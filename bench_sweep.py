@@ -280,7 +280,7 @@ def config4(args, out):
     assert np.array_equal(sub.reshape(-1), exp)
     total = int(res[0].sum())
     gbs = algo / (ms * 1e-3) / 1e9
-    out({"config": 4, "query": "GroupBy(Rows(a), Rows(b)) 256x256", "shards": S, "records": total, "kernel": ("groupby_shard_kernel" if os.environ.get("FBGPU_GROUPBY_HASH") else "groupby_direct_kernel"), "ms": ms, "ms_min": ms_min, "wall_ms": wall,
+    out({"config": 4, "query": "GroupBy(Rows(a), Rows(b)) 256x256", "shards": S, "records": total, "kernel": "groupby_direct_kernel", "ms": ms, "ms_min": ms_min, "wall_ms": wall,
          "records_per_sec": total / (ms * 1e-3), "group_counts_per_sec": 65536 * S / (ms * 1e-3), "algorithmic_bytes": int(algo), "payload_bytes": int(pa + pb),
          "achieved_gbs": gbs, "peak_gbs": pk, "peak_source": src, "frac": gbs / pk, "nonzero_groups": int((res[0] > 0).sum()),
          "note": f"this GPU's 1/8 share ({S} of 4096 shards) of the 100 M-record config; load {time.time() - t0:.1f}s"})

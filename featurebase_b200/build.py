@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = "arch=compute_90a,code=sm_90a"      # H100 (Hopper); the kernels use its cp.async.bulk / mbarrier PTX
+ARCH = "arch=compute_90a,code=sm_90a"      # H100 (Hopper)
 
 
 def _stale(target, sources):

@@ -230,13 +230,10 @@ extern "C" int fbgpu_init(int32_t device_ordinal, fbgpu_ctx** out) try {
     }
     // opt in to large dynamic shared memory once
     CUDA_TRY(cudaFuncSetAttribute(eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 17 * 8192));
-    CUDA_TRY(cudaFuncSetAttribute(eval_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 233472 / 2 - 1024 - 5888));
     CUDA_TRY(cudaFuncSetAttribute(pair_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPcWarps * 8192));
     CUDA_TRY(cudaFuncSetAttribute(row_count_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
     CUDA_TRY(cudaFuncSetAttribute(row_count_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
-    CUDA_TRY(cudaFuncSetAttribute(groupby_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGbSlots * 4 + 8192));
-    CUDA_TRY(cudaFuncSetAttribute(groupby_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGbSlots * 4 + 8192));
-    CUDA_TRY(cudaFuncSetAttribute(groupby_shard_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGhSmemBytes));
+    CUDA_TRY(cudaFuncSetAttribute(groupby_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGbSlots * 4 + 8192));
     CUDA_TRY(cudaFuncSetAttribute(groupby_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGdSmemBytes));
     { int nb = 0; if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, groupby_direct_kernel, kGdThreads, kGdSmemBytes) == cudaSuccess && nb > 0) c->gd_ctas_per_sm = nb; }
     { int nb = 0; if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, pair_count_kernel, kPcWarps * 32, kPcWarps * 8192) == cudaSuccess && nb > 0) c->pair_ctas_per_sm = nb; }
@@ -393,19 +390,14 @@ static int add_items_locked(fbgpu_ctx* c, StoreTxn& txn, uint32_t fv, uint64_t s
         hf.n_desc++; hf.payload_bytes += cont_bytes(d.typ, d.card, d.cnt);
         if (d.typ == kArray) hf.n_arr++; else if (d.typ == kBitmap) hf.n_bmp++; else hf.n_run++;
     }
-    // payloads: row-major (key order) by default: a row's 16 containers are contiguous, which is what the common
-    // few-rows-of-many query streams.  FBGPU_LAYOUT_SLOT_MAJOR=1 stores all rows of slot 0, then slot 1, ... so that a
-    // (shard, slot) unit's consecutive rows are adjacent (it made no significant difference when measured).
+    // payloads: row-major (key order): a row's 16 containers are contiguous, which is what the common
+    // few-rows-of-many query streams.
     // striped order: only for array-dominated fragments, so that bitmap-heavy views (BSI planes) keep every
     // array sorted and stay eligible for the word-parallel kernel, whose slice search needs sorted arrays
     if (!pred) hf.stripe_policy = c->stripe_arrays && (uint64_t)hf.n_arr * 8 > (uint64_t)hf.n_bmp + hf.n_run;
     const bool stripe = hf.stripe_policy;
     if (stripe) for (size_t i = 0; i < items.size(); i++) { const ContDesc& d = c->h_descs[desc0 + i]; if (d.typ == kArray && d.card >= fbgpu_stripe::kMinStripe) hf.n_striped++; }
-    std::vector<uint32_t> order(items.size());
-    for (uint32_t i = 0; i < items.size(); i++) order[i] = i;
-    static const bool slot_major = getenv("FBGPU_LAYOUT_SLOT_MAJOR") != nullptr;   // default: row-major (key order)
-    if (slot_major) std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return items[a].key % kSlotsPerRow < items[b].key % kSlotsPerRow; });
-    for (uint32_t i : order) {
+    for (size_t i = 0; i < items.size(); i++) {
         if (!items[i].pc) continue;                             // kept: its descriptor already points at the payload
         const ParsedCont& pc = *items[i].pc;
         uint64_t pos = c->uploaded + c->staging.len;
@@ -969,7 +961,7 @@ static int upload_inputs(Workspace* w, const std::vector<DevOp>& prog, const uin
     return 0;
 }
 
-// runs of commuting row ops ([k,e) of D_OR_ROW / D_ANDNOT_ROW / D_XOR_ROW): the staged kernel prefetches them by TMA
+// runs of commuting row ops ([k,e) of D_OR_ROW / D_ANDNOT_ROW / D_XOR_ROW): eval_kernel applies each run as one batch
 static std::vector<int2> find_batches(const std::vector<DevOp>& prog) {
     std::vector<int2> b;
     for (size_t k = 0; k < prog.size();) {
@@ -984,8 +976,6 @@ static int launch_eval(fbgpu_ctx* c, Workspace* w, const std::vector<DevOp>& pro
     if (n_units <= 0) return 0;
     const int n_ops = (int)prog.size();
     std::vector<int2> batches = find_batches(prog);
-    size_t staged_rows = 0; for (auto& b : batches) staged_rows += (size_t)(b.y - b.x);
-    // TMA-staged variant: opt-in (FBGPU_STAGED=1) until it beats the direct kernel
     // Word-parallel kernel for bitmap-heavy programs (BSI plane sweeps, dense rows): chosen when the views the
     // program references hold few array containers.  Row results (out.info) need cross-slice run counts: not here.
     if (!out.info && n_ops <= kWpMaxOps && depth <= kWpMaxDepth && !getenv("FBGPU_NO_WORDPAR")) {
@@ -1000,24 +990,8 @@ static int launch_eval(fbgpu_ctx* c, Workspace* w, const std::vector<DevOp>& pro
             return 0;
         }
     }
-    const bool staged = getenv("FBGPU_STAGED") && n_ops <= kStagedMaxOps && staged_rows >= 4;
     // the batch table travels in front of the program in the same H2D copy (upload_inputs); see d_batches()
     const int2* d_batches = reinterpret_cast<const int2*>(w->d_aux.p);
-    if (staged) {
-        // N CTAs per SM (default 2): (depth+1) stack bitmaps + two TMA stages each
-        int ctas = 2;
-        if (const char* e = getenv("FBGPU_STAGE_CTAS")) ctas = std::max(1, std::min(4, atoi(e)));
-        const size_t per_cta = 233472 / ctas - 1024 - 5888;                         // SM smem / N - per-CTA reserve - static smem of the kernel
-        size_t stack = (size_t)(depth + 1) * 8192;
-        if (stack + 2 * 8192 <= per_cta) {
-            uint32_t stg = (uint32_t)(((per_cta - stack) / 2) & ~size_t(127));
-            long long grid = std::min<long long>(n_units, (long long)c->sm_count * ctas);
-            size_t smem = stack + 2 * (size_t)stg;
-            eval_staged_kernel<<<(unsigned)grid, kEvalThreads, smem, w->stream>>>(store_ref(c), d_prog, n_ops, depth, d_batches, (int)batches.size(), stg, d_shards, n_units, out);
-            CUDA_TRY(cudaGetLastError());
-            return 0;
-        }
-    }
     size_t smem = (size_t)(depth + 1) * 8192;
     int per_sm = std::max(1, (int)std::min<size_t>(std::min(FBGPU_EVAL_MIN_BLOCKS, 2048 / kEvalThreads), (227 * 1024) / (smem + 3 * 1024 + 512)));
     long long grid = std::min<long long>(n_units, (long long)c->sm_count * per_sm);
@@ -1607,11 +1581,15 @@ extern "C" int fbgpu_any(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int3
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ GroupBy
-// Slots per CTA of groupby_shard_kernel (16, 8, 4, 2 or 1), or 0 when the fields are not its shape: picked so that a group of
-// slots of field a holds at most ~8 k columns (2/5 of what the table takes), from the cardinality of a sample of the listed shards' fragments.
-static int groupby_slots_per_group(fbgpu_ctx* c, uint32_t fvA, uint32_t fvB, const uint64_t* shards, int64_t n) {
-    if (fvA >= c->shardmaps.size() || fvB >= c->shardmaps.size() || n <= 0) return 0;
-    if (c->view_other[fvA] * 8 > c->view_arr[fvA] || c->view_other[fvB] * 8 > c->view_arr[fvB]) return 0;     // bitmap / run heavy: the per-slot kernels
+// Largest average number of field-a columns per (shard, slot) that groupby_direct_kernel is given: the size its predecessor, a
+// hash table per group of slots, was built for.  Whether the direct kernel is also the faster one above it has not been measured.
+constexpr uint64_t kGdMaxSlotCols = 8192;
+
+// groupby_direct_kernel's shape: both fields array-dominated, and field a holding at most kGdMaxSlotCols columns per slot on
+// average, from the cardinality of a sample of the listed shards' fragments.
+static bool groupby_direct_eligible(fbgpu_ctx* c, uint32_t fvA, uint32_t fvB, const uint64_t* shards, int64_t n) {
+    if (fvA >= c->shardmaps.size() || fvB >= c->shardmaps.size() || n <= 0) return false;
+    if (c->view_other[fvA] * 8 > c->view_arr[fvA] || c->view_other[fvB] * 8 > c->view_arr[fvB]) return false;     // bitmap / run heavy: groupby_kernel
     const auto& sm = c->shardmaps[fvA];
     uint64_t elems = 0, seen = 0;
     const int64_t step = std::max<int64_t>(1, n / 64);
@@ -1620,13 +1598,9 @@ static int groupby_slots_per_group(fbgpu_ctx* c, uint32_t fvA, uint32_t fvB, con
         if (sh >= sm.size() || sm[sh] < 0) continue;
         elems += c->frags[(size_t)sm[sh]].payload_bytes / 2; seen++;
     }
-    if (!seen) return 16;
+    if (!seen) return true;
     const uint64_t avg = elems / seen;                       // columns of field a per shard (all its rows: an upper bound for a row subset)
-    // (BASELINE config 4, 24.4 k columns per shard: 4 slots per group = 6.1 k entries fill the table to 19 %; 8 slots = 12.2 k entries to
-    // 37 %, which is slower — longer probe walks and half as many units to balance over the SMs)
-    static const uint64_t target = [] { const char* e = getenv("FBGPU_GH_TARGET"); const long long n = e ? atoll(e) : 0; return (uint64_t)(n > 0 ? n : (long long)kGhMaxEntries * 2 / 5); }();
-    for (int spg = 16; spg >= 1; spg >>= 1) if (avg * (uint64_t)spg / 16 <= std::min<uint64_t>(target, kGhMaxEntries * 3 / 5)) return spg;
-    return 0;
+    return avg / kSlotsPerRow <= kGdMaxSlotCols;
 }
 
 static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* rowsA, int nA, uint32_t fvB, const uint64_t* rowsB, int nB,
@@ -1652,17 +1626,14 @@ static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* 
         if (have_filter) { rc = eval_filter_batch(c, w, prog, depth, d_prog, d_shards + s0, ns); if (rc) return rc; launches++; }
         long long units = (long long)ns * kSlotsPerRow;
         long long grid = std::min<long long>(units, (long long)c->sm_count * 4);
-        static const bool gb_fast = getenv("FBGPU_GROUPBY_FAST") != nullptr;    // thread-per-row passes of the CTA kernel (kernels.cuh)
         static const bool gb_cta_only = getenv("FBGPU_GROUPBY_CTA") != nullptr; // round-1 path only: one CTA per unit
-        auto cta_kernel = gb_fast ? groupby_kernel<true> : groupby_kernel<false>;
-        const int spg = gb_cta_only ? 0 : groupby_slots_per_group(c, fvA, fvB, shards + s0, ns);
-        const bool gb_hash = getenv("FBGPU_GROUPBY_HASH") != nullptr;           // groupby_shard_kernel (hash table per group of slots) instead of groupby_direct_kernel
-        if (spg > 0 && !gb_hash && units < (1ll << 31)) {
+        if (!gb_cta_only && units < (1ll << 31) && groupby_direct_eligible(c, fvA, fvB, shards + s0, ns)) {
             // array-dominated fields: groupby_direct_kernel, one CTA per (shard, slot), 256 a-rows per launch; what it declines is listed
-            // for the CTA kernel, launched only when the list is not empty (the 4-byte count is read back first, see below)
+            // for groupby_kernel, launched only when the list is not empty (its launch alone costs tens of microseconds next to a kernel
+            // with another shared-memory carve-out) — the 4-byte count is read back first
             if (w->d_emit_units.ensure((size_t)(units + 1) * 4)) return FBGPU_E_NOMEM;
             unsigned int* d_fb = (unsigned int*)w->d_emit_units.p;
-            unsigned int* h_fb = (unsigned int*)w->h_in.p;
+            unsigned int* h_fb = (unsigned int*)w->h_in.p;          // (pinned; upload_inputs sized it, its content is in flight no longer: the stream was synchronised above)
             const long long dgrid = std::min<long long>(units, (long long)c->sm_count * c->gd_ctas_per_sm);
             for (int a0 = 0; a0 < nA; a0 += kGdThreads) {
                 const int na = std::min(kGdThreads, nA - a0);
@@ -1677,39 +1648,15 @@ static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* 
                 CUDA_TRY(cudaStreamSynchronize(w->stream));
                 const unsigned int n_fb = *h_fb;
                 if (n_fb) {
-                    cta_kernel<<<(unsigned)std::min<long long>(n_fb, grid), kGbThreads, smem, w->stream>>>(store_ref(c), fvA, d_ra, na, fvB, (const uint64_t*)w->d_rows.p + nA, nB,
+                    groupby_kernel<<<(unsigned)std::min<long long>(n_fb, grid), kGbThreads, smem, w->stream>>>(store_ref(c), fvA, d_ra, na, fvB, (const uint64_t*)w->d_rows.p + nA, nB,
                         d_shards + s0, units, have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, d_cnt, d_fb);
                     CUDA_TRY(cudaGetLastError()); launches++;
                     CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
                 }
                 fb_units += n_fb; all_units += (uint64_t)units;
             }
-        } else if (spg > 0 && units < (1ll << 31)) {
-            // one CTA per (shard, group of `spg` slots): contiguous descriptor / payload reads.  The units it declines are listed for
-            // the CTA kernel, which is launched only when the list is not empty (its launch alone costs tens of microseconds next to
-            // a kernel with another shared-memory carve-out) — the 4-byte count is read back first.
-            if (w->d_emit_units.ensure((size_t)(units + 1) * 4)) return FBGPU_E_NOMEM;
-            unsigned int* d_fb = (unsigned int*)w->d_emit_units.p;
-            CUDA_TRY(cudaMemsetAsync(d_fb, 0, 4, w->stream));
-            const long long hunits = ns * (kSlotsPerRow / spg);
-            const long long hgrid = std::min<long long>(hunits, (long long)c->sm_count * (1024 / kGhThreads));
-            groupby_shard_kernel<<<(unsigned)hgrid, kGhThreads, kGhSmemBytes, w->stream>>>(store_ref(c), fvA, (const uint64_t*)w->d_rows.p, nA, fvB, (const uint64_t*)w->d_rows.p + nA, nB,
-                d_shards + s0, ns, spg, have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p, d_fb);
-            CUDA_TRY(cudaGetLastError()); launches++;
-            CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
-            unsigned int* h_fb = (unsigned int*)w->h_in.p;          // (pinned; upload_inputs sized it, its content is in flight no longer: the stream was synchronised above)
-            CUDA_TRY(cudaMemcpyAsync(h_fb, d_fb, 4, cudaMemcpyDeviceToHost, w->stream));
-            CUDA_TRY(cudaStreamSynchronize(w->stream));
-            const unsigned int n_fb = *h_fb;
-            if (n_fb) {
-                cta_kernel<<<(unsigned)std::min<long long>(n_fb, grid), kGbThreads, smem, w->stream>>>(store_ref(c), fvA, (const uint64_t*)w->d_rows.p, nA, fvB, (const uint64_t*)w->d_rows.p + nA, nB,
-                    d_shards + s0, units, have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p, d_fb);
-                CUDA_TRY(cudaGetLastError()); launches++;
-                CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
-            }
-            fb_units += n_fb; all_units += (uint64_t)units;
         } else {
-            cta_kernel<<<(unsigned)grid, kGbThreads, smem, w->stream>>>(store_ref(c), fvA, (const uint64_t*)w->d_rows.p, nA, fvB, (const uint64_t*)w->d_rows.p + nA, nB,
+            groupby_kernel<<<(unsigned)grid, kGbThreads, smem, w->stream>>>(store_ref(c), fvA, (const uint64_t*)w->d_rows.p, nA, fvB, (const uint64_t*)w->d_rows.p + nA, nB,
                 d_shards + s0, units, have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p, nullptr);
             CUDA_TRY(cudaGetLastError()); launches++;
             CUDA_TRY(cudaEventRecord(w->ev1, w->stream));

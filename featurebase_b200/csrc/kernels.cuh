@@ -446,278 +446,6 @@ eval_kernel(StoreRef st, const DevOp* __restrict__ prog, int n_ops, int depth,
 }
 
 // ------------------------------------------------------------------------------------------------
-// eval_staged_kernel: same program machine as eval_kernel, but the operands of every batch (run of commuting
-// OR/ANDNOT/XOR row ops) are first copied into a two-stage shared-memory ring by the TMA engine
-// (cp.async.bulk global->shared, one bulk copy per container, completion on an mbarrier) while the previous
-// sub-batch is being scattered, and the next unit's descriptor chains are walked while the current unit runs.
-// The scatter therefore reads its operands from shared memory and never waits on HBM latency; the only steady
-// state limiter left is shared-memory atomic throughput.
-// ------------------------------------------------------------------------------------------------
-constexpr int kStageOps = 32;          // operands per sub-batch (one bulk copy per lane of warp 0)
-constexpr int kStagedMaxOps = 128;     // programs longer than this use eval_kernel
-
-struct SubBatch { int seq, b, o0, n; uint32_t total, pad; uint32_t off[kStageOps]; uint32_t bytes[kStageOps]; };
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory"); }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}" : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
-template <int MODE>
-__device__ __forceinline__ void stage_scatter(uint32_t* T32, const uint8_t* stage, const SubBatch& S, const Resolved* R) {
-    const int tid = threadIdx.x, n = S.n;
-    int G = kEvalThreads / max(n, 1);
-    G = G >= 32 ? 32 : G <= 1 ? 1 : (1 << (31 - __clz(G)));
-    const int groups = kEvalThreads / G, g = tid & (G - 1);
-    for (int j = tid / G; j < n; j += groups) {
-        const uint32_t sz = S.bytes[j];
-        if (!sz) continue;
-        const Resolved r = R[S.o0 + j];
-        const uint4* src = reinterpret_cast<const uint4*>(stage + S.off[j]);
-        if (r.typ == kArray) {
-            const uint32_t n8 = sz >> 4;
-            for (uint32_t i = g; i < n8; i += G) scatter_chunk_unrolled<MODE>(T32, src[i], i * 8, r.card);
-        } else {
-            for (int i = g; i < 512; i += G) {
-                uint4 v = src[i];
-                uint32_t w[4] = { v.x, v.y, v.z, v.w };
-#pragma unroll
-                for (int c = 0; c < 4; c++) {
-                    if (!w[c]) continue;
-                    uint32_t* dst = &T32[4 * i + c];
-                    if (MODE == 0) atomicOr(dst, w[c]); else if (MODE == 1) atomicAnd(dst, ~w[c]); else atomicXor(dst, w[c]);
-                }
-            }
-        }
-    }
-}
-
-#ifndef FBGPU_STAGED_MIN_BLOCKS
-#define FBGPU_STAGED_MIN_BLOCKS 2
-#endif
-__global__ void __launch_bounds__(kEvalThreads, FBGPU_STAGED_MIN_BLOCKS)
-eval_staged_kernel(StoreRef st, const DevOp* __restrict__ prog, int n_ops, int depth,
-                   const int2* __restrict__ batches, int n_batches, uint32_t stg_bytes,
-                   const uint64_t* __restrict__ shards, long long n_units, EvalOut out) {
-    extern __shared__ uint4 smem4[];
-    __shared__ Resolved res2[2][kStagedMaxOps];
-    __shared__ SubBatch sb[2];
-    __shared__ __align__(8) uint64_t mbar[2];
-    __shared__ int it_seq, it_b, it_o, s_ni;
-    __shared__ uint32_t warp_tmp[kEvalThreads / 32], warp_tmp2[kEvalThreads / 32];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    uint8_t* stage0 = reinterpret_cast<uint8_t*>(smem4 + (size_t)(depth + 1) * 512);
-    const long long n_seq = (n_units - blockIdx.x + gridDim.x - 1) / gridDim.x;   // units of this CTA: blockIdx.x + seq*gridDim.x
-    if (n_seq <= 0) return;
-    if (tid == 0) { mbar_init(&mbar[0], 1); mbar_init(&mbar[1], 1); it_seq = 0; it_b = 0; it_o = n_batches ? batches[0].x : 0; s_ni = 0; asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-    int nc = 0;                       // sub-batches consumed so far (uniform)
-    unsigned long long cta_total = 0;
-
-    auto resolve_unit = [&](long long seq) {
-        if (tid < n_ops) {
-            const long long unit = blockIdx.x + seq * gridDim.x;
-            DevOp op = prog[tid];
-            Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
-            if (op.op >= D_PUSH_ROW && op.op <= D_ORANDNOT_ROW && op.op != D_PUSH_EMPTY) r = resolve(st, op.fv, shards[unit >> 4], op.row, (int)(unit & 15));
-            res2[seq & 1][tid] = r;
-        }
-    };
-    // warp 0: issue sub-batches while a stage is free and descriptors are available (units < avail).
-    // Lane j sizes operand o+j; a warp scan gives the packed stage offsets; one bulk copy per operand.
-    auto pump = [&](long long avail) {
-        for (;;) {
-            const int ni = s_ni;
-            if (ni - nc >= 2) break;
-            const int buf = ni & 1;
-            int seq = it_seq, b = it_b, o = it_o;       // uniform across the warp (read after __syncwarp below)
-            bool found = false;
-            while (seq < avail) {
-                if (b >= n_batches) { seq++; b = 0; o = n_batches ? batches[0].x : 0; continue; }
-                const int2 bt = batches[b];
-                if (o >= bt.y) { b++; if (b < n_batches) o = batches[b].x; continue; }
-                const Resolved* R = res2[seq & 1];
-                const bool in_range = o + lane < bt.y;
-                Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
-                if (in_range) r = R[o + lane];
-                const uint32_t sz = !r.ptr ? 0u : r.typ == kArray ? ((r.card + 7) >> 3) * 16u : r.typ == kBitmap ? 8192u : 0u;
-                uint32_t incl = sz;
-#pragma unroll
-                for (int d = 1; d < 32; d <<= 1) { uint32_t x = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += x; }
-                const unsigned bad = __ballot_sync(0xffffffffu, !in_range || (incl > stg_bytes && lane > 0));
-                const int n = bad ? __ffs(bad) - 1 : 32;        // operands taken by this sub-batch (>= 1)
-                const uint32_t total = __shfl_sync(0xffffffffu, incl, n - 1);
-                if (total == 0) { o += n; continue; }            // nothing stageable (absent / run operands)
-                SubBatch& S = sb[buf];
-                if (lane < n) { S.off[lane] = incl - sz; S.bytes[lane] = sz; }
-                if (lane == 0) { S.seq = seq; S.b = b; S.o0 = o; S.n = n; S.total = total; mbar_expect_tx(&mbar[buf], total); }
-                __syncwarp();
-                if (lane < n && sz) tma_bulk_g2s(stage0 + (size_t)buf * stg_bytes + (incl - sz), r.ptr, sz, &mbar[buf]);
-                o += n;
-                found = true;
-                break;
-            }
-            if (lane == 0) { it_seq = seq; it_b = b; it_o = o; if (found) s_ni = ni + 1; }
-            __syncwarp();
-            if (!found) break;
-        }
-    };
-
-    resolve_unit(0);
-    int runs_cur = __syncthreads_or(tid < n_ops && res2[0][tid].typ == kRun && res2[0][tid].ptr != nullptr), runs_next = 0;
-
-    for (long long seq = 0; seq < n_seq; seq++) {
-        const long long unit = blockIdx.x + seq * gridDim.x;
-        const Resolved* res = res2[seq & 1];
-        // descriptors of the next unit are resolved now (the chains overlap with the bulk copies already in flight)
-        if (seq + 1 < n_seq) resolve_unit(seq + 1);
-        runs_next = __syncthreads_or(seq + 1 < n_seq && tid < n_ops && res2[(seq + 1) & 1][tid].typ == kRun && res2[(seq + 1) & 1][tid].ptr != nullptr);
-        const long long avail = min(n_seq, seq + 2);
-        if (wid == 0) pump(avail);
-        uint64_t map = 0xFEDCBA9876543210ull;
-        int top = -1;
-        auto phys = [&](int level) -> uint4* { return smem4 + (size_t)((map >> (4 * level)) & 15u) * 512; };
-        auto swap_levels = [&](int a, int b) {
-            uint64_t pa = (map >> (4 * a)) & 15u, pb = (map >> (4 * b)) & 15u;
-            map &= ~((15ull << (4 * a)) | (15ull << (4 * b)));
-            map |= (pb << (4 * a)) | (pa << (4 * b));
-        };
-        int cur_batch = 0;
-        for (int k = 0; k < n_ops; k++) {
-            const uint8_t opc = prog[k].op;
-            if (opc == D_PUSH_EMPTY) { top++; bm_zero(phys(top)); __syncthreads(); continue; }
-            if (opc == D_SWAP) { swap_levels(top, top - 1); continue; }
-            if (opc == D_POP) { top--; continue; }
-            if (opc >= D_AND && opc <= D_XOR) {
-                int kind = opc == D_AND ? K_AND : opc == D_OR ? K_OR : opc == D_ANDNOT ? K_ANDNOT : K_XOR;
-                bm_apply_smem(kind, phys(top - 1), nullptr, phys(top));
-                top--; __syncthreads(); continue;
-            }
-            if (opc == D_OR_ROW || opc == D_ANDNOT_ROW || opc == D_XOR_ROW) {
-                // this op starts batch `cur_batch` = ops [k, e)
-                const int e = batches[cur_batch].y;
-                uint4* T = phys(top);
-                uint32_t* T32 = reinterpret_cast<uint32_t*>(T);
-                for (;;) {
-                    __syncthreads();                                   // stage info / s_ni written by warp 0 are visible; previous scatter done
-                    const int ni = s_ni;
-                    if (nc >= ni) break;
-                    const int buf = nc & 1;
-                    if (sb[buf].seq != (int)seq || sb[buf].b != cur_batch) break;
-                    if (wid == 0) pump(avail);                         // keep the other stage busy
-                    const uint32_t parity = (uint32_t)(nc >> 1) & 1u;
-                    while (!mbar_try_wait(&mbar[buf], parity)) { }
-                    const uint8_t* stg = stage0 + (size_t)buf * stg_bytes;
-                    if (opc == D_OR_ROW) stage_scatter<0>(T32, stg, sb[buf], res);
-                    else if (opc == D_ANDNOT_ROW) stage_scatter<1>(T32, stg, sb[buf], res);
-                    else stage_scatter<2>(T32, stg, sb[buf], res);
-                    nc++;
-                }
-                if (runs_cur) for (int j = k; j < e; j++) {            // run containers: CTA-wide expansion, one at a time
-                    const Resolved r = res[j];
-                    if (r.ptr == nullptr || r.typ != kRun) continue;
-                    uint4* S = phys(depth);
-                    bm_expand_runs(S, reinterpret_cast<const uint16_t*>(r.ptr), r.cnt, warp_tmp);
-                    bm_apply_smem(opc == D_OR_ROW ? K_OR : opc == D_ANDNOT_ROW ? K_ANDNOT : K_XOR, T, nullptr, S);
-                    __syncthreads();
-                }
-                cur_batch++;
-                k = e - 1;
-                continue;
-            }
-            // single row-operand ops (PUSH_ROW, AND_ROW, ORAND_ROW, ORANDNOT_ROW)
-            int kind = opc == D_PUSH_ROW ? K_PUSH : opc == D_AND_ROW ? K_AND : opc == D_ORAND_ROW ? K_ORAND : K_ORANDNOT;
-            const Resolved r = res[k];
-            if (kind == K_PUSH) top++;
-            uint4* T = phys(top);
-            uint4* B = (kind == K_ORAND || kind == K_ORANDNOT) ? phys(top - 1) : nullptr;
-            if (r.ptr == nullptr) {
-                if (kind == K_PUSH || kind == K_AND) bm_zero(T);
-                else if (kind == K_ORANDNOT) bm_apply_smem(K_OR, B, nullptr, T);
-                __syncthreads();
-            } else if (r.typ == kBitmap) {
-                bm_apply_global(kind, T, B, reinterpret_cast<const uint4*>(r.ptr));
-                __syncthreads();
-            } else if (r.typ == kArray) {
-                const uint16_t* arr = reinterpret_cast<const uint16_t*>(r.ptr);
-                uint32_t* T32 = reinterpret_cast<uint32_t*>(T);
-                if (kind == K_PUSH) { bm_zero(T); __syncthreads(); bm_scatter<0>(T32, arr, r.card); }
-                else if (kind == K_ORAND) bm_filter_scatter(reinterpret_cast<uint32_t*>(B), T32, arr, r.card);
-                else if (kind == K_AND) {
-                    uint4* S = phys(depth);
-                    bm_zero(S); __syncthreads();
-                    bm_filter_scatter(reinterpret_cast<uint32_t*>(S), T32, arr, r.card);
-                    swap_levels(top, depth);
-                } else {
-                    uint4* S = phys(depth);
-                    bm_zero(S); __syncthreads();
-                    bm_scatter<0>(reinterpret_cast<uint32_t*>(S), arr, r.card); __syncthreads();
-                    bm_apply_smem(K_ORANDNOT, T, B, S);
-                }
-                __syncthreads();
-            } else {
-                const uint16_t* runs = reinterpret_cast<const uint16_t*>(r.ptr);
-                if (kind == K_PUSH) bm_expand_runs(T, runs, r.cnt, warp_tmp);
-                else {
-                    uint4* S = phys(depth);
-                    bm_expand_runs(S, runs, r.cnt, warp_tmp);
-                    bm_apply_smem(kind, T, B, S);
-                    __syncthreads();
-                }
-            }
-        }
-        // ---- unit epilogue (same as eval_kernel)
-        uint32_t cnt = 0, nruns = 0;
-        if (top >= 0) {
-            const uint4* R = phys(top);
-            const uint64_t* R64 = reinterpret_cast<const uint64_t*>(R);
-#pragma unroll
-            for (int h = 0; h < kEvalU4PerThread; h++) {
-                int i = tid + h * kEvalThreads;
-                uint4 a = R[i];
-                cnt += popc4(a);
-                if (out.bitmaps) out.bitmaps[(size_t)unit * 512 + i] = a;
-                if (out.info) {
-#pragma unroll
-                    for (int q = 0; q < 2; q++) {
-                        int wi = 2 * i + q;
-                        uint64_t v = R64[wi];
-                        uint64_t prev = wi ? (R64[wi - 1] >> 63) : 0ull;
-                        nruns += __popcll(v & ~((v << 1) | prev));
-                    }
-                }
-            }
-        } else if (out.bitmaps) {
-#pragma unroll
-            for (int h = 0; h < kEvalU4PerThread; h++) out.bitmaps[(size_t)unit * 512 + tid + h * kEvalThreads] = make_uint4(0, 0, 0, 0);
-        }
-        cnt = __reduce_add_sync(0xffffffffu, cnt);
-        nruns = __reduce_add_sync(0xffffffffu, nruns);
-        __syncthreads();
-        if (lane == 0) { warp_tmp[wid] = cnt; warp_tmp2[wid] = nruns; }
-        __syncthreads();
-        if (tid == 0) {
-            uint32_t c = 0, rr = 0;
-#pragma unroll
-            for (int q = 0; q < kEvalThreads / 32; q++) { c += warp_tmp[q]; rr += warp_tmp2[q]; }
-            cta_total += c;
-            if (out.per_shard && c) atomicAdd(&out.per_shard[unit >> 4], (unsigned long long)c);
-            if (out.info) out.info[unit] = make_uint2(c, rr);
-        }
-        runs_cur = runs_next;
-        __syncthreads();
-    }
-    if (tid == 0 && out.total) { if (cta_total) atomicAdd(out.total, cta_total); fused_allreduce_tail(out.fr, out.total, gridDim.x); }
-}
-
-// ------------------------------------------------------------------------------------------------
 // eval_wordpar_kernel: word-parallel evaluation for bitmap-heavy programs (BSI plane sweeps, dense rows).
 // Every thread owns ONE 128-bit slice (uint4) of a (shard, slot) stripe and runs the whole program on it with the
 // operand stack in registers: no shared-memory bitmaps, no barriers between ops, and the operands of the next three
@@ -1729,20 +1457,6 @@ constexpr int kGbSlots = 8192;          // open-addressing table slots per CTA (
 constexpr int kGbPool = kGbSlots / 2;   // entries per pass (load factor <= 0.5)
 constexpr uint32_t kGbEmpty = 0xffffffffu;
 constexpr uint32_t kGbDenseCard = 4096; // a-rows at/above this cardinality (or non-array) use the bitmap pass
-constexpr uint32_t kGbSmallCard = 32;   // kFast: arrays up to this cardinality are walked by one thread each
-
-// one thread walks a small array container, 8 elements per 16-byte load (array payloads start 16-byte aligned and are
-// allocated in 16-byte units, so the last load stays inside the container's allocation; elements past card are skipped)
-template <class F>
-__device__ __forceinline__ void thread_for_each_small(const Resolved& c, F f) {
-    const uint4* p = reinterpret_cast<const uint4*>(c.ptr);
-    for (uint32_t k0 = 0; k0 < c.card; k0 += 8) {
-        const uint4 v = ldg_nc(p + (k0 >> 3));
-        const uint32_t w[4] = { v.x, v.y, v.z, v.w };
-#pragma unroll
-        for (int q = 0; q < 8; q++) if (k0 + q < c.card) f((w[q >> 1] >> ((q & 1) * 16)) & 0xffffu);
-    }
-}
 
 template <class F>
 __device__ __forceinline__ void warp_for_each(const Resolved& c, int lane, F f) {
@@ -1773,12 +1487,6 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* tmp, u
     return base + inc - v;
 }
 
-// kFast (opt-in, FBGPU_GROUPBY_FAST=1, not yet run on a GPU): when every a-row container of the chunk is a small array
-// (<= kGbSmallCard elements) and they fit one pass, each thread inserts its own row's elements straight from a 16-byte
-// load — no offset scan, no per-element binary search; small b-row arrays are probed the same way; the fragment check is
-// done by every thread instead of thread 0 + two barriers, and the b-row descriptors of the first chunk are fetched
-// together with the a-rows so that the two dependent-load chains overlap.  kFast == false is the measured kernel.
-template <bool kFast>
 __global__ void __launch_bounds__(kGbThreads)
 groupby_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ rowsA, int nA,
                uint32_t fvB, const uint64_t* __restrict__ rowsB, int nB,
@@ -1794,18 +1502,12 @@ groupby_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ rowsA, in
     __shared__ uint32_t s_any, s_pass_end;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nwarps = kGbThreads / 32;
 
-    const long long n_work = unit_list ? (long long)unit_list[0] : n_units;     // the units groupby_shard_kernel left for this kernel
+    const long long n_work = unit_list ? (long long)unit_list[0] : n_units;     // the units groupby_direct_kernel declined
     for (long long wi = blockIdx.x; wi < n_work; wi += gridDim.x) {
         const long long unit = unit_list ? (long long)unit_list[1 + wi] : wi;
         const uint64_t shard = shards[unit >> 4];
         const int slot = (int)(unit & 15);
         const uint32_t* flt = filter_bitmaps ? reinterpret_cast<const uint32_t*>(filter_bitmaps + (size_t)unit * 512) : nullptr;
-        int resB_chunk = -1;          // kFast: first b-row of the chunk resB[] holds for this unit (-1: none)
-        if (kFast) {      // same test, made by every thread (uniform; the loads are broadcasts) — no barrier
-            bool ok = fvA < st.n_views && fvB < st.n_views;
-            if (ok) { ViewTab va = st.views[fvA], vb = st.views[fvB]; ok = shard < va.n_shards && shard < vb.n_shards && st.shardmap[va.shard_off + shard] >= 0 && st.shardmap[vb.shard_off + shard] >= 0; }
-            if (!ok) continue;
-        } else {
         __syncthreads();
         if (tid == 0) {   // executor.go:8769-8772: a shard missing either fragment contributes nothing
             bool ok = fvA < st.n_views && fvB < st.n_views;
@@ -1814,46 +1516,15 @@ groupby_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ rowsA, in
         }
         __syncthreads();
         if (!s_any) continue;
-        }
 
         for (int a0 = 0; a0 < nA; a0 += kGbThreads) {
             const int chunkA = min(kGbThreads, nA - a0);
             // all a-row descriptor chains of this chunk are walked concurrently (one per thread)
-            bool fastA = false;
-            if (kFast) {
-                Resolved r, rb; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0; rb = r;
-                const bool fetchB = resB_chunk != 0;               // (uniform)
-                if (tid < chunkA) r = resolve(st, fvA, shard, rowsA[a0 + tid], slot);
-                if (fetchB && tid < min(kGbThreads, nB)) rb = resolve(st, fvB, shard, rowsB[tid], slot);
-                const bool small = !r.ptr || (r.typ == kArray && r.card <= kGbSmallCard);
-                __syncthreads();                                   // previous readers of resA / resB / the table are done
-                resA[tid] = r;
-                if (fetchB) { resB[tid] = rb; resB_chunk = 0; }
-                uint32_t total = 0;
-                block_excl_scan(small ? r.card : 0u, scan_tmp, &total);       // (barriers inside: resA / resB are visible after it)
-                fastA = __syncthreads_and(small) && total <= (uint32_t)kGbPool;
-            } else
             { Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
               if (tid < chunkA) r = resolve(st, fvA, shard, rowsA[a0 + tid], slot);
               __syncthreads(); resA[tid] = r; __syncthreads(); }
             int ia = 0;
             while (ia < chunkA) {
-                int pass_end;
-                if (kFast && fastA) {
-                    // ---- the whole chunk in one pass, one thread per a-row
-                    { uint4* t4 = reinterpret_cast<uint4*>(tab); for (int i = tid; i < kGbSlots / 4; i += kGbThreads) t4[i] = make_uint4(kGbEmpty, kGbEmpty, kGbEmpty, kGbEmpty); }
-                    __syncthreads();
-                    const Resolved c = resA[tid];
-                    if (tid < chunkA && c.ptr)
-                        thread_for_each_small(c, [&](uint32_t col) {
-                            if (flt && !((__ldg(flt + (col >> 5)) >> (col & 31)) & 1u)) return;
-                            const uint32_t ent = (col << 16) | (uint32_t)(a0 + tid);
-                            uint32_t h = (col * 40503u) & (kGbSlots - 1);
-                            while (atomicCAS(&tab[h], kGbEmpty, ent) != kGbEmpty) h = (h + 1) & (kGbSlots - 1);
-                        });
-                    pass_end = chunkA;
-                    __syncthreads();
-                } else {
                 // ---- sparse pass [ia, pass_end): pool offsets = exclusive prefix over row cardinalities (deterministic)
                 const Resolved mine = resA[tid];
                 const bool in_range = tid >= ia && tid < chunkA;
@@ -1866,7 +1537,7 @@ groupby_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ rowsA, in
                 offA[tid] = off;
                 { uint4* t4 = reinterpret_cast<uint4*>(tab); for (int i = tid; i < kGbSlots / 4; i += kGbThreads) t4[i] = make_uint4(kGbEmpty, kGbEmpty, kGbEmpty, kGbEmpty); }
                 __syncthreads();
-                pass_end = (int)s_pass_end;
+                const int pass_end = (int)s_pass_end;
                 {   // flat: one thread per a-element of the pass; the owning row is found by binary search over offA[]
                     const uint32_t total = pass_end < chunkA ? offA[pass_end] : (offA[chunkA - 1] + ((resA[chunkA - 1].ptr && resA[chunkA - 1].typ == kArray && resA[chunkA - 1].card < kGbDenseCard) ? resA[chunkA - 1].card : 0u));
                     for (uint32_t e = tid; e < total; e += kGbThreads) {
@@ -1883,31 +1554,13 @@ groupby_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ rowsA, in
                     }
                 }
                 __syncthreads();
-                }
                 // ---- probe: stream b rows against the table
                 if (pass_end > ia) {
                     for (int b0 = 0; b0 < nB; b0 += kGbThreads) {
                         const int chunkB = min(kGbThreads, nB - b0);
-                        if (!(kFast && resB_chunk == b0))
                         { Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
                           if (tid < chunkB) r = resolve(st, fvB, shard, rowsB[b0 + tid], slot);
-                          __syncthreads(); resB[tid] = r; __syncthreads(); resB_chunk = b0; }
-                        bool fastB = false;
-                        if (kFast) {      // every array of the chunk small: one thread per b-row, straight from its 16-byte loads
-                            const Resolved mb = resB[tid];
-                            fastB = __syncthreads_and(!(tid < chunkB) || !mb.ptr || mb.typ != kArray || mb.card <= kGbSmallCard) != 0;
-                            if (fastB && tid < chunkB && mb.ptr && mb.typ == kArray) {
-                                unsigned long long* cj = counts + (b0 + tid);
-                                thread_for_each_small(mb, [&](uint32_t col) {
-                                    for (uint32_t h = (col * 40503u) & (kGbSlots - 1);; h = (h + 1) & (kGbSlots - 1)) {
-                                        const uint32_t ent = tab[h];
-                                        if (ent == kGbEmpty) break;
-                                        if ((ent >> 16) == col) atomicAdd(cj + (size_t)(ent & 0xffffu) * nB, 1ull);
-                                    }
-                                });
-                            }
-                        }
-                        if (!fastB)
+                          __syncthreads(); resB[tid] = r; __syncthreads(); }
                         {   // arrays: flat thread-per-element (offsets by block scan); bitmap/run rows: warp loop
                             const Resolved mb = resB[tid];
                             const uint32_t nb_ = (tid < chunkB && mb.ptr && mb.typ == kArray) ? mb.card : 0u;
@@ -1965,7 +1618,7 @@ groupby_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ rowsA, in
                             const int chunkB = min(kGbThreads, nB - b0);
                             { Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
                               if (tid < chunkB) r = resolve(st, fvB, shard, rowsB[b0 + tid], slot);
-                              __syncthreads(); resB[tid] = r; __syncthreads(); resB_chunk = b0; }
+                              __syncthreads(); resB[tid] = r; __syncthreads(); }
                             for (int j = wid; j < chunkB; j += nwarps) {
                                 const Resolved bb = resB[j];
                                 if (!bb.ptr) continue;
@@ -1987,171 +1640,14 @@ groupby_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ rowsA, in
 }
 
 // ------------------------------------------------------------------------------------------------
-// groupby_shard_kernel (round 2): the column-keyed join of GroupBy(Rows(a), Rows(b)) for the shape BASELINE config 4 has — hundreds of
-// rows per field, a handful of columns per container — with one CTA per (shard, GROUP OF SLOTS) instead of per (shard, slot).
-// The work of such a query is the descriptor walk (16 B of descriptor for ~12 B of payload).  Per (shard, slot) a unit reads one
-// descriptor out of every row's 16 (a 16-byte read every 256 bytes, and the same for the payload); per group of `spg` adjacent slots
-// thread e = row * spg + slot reads descriptor e and payload chunk e of a contiguous run: whole 128-byte lines, every byte used.
-// Table: kGhSlots x u32 in shared memory (128 KiB, one CTA of 1024 threads per SM), entry = (slot-in-group << 28) | (column << 12) |
-// a-row index in the chunk, linear probing.  A unit goes to `fallback` (-> groupby_kernel per (shard, slot)) before anything is
-// counted when an a- or b-row container is not an array, an a-row holds more than kGhMaxCard columns, or the group holds more entries
-// than 5/8 of the table.
-// ------------------------------------------------------------------------------------------------
-#ifndef FBGPU_GH_THREADS
-#define FBGPU_GH_THREADS 1024
-#endif
-constexpr int kGhThreads = FBGPU_GH_THREADS;      // 1024 (one CTA per SM) or 512 (two)
-constexpr int kGhItems = 2;                       // containers per thread and pass
-constexpr int kGhSlots = kGhThreads * 32;         // 128 KiB (64 KiB)
-constexpr size_t kGhSmemBytes = (size_t)kGhSlots * 4;
-constexpr uint32_t kGhMaxEntries = kGhSlots / 8 * 5;
-constexpr uint32_t kGhMaxCard = 512;
-
-__device__ __forceinline__ uint32_t gh_hash(uint32_t key) { return (key * 2654435761u) >> (kGhThreads == 1024 ? 17 : 18); }   // log2(kGhSlots) bits
-
-__global__ void __launch_bounds__(kGhThreads, 1024 / kGhThreads)
-groupby_shard_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ rowsA, int nA,
-                     uint32_t fvB, const uint64_t* __restrict__ rowsB, int nB,
-                     const uint64_t* __restrict__ shards, long long n_shards, int spg /* slots per group: 1, 2, 4, 8 or 16 */,
-                     const uint4* __restrict__ filter_bitmaps /* per (shard, slot) unit or null */,
-                     unsigned long long* counts /* [nA*nB] */, unsigned int* fallback /* [0] = n, then (shard index * 16 + slot) units */) {
-    extern __shared__ __align__(16) uint32_t gh_tab[];
-    __shared__ uint32_t red[kGhThreads / 32];
-    __shared__ uint32_t s_tot;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int groups = kSlotsPerRow / spg;
-    const int rows_per_pass = (kGhThreads * kGhItems) / spg;         // rows of a field one pass covers (<= 2048: 12-bit row index)
-    const long long n_units = n_shards * groups;
-    for (long long unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
-        const long long si = unit / groups;
-        const int g = (int)(unit - si * groups);
-        const uint64_t shard = shards[si];
-        {   // executor.go:8769-8772: a shard missing either fragment contributes nothing (uniform test, broadcast loads)
-            bool ok = fvA < st.n_views && fvB < st.n_views;
-            if (ok) { const ViewTab va = st.views[fvA], vb = st.views[fvB]; ok = shard < va.n_shards && shard < vb.n_shards && st.shardmap[va.shard_off + shard] >= 0 && st.shardmap[vb.shard_off + shard] >= 0; }
-            if (!ok) continue;
-        }
-        // item e of a pass = (row e / spg of the chunk, slot g * spg + e % spg)
-        auto load_items = [&](uint32_t fv, const uint64_t* rows, int r0, int n, Resolved (&it)[kGhItems]) {
-#pragma unroll
-            for (int k = 0; k < kGhItems; k++) {
-                const int e = tid + k * kGhThreads, i = e / spg;
-                it[k].ptr = nullptr; it[k].card = 0; it[k].typ = 0; it[k].cnt = 0;
-                if (i < n) it[k] = resolve(st, fv, shard, rows[r0 + i], g * spg + (e - i * spg));
-            }
-        };
-        auto block_sum_or = [&](uint32_t v, bool flag, uint32_t& total) -> bool {      // sum of v and OR of flag over the CTA
-            v = __reduce_add_sync(0xffffffffu, v);
-            __syncthreads();                                    // (previous readers of red / s_tot are done)
-            if (lane == 0) red[wid] = v;
-            const int any = __syncthreads_or(flag ? 1 : 0);
-            if (wid == 0) { uint32_t t = lane < kGhThreads / 32 ? red[lane] : 0u; t = __reduce_add_sync(0xffffffffu, t); if (lane == 0) s_tot = t; }
-            __syncthreads();
-            total = s_tot;
-            return any != 0;
-        };
-        // ---- pass 0: nothing may be counted for a unit that ends up in the fallback list, so every a- and b-row of the group is
-        // looked at first when a side needs several passes (a single pass per side is checked on the fly, without extra reads)
-        bool decline = false;
-        const bool multiA = nA > rows_per_pass, multiB = nB > rows_per_pass;
-        if (multiA || multiB) {
-            for (int side = 0; side < 2 && !decline; side++) {
-                const int n = side ? nB : nA;
-                for (int r0 = 0; r0 < n && !decline; r0 += rows_per_pass) {
-                    Resolved it[kGhItems];
-                    load_items(side ? fvB : fvA, side ? rowsB : rowsA, r0, min(rows_per_pass, n - r0), it);
-                    uint32_t cnt = 0; bool bad = false;
-#pragma unroll
-                    for (int k = 0; k < kGhItems; k++) if (it[k].ptr) { bad |= it[k].typ != kArray || (!side && it[k].card > kGhMaxCard); cnt += it[k].card; }
-                    uint32_t tot;
-                    if (block_sum_or(cnt, bad, tot) || (!side && tot > kGhMaxEntries)) decline = true;
-                }
-            }
-        }
-        for (int a0 = 0; a0 < nA && !decline; a0 += rows_per_pass) {
-            const int chunkA = min(rows_per_pass, nA - a0);
-            Resolved ra[kGhItems], rb[kGhItems];
-            load_items(fvA, rowsA, a0, chunkA, ra);
-            if (!multiB) load_items(fvB, rowsB, 0, nB, rb);       // (its descriptor chains run while the a-rows are inserted)
-            uint4 va[kGhItems], vb[kGhItems];                 // first 16-byte chunk of every container, in flight before the first barrier
-            uint32_t cnt = 0; bool bad = false;
-#pragma unroll
-            for (int k = 0; k < kGhItems; k++) {
-                va[k] = vb[k] = make_uint4(0, 0, 0, 0);
-                if (ra[k].ptr) { bad |= ra[k].typ != kArray || ra[k].card > kGhMaxCard; cnt += ra[k].card; if (ra[k].typ == kArray) va[k] = ldg_nc(reinterpret_cast<const uint4*>(ra[k].ptr)); }
-                if (!multiB && rb[k].ptr) { bad |= rb[k].typ != kArray; if (rb[k].typ == kArray) vb[k] = ldg_nc(reinterpret_cast<const uint4*>(rb[k].ptr)); }
-            }
-            uint32_t tot;
-            const bool any_bad = block_sum_or(cnt, bad, tot);
-            if (!multiA && !multiB && (any_bad || tot > kGhMaxEntries)) { decline = true; break; }      // (multi-pass sides were vetted in pass 0)
-            if (tot == 0) continue;
-            {   uint4* t4 = reinterpret_cast<uint4*>(gh_tab);
-#pragma unroll 4
-                for (int k = tid; k < kGhSlots / 4; k += kGhThreads) t4[k] = make_uint4(kGbEmpty, kGbEmpty, kGbEmpty, kGbEmpty); }
-            __syncthreads();
-            // ---- insert the a-rows
-#pragma unroll
-            for (int k = 0; k < kGhItems; k++) {
-                if (!ra[k].ptr) continue;
-                const int e = tid + k * kGhThreads, i = e / spg, sl = e - i * spg;
-                const uint32_t* flt = filter_bitmaps ? reinterpret_cast<const uint32_t*>(filter_bitmaps + ((size_t)si * kSlotsPerRow + g * spg + sl) * 512) : nullptr;
-                const uint4* p = reinterpret_cast<const uint4*>(ra[k].ptr);
-                for (uint32_t k0 = 0; k0 < ra[k].card; k0 += 8) {
-                    const uint4 v = k0 ? ldg_nc(p + (k0 >> 3)) : va[k];
-                    const uint32_t w[4] = { v.x, v.y, v.z, v.w };
-#pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        if (k0 + q >= ra[k].card) break;
-                        const uint32_t col = (w[q >> 1] >> ((q & 1) * 16)) & 0xffffu;
-                        if (flt && !((__ldg(flt + (col >> 5)) >> (col & 31)) & 1u)) continue;
-                        const uint32_t key = ((uint32_t)sl << 16) | col, ent = (key << 12) | (uint32_t)i;
-                        uint32_t h = gh_hash(key);
-                        while (atomicCAS(&gh_tab[h], kGbEmpty, ent) != kGbEmpty) h = (h + 1) & (kGhSlots - 1);
-                    }
-                }
-            }
-            __syncthreads();
-            // ---- probe with the b-rows
-            for (int b0 = 0; b0 < nB; b0 += rows_per_pass) {
-                const int chunkB = min(rows_per_pass, nB - b0);
-                if (multiB) load_items(fvB, rowsB, b0, chunkB, rb);
-#pragma unroll
-                for (int k = 0; k < kGhItems; k++) {
-                    if (!rb[k].ptr) continue;
-                    const int e = tid + k * kGhThreads, i = e / spg, sl = e - i * spg;
-                    unsigned long long* cj = counts + (size_t)a0 * nB + (b0 + i);
-                    const uint4* p = reinterpret_cast<const uint4*>(rb[k].ptr);
-                    for (uint32_t k0 = 0; k0 < rb[k].card; k0 += 8) {
-                        const uint4 v = (k0 || multiB) ? ldg_nc(p + (k0 >> 3)) : vb[k];
-                        const uint32_t w[4] = { v.x, v.y, v.z, v.w };
-#pragma unroll
-                        for (int q = 0; q < 8; q++) {
-                            if (k0 + q >= rb[k].card) break;
-                            const uint32_t key = ((uint32_t)sl << 16) | ((w[q >> 1] >> ((q & 1) * 16)) & 0xffffu);
-                            for (uint32_t h = gh_hash(key);; h = (h + 1) & (kGhSlots - 1)) {
-                                const uint32_t ent = gh_tab[h];
-                                if (ent == kGbEmpty) break;
-                                if ((ent >> 12) == key) atomicAdd(cj + (size_t)(ent & 0xfffu) * nB, 1ull);
-                            }
-                        }
-                    }
-                }
-            }
-            __syncthreads();                                     // the table is cleared for the next a-chunk
-        }
-        if (decline && tid < spg) { const unsigned int k = atomicAdd(&fallback[0], 1u); fallback[1 + k] = (unsigned int)(si * kSlotsPerRow + g * spg + tid); }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// groupby_direct_kernel (round 2): GroupBy(Rows(a), Rows(b)) for the same shape as groupby_shard_kernel — hundreds of rows, a handful of
+// groupby_direct_kernel (round 2): GroupBy(Rows(a), Rows(b)) for array-dominated fields — hundreds of rows, a handful of
 // columns per container — without a hash table.  One CTA of 256 threads per (shard, slot); the 65,536 columns of the slot index a
 // byte table directly: tab[column] = index of the a-row that holds the column (one thread per a-row, at most 256 a-rows per launch:
 // the host chunks longer lists), valid where the 8 KiB presence bitmap has the column's bit.  The presence bit is set with one
 // atomicOr whose return value tells a second a-row of the same column (fields that are not mutually exclusive): that (column, row)
 // goes to a short side list every probe also scans.  Then one thread per b-row looks its columns up: bitmap word, byte, one RED.
-// Per element: ~8 instructions to insert, ~10 to probe, no probe chains, no CAS loops, nothing to clear but the 8 KiB bitmap — the
-// hash kernel spends ~70 warp instructions per probed element at 8-17 of 32 lanes.  72 KiB of shared memory:
+// Per element: ~8 instructions to insert, ~10 to probe, no probe chains, no CAS loops, nothing to clear but the 8 KiB bitmap — a
+// hash table per group of slots (the kernel this one replaced) took ~70 warp instructions per probed element at 8-17 of 32 lanes.  72 KiB of shared memory:
 // three CTAs per SM, so one unit's descriptor chain (views -> row table -> descriptor -> payload) hides behind two other units.
 // Descriptors / payloads are read 16 bytes at a stride of one row (the 16 units of a shard run side by side: the sectors are
 // shared in L2).  A unit is declined — listed in `fallback` for groupby_kernel before anything of it is counted — when a container

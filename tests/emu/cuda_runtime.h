@@ -13,7 +13,7 @@
 //
 // tests/emu/make_emu_source.py rewrites, in a scratch copy of the sources, the three constructs g++ cannot parse:
 // kernel<<<...>>>(...) launches, `extern __shared__ T name[];`, and inline PTX (each known statement is mapped to the
-// emu:: function below; an unknown one becomes emu::unsupported()).
+// emu:: function below; an unknown one fails the rewrite).
 #pragma once
 #include <time.h>
 #include <ucontext.h>
@@ -145,7 +145,6 @@ alignas(128) inline uint8_t g_dyn[kDynSmem];           // dynamic shared memory;
 inline State& S() { return g_state; }
 
 [[noreturn]] inline void die(const char* what) { fprintf(stderr, "[emu] fatal: %s (block %u thread %u)\n", what, S().bid.x, S().cur ? S().cur->tid.x : 0u); abort(); }
-[[noreturn]] inline void unsupported(const char* what) { die(what); }
 
 inline void yield() { State& s = S(); s.switches++; ctx_switch(s.cur->ctx, s.sched); }
 

@@ -6,12 +6,12 @@ gpu-marked parity tests are then re-run against that library in a child process.
 never loads it (featurebase_b200/lib.py loads libfbgpu.so; FBGPU_LIB is the tuning-variant override the child uses), it
 proves nothing about speed, memory-model races or the PTX the rewrites replace, and the device run stays the parity gate.
 What it does give: the scatter / probe / program-loop / group-by code paths written after the round's GPU budget was spent
-(and the opt-in ones: sorted array order, thread-per-row GroupBy, the unrolled word-parallel loop) have executed, statement
-by statement, against the oracle and the reference's goldens.
+(and the opt-in ones: sorted array order, groupby_kernel for every unit, the unrolled word-parallel loop) have executed,
+statement by statement, against the oracle and the reference's goldens.  Every kernel of the library runs on the interpreter.
 
-Default run: everything gpu-marked except the staged (TMA) kernel and the bodies that take a minute or more each when
-interpreted (≈1.5 min in all).  FBGPU_EMU_FULL=1 adds those: the 1024-shard property tests, the reference's 638 x 9
-combination table (in both array orders), Percentile, the random aggregates (≈9 min)."""
+Default run: everything gpu-marked except the bodies that take a minute or more each when interpreted (≈1.5 min in all).
+FBGPU_EMU_FULL=1 adds those: the 1024-shard property tests, the reference's 638 x 9 combination table (in both array
+orders), Percentile, the random aggregates (≈9 min)."""
 import hashlib
 import os
 import subprocess
@@ -59,20 +59,19 @@ def run_on_emulator(args, env=None, defines=(), timeout=1500):
     return tail
 
 
-NOT_HUGE = "not STAGED"                            # the staged kernel is TMA / mbarrier PTX: device only
-SLOW = " and not full_size and not container_combinations and not sorted_order_set_ops and not percentile and not aggregates_random"      # a minute or more each when interpreted
+SLOW = "not full_size and not container_combinations and not sorted_order_set_ops and not percentile and not aggregates_random"      # a minute or more each when interpreted
 
 
 def test_default_kernels_parity():
     """eval / pair-count / row-count / group-by / word-parallel / canonical-emit kernels of the default build against the
     oracle: tests/test_gpu_parity.py and the executor goldens (FULL adds the reference's 638 x 9 combination table)"""
-    run_on_emulator(["tests/test_gpu_parity.py", "tests/test_zz_gpu_executor_goldens.py", "-k", NOT_HUGE + ("" if FULL else SLOW)], timeout=3000)
+    run_on_emulator(["tests/test_gpu_parity.py", "tests/test_zz_gpu_executor_goldens.py"] + ([] if FULL else ["-k", SLOW]), timeout=3000)
 
 
 def test_query_level_bodies_on_interpreted_kernels():
     """the query-level tests written after the GPU budget ran out (aggregates, RBF loader, Distinct, time views, GroupBy
     pass shapes, ...) — on a GPU box these are plain gpu tests"""
-    run_on_emulator(["tests/test_zz_gpu_experimental.py", "-k", NOT_HUGE + " and not sorted_order" + ("" if FULL else SLOW)], timeout=3000)
+    run_on_emulator(["tests/test_zz_gpu_experimental.py", "-k", "not sorted_order" + ("" if FULL else " and " + SLOW)], timeout=3000)
 
 
 def test_node_fan_out_and_merge():
@@ -83,16 +82,14 @@ def test_node_fan_out_and_merge():
 
 def test_sorted_array_order():
     """FBGPU_ARRAY_SORTED=1: the reference's sorted element order (the default is the bank-striped one) under every kernel that reads array payloads"""
-    run_on_emulator(["tests/test_zz_gpu_experimental.py", "-k", "sorted_order and " + NOT_HUGE + ("" if FULL else SLOW)], env={"FBGPU_TEST_EXPERIMENTAL": "1"}, timeout=3000)
+    run_on_emulator(["tests/test_zz_gpu_experimental.py", "-k", "sorted_order" + ("" if FULL else " and " + SLOW)], env={"FBGPU_TEST_EXPERIMENTAL": "1"}, timeout=3000)
 
 
-def test_groupby_thread_per_row_variant():
-    """FBGPU_GROUPBY_FAST=1 (groupby_kernel<true>): the GroupBy goldens and parity tests, and the shapes built for its passes
-    (tiny arrays -> thread-per-row; a bitmap row / a 40-element row -> fallback inside the same kernel; two chunks per side; filter)"""
+def test_groupby_kernel_on_every_unit():
+    """FBGPU_GROUPBY_CTA=1: groupby_kernel for every unit (by default it only sees what groupby_direct_kernel declines) — the
+    GroupBy goldens and parity tests, and the shapes built for its passes (a bitmap row -> dense pass; two chunks per side; filter)"""
     sel = "(groupby or various_queries) and not sorted_order" + ("" if FULL else " and not full_size")
-    # FBGPU_GROUPBY_CTA=1: groupby_kernel for every unit (by default it only sees what groupby_direct_kernel declines)
-    run_on_emulator(["tests/test_gpu_parity.py", "tests/test_zz_gpu_experimental.py", "-k", sel], env={"FBGPU_GROUPBY_FAST": "1", "FBGPU_GROUPBY_CTA": "1"})
-    run_on_emulator(["tests/test_gpu_parity.py", "tests/test_zz_gpu_experimental.py", "-k", "groupby and not sorted_order and not full_size"], env={"FBGPU_GROUPBY_CTA": "1"})
+    run_on_emulator(["tests/test_gpu_parity.py", "tests/test_zz_gpu_experimental.py", "-k", sel], env={"FBGPU_GROUPBY_CTA": "1"})
 
 
 def test_wordpar_loop_variants():
@@ -110,8 +107,8 @@ def test_results_do_not_depend_on_thread_order(order):
     different result under one of the orders"""
     if order == "reverse" and not FULL:
         pytest.skip("reverse order: FBGPU_EMU_FULL=1 (the default suite runs the pseudo-random order)")
-    sel = NOT_HUGE + SLOW + " and not thread_safety and not bsi_diagonal"
-    run_on_emulator(["tests/test_gpu_parity.py", "tests/test_zz_gpu_experimental.py", "-k", sel + " and not sorted_order"], env={"FBGPU_EMU_ORDER": order, "FBGPU_GROUPBY_FAST": "1"}, timeout=3000)
+    sel = SLOW + " and not thread_safety and not bsi_diagonal"
+    run_on_emulator(["tests/test_gpu_parity.py", "tests/test_zz_gpu_experimental.py", "-k", sel + " and not sorted_order"], env={"FBGPU_EMU_ORDER": order}, timeout=3000)
     if FULL:
         run_on_emulator(["tests/test_gpu_parity.py", "-k", "groupby or density_sweep or mixed_encoding"], env={"FBGPU_EMU_ORDER": order}, timeout=3000)
         run_on_emulator(["tests/test_zz_gpu_experimental.py", "-k", "sorted_order_density_sweep or sorted_order_bsi"], env={"FBGPU_EMU_ORDER": order, "FBGPU_TEST_EXPERIMENTAL": "1"}, timeout=3000)
@@ -121,7 +118,7 @@ def test_results_do_not_depend_on_thread_order(order):
 def test_interpreted_library_under_sanitizers(san):
     """kernels and host code compiled with -fsanitize=undefined (shifts, signed overflow, misaligned vector accesses abort)
     or -fsanitize=address (out-of-bounds on `__shared__` statics — plain red-zoned globals in that build —, on host
-    vectors and on thread stacks): the parity tests, the sorted order, the GroupBy variant, the threaded API test"""
+    vectors and on thread stacks): the parity tests, the sorted order, the GroupBy tests, the threaded API test"""
     if not FULL:
         pytest.skip("sanitizer builds: FBGPU_EMU_FULL=1")
     flags = ("-O1", "-g", "-fsanitize=undefined", "-fno-sanitize-recover=undefined") if san == "undefined" else ("-O1", "-g", "-fsanitize=address")
@@ -130,8 +127,8 @@ def test_interpreted_library_under_sanitizers(san):
     base = dict(os.environ, FBGPU_LIB=lib, FBGPU_TEST_ON_EMULATOR="1", LD_PRELOAD=rt, UBSAN_OPTIONS="print_stacktrace=1:halt_on_error=1",
                 ASAN_OPTIONS="detect_leaks=0:halt_on_error=1")
     base.pop("FBGPU_EMU_FULL", None)
-    for extra, sel in (({}, NOT_HUGE + SLOW + " and not sorted_order"),
-                       ({"FBGPU_ARRAY_SORTED": "1", "FBGPU_GROUPBY_FAST": "1", "FBGPU_TEST_EXPERIMENTAL": "1"}, "(sorted_order or groupby or density_sweep) and " + NOT_HUGE + SLOW)):
+    for extra, sel in (({}, SLOW + " and not sorted_order"),
+                       ({"FBGPU_ARRAY_SORTED": "1", "FBGPU_TEST_EXPERIMENTAL": "1"}, "(sorted_order or groupby or density_sweep) and " + SLOW)):
         r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-m", "gpu", "-p", "no:cacheprovider", "tests/test_gpu_parity.py", "tests/test_zz_gpu_experimental.py", "-k", sel],
                            cwd=ROOT, env=dict(base, **extra), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=3000)
         assert r.returncode == 0 and " passed" in r.stdout, r.stdout[-3000:]

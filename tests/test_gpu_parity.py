@@ -394,10 +394,10 @@ def test_full_size_properties_1024_shards():
     assert r.count == i_ab and len(r.columns()) == i_ab
 
 
-@pytest.mark.parametrize("env", ["FBGPU_FORCE_WORDPAR", "FBGPU_STAGED"])
+@pytest.mark.parametrize("env", ["FBGPU_FORCE_WORDPAR"])
 def test_alternative_eval_kernels(env, monkeypatch):
-    """the word-parallel kernel (bitmap-heavy programs) and the TMA-staged kernel are normally picked by a heuristic /
-    opt-in; force each one over array, bitmap and run operands, counts and filter bitmaps, and compare with the oracle"""
+    """the word-parallel kernel (bitmap-heavy programs) is normally picked by a heuristic; force it over array, bitmap and
+    run operands, counts and filter bitmaps, and compare with the oracle"""
     monkeypatch.setenv(env, "1")
     p = Pair()
     p.field("f")

@@ -53,7 +53,7 @@ def test_sorted_order_bsi_topk_groupby(sorted_order):
 
 
 @experimental
-@pytest.mark.parametrize("env", ["FBGPU_FORCE_WORDPAR", "FBGPU_STAGED"])
+@pytest.mark.parametrize("env", ["FBGPU_FORCE_WORDPAR"])
 def test_sorted_order_alternative_kernels(sorted_order, env, monkeypatch):
     G.test_alternative_eval_kernels(env, monkeypatch)       # FORCE_WORDPAR must be ignored for views that hold arrays
 
@@ -449,9 +449,9 @@ def test_min_max_row():
 
 def test_groupby_kernel_pass_shapes():
     """GroupBy over shapes chosen for groupby_kernel's passes: 300 x 270 rows (two a-chunks, two b-chunks) of tiny array
-    containers, a bitmap a-row and a bitmap b-row (dense / warp passes), with and without a filter, either field order —
-    the dense count tensor against the oracle's nested-loop restatement.  (Also run with FBGPU_GROUPBY_FAST=1 by
-    tests/test_emu_kernels.py and tools/r2_first_call.sh.)"""
+    containers, a 40-element a-row, a bitmap a-row and a bitmap b-row (dense / warp passes), with and without a filter, either
+    field order — the dense count tensor against the oracle's nested-loop restatement.  By default groupby_kernel only takes the
+    units groupby_direct_kernel declines; FBGPU_GROUPBY_CTA=1 (tests/test_emu_kernels.py) sends it every unit."""
     from oracle import oracle as O
     SW = 1 << 20
     rng = np.random.default_rng(5)
@@ -467,7 +467,7 @@ def test_groupby_kernel_pass_shapes():
         p.holder.set_bit("i", "a", 7, c)
         if c % 3:
             p.holder.set_bit("i", "b", 11, c)
-    for c in range(SW + 5, SW + 45):                               # an a-row container of 40 elements: above the thread-per-row limit
+    for c in range(SW + 5, SW + 45):                               # an a-row container of 40 elements
         p.holder.set_bit("i", "a", 299, c)
         p.holder.set_bit("i", "b", c % 270, c)
     p.sync_pending()
@@ -525,22 +525,15 @@ def test_groupby_direct_kernel_shapes():
         assert np.array_equal(np.asarray(got).reshape(-1), exp), filt
         assert int(exp.sum()) > 40000 and int(exp.reshape(NA, NB)[17, 9]) >= (300 if filt is None else 200)
         after = p.holder.ctx.counters()
-        if "groupby_fallback_units" in after and not os.environ.get("FBGPU_GROUPBY_CTA") and not os.environ.get("FBGPU_GROUPBY_HASH"):
+        if "groupby_fallback_units" in after and not os.environ.get("FBGPU_GROUPBY_CTA"):
             assert after["groupby_units"] - before["groupby_units"] == 2 * 16 * len(shards)            # two launches (256 + 44 a-rows) over 4 shards
             assert after["groupby_fallback_units"] - before["groupby_fallback_units"] == 2, (filt, before, after)   # (shard 0, slot 3), once per launch
 
 
-def test_groupby_hash_kernel_still_selectable(monkeypatch):
-    """FBGPU_GROUPBY_HASH=1: groupby_shard_kernel (the hash table per group of slots) instead of groupby_direct_kernel, same results"""
-    monkeypatch.setenv("FBGPU_GROUPBY_HASH", "1")
-    test_groupby_slot_groups()
-    test_groupby_direct_kernel_shapes()
-
-
 def test_groupby_slot_groups():
-    """groupby_shard_kernel with several slots per CTA (denser fields -> 2 slots per group instead of 16), one group whose columns
-    overflow the shared-memory table (declined before anything is counted -> groupby_kernel takes its two (shard, slot) units), a
-    row subset, and a filter: the dense count tensor against the oracle's nested loop, and the fallback counter says what ran where"""
+    """groupby_direct_kernel on denser fields whose 3000 columns in two a-rows fill the side list: the two crowded (shard, slot) units
+    overflow it and are declined before anything is counted (groupby_kernel takes them), a row subset, and a filter: the dense count
+    tensor against the oracle's nested loop, and the fallback counter says what ran where"""
     from oracle import oracle as O
     SW = 1 << 20
     rng = np.random.default_rng(11)
@@ -574,7 +567,7 @@ def test_groupby_slot_groups():
         after = p.holder.ctx.counters()
         if "groupby_fallback_units" in after and not os.environ.get("FBGPU_GROUPBY_CTA"):
             assert after["groupby_units"] - before["groupby_units"] == 32
-            assert after["groupby_fallback_units"] - before["groupby_fallback_units"] == 2, (filt, before, after)   # (the crowded slots 0-1 of shard 1; decided on cardinalities, before the filter)
+            assert after["groupby_fallback_units"] - before["groupby_fallback_units"] == 2, (filt, before, after)   # (the crowded slots 0-1 of shard 1: their side lists overflow with or without the filter)
 
 
 def test_topk_time_range():

@@ -4,7 +4,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from featurebase_b200 import build as B
 VARIANTS = {   # name -> -D defines; edit freely, outputs featurebase_b200/libfbgpu_<name>.so (select with FBGPU_LIB=...)
     "gd_nopipe": ["FBGPU_GD_PIPE=0"],
-    "gh512": ["FBGPU_GH_THREADS=512"],          # groupby_shard_kernel: two CTAs of 512 threads per SM with 64 KiB tables
     "pair_nopf": ["FBGPU_PAIR_NO_PF"],          # pair kernel without the L2 prefetch of the next unit's payload lines
     "pair_bm4": ["FBGPU_PAIR_BM_UNROLL=4"],     # pair kernel: bitmap x bitmap loop unrolled 4 (default 8)
     "addr_imad": ["FBGPU_ADDR_IMAD"],            # scatter / probe word addresses with IMAD.HI on the FMA pipe (measured slower: IMAD.HI is half rate)

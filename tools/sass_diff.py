@@ -3,8 +3,9 @@
     python tools/sass_diff.py <commit>         # e.g. the last commit whose library was parity-tested and timed on an H100
 Builds that commit's csrc/ in a scratch directory with the same nvcc line, dumps both libraries with cuobjdump -sass and
 compares the instruction streams per kernel (addresses and encodings stripped; template arguments that did not exist yet
-are matched by kernel name).  No GPU needed.  A kernel reported IDENTICAL is, bit for bit in its instructions, the one that
-was parity-tested and timed on the device."""
+or no longer exist are matched by kernel name: an untemplated kernel and its <false> instantiation).  Kernels of the old
+build that the new one lacks are reported DELETED.  No GPU needed.  A kernel reported IDENTICAL is, bit for bit in its
+instructions, the one that was parity-tested and timed on the device."""
 import os
 import re
 import subprocess
@@ -36,6 +37,10 @@ def short(name):
     return (m.group(1), m.group(3) or "") if m else (name, "")
 
 
+def label(name, targ):
+    return name + ("<%s>" % ("true" if targ == "Lb1" else "false") if targ else "")
+
+
 def main():
     commit = sys.argv[1]
     tmp = tempfile.mkdtemp(prefix="sassdiff_")
@@ -45,18 +50,21 @@ def main():
     subprocess.run(["nvcc", "-O3", "-std=c++17", "-shared", "-Xcompiler", "-fPIC", "-lineinfo", "-gencode", ARCH,
                     "-I", os.path.join(tmp, "include"), "-o", old, os.path.join(tmp, "featurebase_b200/csrc/fbgpu.cu"), "-ldl"], check=True, stdout=subprocess.DEVNULL)
     a, b = kernels(old), kernels(os.path.join(ROOT, "featurebase_b200", "libfbgpu.so"))
-    by_name = {}
+    by_name, matched = {}, set()
     for k, v in a.items():
-        by_name.setdefault(short(k)[0], []).append((short(k)[1], v))
+        by_name.setdefault(short(k)[0], []).append((short(k)[1], v, k))
     for k, v in b.items():
         name, targ = short(k)
         cands = by_name.get(name, [])
-        hit = [x for x in cands if x[0] == targ] or [x for x in cands if not x[0] and targ in ("", "Lb0")]
-        label = name + ("<%s>" % ("true" if targ == "Lb1" else "false") if targ else "")
+        hit = [x for x in cands if x[0] == targ] or [x for x in cands if {x[0], targ} <= {"", "Lb0"}]
         if not hit:
-            print(f"NEW        {label:28s} {len(v):5d} instructions")
+            print(f"NEW        {label(name, targ):28s} {len(v):5d} instructions")
         else:
-            print(f"{'IDENTICAL' if hit[0][1] == v else 'CHANGED  '}  {label:28s} {len(hit[0][1]):5d} -> {len(v):5d} instructions")
+            matched.add(hit[0][2])
+            print(f"{'IDENTICAL' if hit[0][1] == v else 'CHANGED  '}  {label(name, targ):28s} {len(hit[0][1]):5d} -> {len(v):5d} instructions")
+    for k, v in a.items():
+        if k not in matched:
+            print(f"DELETED    {label(*short(k)):28s} {len(v):5d} instructions")
 
 
 if __name__ == "__main__":
