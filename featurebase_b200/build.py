@@ -16,16 +16,14 @@ def _stale(target, sources):
     return any(os.path.getmtime(s) > t for s in sources if os.path.exists(s))
 
 
-def build_fbgpu(force=False, verbose=False, defines=None, out_name="libfbgpu.so"):
+def build_fbgpu(force=False, verbose=False):
     src = os.path.join(HERE, "csrc", "fbgpu.cu")
     deps = [src, os.path.join(HERE, "csrc", "kernels.cuh"), os.path.join(HERE, "csrc", "fbgpu_types.h"), os.path.join(HERE, "csrc", "stripe.h"), os.path.join(HERE, "csrc", "rbf_reader.h"), os.path.join(HERE, "csrc", "bitaddr.h"), os.path.join(HERE, "csrc", "program_compiler.h"), os.path.join(HERE, "csrc", "roaring_parse.h"), os.path.join(HERE, "csrc", "host_error.h"), os.path.join(HERE, "csrc", "wp_machine.h"), os.path.join(HERE, "csrc", "resolve.h"), os.path.join(HERE, "csrc", "node.h"),
             os.path.join(ROOT, "include", "fbgpu.h")]
-    out = os.path.join(HERE, out_name)
+    out = os.path.join(HERE, "libfbgpu.so")
     if force or _stale(out, deps):
         cmd = [NVCC, "-O3", "-std=c++17", "-shared", "-Xcompiler", "-fPIC", "-lineinfo",
                "-gencode", ARCH, "-o", out, src, "-ldl"]
-        for d in (defines or []):
-            cmd.insert(1, "-D" + d)
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         subprocess.check_call(cmd)

@@ -19,34 +19,16 @@ FBGPU_HD uint32_t mulhi_u32(uint32_t a, uint32_t b) {
     return (uint32_t)(((uint64_t)a * b) >> 32);
 #endif
 }
-// Pipe balance: the scatter / probe loops are bound by the integer ALU pipe (LOP3 / SHF / LEA / IADD3), not the FMA pipe (IMAD).
-// -DFBGPU_ADDR_IMAD moves the two word addresses and the `>> 16` of the upper element to IMAD.HI on the FMA pipe (multipliers read
-// from constant memory so that ptxas cannot strength-reduce them, the bitmap's shared-memory base riding along as the 64-bit addend).
-// IMAD.HI issues at half the rate of LEA.HI / SHF / IMAD-low (bench_micro/pipe_rates.cu measures both), which made that form slower,
-// so the shift / LEA forms are the default and the IMAD form is kept only as the record of the experiment.
+// Shift / LEA forms, not IMAD.HI on the FMA pipe: IMAD.HI issues at half their rate (bench_micro/pipe_rates.cu), measured slower.
 // w = (hi << 16) | lo.  4 * (lo >> 5)  and  4 * (hi >> 5)
 FBGPU_HD uint32_t word_off_lo(uint32_t w) { return mulhi_u32(w & 0xffe0u, 1u << 29); }
 FBGPU_HD uint32_t word_off_hi(uint32_t w) { return mulhi_u32(w & 0xffe00000u, 1u << 13); }
-#if defined(__CUDACC__) && defined(FBGPU_ADDR_IMAD)
-__constant__ uint32_t c_mul29 = 1u << 29, c_mul13 = 1u << 13, c_mul16 = 1u << 16;
-#endif
-#if defined(__CUDA_ARCH__) && defined(FBGPU_ADDR_IMAD)
-typedef uint64_t smem_base_t;                        // shared-space address of a bitmap, kept in the upper half of a register pair
-__device__ __forceinline__ smem_base_t smem_base(uint32_t sb) { return (uint64_t)sb << 32; }
-__device__ __forceinline__ uint32_t word_addr_lo(smem_base_t b, uint32_t w) { return (uint32_t)(((uint64_t)(w & 0xffe0u) * c_mul29 + b) >> 32); }
-__device__ __forceinline__ uint32_t word_addr_hi(smem_base_t b, uint32_t w) { return (uint32_t)(((uint64_t)(w & 0xffe00000u) * c_mul13 + b) >> 32); }
-__device__ __forceinline__ uint32_t upper16(uint32_t w) { return __umulhi(w, c_mul16); }
-__device__ __forceinline__ void pin_base(smem_base_t& b) { asm volatile("" : "+l"(b)); }
-#else
-typedef uint32_t smem_base_t;
-FBGPU_HD smem_base_t smem_base(uint32_t sb) { return sb; }
-FBGPU_HD uint32_t word_addr_lo(smem_base_t b, uint32_t w) { return b + word_off_lo(w); }
-FBGPU_HD uint32_t word_addr_hi(smem_base_t b, uint32_t w) { return b + word_off_hi(w); }
-FBGPU_HD uint32_t upper16(uint32_t w) { return w >> 16; }
+// sb: shared-space address of the bitmap
+FBGPU_HD uint32_t word_addr_lo(uint32_t sb, uint32_t w) { return sb + word_off_lo(w); }
+FBGPU_HD uint32_t word_addr_hi(uint32_t sb, uint32_t w) { return sb + word_off_hi(w); }
 #if defined(__CUDA_ARCH__)
-__device__ __forceinline__ void pin_base(smem_base_t& b) { asm volatile("" : "+r"(b)); }
+__device__ __forceinline__ void pin_base(uint32_t& sb) { asm volatile("" : "+r"(sb)); }
 #else
-inline void pin_base(smem_base_t&) {}
-#endif
+inline void pin_base(uint32_t&) {}
 #endif
 }  // namespace fbgpu

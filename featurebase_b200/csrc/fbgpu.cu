@@ -659,7 +659,7 @@ static void build_tables(fbgpu_ctx* c, std::vector<ViewTab>& views, std::vector<
             rmin = std::min(rmin, c->h_rows[hf.row_off].row); rmax = std::max(rmax, c->h_rows[hf.row_off + hf.n_rows - 1].row); nrows = std::max<uint64_t>(nrows, hf.n_rows); }
         if (rmin == ~0ull) continue;
         uint64_t span = rmax - rmin + 1;
-        if (span > 4 * nrows + 64 || span * sm.size() > (64ull << 20) || getenv("FBGPU_NO_ROWTAB")) continue;       // sparse row ids or too large: keep the search chain
+        if (span > 4 * nrows + 64 || span * sm.size() > (64ull << 20)) continue;       // sparse row ids or too large: keep the search chain
         views[v].rt_rows = (uint32_t)span; views[v].rt_off = rowtab.size(); views[v].rmin = rmin;
         rowtab.resize(rowtab.size() + span * sm.size(), RowTabEnt{ 0, 0, 0 });
         for (size_t sh = 0; sh < sm.size(); sh++) if (sm[sh] >= 0) { const HostFrag& hf = c->frags[sm[sh]];
@@ -922,9 +922,7 @@ static int compile_program(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, in
     ViewLookup lookup = [c, index](uint32_t field, uint32_t view) { return view_id_locked(c, ViewKey{ index, field, view }, false); };
     int rc = compile(ops, n_ops, lookup, out, depth, err);
     if (rc) return fail(rc, "%s", err.msg);
-#ifndef FBGPU_WP_LEGACY_LOOP
     expand_push_row(out);          // every kernel accepts the rewritten program; the word-parallel op loop (wp_machine.h) requires it
-#endif
     return 0;
 }
 
@@ -978,13 +976,13 @@ static int launch_eval(fbgpu_ctx* c, Workspace* w, const std::vector<DevOp>& pro
     std::vector<int2> batches = find_batches(prog);
     // Word-parallel kernel for bitmap-heavy programs (BSI plane sweeps, dense rows): chosen when the views the
     // program references hold few array containers.  Row results (out.info) need cross-slice run counts: not here.
-    if (!out.info && n_ops <= kWpMaxOps && depth <= kWpMaxDepth && !getenv("FBGPU_NO_WORDPAR")) {
+    if (!out.info && n_ops <= kWpMaxOps && depth <= kWpMaxDepth) {
         uint64_t arr = 0, other = 0, striped = 0;
         for (const DevOp& o : prog) if (o.op >= D_PUSH_ROW && o.op <= D_ORANDNOT_ROW && o.op != D_PUSH_EMPTY && o.fv < c->view_arr.size()) { arr += c->view_arr[o.fv]; other += c->view_other[o.fv]; striped += c->view_striped[o.fv]; }
         // (wp_slice searches sorted arrays: a view that holds striped arrays can never take this kernel, forced or not)
         if (striped == 0 && ((other > 0 && arr * 8 <= other) || getenv("FBGPU_FORCE_WORDPAR") != nullptr)) {
             long long blocks = n_units * kWpBlocksPerUnit;
-            long long grid = std::min<long long>(blocks, (long long)c->sm_count * std::max(FBGPU_WP_MIN_BLOCKS, 8) * 2);
+            long long grid = std::min<long long>(blocks, (long long)c->sm_count * kWpMinBlocks * 2);
             eval_wordpar_kernel<<<(unsigned)grid, kWpThreads, 0, w->stream>>>(store_ref(c), d_prog, n_ops, d_shards, n_units, out);
             CUDA_TRY(cudaGetLastError());
             return 0;
@@ -993,7 +991,7 @@ static int launch_eval(fbgpu_ctx* c, Workspace* w, const std::vector<DevOp>& pro
     // the batch table travels in front of the program in the same H2D copy (upload_inputs); see d_batches()
     const int2* d_batches = reinterpret_cast<const int2*>(w->d_aux.p);
     size_t smem = (size_t)(depth + 1) * 8192;
-    int per_sm = std::max(1, (int)std::min<size_t>(std::min(FBGPU_EVAL_MIN_BLOCKS, 2048 / kEvalThreads), (227 * 1024) / (smem + 3 * 1024 + 512)));
+    int per_sm = std::max(1, (int)std::min<size_t>(std::min(kEvalMinBlocks, 2048 / kEvalThreads), (227 * 1024) / (smem + 3 * 1024 + 512)));
     long long grid = std::min<long long>(n_units, (long long)c->sm_count * per_sm);
     eval_kernel<<<(unsigned)grid, kEvalThreads, smem, w->stream>>>(store_ref(c), d_prog, n_ops, depth, d_batches, (int)batches.size(), d_shards, n_units, out);
     CUDA_TRY(cudaGetLastError());
@@ -1045,7 +1043,7 @@ static int count_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t
         const DevOp* pa = nullptr; const DevOp* pb = nullptr;
         if (prog.size() == 2 && prog[0].op == D_PUSH_ROW && prog[1].op == D_AND_ROW) { pa = &prog[0]; pb = &prog[1]; }
         else if (prog.size() == 3 && prog[0].op == D_PUSH_EMPTY && prog[1].op == D_OR_ROW && prog[2].op == D_AND_ROW) { pa = &prog[1]; pb = &prog[2]; }
-        if (pa && !getenv("FBGPU_NO_PAIR_KERNEL")) {
+        if (pa) {
             long long grid = std::min<long long>((n_units + kPcWarps - 1) / kPcWarps, (long long)c->sm_count * c->pair_ctas_per_sm);
             c->counters_pair_launches++;
             pair_count_kernel<<<(unsigned)grid, kPcWarps * 32, kPcWarps * 8192, w->stream>>>(store_ref(c), pa->fv, pa->row, pb->fv, pb->row, nullptr, nullptr, n_units,

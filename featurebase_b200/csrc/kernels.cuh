@@ -18,13 +18,8 @@
 
 namespace fbgpu {
 
-#ifndef FBGPU_EVAL_THREADS
-#define FBGPU_EVAL_THREADS 256
-#endif
-#ifndef FBGPU_EVAL_MIN_BLOCKS
-#define FBGPU_EVAL_MIN_BLOCKS 6      // 40 registers: room for three chunk loads in flight per lane (faster on the headline query than 8 CTAs / 32 registers)
-#endif
-constexpr int kEvalThreads = FBGPU_EVAL_THREADS;          // 256 or 512
+constexpr int kEvalThreads = 256;
+constexpr int kEvalMinBlocks = 6;      // 40 registers: room for three chunk loads in flight per lane (faster on the headline query than 8 CTAs / 32 registers)
 constexpr int kEvalU4PerThread = 512 / kEvalThreads;       // uint4 per thread of an 8 KiB bitmap
 constexpr int kEvalW64PerThread = 1024 / kEvalThreads;     // consecutive u64 words per thread in scans
 constexpr int kResolveChunk = 128;
@@ -178,7 +173,7 @@ __device__ __forceinline__ void smem_bit_op_at(uint32_t addr, uint32_t sh) {
 }
 // scatter the (up to) 8 elements of one 16-byte array chunk; sb = shared-space address of the target bitmap
 template <int MODE>
-__device__ __forceinline__ void scatter_chunk_sb(smem_base_t sb, uint4 v, uint32_t base, uint32_t n) {
+__device__ __forceinline__ void scatter_chunk_sb(uint32_t sb, uint4 v, uint32_t base, uint32_t n) {
     uint32_t w[4] = { v.x, v.y, v.z, v.w };
     // OR / AND-NOT: the loader pads the last chunk with copies of the last element (stripe.h pad_array_tail), setting or
     // clearing a bit twice is harmless, so every chunk takes the unguarded path and the warp never diverges on a tail
@@ -186,7 +181,7 @@ __device__ __forceinline__ void scatter_chunk_sb(smem_base_t sb, uint4 v, uint32
 #pragma unroll
         for (int q = 0; q < 4; q++) {            // LOP3 + LEA.HI + SHF.L.W (+ SHF.R for the upper element) + ATOMS, see bitaddr.h
             smem_bit_op_at<MODE>(word_addr_lo(sb, w[q]), w[q]);
-            smem_bit_op_at<MODE>(word_addr_hi(sb, w[q]), upper16(w[q]));
+            smem_bit_op_at<MODE>(word_addr_hi(sb, w[q]), w[q] >> 16);
         }
     } else {
 #pragma unroll
@@ -198,19 +193,17 @@ __device__ __forceinline__ void scatter_chunk_sb(smem_base_t sb, uint4 v, uint32
 }
 template <int MODE>
 __device__ __forceinline__ void scatter_chunk_unrolled(uint32_t* bm, uint4 v, uint32_t base, uint32_t n) {
-    scatter_chunk_sb<MODE>(smem_base((uint32_t)__cvta_generic_to_shared(bm)), v, base, n);
+    scatter_chunk_sb<MODE>((uint32_t)__cvta_generic_to_shared(bm), v, base, n);
 }
 // Batch of commuting row operands (OR / ANDNOT / XOR onto the same target), no barrier in between: warp w takes
 // operands w, w+8, ...; arrays are scattered with red.shared, bitmaps applied with word atomics.  (Tried and slower:
 // 4 loads in flight per thread, register double-buffering, L2 prefetch, TMA staging.)
 static_assert(sizeof(Resolved) == 16, "batch_rows reads a Resolved with one 16-byte shared load");
-#ifndef FBGPU_EVAL_DEEP
-#define FBGPU_EVAL_DEEP 3
-#endif
+constexpr int kEvalDeep = 3;
 template <int MODE>
 __device__ __forceinline__ void batch_rows(uint32_t* T32, const Resolved* res, int n) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    smem_base_t sb = smem_base((uint32_t)__cvta_generic_to_shared(T32));
+    uint32_t sb = (uint32_t)__cvta_generic_to_shared(T32);
     pin_base(sb);                          // keep the shared address live: ptxas otherwise rebuilds it for every chunk
     for (int j = wid; j < n; j += kEvalThreads / 32) {
         const uint4 raw = *reinterpret_cast<const uint4*>(res + j);        // one LDS.128: {ptr lo, ptr hi, card, typ | cnt << 16}
@@ -219,17 +212,17 @@ __device__ __forceinline__ void batch_rows(uint32_t* T32, const Resolved* res, i
         const uint32_t typ = raw.w & 0xffffu;
         if (typ == kArray) {
             const uint32_t card = raw.z, n8 = (card + 7) >> 3;
-            // the first FBGPU_EVAL_DEEP chunks of the lane are all in flight before the first reduction is issued: a ~650-element
+            // the first kEvalDeep chunks of the lane are all in flight before the first reduction is issued: a ~650-element
             // container is 82 chunks = at most 3 per lane, so its whole payload costs the warp ONE exposed HBM latency instead of
             // three (most stall samples of the old one-chunk loop sat on its single load)
             // (the loads are unconditional — index clamped to the last chunk — so that no register of v[] is ever undefined:
             // predicated loads made ptxas park the chunks in local memory)
-            uint4 v[FBGPU_EVAL_DEEP];
+            uint4 v[kEvalDeep];
 #pragma unroll
-            for (int q = 0; q < FBGPU_EVAL_DEEP; q++) v[q] = ldg_nc(a4 + min((uint32_t)lane + 32u * q, n8 - 1u));
+            for (int q = 0; q < kEvalDeep; q++) v[q] = ldg_nc(a4 + min((uint32_t)lane + 32u * q, n8 - 1u));
 #pragma unroll
-            for (int q = 0; q < FBGPU_EVAL_DEEP; q++) if (lane + 32 * q < n8) scatter_chunk_sb<MODE>(sb, v[q], (lane + 32 * q) * 8, card);
-            for (uint32_t i = lane + 32 * FBGPU_EVAL_DEEP; i < n8; i += 32) scatter_chunk_sb<MODE>(sb, ldg_nc(a4 + i), i * 8, card);
+            for (int q = 0; q < kEvalDeep; q++) if (lane + 32 * q < n8) scatter_chunk_sb<MODE>(sb, v[q], (lane + 32 * q) * 8, card);
+            for (uint32_t i = lane + 32 * kEvalDeep; i < n8; i += 32) scatter_chunk_sb<MODE>(sb, ldg_nc(a4 + i), i * 8, card);
         } else if (typ == kBitmap) warp_bitmap_atomic<MODE>(T32, a4, lane);
     }
 }
@@ -290,7 +283,7 @@ struct EvalOut {
 };
 
 // One CTA per (shard, slot) unit, persistent over units.  Dynamic smem: (depth+1) x 8 KiB.
-__global__ void __launch_bounds__(kEvalThreads, FBGPU_EVAL_MIN_BLOCKS)
+__global__ void __launch_bounds__(kEvalThreads, kEvalMinBlocks)
 eval_kernel(StoreRef st, const DevOp* __restrict__ prog, int n_ops, int depth,
             const int2* __restrict__ batches, int n_batches,
             const uint64_t* __restrict__ shards, long long n_units, EvalOut out) {
@@ -447,21 +440,17 @@ eval_kernel(StoreRef st, const DevOp* __restrict__ prog, int n_ops, int depth,
 
 // ------------------------------------------------------------------------------------------------
 // eval_wordpar_kernel: word-parallel evaluation for bitmap-heavy programs (BSI plane sweeps, dense rows).
-// Every thread owns ONE 128-bit slice (uint4) of a (shard, slot) stripe and runs the whole program on it with the
-// operand stack in registers: no shared-memory bitmaps, no barriers between ops, and the operands of the next three
-// row ops are already in flight (register prefetch ring) while the current op is applied.  Arrays and runs are
-// handled by a per-thread search for the slice's elements, so any program is valid here; the host only picks this
-// kernel when the referenced views are dominated by bitmap/run containers.
+// Every thread owns 32 bytes (two adjacent 128-bit slices) of a (shard, slot) stripe and runs the whole program on them with the
+// operand stack in registers (wp_machine.h): no shared-memory bitmaps and no barriers between ops.  Arrays and runs are handled by
+// a per-thread search for the slice's elements, so any program is valid here; the host only picks this kernel when the referenced
+// views are dominated by bitmap/run containers.
 // ------------------------------------------------------------------------------------------------
-// FBGPU_WP_WIDE (default, with the cp.async operand ring): a thread owns 32 bytes (two adjacent 128-bit slices) instead of 16, in CTAs
-// of 64 threads — the same 2 KiB per CTA and row op, but the program loop's per-op overhead (ring bookkeeping, op decode, branches:
-// ~32 of the ~36 instructions per op and thread; the kernel issued 43 % of its cycles with DRAM 30 % busy) is paid once per 32 bytes.
-#if !defined(FBGPU_WP_LEGACY_LOOP) && !defined(FBGPU_WP_REG_RING) && !defined(FBGPU_WP_NARROW)
-#define FBGPU_WP_WIDE 1
+// 32 bytes per thread in CTAs of 64 threads rather than 16 bytes in CTAs of 128: the same 2 KiB per CTA and row op, but the program
+// loop's per-op overhead (ring bookkeeping, op decode, branches: ~32 of the ~36 instructions per op and thread; the 16-byte form issued
+// 43 % of its cycles with DRAM 30 % busy) is paid once per 32 bytes.
 constexpr int kWpThreads = 64;
-#else
-constexpr int kWpThreads = 128;              // 512 / (128 * slices-per-thread) CTAs per unit
-#endif
+constexpr int kWpBlocksPerUnit = 512 / (kWpThreads * 2);       // CTAs per (shard, slot) unit
+constexpr int kWpMinBlocks = 8;
 struct __align__(16) WpV32 { unsigned long long x, y, z, w; };      // 32 bytes of a stripe; member-wise bit ops (wp_machine.h)
 constexpr int kWpMaxOps = 256;
 constexpr int kWpMaxDepth = 4;
@@ -496,52 +485,34 @@ __device__ __forceinline__ uint4 wp_slice(const Resolved& r, int i) {
     return make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-#ifndef FBGPU_WP_SLICES
-#define FBGPU_WP_SLICES 1
-#endif
-#ifndef FBGPU_WP_MIN_BLOCKS
-#define FBGPU_WP_MIN_BLOCKS 8
-#endif
-constexpr int kWpSlices = FBGPU_WP_SLICES;       // uint4 slices per thread (slice q of a thread: i0 + q * kWpThreads => coalesced)
-#if defined(FBGPU_WP_WIDE)
-constexpr int kWpBlocksPerUnit = 512 / (kWpThreads * 2);
-#else
-constexpr int kWpBlocksPerUnit = 512 / (kWpThreads * kWpSlices);
-#endif
-
 struct WpOp { const void* ptr; uint32_t card; uint16_t typ, cnt; uint8_t opc, is_row, pad[6]; };   // pre-decoded op, 24 B
 
-#ifndef FBGPU_WP_ASYNC_DEPTH
-#define FBGPU_WP_ASYNC_DEPTH 8
-#endif
-constexpr int kWpAsyncDepth = FBGPU_WP_ASYNC_DEPTH;       // ring slots per thread: depth - 1 operand slices in flight
+// Operand ring in shared memory, filled by cp.async (LDGSTS): every thread copies ITS 32 bytes of the next kWpAsyncDepth - 1 row
+// operands into its own ring slots — no registers and no scoreboard entry per load in flight (a register ring stalled on shared
+// scoreboards beyond 3 loads: depth 6 was slower than depth 3 on BASELINE config 3), no barrier (a slot is written and read by the
+// same thread), and the depth is a shared-memory size, not a register count.  One commit group per row op, empty when the operand
+// is absent or not a bitmap (its slice is computed into the slot right away), so that `wait_group depth - 1` at row op ri always
+// means "group ri has landed".
+constexpr int kWpAsyncDepth = 8;       // ring slots per thread: depth - 1 operand slices in flight
 __device__ __forceinline__ void cp_async_16(uint4* dst_smem, const uint4* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait_group() { asm volatile("cp.async.wait_group %0;" :: "n"(N) : "memory"); }
 
-__global__ void __launch_bounds__(kWpThreads, FBGPU_WP_MIN_BLOCKS)
+__global__ void __launch_bounds__(kWpThreads, kWpMinBlocks)
 eval_wordpar_kernel(StoreRef st, const DevOp* __restrict__ prog, int n_ops,
                     const uint64_t* __restrict__ shards, long long n_units, EvalOut out) {
     __shared__ WpOp ops[kWpMaxOps];
     __shared__ uint16_t rowops[kWpMaxOps];     // indices of the row ops, in program order
     __shared__ int n_rowops;
     __shared__ uint32_t wsum[kWpThreads / 32];
-#if defined(FBGPU_WP_WIDE)
     __shared__ __align__(16) WpV32 wp_ring[kWpAsyncDepth][kWpThreads];
-#elif !defined(FBGPU_WP_LEGACY_LOOP) && FBGPU_WP_SLICES == 1 && !defined(FBGPU_WP_REG_RING)
-    __shared__ __align__(16) uint4 wp_ring[kWpAsyncDepth][kWpThreads];
-#endif
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const long long n_blocks = n_units * kWpBlocksPerUnit;
     for (long long blk = blockIdx.x; blk < n_blocks; blk += gridDim.x) {
         const long long unit = blk / kWpBlocksPerUnit;
-#if defined(FBGPU_WP_WIDE)
         const int i0 = (int)(blk % kWpBlocksPerUnit) * kWpThreads * 2 + 2 * tid;       // the thread's two adjacent uint4 slices: i0, i0 + 1
-#else
-        const int i0 = (int)(blk % kWpBlocksPerUnit) * kWpThreads * kWpSlices + tid;
-#endif
         __syncthreads();
         for (int k = tid; k < n_ops; k += kWpThreads) {        // decode + resolve: one op per thread
             DevOp op = prog[k];
@@ -565,20 +536,6 @@ eval_wordpar_kernel(StoreRef st, const DevOp* __restrict__ prog, int n_ops,
         }
         __syncthreads();
         const int nr = n_rowops;
-        auto fetch = [&](uint4* dst, int ri) {
-            const WpOp w = ops[rowops[ri]];
-            if (w.ptr != nullptr && w.typ == kBitmap) {
-#pragma unroll
-                for (int q = 0; q < kWpSlices; q++) dst[q] = ldg_nc(reinterpret_cast<const uint4*>(w.ptr) + i0 + q * kWpThreads);
-            } else {
-                Resolved r; r.ptr = w.ptr; r.card = w.card; r.typ = w.typ; r.cnt = w.cnt;
-#pragma unroll
-                for (int q = 0; q < kWpSlices; q++) dst[q] = wp_slice(r, i0 + q * kWpThreads);
-            }
-        };
-        const uint4 z = make_uint4(0, 0, 0, 0);
-#if defined(FBGPU_WP_WIDE)
-        // Operand ring in shared memory, filled by cp.async (see the 16-byte form below); 32 bytes per thread and row op
         auto issue = [&](int ri) {
             if (ri < nr) {
                 const WpOp w = ops[rowops[ri]];
@@ -600,99 +557,12 @@ eval_wordpar_kernel(StoreRef st, const DevOp* __restrict__ prog, int n_ops,
         uint4 T[2];
         T[0] = make_uint4((uint32_t)T32.x, (uint32_t)(T32.x >> 32), (uint32_t)T32.y, (uint32_t)(T32.y >> 32));
         T[1] = make_uint4((uint32_t)T32.z, (uint32_t)(T32.z >> 32), (uint32_t)T32.w, (uint32_t)(T32.w >> 32));
-#elif !defined(FBGPU_WP_LEGACY_LOOP) && FBGPU_WP_SLICES == 1 && !defined(FBGPU_WP_REG_RING)
-        // Operand ring in shared memory, filled by cp.async (LDGSTS): every thread copies ITS 16-byte slice of the next kWpAsyncDepth - 1
-        // row operands into its own ring slots — no registers and no scoreboard entry per load in flight (the register ring of
-        // wp_run_unrolled stalled on shared scoreboards beyond 3 loads: depth 6 was slower than depth 3 on BASELINE config 3),
-        // no barrier (a slot is written and read by the same thread), and the depth is a shared-memory size, not a register count.
-        // One commit group per row op, empty when the operand is absent or not a bitmap (its slice is computed into the slot right
-        // away), so that `wait_group depth - 1` at row op ri always means "group ri has landed".
-        auto issue = [&](int ri) {
-            if (ri < nr) {
-                const WpOp w = ops[rowops[ri]];
-                uint4* slot = &wp_ring[ri % kWpAsyncDepth][tid];
-                if (w.ptr != nullptr && w.typ == kBitmap) cp_async_16(slot, reinterpret_cast<const uint4*>(w.ptr) + i0);
-                else { Resolved r; r.ptr = w.ptr; r.card = w.card; r.typ = w.typ; r.cnt = w.cnt; *slot = wp_slice(r, i0); }
-            }
-            cp_async_commit();
-        };
-        for (int ri = 0; ri < kWpAsyncDepth - 1; ri++) issue(ri);
-        uint4 T[1];
-        T[0] = wp_run_unrolled<uint4, true, 1>(n_ops, nr, [&](int k) { return ops[k].opc; }, [&](int k) { return ops[k].is_row != 0; },
-                                         [&](int ri) { return (int)rowops[ri]; },
-                                         [&](int ri) {      // called once per row op, in order, after the previous operand has been consumed
-                                             issue(ri + kWpAsyncDepth - 1);          // into the slot the previous row op was read from
-                                             cp_async_wait_group<kWpAsyncDepth - 1>();
-                                             return wp_ring[ri % kWpAsyncDepth][tid];
-                                         });
-        cp_async_wait_group<0>();
-        const int depth_now = 1;                       // (wp_run_unrolled already returns zero for an empty stack)
-#elif !defined(FBGPU_WP_LEGACY_LOOP) && FBGPU_WP_SLICES == 1
-        // op loop with fixed register roles and a register operand ring (wp_machine.h); same program semantics
-        uint4 T[1];
-        T[0] = wp_run_unrolled<uint4, true>(n_ops, nr, [&](int k) { return ops[k].opc; }, [&](int k) { return ops[k].is_row != 0; },
-                                      [&](int ri) { return (int)rowops[ri]; }, [&](int ri) { uint4 d[1]; fetch(d, ri); return d[0]; });
-        const int depth_now = 1;                       // (wp_run_unrolled already returns zero for an empty stack)
-#else
-        // prefetch ring: operands of the next three row ops are in flight while the current one is applied
-        uint4 p0[kWpSlices], p1[kWpSlices], p2[kWpSlices];
-#pragma unroll
-        for (int q = 0; q < kWpSlices; q++) { p0[q] = z; p1[q] = z; p2[q] = z; }
-        int ri = 0;
-        if (ri < nr) fetch(p0, ri++);
-        if (ri < nr) fetch(p1, ri++);
-        if (ri < nr) fetch(p2, ri++);
-        // operand stack as a shift register: T = top, B = below, S2, S3 deeper (depth <= 4 checked by the host)
-        uint4 T[kWpSlices], B[kWpSlices], S2[kWpSlices], S3[kWpSlices];
-#pragma unroll
-        for (int q = 0; q < kWpSlices; q++) { T[q] = z; B[q] = z; S2[q] = z; S3[q] = z; }
-        int depth_now = 0;
-        for (int k = 0; k < n_ops; k++) {
-            const uint8_t opc = ops[k].opc;
-            if (!ops[k].is_row) {
-#pragma unroll
-                for (int q = 0; q < kWpSlices; q++) {
-                    if (opc == D_PUSH_EMPTY) { S3[q] = S2[q]; S2[q] = B[q]; B[q] = T[q]; T[q] = z; }
-                    else if (opc == D_SWAP) { uint4 t = T[q]; T[q] = B[q]; B[q] = t; }
-                    else if (opc == D_POP) { T[q] = B[q]; B[q] = S2[q]; S2[q] = S3[q]; }
-                    else { T[q] = opc == D_AND ? and4(B[q], T[q]) : opc == D_OR ? or4(B[q], T[q]) : opc == D_ANDNOT ? andn4(B[q], T[q]) : xor4(B[q], T[q]); B[q] = S2[q]; S2[q] = S3[q]; }
-                }
-                depth_now += opc == D_PUSH_EMPTY ? 1 : opc == D_SWAP ? 0 : -1;
-                continue;
-            }
-#pragma unroll
-            for (int q = 0; q < kWpSlices; q++) {
-                const uint4 x = p0[q];
-                switch (opc) {
-                    case D_PUSH_ROW: S3[q] = S2[q]; S2[q] = B[q]; B[q] = T[q]; T[q] = x; break;
-                    case D_OR_ROW: T[q] = or4(T[q], x); break;
-                    case D_AND_ROW: T[q] = and4(T[q], x); break;
-                    case D_ANDNOT_ROW: T[q] = andn4(T[q], x); break;
-                    case D_XOR_ROW: T[q] = xor4(T[q], x); break;
-                    case D_ORAND_ROW: B[q] = or4(B[q], and4(T[q], x)); break;
-                    default: B[q] = or4(B[q], andn4(T[q], x)); break;       // D_ORANDNOT_ROW
-                }
-                p0[q] = p1[q]; p1[q] = p2[q]; p2[q] = z;
-            }
-            if (opc == D_PUSH_ROW) depth_now++;
-            if (ri < nr) fetch(p2, ri++);
-        }
-#endif
         uint32_t cnt = 0;
-#if defined(FBGPU_WP_WIDE)
 #pragma unroll
         for (int q = 0; q < 2; q++) {                   // (wp_run_unrolled already returns zero for an empty stack)
             if (out.bitmaps) out.bitmaps[(size_t)unit * 512 + i0 + q] = T[q];
             cnt += (uint32_t)popc4(T[q]);
         }
-#else
-#pragma unroll
-        for (int q = 0; q < kWpSlices; q++) {
-            const uint4 rsl = depth_now > 0 ? T[q] : z;
-            if (out.bitmaps) out.bitmaps[(size_t)unit * 512 + i0 + q * kWpThreads] = rsl;
-            cnt += (uint32_t)popc4(rsl);
-        }
-#endif
         cnt = __reduce_add_sync(0xffffffffu, cnt);
         if (lane == 0) wsum[wid] = cnt;
         __syncthreads();
@@ -773,22 +643,11 @@ __device__ __forceinline__ uint2 ldg_nc64(const uint2* p) {
     return r;
 }
 constexpr int kPairWarps = 8;           // row_count_kernel
-#ifndef FBGPU_PAIR_WARPS
-#define FBGPU_PAIR_WARPS 8
-#endif
-#ifndef FBGPU_PAIR_MIN_BLOCKS
-#define FBGPU_PAIR_MIN_BLOCKS 3
-#endif
-constexpr int kPcWarps = FBGPU_PAIR_WARPS;                  // warps per CTA of pair_count_kernel, one 8 KiB bitmap each; 3 CTAs per SM (8 warps measured faster than 9)
+constexpr int kPcWarps = 8;                                 // warps per CTA of pair_count_kernel, one 8 KiB bitmap each; 3 CTAs per SM (8 warps measured faster than 9)
+constexpr int kPcMinBlocks = 3;
 constexpr int kPcPairSlots = 256;                           // row pairs per launch whose counts are summed in shared memory first
-#ifndef FBGPU_PAIR_BM_UNROLL
-#define FBGPU_PAIR_BM_UNROLL 8
-#endif
-#ifndef FBGPU_PAIR_PF_DIST
-#define FBGPU_PAIR_PF_DIST 1
-#endif
-constexpr int kPcPfDist = FBGPU_PAIR_PF_DIST;               // how many units ahead the payload lines are prefetched into L2
-constexpr int kPcBmUnroll = FBGPU_PAIR_BM_UNROLL;           // bitmap x bitmap: pairs of 16-byte loads in flight per lane
+constexpr int kPcPfDist = 1;                                // how many units ahead the payload lines are prefetched into L2
+constexpr int kPcBmUnroll = 8;                              // bitmap x bitmap: pairs of 16-byte loads in flight per lane
 constexpr uint32_t kPcFastCard = 768;                       // arrays up to this size take the register-window path (3 chunks per lane)
 
 // Pairs with a run container on at least one side; returns the per-lane partial count.  The searched interval list (<= 2048 runs =
@@ -865,7 +724,7 @@ __device__ __noinline__ uint32_t warp_intersection_count_generic(Resolved a, Res
         if (a.card > b.card) { Resolved t = a; a = b; b = t; }
         const uint4* a4 = reinterpret_cast<const uint4*>(a.ptr); const uint4* b4 = reinterpret_cast<const uint4*>(b.ptr);
         const uint32_t na8 = (a.card + 7) >> 3, nb8 = (b.card + 7) >> 3;
-        const smem_base_t sb = smem_base((uint32_t)__cvta_generic_to_shared(bm));
+        const uint32_t sb = (uint32_t)__cvta_generic_to_shared(bm);
         for (uint32_t i = lane; i < na8; i += 32) scatter_chunk_sb<0>(sb, ldg_nc(a4 + i), i * 8, a.card);
         __syncwarp();
         for (uint32_t i = lane; i < nb8; i += 32) {           // whole chunks: the pad copies of b's last element are taken out below
@@ -873,7 +732,7 @@ __device__ __noinline__ uint32_t warp_intersection_count_generic(Resolved a, Res
 #pragma unroll
             for (int q = 0; q < 4; q++) {
                 c += (lds_u32(word_addr_lo(sb, w[q])) >> (w[q] & 31)) & 1u;
-                c += (lds_u32(word_addr_hi(sb, w[q])) >> (upper16(w[q]) & 31)) & 1u;
+                c += (lds_u32(word_addr_hi(sb, w[q])) >> ((w[q] >> 16) & 31)) & 1u;
             }
         }
         const uint32_t pads = nb8 * 8u - b.card;
@@ -902,7 +761,7 @@ __device__ __noinline__ uint32_t warp_intersection_count_generic(Resolved a, Res
 // dispatch left: six shuffles, six 16-byte loads per lane, scatter / probe / clear out of a register window.
 // The path is bound by the integer ALU pipe (LOP3 / LEA / SHF), about half of whose instructions per pair are the scatter and probe
 // arithmetic itself: every instruction that is not per-element work was taken out of the per-unit loop.
-__global__ void __launch_bounds__(kPcWarps * 32, FBGPU_PAIR_MIN_BLOCKS)
+__global__ void __launch_bounds__(kPcWarps * 32, kPcMinBlocks)
 pair_count_kernel(StoreRef st, uint32_t fvA, uint64_t rowA, uint32_t fvB, uint64_t rowB,
                   const uint64_t* __restrict__ rowsA, const uint64_t* __restrict__ rowsB, long long units_per_pair,
                   const uint64_t* __restrict__ shards, uint64_t shard0, long long n_units,
@@ -920,7 +779,7 @@ pair_count_kernel(StoreRef st, uint32_t fvA, uint64_t rowA, uint32_t fvB, uint64
 #pragma unroll 4
         for (int i = lane; i < 512; i += 32) b4[i] = make_uint4(0, 0, 0, 0); }
     __syncwarp();
-    smem_base_t sb = smem_base((uint32_t)__cvta_generic_to_shared(bm));
+    uint32_t sb = (uint32_t)__cvta_generic_to_shared(bm);
     pin_base(sb);
     unsigned long long acc = 0, run_sum = 0;               // run_sum: count of the current pair index / shard, flushed when it changes
     long long run_key = -1;
@@ -965,19 +824,15 @@ pair_count_kernel(StoreRef st, uint32_t fvA, uint64_t rowA, uint32_t fvB, uint64
                 if (np != 0 && (lane & 15) < 12) asm volatile("prefetch.global.L2 [%0];" :: "l"(np + (unsigned long long)(lane & 15) * 128ull));
             }
         };
-#ifndef FBGPU_PAIR_NO_PF
 #pragma unroll
         for (int j = 1; j < kPcPfDist; j++) prefetch_unit(j);
-#endif
         const int n_k = (int)min((long long)16, (n_units - base + stride - 1) / stride);      // units of this round (one division per round instead of a 64-bit compare per unit)
         long long unit = base - stride;
         for (int k = 0; k < n_k; k++) {
             unit += stride;
             const uint32_t ca = __shfl_sync(0xffffffffu, my_card, 2 * k), cb = __shfl_sync(0xffffffffu, my_card, 2 * k + 1);
             uint32_t c = 0;
-#ifndef FBGPU_PAIR_NO_PF
             prefetch_unit(k + kPcPfDist);       // payloads of a later unit on their way to L2 while this one is intersected
-#endif
             if ((ca >> 20) == 1u) {
                 // ---- two small arrays: a (even lane) is scattered, b probed; lane L owns chunks L, L+32, L+64 of both
                 const uint4* a4 = reinterpret_cast<const uint4*>(__shfl_sync(0xffffffffu, my_ptr, 2 * k)) + lane;
@@ -994,7 +849,7 @@ pair_count_kernel(StoreRef st, uint32_t fvA, uint64_t rowA, uint32_t fvB, uint64
                     for (int q = 0; q < 4; q++) { ad[2 * q] = word_addr_lo(sb, x[q]); ad[2 * q + 1] = word_addr_hi(sb, x[q]); }
                     if (on) {       // (array tails are padded with copies of the last element: setting a bit twice is harmless)
 #pragma unroll
-                        for (int q = 0; q < 4; q++) { red_or_at(ad[2 * q], 1u << (x[q] & 31)); red_or_at(ad[2 * q + 1], 1u << (upper16(x[q]) & 31)); }
+                        for (int q = 0; q < 4; q++) { red_or_at(ad[2 * q], 1u << (x[q] & 31)); red_or_at(ad[2 * q + 1], 1u << ((x[q] >> 16) & 31)); }
                     }
                 };
                 scatter(va0, addr[0], pa0); scatter(va1, addr[1], pa1); scatter(va2, addr[2], pa2);
@@ -1007,7 +862,7 @@ pair_count_kernel(StoreRef st, uint32_t fvA, uint64_t rowA, uint32_t fvB, uint64
 #pragma unroll
                     for (int q = 0; q < 4; q++) {
                         n += (lds_u32(word_addr_lo(sb, x[q])) >> (x[q] & 31)) & 1u;
-                        n += (lds_u32(word_addr_hi(sb, x[q])) >> (upper16(x[q]) & 31)) & 1u;
+                        n += (lds_u32(word_addr_hi(sb, x[q])) >> ((x[q] >> 16) & 31)) & 1u;
                     }
                     return n;
                 };
@@ -1681,10 +1536,6 @@ __device__ __forceinline__ void thread_for_each_col(const Resolved& c, const uin
     }
 }
 
-#ifndef FBGPU_GD_PIPE
-#define FBGPU_GD_PIPE 1
-#endif
-
 __global__ void __launch_bounds__(kGdThreads, 3)
 groupby_direct_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ rowsA, int nA /* <= kGdThreads */,
                       uint32_t fvB, const uint64_t* __restrict__ rowsB, int nB,
@@ -1742,7 +1593,7 @@ groupby_direct_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ ro
     };
 
     const ViewTab vA = st.views[fvA], vB = st.views[fvB];
-    if (FBGPU_GD_PIPE && !multiB && vA.rt_rows && vB.rt_rows) {
+    if (!multiB && vA.rt_rows && vB.rt_rows) {
         // Both views have the dense (shard, row) directory: the three dependent loads of a unit — directory entry, descriptor, first
         // payload chunk — are issued one unit apart each, so that every level has a whole phase of another unit to arrive in:
         //   iteration i:  shard id(i+3), directory(i+2), descriptor(i+1) <- directory(i+1) | insert(i) | payload(i+1) <- descriptor(i+1) | probe(i)

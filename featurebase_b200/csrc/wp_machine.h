@@ -1,12 +1,12 @@
 // Op loop of the word-parallel program machine (eval_wordpar_kernel), restructured to keep every value in a register with a
-// fixed role.  The default since round 2 (-DFBGPU_WP_LEGACY_LOOP restores the original rotating-ring loop).  Host-compilable on purpose: tests/test_wp_machine.py checks it on the CPU against a plain
-// stack-machine model for random programs.
+// fixed role.  Host-compilable on purpose: tests/test_program_compiler.py::test_wordpar_unrolled_loop_matches_stack_model checks it
+// on the CPU against a plain stack-machine model for random programs.
 //
-// Why: in the original loop the operand prefetch ring (p0 <- p1 <- p2) rotates and the 4-deep register stack shifts inside
-// one generic loop body, so ptxas emits ~40-60 register moves per op around 4 useful logic instructions (cuobjdump: blocks
-// of IMAD.MOV per switch case) — interpretive overhead that limited that kernel.  Here the
-// loop walks ROW ops three at a time; ring slot j always serves row op 3t+j, so there is no rotation, and the ops that do
-// move the stack (PUSH_EMPTY / SWAP / POP / binary ops, rare in BSI sweeps) run in a separate small loop between row ops.
+// Why: in a loop where the operand prefetch ring (p0 <- p1 <- p2) rotates and the 4-deep register stack shifts inside one
+// generic loop body, ptxas emits ~40-60 register moves per op around 4 useful logic instructions (cuobjdump: blocks of
+// IMAD.MOV per switch case) — interpretive overhead that limited the first form of the kernel.  Here the loop walks ROW ops
+// R at a time; ring slot j always serves row op R*t+j, so there is no rotation, and the ops that do move the stack
+// (PUSH_EMPTY / SWAP / POP / binary ops, rare in BSI sweeps) run in a separate small loop between row ops.
 #pragma once
 #include <stdint.h>
 
@@ -61,13 +61,10 @@ FBGPU_HD void wp_row_op(WpStack<V>& s, uint8_t opc, V x) {
 }
 
 // opc(k): opcode of program op k; is_row(k); rowops[ri]: program index of the ri-th row op; fetch(ri): its operand slice.
-// Returns the top of stack (zero when the program leaves the stack empty).  R = operand slices in flight per thread: ring slot j
-// always serves row op R*t + j, so the ring never rotates.  (The 10 M-record BASELINE config 3 is latency-bound — 34 plane loads
-// per thread — so the default ring is deeper than 3.)
-#ifndef FBGPU_WP_RING
-#define FBGPU_WP_RING 6
-#endif
-template <class V, bool NO_PUSH = false, int R = FBGPU_WP_RING, class OpcAt, class IsRowAt, class RowOpAt, class Fetch>
+// Returns the top of stack (zero when the program leaves the stack empty).  R = operand slices fetched ahead per thread: ring slot j
+// always serves row op R*t + j, so the ring never rotates.  The default R = 1 is what eval_wordpar_kernel runs: its fetch() reads a
+// cp.async ring in shared memory that already keeps the loads in flight.
+template <class V, bool NO_PUSH, int R = 1, class OpcAt, class IsRowAt, class RowOpAt, class Fetch>
 FBGPU_HD V wp_run_unrolled(int n_ops, int nr, OpcAt opc_at, IsRowAt is_row_at, RowOpAt rowop_at, Fetch fetch) {
     WpStack<V> s; s.T = s.B = s.S2 = s.S3 = wp_zero<V>(); s.depth = 0;
     V p[R];

@@ -51,7 +51,7 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
 
 
 def lib_path():
-    return os.environ.get("FBGPU_LIB") or os.path.join(_HERE, "libfbgpu.so")   # FBGPU_LIB: tuning variants only
+    return os.environ.get("FBGPU_LIB") or os.path.join(_HERE, "libfbgpu.so")   # FBGPU_LIB: another build of the library (the test suite's CPU kernel interpreter)
 
 
 def load():
@@ -101,9 +101,6 @@ def load():
     L.fbgpu_get_counters.argtypes, L.fbgpu_get_counters.restype = [vp, C.POINTER(Counters)], C.c_int
     L.fbgpu_stream.argtypes, L.fbgpu_stream.restype = [vp], vp
     L.fbgpu_rows_payload_bytes.argtypes, L.fbgpu_rows_payload_bytes.restype = [vp, u32, u32, u32, vp, i32, vp, i64, C.POINTER(u64), C.POINTER(u64)], C.c_int
-    if os.environ.get("FBGPU_LIB") and not hasattr(L, "fbgpu_node_init"):      # an older tuning build (A/B runs only): round-1 entry points only
-        _LIB = L
-        return L
     L.fbgpu_comm_p2p_open_local.argtypes, L.fbgpu_comm_p2p_open_local.restype = [vp, i32], C.c_int
     L.fbgpu_any.argtypes, L.fbgpu_any.restype = [vp, u32, vp, i32, vp, i64, C.POINTER(i32)], C.c_int
     L.fbgpu_pair_types.argtypes, L.fbgpu_pair_types.restype = [vp, u32, u32, u32, u64, u32, u32, u64, vp, i64, vp], C.c_int

@@ -124,8 +124,7 @@ struct Fiber {
     Ctx ctx; char* stack = nullptr; bool done = true;
     dim3 tid; int lane = 0, warp = 0;
     long blk_gen = 0, warp_gen = 0;          // barriers this thread has arrived at
-    int wait = 0;                             // 0 runnable, 1 block barrier, 2 warp barrier, 3 named barrier
-    int nb = 0; long nb_gen = 0;              // the named barrier (and its generation) this thread waits at
+    int wait = 0;                             // 0 runnable, 1 block barrier, 2 warp barrier
     unsigned red_n = 0;
 };
 struct State {
@@ -165,17 +164,6 @@ inline void warp_barrier() {
     if (++w.arrived == w.alive) { release_warp(w); return; }
     me.wait = 2;
     while (w.gen < g) yield();
-    me.wait = 0;
-}
-// bar.sync id, count: the first `count` threads to arrive at barrier `id` of this generation release each other
-struct NamedBar { int arrived = 0; long gen = 0; };
-inline NamedBar g_named[16];
-inline void named_barrier(int id, int count) {
-    State& s = S(); Fiber& me = *s.cur; NamedBar& b = g_named[id & 15];
-    const long g = b.gen;
-    if (++b.arrived == count) { b.arrived = 0; b.gen++; return; }
-    me.wait = 3; me.nb = id & 15; me.nb_gen = g;
-    while (b.gen == g) yield();
     me.wait = 0;
 }
 inline int block_reduce(int pred, int mode /*0 count, 1 and, 2 or*/) {
@@ -230,7 +218,6 @@ inline bool runnable(const State& s, const Fiber& f) {
     if (f.done) return false;
     if (f.wait == 1) return s.bar_gen >= f.blk_gen;
     if (f.wait == 2) return s.warps[f.warp].gen >= f.warp_gen;
-    if (f.wait == 3) return g_named[f.nb].gen != f.nb_gen;
     return true;
 }
 
@@ -245,7 +232,6 @@ inline void launch(dim3 grid, dim3 block, size_t smem, const std::function<void(
     s.grid = grid; s.block = block; s.nthreads = T; s.body = &body; s.launches++;
     for (unsigned b = 0; b < grid.x; b++) {
         s.bid = dim3(b); s.alive = T; s.arrived = 0; s.bar_gen = 0; s.red_cnt[0] = s.red_cnt[1] = 0;
-        for (NamedBar& nb : g_named) nb = NamedBar();
         memset(g_dyn, 0xCD, smem ? smem : 16);
         if (__start_fbgpu_smem && __stop_fbgpu_smem > __start_fbgpu_smem) memset(__start_fbgpu_smem, 0xCD, (size_t)(__stop_fbgpu_smem - __start_fbgpu_smem));
         for (int w = 0; w < W; w++) { s.warps[w] = Warp(); s.warps[w].alive = std::min(32, T - 32 * w); }

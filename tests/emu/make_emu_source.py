@@ -79,15 +79,12 @@ def rewrite_launches(s):
 
 ASM = [
     (r'asm volatile\("ld\.global\.nc\.L1::no_allocate\.v4\.u32 \{%0,%1,%2,%3\}, \[%4\];" : "=r"\(r\.x\), "=r"\(r\.y\), "=r"\(r\.z\), "=r"\(r\.w\) : "l"\(p\)\);', "r = *p;"),
-    (r'asm volatile\("prefetch\.global\.L2 \[%0\];" :: "l"\(p\)\);', "(void)p;"),
     (r'asm volatile\("prefetch\.global\.L2 \[%0\];" :: "l"\(np \+ \(unsigned long long\)\(lane & 15\) \* 128ull\)\);', "(void)np;"),
     (r'asm volatile\("ld\.global\.nc\.L1::no_allocate\.v2\.u32 \{%0,%1\}, \[%2\];" : "=r"\(r\.x\), "=r"\(r\.y\) : "l"\(p\)\);', "r = *p;"),
-    (r'asm volatile\("bar\.sync %0, 64;" :: "r"\(id\) : "memory"\);', "emu::named_barrier(id, 64);"),
     (r'asm volatile\("red\.shared\.or\.b32 \[%0\], %1;" :: "r"\((\w+)\), "r"\(([^()]+)\) : "memory"\);', r"emu::red_or(\1, \2);"),
     (r'asm volatile\("red\.shared\.and\.b32 \[%0\], %1;" :: "r"\((\w+)\), "r"\(([^()]+)\) : "memory"\);', r"emu::red_and(\1, \2);"),
     (r'asm volatile\("red\.shared\.xor\.b32 \[%0\], %1;" :: "r"\((\w+)\), "r"\(([^()]+)\) : "memory"\);', r"emu::red_xor(\1, \2);"),
     (r'asm volatile\("" : "\+r"\(([\w\[\].]+)\)\);', r"(void)\1;"),
-    (r'asm volatile\("" : "\+l"\((\w+)\)\);', r"(void)\1;"),
     (r'asm volatile\("cp\.async\.cg\.shared\.global \[%0\], \[%1\], 16;" :: "r"\(\(uint32_t\)__cvta_generic_to_shared\(dst_smem\)\), "l"\(src\) : "memory"\);', r"*dst_smem = *src;"),
     (r'asm volatile\("cp\.async\.commit_group;" ::: "memory"\);', r"(void)0;"),
     (r'asm volatile\("cp\.async\.wait_group %0;" :: "n"\(N\) : "memory"\);', r"(void)0;"),

@@ -3,11 +3,11 @@
 tests/emu/ compiles a scratch copy of the library's own sources (fbgpu.cu + kernels.cuh, launches / `extern __shared__` /
 inline PTX rewritten mechanically) with g++ against a stand-in <cuda_runtime.h> that runs every CUDA thread as a fibre, and the
 gpu-marked parity tests are then re-run against that library in a child process.  This is test infrastructure: the product
-never loads it (featurebase_b200/lib.py loads libfbgpu.so; FBGPU_LIB is the tuning-variant override the child uses), it
+never loads it (featurebase_b200/lib.py loads libfbgpu.so; the child points FBGPU_LIB at the interpreted library), it
 proves nothing about speed, memory-model races or the PTX the rewrites replace, and the device run stays the parity gate.
 What it does give: the scatter / probe / program-loop / group-by code paths written after the round's GPU budget was spent
-(and the opt-in ones: sorted array order, groupby_kernel for every unit, the unrolled word-parallel loop) have executed,
-statement by statement, against the oracle and the reference's goldens.  Every kernel of the library runs on the interpreter.
+(and the opt-in ones: sorted array order, groupby_kernel for every unit) have executed, statement by statement, against the
+oracle and the reference's goldens.  Every kernel of the library runs on the interpreter.
 
 Default run: everything gpu-marked except the bodies that take a minute or more each when interpreted (≈1.5 min in all).
 FBGPU_EMU_FULL=1 adds those: the 1024-shard property tests, the reference's 638 x 9 combination table (in both array
@@ -48,8 +48,8 @@ def emu_lib(defines=(), flags=()):
     return lib
 
 
-def run_on_emulator(args, env=None, defines=(), timeout=1500):
-    e = dict(os.environ, FBGPU_LIB=emu_lib(defines), FBGPU_TEST_ON_EMULATOR="1", **(env or {}))
+def run_on_emulator(args, env=None, timeout=1500):
+    e = dict(os.environ, FBGPU_LIB=emu_lib(), FBGPU_TEST_ON_EMULATOR="1", **(env or {}))
     e.pop("FBGPU_EMU_FULL", None)
     r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-m", "gpu", "-p", "no:cacheprovider"] + args, cwd=ROOT, env=e,
                        stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=timeout)
@@ -90,14 +90,6 @@ def test_groupby_kernel_on_every_unit():
     GroupBy goldens and parity tests, and the shapes built for its passes (a bitmap row -> dense pass; two chunks per side; filter)"""
     sel = "(groupby or various_queries) and not sorted_order" + ("" if FULL else " and not full_size")
     run_on_emulator(["tests/test_gpu_parity.py", "tests/test_zz_gpu_experimental.py", "-k", sel], env={"FBGPU_GROUPBY_CTA": "1"})
-
-
-def test_wordpar_loop_variants():
-    """the word-parallel op loop (wp_machine.h) with its register operand ring (-DFBGPU_WP_REG_RING), a shallower cp.async ring, and the
-    round-1 rotating-ring loop (-DFBGPU_WP_LEGACY_LOOP), on the BSI programs (the default build's cp.async ring runs in test_default_kernels_parity)"""
-    run_on_emulator(["tests/test_gpu_parity.py", "-k", "bsi_range or bsi_uniform or FORCE_WORDPAR or bsi_diagonal"], defines=("FBGPU_WP_REG_RING", "FBGPU_WP_RING=3"), timeout=3000)
-    run_on_emulator(["tests/test_gpu_parity.py", "-k", "bsi_range or bsi_uniform or FORCE_WORDPAR"], defines=("FBGPU_WP_ASYNC_DEPTH=3",), timeout=3000)
-    run_on_emulator(["tests/test_gpu_parity.py", "-k", "bsi_range or bsi_uniform or FORCE_WORDPAR"], defines=("FBGPU_WP_LEGACY_LOOP",), timeout=3000)
 
 
 @pytest.mark.parametrize("order", ["reverse", "random"])

@@ -261,7 +261,7 @@ def test_wordpar_unrolled_loop_matches_stack_model(cc):
         arr = (DevOp * max(len(prog), 1))()
         for i, (op, fv, row) in enumerate(prog):
             arr[i].op, arr[i].fv, arr[i].row = op, fv, row
-        for no_push in (0, 1):                               # 1: PUSH_ROW rewritten to PUSH_EMPTY + OR_ROW first (what the variant build runs)
+        for no_push in (0, 1):                               # 1: PUSH_ROW rewritten to PUSH_EMPTY + OR_ROW first (what the kernel runs)
             out = (C.c_uint32 * 4)()
             cc.wp_run(arr, len(prog), np.ascontiguousarray(words).ctypes.data_as(C.c_void_p), out, no_push)
             got = out[0] | out[1] << 32 | out[2] << 64 | out[3] << 96
