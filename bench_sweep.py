@@ -6,6 +6,8 @@
   config 3: BSI Count(Row(v > k)) over 10 M records, 32-bit values (eval_kernel plane sweep).
   config 4: GroupBy(Rows(a), Rows(b)) 256 x 256 over this GPU's share (512 shards) of 100 M records / 4096 shards.
   config X: fbgpu_columns / fbgpu_extract (device-side column-id and int-value expansion), wall clock; R: fbgpu_row.
+  config P: Percentile over config X's 32-bit field, order statistics (fbgpu_bsi_select) against the query-driven bisection
+            (only when named in --configs).
 Every point is spot-checked against the CPU oracle on a few shards (the checker, not the thing measured)."""
 import argparse
 import json
@@ -199,6 +201,73 @@ def config_extract(args, out):
     h.ctx.close()
 
 
+class _KernelMs:
+    """a context proxy that sums last_query_gpu_ms over every library query issued through it"""
+
+    def __init__(self, ctx):
+        self.ctx, self.ms = ctx, 0.0
+
+    def __getattr__(self, name):
+        fn = getattr(self.ctx, name)
+        if name in ("counters", "close", "commit") or not callable(fn):
+            return fn
+
+        def call(*a, **kw):
+            r = fn(*a, **kw)
+            self.ms += self.ctx.counters()["last_query_gpu_ms"]
+            return r
+        return call
+
+
+def config_percentile(args, out):
+    """Percentile(field=v, nth) over config X's data (10 M records, 32-bit values), with and without a 1 % filter row, through
+    the executor: the select arm (one Count + one fbgpu_bsi_select) and the bisection arm (Count, Min, Max, then up to two
+    Counts per bisection step), alternated query by query.  Both arms must give the same ValCount."""
+    from featurebase_b200 import datagen as D, executor as X
+    n_rec = min(10_000_000, args.shards * SW)
+    n_sh = (n_rec + SW - 1) // SW
+    shards = np.arange(n_sh, dtype=np.uint64)
+    h = X.Holder()
+    idx = h.create_index("i", track_existence=False)
+    f = idx.create_field("f")
+    v = idx.create_field("v", "int", min=0, max=(1 << 32) - 1)
+    bulk = D.fragments(11, shards, [0], 0.01)
+    h.ctx.load_fragments(idx.id, f.id, X.VIEW_STANDARD, shards, bulk.buf, bulk.offsets)
+    for s in range(n_sh):
+        h.ctx.load_fragment(idx.id, v.id, X.VIEW_BSI, s, D.bsi_fragment(12, s, min(SW, n_rec - s * SW), 32, 0, (1 << 32) - 1))
+    h.ctx.commit()
+    idx.shards.update(range(n_sh))
+    real = h.ctx
+    h.ctx = prox = _KernelMs(real)
+    arms = {"select": X.Executor(h), "bisection": X.Executor(h)}
+    arms["bisection"].percentile_select = False
+    for nth in (1, 50, 99.9):
+        for q_filter in (False, True):
+            q = f"Percentile(field=v, nth={nth}" + (", filter=Row(f=0))" if q_filter else ")")
+            rec = {name: {"wall": [], "kernel_ms": [], "queries": []} for name in arms}
+            res = {}
+            for i in range(2 + args.steps):                  # two warm-up rounds, then alternate the arms
+                for name in (("select", "bisection") if i % 2 == 0 else ("bisection", "select")):
+                    q0, prox.ms = real.counters()["queries"], 0.0
+                    t0 = time.perf_counter()
+                    r = arms[name].execute("i", q)[0]
+                    wall = (time.perf_counter() - t0) * 1e3
+                    res.setdefault(name, r)
+                    assert r == res[name], (q, name)
+                    if i >= 2:
+                        rec[name]["wall"].append(wall)
+                        rec[name]["kernel_ms"].append(prox.ms)
+                        rec[name]["queries"].append(real.counters()["queries"] - q0)
+            assert res["select"] == res["bisection"], (q, res)
+            for name, d in rec.items():
+                out({"config": "P", "query": q, "arm": name, "records": n_rec, "shards": n_sh, "result": [res[name].val, res[name].count],
+                     "wall_ms": float(np.median(d["wall"])), "wall_ms_min": float(np.min(d["wall"])), "wall_ms_max": float(np.max(d["wall"])),
+                     "kernel_ms": float(np.median(d["kernel_ms"])), "queries": int(np.median(d["queries"])), "steps": args.steps,
+                     "kernel": "eval_kernel + bsi_select_step_kernel + bsi_select_decide_kernel" if name == "select" else "eval_kernel + bsi_minmax_kernel (Count / Min / Max / bisection Counts)",
+                     "note": "median over the timed steps of the executor call (wall clock) and of the summed last_query_gpu_ms of its library queries"})
+    real.close()
+
+
 def config3(args, out, n_rec=10_000_000, nf=4):
     """nf fields are rotated between steps so that the touched planes exceed L2 (the 10 M-record config is 42.5 MB)"""
     from featurebase_b200 import datagen as D, executor as X, pql
@@ -307,6 +376,8 @@ def main():
             config_row(args, out)
         elif c == "X":
             config_extract(args, out)
+        elif c == "P":
+            config_percentile(args, out)
         elif c == "3L":     # the same BSI query at 256 shards (268 M records, 1.1 GB of planes): shows the kernel away from the launch-bound regime
             config3(args, out, n_rec=256 * SW, nf=1)
         else:

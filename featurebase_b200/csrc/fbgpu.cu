@@ -145,6 +145,7 @@ struct Workspace {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     DevBuf d_in, d_counts, d_bitmaps, d_info, d_emit_units, d_emit, d_rows, d_aux;
+    DevBuf d_select;                     // fbgpu_bsi_select: per-rank candidate bitmaps of every unit of the call
     PinBuf h_in, h_out;
     bool busy = false;
 };
@@ -249,7 +250,7 @@ extern "C" void fbgpu_shutdown(fbgpu_ctx* c) {
     cudaDeviceSynchronize();
     if (c->comm && nccl_load()) g_nccl.CommDestroy(c->comm);
     for (auto& w : c->wss) {
-        for (DevBuf* b : { &w->d_in, &w->d_counts, &w->d_bitmaps, &w->d_info, &w->d_emit_units, &w->d_emit, &w->d_rows, &w->d_aux }) b->release();
+        for (DevBuf* b : { &w->d_in, &w->d_counts, &w->d_bitmaps, &w->d_info, &w->d_emit_units, &w->d_emit, &w->d_rows, &w->d_aux, &w->d_select }) b->release();
         w->h_in.release(); w->h_out.release();
         if (w->ev0) cudaEventDestroy(w->ev0);
         if (w->ev1) cudaEventDestroy(w->ev1);
@@ -1384,6 +1385,93 @@ extern "C" int fbgpu_bsi_sum(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, 
     float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1);
     bump(c, launches, ms);
     lease.ok = true;
+    return FBGPU_OK;
+} FBGPU_CATCH
+
+// ------------------------------------------------------------------ BSI order statistics (radix select over the planes, kernels.cuh)
+// The row is evaluated batch by batch straight into rank 0's slot of the call's candidate buffer (d_select: 8 KiB per unit per
+// distinct rank, plus one live mask per unit), then the select steps run over every unit of the call at once, chained on the
+// stream: no host round trip until the one D2H copy of the rank states.
+static_assert(kSelMaxRanks == FBGPU_SELECT_MAX_RANKS, "kernels.cuh and fbgpu.h disagree on the rank cap");
+extern "C" int fbgpu_bsi_select(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
+                                const uint64_t* shards, int64_t n_shards, const uint64_t* ranks, int32_t n_ranks,
+                                int64_t* out_vals, uint64_t* out_counts, uint64_t* out_total) try {
+    if (!c || !out_total || n_shards < 0 || (n_shards && !shards) || n_ops < 0 || (n_ops && !ops) || n_ranks < 0 || (n_ranks && (!ranks || !out_vals)))
+        return fail(FBGPU_E_INVALID, "null argument");
+    if (bit_depth < 0 || bit_depth > 63) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..63", bit_depth);
+    if (n_ranks > FBGPU_SELECT_MAX_RANKS) return fail(FBGPU_E_INVALID, "%d ranks: at most %d per call", n_ranks, FBGPU_SELECT_MAX_RANKS);
+    if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_bsi_select is local to one context: order statistics of the ranks' shares do not merge");
+    USE_DEVICE(c);
+    std::shared_lock<std::shared_mutex> lk;
+    int rc = lock_committed(c, lk); if (rc) return rc;
+    *out_total = 0;
+    std::vector<uint64_t> uniq(ranks, ranks + n_ranks);     // the device works on distinct ranks (at least one: slot 0 holds the row)
+    std::sort(uniq.begin(), uniq.end());
+    uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
+    const int nr = std::max(1, (int)uniq.size());
+    std::vector<fbgpu_op> full(ops, ops + n_ops);           // the row = <filter> ∩ exists, as for Min / Max
+    fbgpu_op ex{}; ex.opcode = FBGPU_OP_ROW; ex.field = field; ex.view = view; ex.a = 0;
+    full.push_back(ex);
+    if (n_ops) { fbgpu_op in{}; in.opcode = FBGPU_OP_INTERSECT; in.argc = 2; full.push_back(in); }
+    std::vector<DevOp> prog; int depth = 1;
+    rc = compile_program(c, index, full.data(), (int32_t)full.size(), prog, depth); if (rc) return rc;
+    const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
+    WsLease lease(c); Workspace* w = lease.w;
+    const DevOp* d_prog; const uint64_t* d_shards;
+    rc = upload_inputs(w, prog, shards, n_shards, &d_prog, &d_shards); if (rc) return rc;
+    const long long n_units = (long long)n_shards * kSlotsPerRow;
+    // d_counts: [SelRank x kSelMaxRanks][buckets kSelMaxRanks x kSelBuckets][total]
+    const size_t st_bytes = kSelMaxRanks * sizeof(SelRank), bk_bytes = kSelMaxRanks * kSelBuckets * 8, ctl_bytes = st_bytes + bk_bytes + 8;
+    if (w->d_counts.ensure(ctl_bytes) || w->h_out.ensure(ctl_bytes)) return FBGPU_E_NOMEM;
+    const size_t cand_bytes = (size_t)n_units * (size_t)nr * 8192;
+    if (n_units > 0 && w->d_select.ensure(cand_bytes + (size_t)n_units * 4)) return FBGPU_E_NOMEM;
+    memset(w->h_out.p, 0, ctl_bytes);                       // (h_out is free: the previous user of the lease drained its copies)
+    SelRank* hs = (SelRank*)w->h_out.p;
+    for (int r = 0; r < (int)uniq.size(); r++) hs[r].rank = uniq[(size_t)r];
+    CUDA_TRY(cudaMemcpyAsync(w->d_counts.p, w->h_out.p, ctl_bytes, cudaMemcpyHostToDevice, w->stream));
+    SelRank* d_state = (SelRank*)w->d_counts.p;
+    unsigned long long* d_buckets = (unsigned long long*)((uint8_t*)w->d_counts.p + st_bytes);
+    unsigned long long* d_total = d_buckets + kSelMaxRanks * kSelBuckets;
+    uint4* d_cand = (uint4*)w->d_select.p;
+    unsigned int* d_live = n_units > 0 ? (unsigned int*)((uint8_t*)w->d_select.p + cand_bytes) : nullptr;
+    uint64_t launches = 0;
+    CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
+    if (n_units > 0) {
+        for (long long u0 = 0; u0 < n_units; u0 += c->unit_batch) {
+            const long long nu = std::min(c->unit_batch, n_units - u0);
+            EvalOut eo{ nullptr, nullptr, d_cand + (size_t)u0 * 512, nullptr, FuseReduce{} };
+            rc = launch_eval(c, w, prog, d_prog, depth, d_shards + u0 / kSlotsPerRow, nu, eo); if (rc) return rc;
+            launches++;
+        }
+        const int n_steps = (bit_depth + 1 + kSelDigit - 1) / kSelDigit;
+        const long long grid = std::min<long long>(n_units, (long long)c->sm_count * 4);
+        for (int s = 0; s < n_steps; s++) {
+            bsi_select_step_kernel<<<(unsigned)grid, kEvalThreads, 0, w->stream>>>(store_ref(c), fv, bit_depth, s, s == n_steps - 1 ? 1 : 0, d_cand, d_shards, n_units, nr,
+                                                                                   d_state, d_live, d_buckets);
+            CUDA_TRY(cudaGetLastError());
+            bsi_select_decide_kernel<<<1, 32, 0, w->stream>>>(bit_depth, s, nr, d_state, d_buckets, d_total);
+            CUDA_TRY(cudaGetLastError());
+            launches += 2;
+        }
+    }
+    CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, ctl_bytes, cudaMemcpyDeviceToHost, w->stream));
+    CUDA_TRY(cudaStreamSynchronize(w->stream));
+    float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1);
+    bump(c, launches, ms);
+    lease.ok = true;
+    const SelRank* rs = (const SelRank*)w->h_out.p;
+    const uint64_t total = *(const uint64_t*)((const uint8_t*)w->h_out.p + st_bytes + bk_bytes);
+    *out_total = total;
+    const uint64_t low = bit_depth ? ~0ull >> (64 - bit_depth) : 0ull;
+    for (int i = 0; i < n_ranks; i++) {
+        if (ranks[i] >= total) return fail(FBGPU_E_INVALID, "rank %llu outside the %llu sorted values", (unsigned long long)ranks[i], (unsigned long long)total);
+        const SelRank& R = rs[std::lower_bound(uniq.begin(), uniq.end(), ranks[i]) - uniq.begin()];
+        const bool neg = ((R.key >> bit_depth) & 1ull) == 0;   // key -> sign-magnitude (kernels.cuh)
+        const uint64_t mag = neg ? ~R.key & low : R.key & low;
+        out_vals[i] = neg ? -(int64_t)mag : (int64_t)mag;
+        if (out_counts) out_counts[i] = R.count;
+    }
     return FBGPU_OK;
 } FBGPU_CATCH
 

@@ -1301,6 +1301,207 @@ bsi_sum_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restrict__ co
 }
 
 // ------------------------------------------------------------------------------------------------
+// k-th smallest values of an int field over a row (fbgpu_bsi_select; the order statistics executePercentile's bisection
+// :1310-1600 depends on): an MSB-first radix select over a (depth + 1)-bit sort key per column,
+//     key = (sign ? 0 : 1) << depth  |  (sign ? ~magnitude : magnitude)  (low depth bits),
+// which orders negatives first, larger magnitudes first among them, then non-negatives by magnitude.  Step s fixes the key
+// bits [lo, hi] with hi = depth - s * kSelDigit: bsi_select_step_kernel counts, per (shard, slot) unit and per rank, the live
+// candidates in each of the 2^kSelDigit buckets of those bits (summed over all units with atomics), then the one-CTA
+// bsi_select_decide_kernel picks each rank's bucket, takes the columns below it off the remaining rank and zeroes the
+// counters.  The next step first narrows each rank's candidate bitmap (kept per unit in a call-scoped buffer) to the chosen
+// bucket, re-reading the previous step's planes once, then counts its own bits: every plane container of a unit is read at
+// most twice per call, however many ranks there are.  Step 0 holds the sign bit: all ranks start from the same set
+// (consider = filter ∩ exists, from eval_kernel), so it counts one set, and it xors the magnitude planes with the sign row per
+// column; later steps see one sign side per rank and flip the digit of a negative rank instead.  A unit without a live
+// candidate for any rank is skipped from then on.  The final bucket of a rank holds exactly the columns with its value.
+constexpr int kSelDigit = 4;                         // key bits per step: 33 key bits of a 32-bit field take 9 steps
+constexpr int kSelBuckets = 1 << kSelDigit;
+constexpr int kSelMaxRanks = 8;                      // = FBGPU_SELECT_MAX_RANKS (distinct ranks per call)
+
+struct SelRank {                                     // one distinct rank, host-initialised, advanced by bsi_select_decide_kernel
+    unsigned long long rank;                         // 0-based position in the ascending order
+    unsigned long long rem;                          // position still to find inside the rank's current candidate set
+    unsigned long long key;                          // key bits fixed so far
+    unsigned long long count;                        // size of the chosen bucket (after the last step: the value's multiplicity)
+    unsigned int digit;                              // key digit chosen by the last step
+    int neg;                                         // the candidates hold negative values (known after step 0)
+    int valid;                                       // rank < |row| (known after step 0)
+    int pad;
+};
+
+__host__ __device__ __forceinline__ int sel_step_bits(int depth, int step, int* lo) {
+    const int hi = depth - step * kSelDigit;
+    *lo = hi - kSelDigit + 1 > 0 ? hi - kSelDigit + 1 : 0;
+    return hi - *lo + 1;
+}
+
+// kb[j] = key bit lo + j of the unit's columns for the bits of `step` (zero for j >= the step's width).  Step 0 xors the
+// magnitude planes with the sign row, later steps return the raw planes.  CTA-wide call.
+__device__ __forceinline__ void sel_load_step(const StoreRef& st, uint32_t fv, uint64_t shard, int slot, int depth, int step,
+                                              uint4* X, Resolved* s_res, uint32_t* warp_tmp, uint4 kb[kSelDigit][kEvalU4PerThread]) {
+    int lo; const int w = sel_step_bits(depth, step, &lo);
+    uint4 sg[kEvalU4PerThread], x[kEvalU4PerThread];
+    if (step == 0) unit_load_plane(st, fv, shard, slot, 1, X, s_res, warp_tmp, sg);                 // bsiSignBit
+#pragma unroll
+    for (int h = 0; h < kEvalU4PerThread; h++) { if (step != 0) sg[h] = make_uint4(0, 0, 0, 0); }
+    for (int j = 0; j < kSelDigit; j++) {
+        if (j >= w) {
+#pragma unroll
+            for (int h = 0; h < kEvalU4PerThread; h++) x[h] = make_uint4(0, 0, 0, 0);
+        } else if (lo + j == depth) {                                                              // sign key bit: 1 = non-negative
+#pragma unroll
+            for (int h = 0; h < kEvalU4PerThread; h++) x[h] = xor4(sg[h], make_uint4(~0u, ~0u, ~0u, ~0u));
+        } else {
+            unit_load_plane(st, fv, shard, slot, (uint64_t)(2 + lo + j), X, s_res, warp_tmp, x);
+#pragma unroll
+            for (int h = 0; h < kEvalU4PerThread; h++) x[h] = xor4(x[h], sg[h]);
+        }
+#pragma unroll
+        for (int jj = 0; jj < kSelDigit; jj++) {                                                   // (constant indices: kb stays in registers)
+            if (jj == j) {
+#pragma unroll
+                for (int h = 0; h < kEvalU4PerThread; h++) kb[jj][h] = x[h];
+            }
+        }
+    }
+}
+
+// c &= the columns whose bits under kb equal digit d
+__device__ __forceinline__ void sel_narrow(uint4 c[kEvalU4PerThread], const uint4 kb[kSelDigit][kEvalU4PerThread], uint32_t d) {
+#pragma unroll
+    for (int j = 0; j < kSelDigit; j++) {
+#pragma unroll
+        for (int h = 0; h < kEvalU4PerThread; h++) c[h] = ((d >> j) & 1u) ? and4(c[h], kb[j][h]) : andn4(c[h], kb[j][h]);
+    }
+}
+
+__device__ __forceinline__ uint32_t u4_word(const uint4& v, int k) { return k == 0 ? v.x : k == 1 ? v.y : k == 2 ? v.z : v.w; }
+
+// adds the CTA's bucket counts of candidate set c (digits under kb) to cnt[0 .. kSelBuckets)
+__device__ __forceinline__ void sel_count(const uint4 c[kEvalU4PerThread], const uint4 kb[kSelDigit][kEvalU4PerThread], unsigned long long* cnt) {
+    uint32_t n[kSelBuckets];
+#pragma unroll
+    for (int b = 0; b < kSelBuckets; b++) n[b] = 0;
+#pragma unroll
+    for (int h = 0; h < kEvalU4PerThread; h++) {
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const uint32_t cw = u4_word(c[h], k);
+            if (!cw) continue;
+            uint32_t kw[kSelDigit];
+#pragma unroll
+            for (int j = 0; j < kSelDigit; j++) kw[j] = u4_word(kb[j][h], k);
+#pragma unroll
+            for (int b = 0; b < kSelBuckets; b++) {
+                uint32_t m = cw;
+#pragma unroll
+                for (int j = 0; j < kSelDigit; j++) m &= ((b >> j) & 1) ? kw[j] : ~kw[j];
+                n[b] += (uint32_t)__popc(m);
+            }
+        }
+    }
+#pragma unroll
+    for (int b = 0; b < kSelBuckets; b++) {
+        const uint32_t v = __reduce_add_sync(0xffffffffu, n[b]);
+        if ((threadIdx.x & 31) == 0 && v) atomicAdd(&cnt[b], (unsigned long long)v);
+    }
+}
+
+__global__ void __launch_bounds__(kEvalThreads)
+bsi_select_step_kernel(StoreRef st, uint32_t fv, int depth, int step, int last, uint4* __restrict__ cand /* [n_ranks][n_units] bitmaps; rank 0's = consider before step 1 */,
+                       const uint64_t* __restrict__ shards, long long n_units, int n_ranks, const SelRank* __restrict__ ranks,
+                       unsigned int* __restrict__ live /* [n_units] bit r: rank r has candidates in the unit */,
+                       unsigned long long* __restrict__ buckets /* [n_ranks][kSelBuckets], zero on entry */) {
+    __shared__ __align__(16) uint4 X[512];
+    __shared__ Resolved s_res;
+    __shared__ uint32_t warp_tmp[kEvalThreads / 32];
+    __shared__ unsigned long long s_cnt[kSelMaxRanks * kSelBuckets];
+    __shared__ uint32_t s_live;
+    const int tid = threadIdx.x;
+    for (int i = tid; i < kSelMaxRanks * kSelBuckets; i += kEvalThreads) s_cnt[i] = 0;
+    for (long long unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
+        const uint64_t shard = shards[unit >> 4];
+        const int slot = (int)(unit & 15);
+        __syncthreads();                                   // s_live of the previous unit has been read
+        if (tid == 0) s_live = step == 0 ? 1u : live[unit];
+        __syncthreads();
+        uint32_t lv = s_live;
+        if (!lv) continue;
+        uint4 base[kEvalU4PerThread], kb[kSelDigit][kEvalU4PerThread];
+        if (step <= 1) {
+#pragma unroll
+            for (int h = 0; h < kEvalU4PerThread; h++) base[h] = cand[(size_t)unit * 512 + tid + h * kEvalThreads];
+        }
+        if (step == 0) {
+            const int any = __syncthreads_or(any_u4(base));
+            if (tid == 0) live[unit] = any ? (n_ranks >= 32 ? ~0u : (1u << n_ranks) - 1u) : 0u;
+            if (!any) continue;
+            sel_load_step(st, fv, shard, slot, depth, 0, X, &s_res, warp_tmp, kb);
+            sel_count(base, kb, s_cnt);                    // every rank's set: the decide kernel reads row 0 for all
+            continue;
+        }
+        uint4 kp[kSelDigit][kEvalU4PerThread];
+        sel_load_step(st, fv, shard, slot, depth, step - 1, X, &s_res, warp_tmp, kp);
+        sel_load_step(st, fv, shard, slot, depth, step, X, &s_res, warp_tmp, kb);
+        int plo; const uint32_t pmask = (1u << sel_step_bits(depth, step - 1, &plo)) - 1u;
+        for (int r = 0; r < n_ranks; r++) {
+            if (!((lv >> r) & 1u)) continue;
+            const SelRank R = ranks[r];
+            if (!R.valid) { lv &= ~(1u << r); continue; }
+            uint4 c[kEvalU4PerThread];
+            uint4* slot_r = cand + ((size_t)r * (size_t)n_units + (size_t)unit) * 512;
+#pragma unroll
+            for (int h = 0; h < kEvalU4PerThread; h++) c[h] = step == 1 ? base[h] : slot_r[tid + h * kEvalThreads];
+            sel_narrow(c, kp, R.digit ^ (step - 1 > 0 && R.neg ? pmask : 0u));     // (step 0's planes are already key bits)
+            if (!__syncthreads_or(any_u4(c))) { lv &= ~(1u << r); continue; }
+            if (!last) {
+#pragma unroll
+                for (int h = 0; h < kEvalU4PerThread; h++) slot_r[tid + h * kEvalThreads] = c[h];
+            }
+            sel_count(c, kb, s_cnt + r * kSelBuckets);
+        }
+        if (tid == 0) live[unit] = lv;
+    }
+    __syncthreads();
+    for (int i = tid; i < kSelMaxRanks * kSelBuckets; i += kEvalThreads)
+        if (s_cnt[i]) atomicAdd(&buckets[i], s_cnt[i]);
+}
+
+// one CTA of 32 threads, thread r = rank r: picks the bucket of each rank from the summed counts of the step that just ran
+// (counts in plane-digit order after step 0; a negative rank walks them flipped), then zeroes the counters for the next step.
+// Step 0 also sets *total = |row| (the sum of row 0) and marks the ranks >= |row| invalid.
+__global__ void __launch_bounds__(32)
+bsi_select_decide_kernel(int depth, int step, int n_ranks, SelRank* __restrict__ ranks, unsigned long long* __restrict__ buckets, unsigned long long* __restrict__ total) {
+    const int r = threadIdx.x;
+    int lo; const int w = sel_step_bits(depth, step, &lo);
+    const uint32_t mask = (1u << w) - 1u;
+    if (r < n_ranks) {
+        SelRank R = ranks[r];
+        const unsigned long long* row = buckets + (size_t)(step == 0 ? 0 : r) * kSelBuckets;
+        if (step == 0) {
+            unsigned long long t = 0;
+            for (int b = 0; b < kSelBuckets; b++) t += row[b];
+            if (r == 0) *total = t;
+            R.valid = R.rank < t ? 1 : 0; R.rem = R.rank; R.key = 0;
+        }
+        if (R.valid) {
+            const uint32_t flip = step > 0 && R.neg ? mask : 0u;
+            unsigned long long below = 0;
+            for (uint32_t d = 0; d <= mask; d++) {
+                const unsigned long long n = row[d ^ flip];
+                if (R.rem < below + n) { R.digit = d; R.rem -= below; R.count = n; break; }
+                below += n;
+            }
+            R.key = (R.key << w) | R.digit;
+            if (step == 0) R.neg = (R.digit >> (w - 1)) == 0u ? 1 : 0;
+        }
+        ranks[r] = R;
+    }
+    __syncthreads();
+    for (int i = r; i < kSelMaxRanks * kSelBuckets; i += 32) buckets[i] = 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // GroupBy(Rows(a), Rows(b)) [+ filter]: one CTA per (shard, slot).  Column-keyed hash join instead of the
 // reference's |A|x|B| nested intersectionCount loop (executor.go:8880-8934): the elements of field-a rows are inserted
 // as (column, row) entries into an open-addressing table in shared memory (linear probing, duplicates allowed, so

@@ -857,10 +857,16 @@ class Executor:
         lim = c.args.get("limit")
         return kvs[:int(lim)] if lim is not None else kvs
 
+    percentile_select = True            # False: Percentile always runs the query-driven bisection (the reference's own flow)
+
     def _percentile(self, idx, c, shards):
         """executePercentile :1310-1600 (int fields): total = Count(filter ∩ notNull); the wanted numbers of smaller / larger
-        values; Min and Max under the filter; then a bisection on the value, two Count(Row(f < x) [∩ filter]) style queries
-        per step.  Every step is a whole-batch device query, exactly as every step is a cluster-wide query in the reference.
+        values (float64 arithmetic, as the reference); Min and Max under the filter; then a bisection on the value.
+        The reference asks two Count(Row(f < x) [∩ filter]) style queries per bisection step.  Every guess g lies in
+        [min, max], so with v[0..T-1] the sorted values: Count(f < g) > desiredLess exactly when v[desiredLess] < g, and
+        Count(f > g) > desiredGreater exactly when v[T-1-desiredGreater] > g.  One fbgpu_bsi_select call for the ranks
+        0, T-1, desiredLess, T-1-desiredGreater therefore fixes the answer bit for bit, and the bisection runs on the host.
+        Contexts without the call (a node handle, a context with a communicator) take the query-driven bisection.
         Returns None ("the median of nothing is NULL") or ValCount(value, 1) / the Min / Max ValCount at the ends."""
         nth = c.args.get("nth")
         if nth is None:
@@ -876,15 +882,70 @@ class Executor:
         f = self._field(idx, name)
         filt = c.args.get("filter") if isinstance(c.args.get("filter"), pql.Call) else None
         not_null = pql.Call("Row", {name: pql.Condition("!=", None)})
-
-        def count_of(row_call):
-            inner = row_call if filt is None else pql.Call("Intersect", {}, [row_call, filt])
-            return self._count(idx, pql.Call("Count", {}, [inner]), shards)
-        total = count_of(not_null) if filt is None else self._count(idx, pql.Call("Count", {}, [pql.Call("Intersect", {}, [filt, not_null])]), shards)
+        total = self._count(idx, pql.Call("Count", {}, [not_null if filt is None else pql.Call("Intersect", {}, [filt, not_null])]), shards)
         if total == 0:
             return None
         want_less = int(total * nth / 100.0)
         want_greater = int(total * (100 - nth) / 100.0)
+        if self.percentile_select and f.type == "int" and hasattr(self.ctx, "bsi_select"):
+            try:
+                return self._percentile_select(idx, f, filt, shards, total, want_less, want_greater)
+            except NotImplementedError:
+                pass
+            except L.FbgpuError as e:
+                if e.code != L.E_COMM:
+                    raise
+        return self._percentile_bisect(idx, f, filt, shards, want_less, want_greater)
+
+    @staticmethod
+    def _midpoint(lo, hi):
+        """the reference's overflow-free midpoint (:1493-1497) in Go's truncating integer arithmetic"""
+        tdiv = lambda a, b: int(a / b) if abs(a) < (1 << 52) else (abs(a) // b) * (1 if a >= 0 else -1)      # Go's truncating division
+        tmod = lambda a, b: a - b * tdiv(a, b)                                                                  # Go's %: sign of the dividend
+        return tdiv(lo, 2) + tdiv(hi, 2) + tdiv(tmod(lo, 2) + tmod(hi, 2), 2)
+
+    def _percentile_select(self, idx, f, filt, shards, total, want_less, want_greater):
+        """the bisection over order statistics: one device call, no Count query per step.  A rank >= total (float rounding
+        can make desiredLess reach it) or < 0 names a branch that is never taken."""
+        wanted = {0, total - 1}
+        i_less, i_greater = want_less, total - 1 - want_greater
+        for r in (i_less, i_greater):
+            if 0 <= r < total:
+                wanted.add(r)
+        ranks = sorted(wanted)
+        filt_ops = self._bitmap_call(idx, filt) if filt is not None else None
+        vals, cnts, _ = self.ctx.bsi_select(idx.id, f.id, VIEW_BSI, min(f.bit_depth, 63), shards, ranks, filter_ops=filt_ops)
+        at = {r: (int(v) + f.base, int(n)) for r, v, n in zip(ranks, vals.tolist(), cnts.tolist())}
+        mn = ValCount()
+        if want_greater != 0:
+            mn = ValCount(*at[0])                                       # Min under the filter, with its multiplicity
+            if want_less == 0:
+                return mn
+        mx = ValCount(*at[total - 1])
+        if want_greater == 0:
+            return mx
+        v_less = at[i_less][0] if i_less < total else None
+        v_greater = at[i_greater][0] if i_greater >= 0 else None
+        lo, hi, guess = mn.val, mx.val, mn.val
+        while lo < hi:
+            guess = self._midpoint(lo, hi)
+            if v_less is not None and v_less < guess:                   # Count(f < guess) > desiredLess
+                hi = guess - 1
+                continue
+            if v_greater is not None and v_greater > guess:             # Count(f > guess) > desiredGreater
+                lo = guess + 1
+                continue
+            break
+        return ValCount(guess, 1)
+
+    def _percentile_bisect(self, idx, f, filt, shards, want_less, want_greater):
+        """the reference's flow: Min, Max, then two Count(Row(f < x) [∩ filter]) style queries per bisection step, every one a
+        whole-batch device query, exactly as every step is a cluster-wide query in the reference"""
+        name = f.name
+
+        def count_of(row_call):
+            inner = row_call if filt is None else pql.Call("Intersect", {}, [row_call, filt])
+            return self._count(idx, pql.Call("Count", {}, [inner]), shards)
         kids = [filt] if filt is not None else []
         mn = ValCount()
         if want_greater != 0:
@@ -895,10 +956,8 @@ class Executor:
         if want_greater == 0:
             return mx
         lo, hi, guess = mn.val, mx.val, mn.val
-        tdiv = lambda a, b: int(a / b) if abs(a) < (1 << 52) else (abs(a) // b) * (1 if a >= 0 else -1)      # Go's truncating division
-        tmod = lambda a, b: a - b * tdiv(a, b)                                                                  # Go's %: sign of the dividend
         while lo < hi:
-            guess = tdiv(lo, 2) + tdiv(hi, 2) + tdiv(tmod(lo, 2) + tmod(hi, 2), 2)       # overflow-free midpoint (:1493-1497)
+            guess = self._midpoint(lo, hi)
             if count_of(pql.Call("Row", {name: pql.Condition("<", guess)})) > want_less:
                 hi = guess - 1
                 continue

@@ -13,6 +13,7 @@ OP_ROW, OP_INTERSECT, OP_UNION, OP_DIFFERENCE, OP_XOR, OP_NOT, OP_BSI_RANGE, OP_
 CMP = {"==": 1, "!=": 2, "<": 3, "<=": 4, ">": 5, ">=": 6, "><": 7}
 E_INVALID, E_QUERY, E_FORMAT, E_NOSPACE, E_CUDA, E_NOMEM, E_COMM = -1, -2, -3, -4, -5, -6, -7
 DEVICE_NONE = -1            # fbgpu_init(FBGPU_DEVICE_NONE): inspection-only context (no device, no queries)
+SELECT_MAX_RANKS = 8        # FBGPU_SELECT_MAX_RANKS: ranks per fbgpu_bsi_select call
 
 
 _row_tls = threading.local()
@@ -43,7 +44,7 @@ class Counters(C.Structure):
 EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_version", "fbgpu_load_fragment",
            "fbgpu_load_fragments", "fbgpu_drop_fragment", "fbgpu_commit", "fbgpu_get_stats", "fbgpu_count", "fbgpu_row",
            "fbgpu_row_counts", "fbgpu_row_counts_per_shard", "fbgpu_groupby", "fbgpu_comm_unique_id", "fbgpu_comm_init", "fbgpu_comm_destroy",
-           "fbgpu_get_counters", "fbgpu_stream", "fbgpu_rows_payload_bytes", "fbgpu_count_pairs", "fbgpu_columns", "fbgpu_extract", "fbgpu_load_rbf", "fbgpu_load_rbf_dir", "fbgpu_bsi_minmax", "fbgpu_bsi_sum", "fbgpu_compact", "fbgpu_comm_p2p_handle", "fbgpu_comm_p2p_open", "fbgpu_comm_p2p_disable",
+           "fbgpu_get_counters", "fbgpu_stream", "fbgpu_rows_payload_bytes", "fbgpu_count_pairs", "fbgpu_columns", "fbgpu_extract", "fbgpu_load_rbf", "fbgpu_load_rbf_dir", "fbgpu_bsi_minmax", "fbgpu_bsi_sum", "fbgpu_bsi_select", "fbgpu_compact", "fbgpu_comm_p2p_handle", "fbgpu_comm_p2p_open", "fbgpu_comm_p2p_disable",
            "fbgpu_any", "fbgpu_pair_types", "fbgpu_node_any", "fbgpu_apply_containers", "fbgpu_node_apply_containers",
            "fbgpu_comm_p2p_open_local", "fbgpu_node_init", "fbgpu_node_shutdown", "fbgpu_node_devices", "fbgpu_node_owner", "fbgpu_node_ctx", "fbgpu_node_load_fragment",
            "fbgpu_node_load_fragments", "fbgpu_node_load_rbf_dir", "fbgpu_node_drop_fragment", "fbgpu_node_commit", "fbgpu_node_get_stats", "fbgpu_node_count", "fbgpu_node_row",
@@ -88,6 +89,8 @@ def load():
     L.fbgpu_bsi_minmax.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, i32, C.POINTER(C.c_int64), C.POINTER(u64)]
     L.fbgpu_bsi_minmax.restype = C.c_int
     L.fbgpu_bsi_sum.argtypes, L.fbgpu_bsi_sum.restype = [vp, u32, vp, i32, u32, u32, i32, vp, i64, C.POINTER(C.c_int64), C.POINTER(u64)], C.c_int
+    L.fbgpu_bsi_select.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, vp, i32, vp, vp, C.POINTER(u64)]
+    L.fbgpu_bsi_select.restype = C.c_int
     L.fbgpu_row_counts.argtypes, L.fbgpu_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp, vp, i32, C.POINTER(i32)], C.c_int
     L.fbgpu_row_counts_per_shard.argtypes, L.fbgpu_row_counts_per_shard.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_groupby.argtypes, L.fbgpu_groupby.restype = [vp, u32, vp, vp, i32, vp, vp, vp, i32, vp, i64, vp], C.c_int
@@ -341,6 +344,17 @@ class Context:
                                          C.byref(tot), C.byref(cnt)))
         return tot.value, cnt.value
 
+    def bsi_select(self, index, field, view, bit_depth, shards, ranks, filter_ops=None):
+        """order statistics over <filter> ∩ not-null: (vals, counts, total) — vals[i] = the stored value (value - Base) at
+        0-based position ranks[i] of the ascending sorted values, counts[i] = how many columns hold it, total = number of
+        columns with a value under the filter.  A rank >= total raises FbgpuError(E_INVALID)."""
+        sh, rk = _u64arr(shards), _u64arr(ranks)
+        arr = ops_array(filter_ops) if filter_ops else None
+        vals, cnts, total = np.zeros(max(len(rk), 1), dtype=np.int64), np.zeros(max(len(rk), 1), dtype=np.uint64), C.c_uint64(0)
+        self._check(self.L.fbgpu_bsi_select(self.h, index, arr, len(filter_ops) if filter_ops else 0, field, view, int(bit_depth), sh.ctypes.data, len(sh),
+                                            rk.ctypes.data, len(rk), vals.ctypes.data, cnts.ctypes.data, C.byref(total)))
+        return vals[: len(rk)], cnts[: len(rk)], total.value
+
     def row_counts(self, index, field, view, shards, row_ids=None, filter_ops=None, cap=1 << 20):
         sh = _u64arr(shards)
         f = ops_array(filter_ops) if filter_ops else None
@@ -469,6 +483,9 @@ class Node(Context):
         per = [self.device_counters(i) for i in range(self.n_devices)]
         return {"kernel_launches": sum(p["kernel_launches"] for p in per), "queries": sum(p["queries"] for p in per),
                 "last_query_gpu_ms": max(p["last_query_gpu_ms"] for p in per)}
+
+    def bsi_select(self, index, field, view, bit_depth, shards, ranks, filter_ops=None):
+        raise NotImplementedError("fbgpu_bsi_select has no node form: order statistics of the devices' shares do not merge")
 
     def row_counts(self, index, field, view, shards, row_ids=None, filter_ops=None, cap=1 << 20):
         if row_ids is None:

@@ -195,6 +195,21 @@ int fbgpu_bsi_minmax(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_
 int fbgpu_bsi_sum(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                   const uint64_t *shards, int64_t n_shards, int64_t *out_sum, uint64_t *out_count);
 
+/* Order statistics of an int field over a row: the row is <filter program> ∩ not-null(field) (n_ops == 0: every column with a
+ * value).  Sort the stored values (value - bsiGroup.Base, sign-magnitude planes as fbgpu_extract reads them) of its columns
+ * ascending, keeping duplicates.  out_vals[i] = the value at 0-based position ranks[i], and out_counts[i] = how many columns hold
+ * that value (may be NULL).  *out_total = |row|.  ranks need not be sorted or distinct; n_ranks == 0 only reports the total
+ * (out_vals may then be NULL).  At most FBGPU_SELECT_MAX_RANKS ranks per call.  A rank >= *out_total is FBGPU_E_INVALID
+ * (*out_total is still set).  One evaluation of the row, then an MSB-first radix select over the bit planes chained on the
+ * device (every plane container read at most twice) and one D2H copy.  Device memory held by the call: 8 KiB per (shard, slot)
+ * unit per distinct rank (at least one).  Local to this context: a context with a communicator attached returns FBGPU_E_COMM,
+ * because per-rank order statistics do not merge.  Percentile (executePercentile :1310-1600) needs the ranks 0, T-1,
+ * desiredLess and T-1-desiredGreater: its bisection then runs on the host over these values without further queries. */
+#define FBGPU_SELECT_MAX_RANKS 8
+int fbgpu_bsi_select(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view,
+                     int32_t bit_depth, const uint64_t *shards, int64_t n_shards, const uint64_t *ranks, int32_t n_ranks,
+                     int64_t *out_vals, uint64_t *out_counts, uint64_t *out_total);
+
 /* Per-row counts of one field, optionally intersected with a filter program: the exact part of TopN
  * (fragment.top with explicit ids, fragment.go:1317-1437) and TopK (doTopK executor.go:2705-2746).
  * row_ids != NULL: counts for exactly those rows (out_counts[i] for row_ids[i]).
