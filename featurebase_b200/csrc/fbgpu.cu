@@ -1235,7 +1235,8 @@ static int columns_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32
             seen += N;
         }
         if (batch_out && written + batch_out <= cap) {
-            const size_t ub = units.size() * sizeof(ColUnit), ob = batch_out * 8 * (want_vals ? 2 : 1);
+            // d_emit: columns [batch_out] u64, then for Extract magnitudes [batch_out] u64 and sign bits [ceil(batch_out / 32)] u32
+            const size_t ub = units.size() * sizeof(ColUnit), vb = want_vals ? batch_out * 8 + ((batch_out + 31) / 32) * 4 : 0, ob = batch_out * 8 + vb;
             if (w->d_emit_units.ensure(ub) || w->d_emit.ensure(ob) || w->h_in.ensure(std::max<size_t>(ub, ob))) return FBGPU_E_NOMEM;
             memcpy(w->h_in.p, units.data(), ub);
             CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, w->h_in.p, ub, cudaMemcpyHostToDevice, w->stream));
@@ -1244,8 +1245,9 @@ static int columns_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32
             columns_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>((const uint4*)w->d_bitmaps.p, (const ColUnit*)w->d_emit_units.p, (int)units.size(), d_cols);
             CUDA_TRY(cudaGetLastError()); launches++;
             if (want_vals) {
-                CUDA_TRY(cudaMemsetAsync(d_vals, 0, batch_out * 8, w->stream));
-                extract_values_kernel<<<grid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv_vals, depth_vals, (const uint4*)w->d_bitmaps.p, (const ColUnit*)w->d_emit_units.p, (int)units.size(), d_vals);
+                CUDA_TRY(cudaMemsetAsync(d_vals, 0, vb, w->stream));
+                extract_values_kernel<<<grid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv_vals, depth_vals, (const uint4*)w->d_bitmaps.p, (const ColUnit*)w->d_emit_units.p, (int)units.size(),
+                                                                               d_vals, (unsigned int*)(d_vals + batch_out));
                 CUDA_TRY(cudaGetLastError()); launches++;
             }
             CUDA_TRY(cudaStreamSynchronize(w->stream));   // h_in is reused as the D2H landing buffer below
@@ -1253,9 +1255,10 @@ static int columns_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32
             CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
             CUDA_TRY(cudaStreamSynchronize(w->stream));
             memcpy(out_cols + written, w->h_in.p, batch_out * 8);
-            if (want_vals) {                               // sign-magnitude (bit 63 = sign row) -> int64
-                const uint64_t* raw = (const uint64_t*)w->h_in.p + batch_out;
-                for (uint64_t i = 0; i < batch_out; i++) { const int64_t m = (int64_t)(raw[i] & ~(1ull << 63)); out_vals[written + i] = (raw[i] >> 63) ? -m : m; }
+            if (want_vals) {                               // sign-magnitude -> int64, wrapping like fragment.value: sign + 2^63 is INT64_MIN
+                const uint64_t* mag = (const uint64_t*)w->h_in.p + batch_out;
+                const uint32_t* sgn = (const uint32_t*)(mag + batch_out);
+                for (uint64_t i = 0; i < batch_out; i++) out_vals[written + i] = (int64_t)(((sgn[i >> 5] >> (i & 31)) & 1u) ? 0ull - mag[i] : mag[i]);
             }
             float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1); ms_total += ms;
         }
@@ -1282,7 +1285,7 @@ extern "C" int fbgpu_extract(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, 
                              const uint64_t* shards, int64_t n_shards, uint64_t offset, int64_t limit,
                              uint64_t* out_cols, int64_t* out_vals, uint64_t cap, uint64_t* out_n, uint64_t* out_total) try {
     if (!c || !out_n || n_shards < 0 || (n_shards && !shards) || (cap && (!out_cols || !out_vals)) || n_ops < 0 || (n_ops && !ops)) return fail(FBGPU_E_INVALID, "null argument");
-    if (bit_depth < 0 || bit_depth > 63) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..63", bit_depth);
+    if (bit_depth < 0 || bit_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", bit_depth);
     USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
     int rc = lock_committed(c, lk); if (rc) return rc;
@@ -1299,7 +1302,7 @@ extern "C" int fbgpu_extract(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, 
 extern "C" int fbgpu_bsi_minmax(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                                 const uint64_t* shards, int64_t n_shards, int32_t want_max, int64_t* out_val, uint64_t* out_count) try {
     if (!c || !out_val || !out_count || n_shards < 0 || (n_shards && !shards) || n_ops < 0 || (n_ops && !ops)) return fail(FBGPU_E_INVALID, "null argument");
-    if (bit_depth < 0 || bit_depth > 63) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..63", bit_depth);
+    if (bit_depth < 0 || bit_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", bit_depth);
     USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
     int rc = lock_committed(c, lk); if (rc) return rc;
@@ -1345,7 +1348,7 @@ extern "C" int fbgpu_bsi_minmax(fbgpu_ctx* c, uint32_t index, const fbgpu_op* op
 extern "C" int fbgpu_bsi_sum(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                              const uint64_t* shards, int64_t n_shards, int64_t* out_sum, uint64_t* out_count) try {
     if (!c || !out_sum || !out_count || n_shards < 0 || (n_shards && !shards) || n_ops < 0 || (n_ops && !ops)) return fail(FBGPU_E_INVALID, "null argument");
-    if (bit_depth < 0 || bit_depth > 63) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..63", bit_depth);
+    if (bit_depth < 0 || bit_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", bit_depth);
     USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
     int rc = lock_committed(c, lk); if (rc) return rc;
@@ -1398,7 +1401,7 @@ extern "C" int fbgpu_bsi_select(fbgpu_ctx* c, uint32_t index, const fbgpu_op* op
                                 int64_t* out_vals, uint64_t* out_counts, uint64_t* out_total) try {
     if (!c || !out_total || n_shards < 0 || (n_shards && !shards) || n_ops < 0 || (n_ops && !ops) || n_ranks < 0 || (n_ranks && (!ranks || !out_vals)))
         return fail(FBGPU_E_INVALID, "null argument");
-    if (bit_depth < 0 || bit_depth > 63) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..63", bit_depth);
+    if (bit_depth < 0 || bit_depth > 63) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..63", bit_depth);     // the sort key takes depth + 1 bits
     if (n_ranks > FBGPU_SELECT_MAX_RANKS) return fail(FBGPU_E_INVALID, "%d ranks: at most %d per call", n_ranks, FBGPU_SELECT_MAX_RANKS);
     if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_bsi_select is local to one context: order statistics of the ranks' shares do not merge");
     USE_DEVICE(c);

@@ -1092,12 +1092,13 @@ columns_emit_kernel(const uint4* __restrict__ bitmaps, const ColUnit* __restrict
 // executeDistinctShardBSI :2034 transpose column by column): one CTA per non-empty unit.  The unit's base bitmap
 // (filter ∩ exists, produced by eval_kernel) is staged in shared memory with a per-word rank table; warp w then walks the
 // planes w, w+8, ... — sign row 1 and magnitude rows 2..depth+1 of the BSI view — each container read once, in its own
-// encoding, and every base column found in plane b gets bit b (sign: bit 63) or-ed into its output slot
-// out[out_off + rank - first].  Ranks match columns_emit_kernel, so the two outputs line up.
+// encoding, and every base column found in magnitude plane b gets bit b or-ed into its output slot i = out_off + rank - first,
+// a column found in the sign row gets bit i of the `sign` bit array.  The sign is kept apart because a depth-64 magnitude
+// fills all 64 bits (INT64_MIN is stored as sign + 2^63).  Ranks match columns_emit_kernel, so the outputs line up.
 constexpr int kExtractThreads = 256;
 __global__ void __launch_bounds__(kExtractThreads)
 extract_values_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restrict__ bitmaps, const ColUnit* __restrict__ units, int n_units,
-                      unsigned long long* __restrict__ out) {
+                      unsigned long long* __restrict__ out, unsigned int* __restrict__ sign) {
     __shared__ __align__(16) uint64_t base[1024];
     __shared__ uint32_t rank0[1024];            // number of base bits before word i
     __shared__ uint32_t wsum[kExtractThreads / 32];
@@ -1120,12 +1121,15 @@ extract_values_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restri
         for (int k = 0; k < 4; k++) { rank0[4 * tid + k] = r; r += __popcll(w[k]); }
         __syncthreads();
         const uint64_t shard = u.col_base >> 20; const int slot = (int)((u.col_base >> 16) & 15);
-        // or `flag` into the slot of base column v (a column outside the base or outside the window is skipped)
-        auto hit = [&](uint32_t v, unsigned long long flag) {
+        // plane pl of base column v into its slot (a column outside the base or outside the window is skipped)
+        auto hit = [&](uint32_t v, int pl) {
             const uint64_t bw = base[v >> 6];
             if (!((bw >> (v & 63)) & 1ull)) return;
             const uint32_t rk = rank0[v >> 6] + __popcll(bw & ((1ull << (v & 63)) - 1ull));
-            if (rk >= u.first && rk < u.last) atomicOr(&out[u.out_off + (rk - u.first)], flag);
+            if (rk < u.first || rk >= u.last) return;
+            const uint64_t i = u.out_off + (rk - u.first);
+            if (pl == 0) atomicOr(&sign[i >> 5], 1u << (i & 31));
+            else atomicOr(&out[i], 1ull << (pl - 1));
         };
         for (int pl = wid; pl < depth + 1; pl += nwarps) {                 // pl 0: sign row 1; pl 1..depth: value rows 2..depth+1
             Resolved rc; rc.ptr = nullptr; rc.card = 0; rc.typ = 0; rc.cnt = 0;
@@ -1134,16 +1138,15 @@ extract_values_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restri
             const uint32_t card = __shfl_sync(0xffffffffu, rc.card, 0);
             const uint32_t meta = __shfl_sync(0xffffffffu, ((uint32_t)rc.typ << 16) | rc.cnt, 0);
             if (ptr == nullptr) continue;
-            const unsigned long long flag = pl == 0 ? (1ull << 63) : (1ull << (pl - 1));
             const uint32_t typ = meta >> 16, cnt = meta & 0xffffu;
             if (typ == kArray) {
                 const uint16_t* a = reinterpret_cast<const uint16_t*>(ptr);
-                for (uint32_t i = lane; i < card; i += 32) hit((uint32_t)__ldg(a + i), flag);
+                for (uint32_t i = lane; i < card; i += 32) hit((uint32_t)__ldg(a + i), pl);
             } else if (typ == kBitmap) {
                 const uint64_t* g = reinterpret_cast<const uint64_t*>(ptr);
                 for (int i = lane; i < 1024; i += 32) {
                     uint64_t v = __ldg(g + i) & base[i];
-                    while (v) { const int bit = __ffsll((long long)v) - 1; hit((uint32_t)(i * 64 + bit), flag); v &= v - 1; }
+                    while (v) { const int bit = __ffsll((long long)v) - 1; hit((uint32_t)(i * 64 + bit), pl); v &= v - 1; }
                 }
             } else {
                 const uint32_t* r32 = reinterpret_cast<const uint32_t*>(ptr);
@@ -1154,7 +1157,7 @@ extract_values_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restri
                         if (i == (s0 >> 6)) m &= ~0ull << (s0 & 63);
                         if (i == (l0 >> 6)) m &= ~0ull >> (63 - (l0 & 63));
                         uint64_t v = base[i] & m;
-                        while (v) { const int bit = __ffsll((long long)v) - 1; hit(i * 64 + (uint32_t)bit, flag); v &= v - 1; }
+                        while (v) { const int bit = __ffsll((long long)v) - 1; hit(i * 64 + (uint32_t)bit, pl); v &= v - 1; }
                     }
                 }
             }
@@ -1248,7 +1251,7 @@ bsi_minmax_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restrict__
         if (tid == 0) {
             uint32_t n = 0;
             for (int k = 0; k < kEvalThreads / 32; k++) n += warp_tmp[k];
-            out[unit].val = use_neg ? -(long long)mag : (long long)mag;
+            out[unit].val = (long long)(use_neg ? 0ull - mag : mag);          // mag = 2^63 (INT64_MIN at depth 64) wraps, no overflow
             out[unit].cnt = n;
         }
     }

@@ -319,7 +319,7 @@ class Executor:
                     raise QueryError(f"field {name} is not an int field")
                 col = int(c.args["column"])
                 ef, erow = self.holder.embed_row(idx.name, [col])
-                _, vals, n = self.ctx.extract(idx.id, f.id, VIEW_BSI, min(f.bit_depth, 63), [col // SHARD_WIDTH],
+                _, vals, n = self.ctx.extract(idx.id, f.id, VIEW_BSI, f.bit_depth, [col // SHARD_WIDTH],
                                               filter_ops=[L.Op(L.OP_ROW, ef.id, VIEW_STANDARD, 0, erow, 0, 0, 0)])
                 return ValCount(int(vals[0]) + f.base, 1) if n else ValCount()
             if c.name == "Options":                              # executeOptionsCall :869: shards=[..] narrows the shard list of the child call
@@ -683,7 +683,7 @@ class Executor:
         if f.type != "int":
             return ValCount()                                           # bsig == nil (:2187-2190)
         filt = self._bitmap_call(idx, c.children[0]) if c.children else None
-        total, count = self.ctx.bsi_sum(idx.id, f.id, VIEW_BSI, min(f.bit_depth, 63), shards, filter_ops=filt)
+        total, count = self.ctx.bsi_sum(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, filter_ops=filt)
         if count == 0:
             return ValCount()                                           # executeSum :1147-1149
         return ValCount(_i64(total + count * f.base), count)
@@ -701,7 +701,7 @@ class Executor:
         if f.type != "int":
             raise QueryError("bsigroup not found")                      # ErrBSIGroupNotFound field.go:1571
         filt = self._bitmap_call(idx, c.children[0]) if c.children else None
-        v, n = self.ctx.bsi_minmax(idx.id, f.id, VIEW_BSI, min(f.bit_depth, 63), shards, what == "Max", filter_ops=filt)
+        v, n = self.ctx.bsi_minmax(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, what == "Max", filter_ops=filt)
         if n == 0:
             return ValCount()                                           # :1252-1254
         return ValCount(v + f.base, n)                                  # valCountize field.go:1640
@@ -757,7 +757,7 @@ class Executor:
         if f.type != "int":
             rid, cnt = self.ctx.row_counts(idx.id, f.id, VIEW_STANDARD, shards, filter_ops=filt)
             return sorted(int(r) for r, n in zip(rid, cnt) if n > 0)
-        _, vals, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, min(f.bit_depth, 63), shards, filter_ops=filt)
+        _, vals, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, filter_ops=filt)
         pos, neg = set(), set()
         for m in np.unique(vals).tolist():
             v = int(m) + f.base                                        # value += offset (:2125)
@@ -805,7 +805,7 @@ class Executor:
         for k, f in enumerate(fields):
             if f.type == "int":
                 types.append("int64")
-                vc, vv, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, min(f.bit_depth, 63), shards, filter_ops=filt)
+                vc, vv, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, filter_ops=filt)
                 for col, v in zip(vc.tolist(), vv.tolist()):
                     if col in pos:
                         table[pos[col]][k] = int(v) + f.base
@@ -841,7 +841,7 @@ class Executor:
         desc = bool(c.args.get("sort-desc", False))
         filt = self._bitmap_call(idx, c.children[0])
         if f.type == "int":
-            cols, vals, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, min(f.bit_depth, 63), shards, filter_ops=filt)
+            cols, vals, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, filter_ops=filt)
             kvs = [(int(col), int(v) + f.base) for col, v in zip(cols.tolist(), vals.tolist())]
         elif f.type in ("bool", "mutex"):
             kvs = []
@@ -866,7 +866,7 @@ class Executor:
         [min, max], so with v[0..T-1] the sorted values: Count(f < g) > desiredLess exactly when v[desiredLess] < g, and
         Count(f > g) > desiredGreater exactly when v[T-1-desiredGreater] > g.  One fbgpu_bsi_select call for the ranks
         0, T-1, desiredLess, T-1-desiredGreater therefore fixes the answer bit for bit, and the bisection runs on the host.
-        Contexts without the call (a node handle, a context with a communicator) take the query-driven bisection.
+        Contexts without the call (a node handle, a context with a communicator) and depth-64 fields take the query-driven bisection.
         Returns None ("the median of nothing is NULL") or ValCount(value, 1) / the Min / Max ValCount at the ends."""
         nth = c.args.get("nth")
         if nth is None:
@@ -887,7 +887,7 @@ class Executor:
             return None
         want_less = int(total * nth / 100.0)
         want_greater = int(total * (100 - nth) / 100.0)
-        if self.percentile_select and f.type == "int" and hasattr(self.ctx, "bsi_select"):
+        if self.percentile_select and f.type == "int" and f.bit_depth <= 63 and hasattr(self.ctx, "bsi_select"):      # select keys take depth + 1 bits
             try:
                 return self._percentile_select(idx, f, filt, shards, total, want_less, want_greater)
             except NotImplementedError:
@@ -914,7 +914,7 @@ class Executor:
                 wanted.add(r)
         ranks = sorted(wanted)
         filt_ops = self._bitmap_call(idx, filt) if filt is not None else None
-        vals, cnts, _ = self.ctx.bsi_select(idx.id, f.id, VIEW_BSI, min(f.bit_depth, 63), shards, ranks, filter_ops=filt_ops)
+        vals, cnts, _ = self.ctx.bsi_select(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, ranks, filter_ops=filt_ops)
         at = {r: (int(v) + f.base, int(n)) for r, v, n in zip(ranks, vals.tolist(), cnts.tolist())}
         mn = ValCount()
         if want_greater != 0:

@@ -310,7 +310,8 @@ class Context:
 
     def extract(self, index, field, view, bit_depth, shards, filter_ops=None, offset=0, limit=None):
         """(column ids, int64 values relative to the field's Base, number of columns with a value under the filter): the int
-        field's values for the columns of <filter> ∩ not-null, ascending by column, gathered from the bit planes on the device"""
+        field's values for the columns of <filter> ∩ not-null, ascending by column, gathered from the bit planes on the device.
+        bit_depth 0..64 (a field over [MinInt64, MaxInt64] has depth 64 and stores INT64_MIN as sign + magnitude 2^63)"""
         sh = _u64arr(shards)
         arr = ops_array(filter_ops) if filter_ops else None
         nf = len(filter_ops) if filter_ops else 0
@@ -327,7 +328,8 @@ class Context:
             return cols[: n.value].copy(), vals[: n.value].copy(), total.value
 
     def bsi_minmax(self, index, field, view, bit_depth, shards, want_max, filter_ops=None):
-        """(extreme stored value = value - Base, number of columns holding it) over <filter> ∩ not-null; count 0: empty row"""
+        """(extreme stored value = value - Base, number of columns holding it) over <filter> ∩ not-null; count 0: empty row.
+        bit_depth 0..64"""
         sh = _u64arr(shards)
         arr = ops_array(filter_ops) if filter_ops else None
         val, cnt = C.c_int64(0), C.c_uint64(0)
@@ -336,7 +338,7 @@ class Context:
         return val.value, cnt.value
 
     def bsi_sum(self, index, field, view, bit_depth, shards, filter_ops=None):
-        """(Σ stored values = Σ (value - Base) in wrapping int64, number of columns) over <filter> ∩ not-null"""
+        """(Σ stored values = Σ (value - Base) in wrapping int64, number of columns) over <filter> ∩ not-null; bit_depth 0..64"""
         sh = _u64arr(shards)
         arr = ops_array(filter_ops) if filter_ops else None
         tot, cnt = C.c_int64(0), C.c_uint64(0)
@@ -347,7 +349,8 @@ class Context:
     def bsi_select(self, index, field, view, bit_depth, shards, ranks, filter_ops=None):
         """order statistics over <filter> ∩ not-null: (vals, counts, total) — vals[i] = the stored value (value - Base) at
         0-based position ranks[i] of the ascending sorted values, counts[i] = how many columns hold it, total = number of
-        columns with a value under the filter.  A rank >= total raises FbgpuError(E_INVALID)."""
+        columns with a value under the filter.  A rank >= total raises FbgpuError(E_INVALID).  bit_depth 0..63: the sort key
+        takes depth + 1 bits."""
         sh, rk = _u64arr(shards), _u64arr(ranks)
         arr = ops_array(filter_ops) if filter_ops else None
         vals, cnts, total = np.zeros(max(len(rk), 1), dtype=np.int64), np.zeros(max(len(rk), 1), dtype=np.uint64), C.c_uint64(0)
@@ -443,15 +446,23 @@ class Context:
 
 
 class _NodeCalls:
-    """routes Context's `self.L.fbgpu_<call>` to `fbgpu_node_<call>` where the node has that call"""
+    """routes Context's `self.L.fbgpu_<call>` to `fbgpu_node_<call>` where the node has that call.  A context call without a
+    node form would read the node handle as a context, so calling it raises NotImplementedError; the calls that take no
+    handle pass through."""
+    NO_HANDLE = ("fbgpu_last_error", "fbgpu_abi_version", "fbgpu_comm_unique_id")
 
     def __init__(self, real):
         self._real = real
 
     def __getattr__(self, name):
-        if name.startswith("fbgpu_") and not name.startswith("fbgpu_node_") and hasattr(self._real, "fbgpu_node_" + name[6:]):
+        if not name.startswith("fbgpu_") or name.startswith("fbgpu_node_") or name in self.NO_HANDLE:
+            return getattr(self._real, name)
+        if hasattr(self._real, "fbgpu_node_" + name[6:]):
             return getattr(self._real, "fbgpu_node_" + name[6:])
-        return getattr(self._real, name)
+
+        def missing(*args, **kw):
+            raise NotImplementedError(f"{name} has no node form")
+        return missing
 
 
 class Node(Context):

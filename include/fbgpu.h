@@ -174,7 +174,8 @@ int fbgpu_columns(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n
  * <filter program> ∩ not-null(field) (n_ops == 0: every column that has a value); for its columns, in ascending order and
  * inside the offset / limit window, out_cols[i] receives the column id and out_vals[i] the stored sign-magnitude value as
  * an int64, i.e. value - bsiGroup.Base (the caller adds Base, field.go:1640).  `view` is the field's bsig_ view,
- * bit_depth <= 63 its current depth.  Same capacity contract as fbgpu_columns. */
+ * bit_depth (0..64) its current depth.  A field over [MinInt64, MaxInt64] has depth 64: INT64_MIN is stored as the sign
+ * row plus magnitude 2^63, and -magnitude wraps to INT64_MIN as in fragment.value.  Same capacity contract as fbgpu_columns. */
 int fbgpu_extract(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                   const uint64_t *shards, int64_t n_shards, uint64_t offset, int64_t limit,
                   uint64_t *out_cols, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
@@ -182,7 +183,7 @@ int fbgpu_extract(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n
 /* Min / Max of an int field over a row (executeMin :1225 / executeMax :1261, fragment.min / max fragment.go:752-838): the row
  * is <filter program> ∩ not-null(field) (n_ops == 0: every column with a value).  *out_val receives the extreme stored
  * value, i.e. value - bsiGroup.Base (the caller adds Base), *out_count how many columns hold it — the reference's ValCount;
- * *out_count == 0 when the row is empty.  One evaluation of the row plus one pass over the bit planes, every plane container
+ * *out_count == 0 when the row is empty.  bit_depth 0..64, as for fbgpu_extract.  One evaluation of the row plus one pass over the bit planes, every plane container
  * read once (the composition from fbgpu_count calls re-reads the planes it has kept).  Not reduced over the communicator:
  * the caller merges per-node ValCounts as it does today (ValCount.Smaller / Larger executor.go:8446-8560). */
 int fbgpu_bsi_minmax(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
@@ -190,7 +191,7 @@ int fbgpu_bsi_minmax(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_
 
 /* Sum of an int field over a row (executeSum :1119, fragment.sum fragment.go:722-750): *out_count = |<filter> ∩ not-null|,
  * *out_sum = Σ (stored value) over those columns in wrapping int64 arithmetic, i.e. Σ (value - Base); the caller adds
- * count * Base (executeSumCountShard :2203-2206).  One evaluation of the row, one pass over the planes.  Per-node result,
+ * count * Base (executeSumCountShard :2203-2206).  bit_depth 0..64.  One evaluation of the row, one pass over the planes.  Per-node result,
  * like fbgpu_bsi_minmax (ValCount.Add merges nodes). */
 int fbgpu_bsi_sum(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                   const uint64_t *shards, int64_t n_shards, int64_t *out_sum, uint64_t *out_count);
@@ -204,7 +205,8 @@ int fbgpu_bsi_sum(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n
  * device (every plane container read at most twice) and one D2H copy.  Device memory held by the call: 8 KiB per (shard, slot)
  * unit per distinct rank (at least one).  Local to this context: a context with a communicator attached returns FBGPU_E_COMM,
  * because per-rank order statistics do not merge.  Percentile (executePercentile :1310-1600) needs the ranks 0, T-1,
- * desiredLess and T-1-desiredGreater: its bisection then runs on the host over these values without further queries. */
+ * desiredLess and T-1-desiredGreater: its bisection then runs on the host over these values without further queries.
+ * bit_depth 0..63: the sort key takes depth + 1 bits (a depth-64 field takes Percentile's query-driven bisection). */
 #define FBGPU_SELECT_MAX_RANKS 8
 int fbgpu_bsi_select(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view,
                      int32_t bit_depth, const uint64_t *shards, int64_t n_shards, const uint64_t *ranks, int32_t n_ranks,

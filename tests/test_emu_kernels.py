@@ -110,7 +110,8 @@ def test_results_do_not_depend_on_thread_order(order):
 def test_interpreted_library_under_sanitizers(san):
     """kernels and host code compiled with -fsanitize=undefined (shifts, signed overflow, misaligned vector accesses abort)
     or -fsanitize=address (out-of-bounds on `__shared__` statics — plain red-zoned globals in that build —, on host
-    vectors and on thread stacks): the parity tests, the sorted order, the GroupBy tests, the threaded API test"""
+    vectors and on thread stacks): the parity tests, the sorted order, the GroupBy tests, the threaded API test, the int64-range
+    value tests (a negation of magnitude 2^63 in int64 would abort the UBSan build)"""
     if not FULL:
         pytest.skip("sanitizer builds: FBGPU_EMU_FULL=1")
     flags = ("-O1", "-g", "-fsanitize=undefined", "-fno-sanitize-recover=undefined") if san == "undefined" else ("-O1", "-g", "-fsanitize=address")
@@ -121,8 +122,8 @@ def test_interpreted_library_under_sanitizers(san):
     base.pop("FBGPU_EMU_FULL", None)
     for extra, sel in (({}, SLOW + " and not sorted_order"),
                        ({"FBGPU_ARRAY_SORTED": "1", "FBGPU_TEST_EXPERIMENTAL": "1"}, "(sorted_order or groupby or density_sweep) and " + SLOW)):
-        r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-m", "gpu", "-p", "no:cacheprovider", "tests/test_gpu_parity.py", "tests/test_zz_gpu_experimental.py", "-k", sel],
-                           cwd=ROOT, env=dict(base, **extra), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=3000)
+        r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-m", "gpu", "-p", "no:cacheprovider", "tests/test_gpu_parity.py", "tests/test_zz_gpu_experimental.py",
+                            "tests/test_bsi_wide_values.py", "-k", sel], cwd=ROOT, env=dict(base, **extra), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=3000)
         assert r.returncode == 0 and " passed" in r.stdout, r.stdout[-3000:]
 
 

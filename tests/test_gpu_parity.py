@@ -224,7 +224,7 @@ def test_bsi_range_goldens_on_gpu():
     """fragment_internal_test.go:606-916 literal cases through Row(v <op> k)"""
     for values, depth, checks in V.BSI_RANGE_CASES:
         if depth == 64:
-            continue  # covered at the C-ABI level below (host mirror uses Python ints for min/max)
+            continue  # covered at the C-ABI level by tests/test_bsi_wide_values.py::test_between_common_bits_regression_depth_64
         p = _bsi_pair(values, depth)
         for op, pred, exp in checks:
             q = f"Row(v >< [{pred[0]},{pred[1]}])" if op == "><" else f"Row(v {op} {pred})"
