@@ -898,15 +898,20 @@ extern "C" int fbgpu_compact(fbgpu_ctx* c) try {
 } FBGPU_CATCH
 // Takes the store's shared lock for a query with the device tables in sync with the host mirrors: the "is anything
 // pending" check and the query run under the SAME lock acquisition, so a load that slips in between a commit and the
-// query cannot leave the query reading host mirrors that are newer than what is in HBM.
+// query cannot leave the query reading host mirrors that are newer than what is in HBM.  (After USE_DEVICE.)
 static int lock_committed(fbgpu_ctx* c, std::shared_lock<std::shared_mutex>& lk) {
-    if (c->inspect_only) return fail(FBGPU_E_CUDA, "this context was created with FBGPU_DEVICE_NONE: it holds no device and answers no query");
     for (;;) {
         lk = std::shared_lock<std::shared_mutex>(c->store_mu);
         if (!c->meta_dirty && c->staging.empty()) return 0;
         lk.unlock();
         int rc = fbgpu_commit(c); if (rc) return rc;
     }
+}
+
+// the start of every query once its arguments are checked: refuses an inspection-only context, selects the device, locks the store
+static int begin_query(fbgpu_ctx* c, std::shared_lock<std::shared_mutex>& lk) {
+    USE_DEVICE(c);
+    return lock_committed(c, lk);
 }
 
 extern "C" int fbgpu_get_stats(fbgpu_ctx* c, fbgpu_stats* out) try {
@@ -999,25 +1004,99 @@ static int launch_eval(fbgpu_ctx* c, Workspace* w, const std::vector<DevOp>& pro
     return 0;
 }
 
-// the usual shard list is a contiguous range (a node's share, SURVEY §8e): kernels then compute the shard id instead of loading it
-static bool contiguous_shards(const uint64_t* shards, int64_t n) {
-    for (int64_t i = 1; i < n; i++) if (shards[i] != shards[0] + (uint64_t)i) return false;
-    return n > 0;
+// pair_count_kernel's shard arguments: the usual shard list is a contiguous range (a node's share, SURVEY §8e), for which the
+// kernel is given no list and computes each shard id from the first instead of loading it
+struct PairShards { const uint64_t* list; uint64_t first; };
+static PairShards pair_shards(const uint64_t* shards, int64_t n, const uint64_t* d_shards) {
+    for (int64_t i = 1; i < n; i++) if (shards[i] != shards[0] + (uint64_t)i) return { d_shards, shards[0] };
+    return { n > 0 ? nullptr : d_shards, n ? shards[0] : 0 };
 }
+
+static std::vector<uint64_t> sorted_unique(const uint64_t* v, int64_t n) {
+    std::vector<uint64_t> s(v, v + n);
+    std::sort(s.begin(), s.end());
+    s.erase(std::unique(s.begin(), s.end()), s.end());
+    return s;
+}
+
+// the program "<ops> ∩ Row(field, view, row)": the row alone when there are no ops
+static std::vector<fbgpu_op> and_row(const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, uint64_t row) {
+    std::vector<fbgpu_op> full(ops, ops + n_ops);
+    fbgpu_op r{}; r.opcode = FBGPU_OP_ROW; r.field = field; r.view = view; r.a = row;
+    full.push_back(r);
+    if (n_ops) { fbgpu_op in{}; in.opcode = FBGPU_OP_INTERSECT; in.argc = 2; full.push_back(in); }
+    return full;
+}
+
+// One query call on a leased workspace: the device program and its operand stack depth, the uploaded program and shard list,
+// and the call's kernel launches and GPU milliseconds, which finish() adds to the counters.
+struct Query {
+    fbgpu_ctx* c; WsLease lease; Workspace* w;
+    std::vector<DevOp> prog; int depth = 1;
+    const DevOp* d_prog = nullptr; const uint64_t* d_shards = nullptr;
+    long long n_units = 0;                   // (shard, slot) units of the shard list
+    uint64_t launches = 0; float ms = 0;
+    explicit Query(fbgpu_ctx* ctx) : c(ctx), lease(ctx), w(lease.w) {}
+
+    int open(uint32_t index, const fbgpu_op* ops, int32_t n_ops, const uint64_t* shards, int64_t n_shards) {
+        int rc = compile_program(c, index, ops, n_ops, prog, depth); if (rc) return rc;
+        return open(shards, n_shards);
+    }
+    int open(const uint64_t* shards, int64_t n_shards) {      // no program
+        n_units = (long long)n_shards * kSlotsPerRow;
+        return upload_inputs(w, prog, shards, n_shards, &d_prog, &d_shards);
+    }
+    // evaluates the program for units [u0, u0 + nu) into `bits` (w->d_bitmaps when null), with `info` also their {N, runs} into w->d_info
+    int eval(long long u0, long long nu, bool info = false, uint4* bits = nullptr) {
+        if (!bits) { if (w->d_bitmaps.ensure((size_t)nu * 8192)) return FBGPU_E_NOMEM; bits = (uint4*)w->d_bitmaps.p; }
+        if (info && w->d_info.ensure((size_t)nu * 8)) return FBGPU_E_NOMEM;
+        EvalOut eo{ nullptr, nullptr, bits, info ? (uint2*)w->d_info.p : nullptr, FuseReduce{} };
+        int rc = launch_eval(c, w, prog, d_prog, depth, d_shards + u0 / kSlotsPerRow, nu, eo); if (rc) return rc;
+        launches++;
+        return 0;
+    }
+    // Row / Columns: eval() with the units' {N, runs} read back into h_out; ev0 opens the batch's timed bracket
+    int eval_info(long long u0, long long nu, const uint2*& info) {
+        // (the buffers are grown before ev0: the bracket holds no allocation)
+        if (w->d_bitmaps.ensure((size_t)nu * 8192) || w->d_info.ensure((size_t)nu * 8) || w->h_out.ensure((size_t)nu * 8)) return FBGPU_E_NOMEM;
+        CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
+        int rc = eval(u0, nu, true); if (rc) return rc;
+        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_info.p, (size_t)nu * 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        info = (const uint2*)w->h_out.p;
+        return 0;
+    }
+    // Row / Columns: copies the unit list to d_emit_units, runs launch(d_units, units.size(), grid) (emit kernels that write d_emit) and
+    // reads `out_bytes` of d_emit back into h_in; ev1 closes the batch's timed bracket
+    template <class Unit, class Launch>
+    int emit(const std::vector<Unit>& units, size_t out_bytes, Launch launch) {
+        const size_t ub = units.size() * sizeof(Unit);
+        if (w->d_emit_units.ensure(ub) || w->d_emit.ensure(out_bytes) || w->h_in.ensure(std::max(ub, out_bytes))) return FBGPU_E_NOMEM;
+        memcpy(w->h_in.p, units.data(), ub);
+        CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, w->h_in.p, ub, cudaMemcpyHostToDevice, w->stream));
+        const int grid = (int)std::min<size_t>(units.size(), (size_t)c->sm_count * 8);
+        int rc = launch((const Unit*)w->d_emit_units.p, (int)units.size(), grid); if (rc) return rc;
+        CUDA_TRY(cudaStreamSynchronize(w->stream));   // h_in is reused as the D2H landing buffer below
+        CUDA_TRY(cudaMemcpyAsync(w->h_in.p, w->d_emit.p, out_bytes, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        add_elapsed();
+        return 0;
+    }
+    void add_elapsed() { float t = 0; cudaEventElapsedTime(&t, w->ev0, w->ev1); ms += t; }
+    void finish() { bump(c, launches, ms); lease.ok = true; }
+};
 
 // ------------------------------------------------------------------ Count
 // collective == false: this context's shards only — no cross-GPU merge (fbgpu_any's early exit must not desynchronise the ranks)
 static int count_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, const uint64_t* shards, int64_t n_shards,
                       uint64_t* out_total, uint64_t* out_per_shard, bool collective) {
     if (!c || !out_total || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "null argument");
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
-    std::vector<DevOp> prog; int depth = 1;
-    rc = compile_program(c, index, ops, n_ops, prog, depth); if (rc) return rc;
-    WsLease lease(c); Workspace* w = lease.w;
-    const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, prog, shards, n_shards, &d_prog, &d_shards); if (rc) return rc;
+    int rc = begin_query(c, lk); if (rc) return rc;
+    Query q(c); Workspace* w = q.w;
+    rc = q.open(index, ops, n_ops, shards, n_shards); if (rc) return rc;
+    const std::vector<DevOp>& prog = q.prog;
     // layout of d_counts: [total][per-shard counts ...][ticket][reduced result][error]
     const size_t nper = out_per_shard ? (size_t)n_shards : 0, nc = 1 + nper + 3;
     if (w->d_counts.ensure(nc * 8)) return FBGPU_E_NOMEM;
@@ -1025,7 +1104,7 @@ static int count_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t
     CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, nc * 8, w->stream));
     unsigned long long* d_total = (unsigned long long*)w->d_counts.p;
     unsigned long long* d_per = out_per_shard ? d_total + 1 : nullptr;
-    long long n_units = (long long)n_shards * kSlotsPerRow;
+    const long long n_units = q.n_units;
     // cross-GPU merge of the count: fused into the kernel over peer memory when the mailboxes are mapped, else NCCL
     std::unique_lock<std::mutex> coll_lk(c->coll_mu, std::defer_lock);
     FuseReduce fr{};
@@ -1047,12 +1126,13 @@ static int count_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t
         if (pa) {
             long long grid = std::min<long long>((n_units + kPcWarps - 1) / kPcWarps, (long long)c->sm_count * c->pair_ctas_per_sm);
             c->counters_pair_launches++;
+            const PairShards ps = pair_shards(shards, n_shards, q.d_shards);
             pair_count_kernel<<<(unsigned)grid, kPcWarps * 32, kPcWarps * 8192, w->stream>>>(store_ref(c), pa->fv, pa->row, pb->fv, pb->row, nullptr, nullptr, n_units,
-                contiguous_shards(shards, n_shards) ? nullptr : d_shards, n_shards ? shards[0] : 0, n_units, d_total, d_per, nullptr, fr);
+                ps.list, ps.first, n_units, d_total, d_per, nullptr, fr);
             CUDA_TRY(cudaGetLastError());
         } else {
             EvalOut eo{ d_total, d_per, nullptr, nullptr, fr };
-            rc = launch_eval(c, w, prog, d_prog, depth, d_shards, n_units, eo); if (rc) return rc;
+            rc = launch_eval(c, w, prog, q.d_prog, q.depth, q.d_shards, n_units, eo); if (rc) return rc;
         }
     } else if (p2p) {
         p2p_reduce_only_kernel<<<1, 1, 0, w->stream>>>(fr, d_total);
@@ -1063,15 +1143,15 @@ static int count_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t
     CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, nc * 8, cudaMemcpyDeviceToHost, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
     if (p2p && ((uint64_t*)w->h_out.p)[1 + nper + 2] != 0) {
-        lease.ok = true;                     // the stream is drained; the exchange state is not: the caller re-opens the peers
+        q.lease.ok = true;                   // the stream is drained; the exchange state is not: the caller re-opens the peers
         return fail(FBGPU_E_COMM, "rank %d did not publish its count for exchange %llu in time (peer dead, or the ranks issued their collective queries in different orders); re-open with fbgpu_comm_p2p_open",
                     (int)((uint64_t*)w->h_out.p)[1 + nper + 2] - 1, (unsigned long long)fr.epoch);
     }
     *out_total = p2p ? ((uint64_t*)w->h_out.p)[1 + nper + 1] : ((uint64_t*)w->h_out.p)[0];
     if (out_per_shard) memcpy(out_per_shard, (uint64_t*)w->h_out.p + 1, (size_t)n_shards * 8);
-    float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1);
-    bump(c, (n_units > 0 || p2p) ? 1 : 0, ms);
-    lease.ok = true;
+    q.add_elapsed();
+    q.launches = (n_units > 0 || p2p) ? 1 : 0;
+    q.finish();
     return FBGPU_OK;
 }
 extern "C" int fbgpu_count(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, const uint64_t* shards, int64_t n_shards,
@@ -1086,41 +1166,26 @@ static int fbgpu_count_local(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, 
 extern "C" int fbgpu_row(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, const uint64_t* shards, int64_t n_shards,
                          uint8_t* out_buf, uint64_t out_cap, uint64_t* out_len, uint64_t* out_count) try {
     if (!c || !out_len || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "null argument");
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
-    std::vector<DevOp> prog; int depth = 1;
-    rc = compile_program(c, index, ops, n_ops, prog, depth); if (rc) return rc;
+    int rc = begin_query(c, lk); if (rc) return rc;
+    Query q(c); Workspace* w = q.w;
     // Row.Merge concatenates disjoint shard segments (row.go:202); emit in ascending shard order
-    std::vector<uint64_t> sorted(shards, shards + n_shards);
-    std::sort(sorted.begin(), sorted.end());
-    sorted.erase(std::unique(sorted.begin(), sorted.end()), sorted.end());
-    n_shards = (int64_t)sorted.size();
-    WsLease lease(c); Workspace* w = lease.w;
-    const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, prog, sorted.data(), n_shards, &d_prog, &d_shards); if (rc) return rc;
-    long long n_units = (long long)n_shards * kSlotsPerRow;
+    const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);
+    rc = q.open(index, ops, n_ops, sorted.data(), (int64_t)sorted.size()); if (rc) return rc;
+    const long long n_units = q.n_units;
     struct OutCont { uint64_t key; uint16_t typ; uint32_t n; uint64_t size; uint32_t batch; uint64_t src_off; };
     std::vector<OutCont> conts; std::vector<std::vector<uint8_t>> batch_bufs;   // one host copy of the emitted payloads per batch
     // a single batch (<= 1024 shards, the usual call) needs no such copy: its payloads are assembled straight from the pinned
     // D2H landing buffer, which stays leased until this function returns
     const bool single_batch = n_units <= c->unit_batch;
     const uint8_t* single_src = nullptr;
-    uint64_t total_count = 0; uint64_t launches = 0; float ms_total = 0;
+    uint64_t total_count = 0;
     for (long long u0 = 0; u0 < n_units; u0 += c->unit_batch) {
-        long long nu = std::min(c->unit_batch, n_units - u0);
-        if (w->d_bitmaps.ensure((size_t)nu * 8192)) return FBGPU_E_NOMEM;
-        if (w->d_info.ensure((size_t)nu * 8)) return FBGPU_E_NOMEM;
-        if (w->h_out.ensure((size_t)nu * 8)) return FBGPU_E_NOMEM;
-        EvalOut eo{ nullptr, nullptr, (uint4*)w->d_bitmaps.p, (uint2*)w->d_info.p, FuseReduce{} };
-        CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
-        rc = launch_eval(c, w, prog, d_prog, depth, d_shards + u0 / kSlotsPerRow, nu, eo); if (rc) return rc;
-        launches++;
-        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_info.p, (size_t)nu * 8, cudaMemcpyDeviceToHost, w->stream));
-        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        const long long nu = std::min(c->unit_batch, n_units - u0);
+        const uint2* info;
+        rc = q.eval_info(u0, nu, info); if (rc) return rc;
         // optimize(): roaring.go:3412-3426
-        std::vector<EmitUnit> emits; uint64_t off = 0; size_t first = conts.size();
-        const uint2* info = (const uint2*)w->h_out.p;
+        std::vector<EmitUnit> emits; uint64_t off = 0;
         for (long long u = 0; u < nu; u++) {
             uint32_t N = info[u].x, runs = info[u].y;
             if (!N) continue;
@@ -1136,24 +1201,17 @@ extern "C" int fbgpu_row(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int3
         }
         if (emits.empty()) batch_bufs.emplace_back();
         if (!emits.empty()) {
-            if (w->d_emit_units.ensure(emits.size() * sizeof(EmitUnit))) return FBGPU_E_NOMEM;
-            if (w->d_emit.ensure(off)) return FBGPU_E_NOMEM;
-            if (w->h_in.ensure(std::max<size_t>(emits.size() * sizeof(EmitUnit), off))) return FBGPU_E_NOMEM;
-            memcpy(w->h_in.p, emits.data(), emits.size() * sizeof(EmitUnit));
-            CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, w->h_in.p, emits.size() * sizeof(EmitUnit), cudaMemcpyHostToDevice, w->stream));
-            int grid = (int)std::min<size_t>(emits.size(), (size_t)c->sm_count * 8);
-            canon_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>((const uint4*)w->d_bitmaps.p, (const EmitUnit*)w->d_emit_units.p, (int)emits.size(), (uint8_t*)w->d_emit.p);
-            CUDA_TRY(cudaGetLastError()); launches++;
-            CUDA_TRY(cudaStreamSynchronize(w->stream));   // h_in is reused as the D2H landing buffer below
-            CUDA_TRY(cudaMemcpyAsync(w->h_in.p, w->d_emit.p, off, cudaMemcpyDeviceToHost, w->stream));
-            CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
-            CUDA_TRY(cudaStreamSynchronize(w->stream));
+            rc = q.emit(emits, off, [&](const EmitUnit* d_units, int n, int grid) {
+                canon_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>((const uint4*)w->d_bitmaps.p, d_units, n, (uint8_t*)w->d_emit.p);
+                CUDA_TRY(cudaGetLastError()); q.launches++;
+                return 0;
+            });
+            if (rc) return rc;
             if (single_batch) { single_src = (const uint8_t*)w->h_in.p; batch_bufs.emplace_back(); }
             else batch_bufs.emplace_back((uint8_t*)w->h_in.p, (uint8_t*)w->h_in.p + off);
-            float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1); ms_total += ms;
         }
     }
-    bump(c, launches, ms_total);
+    bump(c, q.launches, q.ms);
     // writeToUnoptimized layout: roaring.go:1738-1817
     uint64_t need = 8 + conts.size() * 16;
     for (auto& oc : conts) need += oc.size;
@@ -1188,7 +1246,7 @@ extern "C" int fbgpu_row(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int3
         for (int t = 0; t < n_threads; t++) th.emplace_back(copy_range, conts.size() * t / n_threads, conts.size() * (t + 1) / n_threads);
         for (auto& t : th) t.join();
     }
-    lease.ok = true;
+    q.lease.ok = true;                       // (not before the size checks above: their error returns drain the stream)
     return FBGPU_OK;
 } FBGPU_CATCH
 
@@ -1198,28 +1256,16 @@ extern "C" int fbgpu_row(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int3
 static int columns_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, const uint64_t* shards, int64_t n_shards,
                         uint64_t offset, int64_t limit, bool want_vals, uint32_t fv_vals, int depth_vals,
                         uint64_t* out_cols, int64_t* out_vals, uint64_t cap, uint64_t* out_n, uint64_t* out_total) {
-    std::vector<DevOp> prog; int depth = 1;
-    int rc = compile_program(c, index, ops, n_ops, prog, depth); if (rc) return rc;
-    std::vector<uint64_t> sorted(shards, shards + n_shards);
-    std::sort(sorted.begin(), sorted.end());
-    sorted.erase(std::unique(sorted.begin(), sorted.end()), sorted.end());
-    n_shards = (int64_t)sorted.size();
-    WsLease lease(c); Workspace* w = lease.w;
-    const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, prog, sorted.data(), n_shards, &d_prog, &d_shards); if (rc) return rc;
-    const long long n_units = (long long)n_shards * kSlotsPerRow;
+    Query q(c); Workspace* w = q.w;
+    const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);
+    int rc = q.open(index, ops, n_ops, sorted.data(), (int64_t)sorted.size()); if (rc) return rc;
+    const long long n_units = q.n_units;
     const uint64_t win_end = limit < 0 ? ~0ull : (offset + (uint64_t)limit < offset ? ~0ull : offset + (uint64_t)limit);
-    uint64_t seen = 0, written = 0, launches = 0; float ms_total = 0;
+    uint64_t seen = 0, written = 0;
     for (long long u0 = 0; u0 < n_units; u0 += c->unit_batch) {
         const long long nu = std::min(c->unit_batch, n_units - u0);
-        if (w->d_bitmaps.ensure((size_t)nu * 8192) || w->d_info.ensure((size_t)nu * 8) || w->h_out.ensure((size_t)nu * 8)) return FBGPU_E_NOMEM;
-        EvalOut eo{ nullptr, nullptr, (uint4*)w->d_bitmaps.p, (uint2*)w->d_info.p, FuseReduce{} };
-        CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
-        rc = launch_eval(c, w, prog, d_prog, depth, d_shards + u0 / kSlotsPerRow, nu, eo); if (rc) return rc;
-        launches++;
-        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_info.p, (size_t)nu * 8, cudaMemcpyDeviceToHost, w->stream));
-        CUDA_TRY(cudaStreamSynchronize(w->stream));
-        const uint2* info = (const uint2*)w->h_out.p;
+        const uint2* info;
+        rc = q.eval_info(u0, nu, info); if (rc) return rc;
         std::vector<ColUnit> units; uint64_t batch_out = 0;
         for (long long u = 0; u < nu; u++) {
             const uint64_t N = info[u].x;
@@ -1236,38 +1282,32 @@ static int columns_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32
         }
         if (batch_out && written + batch_out <= cap) {
             // d_emit: columns [batch_out] u64, then for Extract magnitudes [batch_out] u64 and sign bits [ceil(batch_out / 32)] u32
-            const size_t ub = units.size() * sizeof(ColUnit), vb = want_vals ? batch_out * 8 + ((batch_out + 31) / 32) * 4 : 0, ob = batch_out * 8 + vb;
-            if (w->d_emit_units.ensure(ub) || w->d_emit.ensure(ob) || w->h_in.ensure(std::max<size_t>(ub, ob))) return FBGPU_E_NOMEM;
-            memcpy(w->h_in.p, units.data(), ub);
-            CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, w->h_in.p, ub, cudaMemcpyHostToDevice, w->stream));
-            const int grid = (int)std::min<size_t>(units.size(), (size_t)c->sm_count * 8);
-            unsigned long long* d_cols = (unsigned long long*)w->d_emit.p; unsigned long long* d_vals = d_cols + batch_out;
-            columns_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>((const uint4*)w->d_bitmaps.p, (const ColUnit*)w->d_emit_units.p, (int)units.size(), d_cols);
-            CUDA_TRY(cudaGetLastError()); launches++;
-            if (want_vals) {
-                CUDA_TRY(cudaMemsetAsync(d_vals, 0, vb, w->stream));
-                extract_values_kernel<<<grid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv_vals, depth_vals, (const uint4*)w->d_bitmaps.p, (const ColUnit*)w->d_emit_units.p, (int)units.size(),
-                                                                               d_vals, (unsigned int*)(d_vals + batch_out));
-                CUDA_TRY(cudaGetLastError()); launches++;
-            }
-            CUDA_TRY(cudaStreamSynchronize(w->stream));   // h_in is reused as the D2H landing buffer below
-            CUDA_TRY(cudaMemcpyAsync(w->h_in.p, w->d_emit.p, ob, cudaMemcpyDeviceToHost, w->stream));
-            CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
-            CUDA_TRY(cudaStreamSynchronize(w->stream));
+            const size_t vb = want_vals ? batch_out * 8 + ((batch_out + 31) / 32) * 4 : 0;
+            rc = q.emit(units, batch_out * 8 + vb, [&](const ColUnit* d_units, int n, int grid) {
+                unsigned long long* d_cols = (unsigned long long*)w->d_emit.p; unsigned long long* d_vals = d_cols + batch_out;
+                columns_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>((const uint4*)w->d_bitmaps.p, d_units, n, d_cols);
+                CUDA_TRY(cudaGetLastError()); q.launches++;
+                if (want_vals) {
+                    CUDA_TRY(cudaMemsetAsync(d_vals, 0, vb, w->stream));
+                    extract_values_kernel<<<grid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv_vals, depth_vals, (const uint4*)w->d_bitmaps.p, d_units, n,
+                                                                                   d_vals, (unsigned int*)(d_vals + batch_out));
+                    CUDA_TRY(cudaGetLastError()); q.launches++;
+                }
+                return 0;
+            });
+            if (rc) return rc;
             memcpy(out_cols + written, w->h_in.p, batch_out * 8);
             if (want_vals) {                               // sign-magnitude -> int64, wrapping like fragment.value: sign + 2^63 is INT64_MIN
                 const uint64_t* mag = (const uint64_t*)w->h_in.p + batch_out;
                 const uint32_t* sgn = (const uint32_t*)(mag + batch_out);
                 for (uint64_t i = 0; i < batch_out; i++) out_vals[written + i] = (int64_t)(((sgn[i >> 5] >> (i & 31)) & 1u) ? 0ull - mag[i] : mag[i]);
             }
-            float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1); ms_total += ms;
         }
         written += batch_out;                              // (past cap: counted, not written)
     }
-    bump(c, launches, ms_total);
     *out_n = written;
     if (out_total) *out_total = seen;
-    lease.ok = true;
+    q.finish();
     if (written > cap) return fail(FBGPU_E_NOSPACE, "output needs room for %llu columns", (unsigned long long)written);
     return FBGPU_OK;
 }
@@ -1275,9 +1315,8 @@ static int columns_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32
 extern "C" int fbgpu_columns(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, const uint64_t* shards, int64_t n_shards,
                              uint64_t offset, int64_t limit, uint64_t* out_cols, uint64_t cap, uint64_t* out_n, uint64_t* out_total) try {
     if (!c || !out_n || n_shards < 0 || (n_shards && !shards) || (cap && !out_cols)) return fail(FBGPU_E_INVALID, "null argument");
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
+    int rc = begin_query(c, lk); if (rc) return rc;
     return columns_impl(c, index, ops, n_ops, shards, n_shards, offset, limit, false, 0, 0, out_cols, nullptr, cap, out_n, out_total);
 } FBGPU_CATCH
 
@@ -1286,14 +1325,9 @@ extern "C" int fbgpu_extract(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, 
                              uint64_t* out_cols, int64_t* out_vals, uint64_t cap, uint64_t* out_n, uint64_t* out_total) try {
     if (!c || !out_n || n_shards < 0 || (n_shards && !shards) || (cap && (!out_cols || !out_vals)) || n_ops < 0 || (n_ops && !ops)) return fail(FBGPU_E_INVALID, "null argument");
     if (bit_depth < 0 || bit_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", bit_depth);
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
-    // the row: <filter> ∩ exists (bsiExistsBit, row 0 of the bsig_ view; fragment.go:44)
-    std::vector<fbgpu_op> full(ops, ops + n_ops);
-    fbgpu_op ex{}; ex.opcode = FBGPU_OP_ROW; ex.field = field; ex.view = view; ex.a = 0;
-    full.push_back(ex);
-    if (n_ops) { fbgpu_op in{}; in.opcode = FBGPU_OP_INTERSECT; in.argc = 2; full.push_back(in); }
+    int rc = begin_query(c, lk); if (rc) return rc;
+    const std::vector<fbgpu_op> full = and_row(ops, n_ops, field, view, 0);    // <filter> ∩ exists (bsiExistsBit, row 0 of the bsig_ view; fragment.go:44)
     const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
     return columns_impl(c, index, full.data(), (int32_t)full.size(), shards, n_shards, offset, limit, true, fv, bit_depth, out_cols, out_vals, cap, out_n, out_total);
 } FBGPU_CATCH
@@ -1303,31 +1337,23 @@ extern "C" int fbgpu_bsi_minmax(fbgpu_ctx* c, uint32_t index, const fbgpu_op* op
                                 const uint64_t* shards, int64_t n_shards, int32_t want_max, int64_t* out_val, uint64_t* out_count) try {
     if (!c || !out_val || !out_count || n_shards < 0 || (n_shards && !shards) || n_ops < 0 || (n_ops && !ops)) return fail(FBGPU_E_INVALID, "null argument");
     if (bit_depth < 0 || bit_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", bit_depth);
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
+    int rc = begin_query(c, lk); if (rc) return rc;
     *out_val = 0; *out_count = 0;
-    std::vector<fbgpu_op> full(ops, ops + n_ops);           // consider = <filter> ∩ exists (fragment.go:753-757)
-    fbgpu_op ex{}; ex.opcode = FBGPU_OP_ROW; ex.field = field; ex.view = view; ex.a = 0;
-    full.push_back(ex);
-    if (n_ops) { fbgpu_op in{}; in.opcode = FBGPU_OP_INTERSECT; in.argc = 2; full.push_back(in); }
-    std::vector<DevOp> prog; int depth = 1;
-    rc = compile_program(c, index, full.data(), (int32_t)full.size(), prog, depth); if (rc) return rc;
+    const std::vector<fbgpu_op> full = and_row(ops, n_ops, field, view, 0);    // consider = <filter> ∩ exists (fragment.go:753-757)
+    Query q(c); Workspace* w = q.w;
+    rc = q.open(index, full.data(), (int32_t)full.size(), shards, n_shards); if (rc) return rc;
     const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
-    WsLease lease(c); Workspace* w = lease.w;
-    const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, prog, shards, n_shards, &d_prog, &d_shards); if (rc) return rc;
-    const long long n_units = (long long)n_shards * kSlotsPerRow;
-    bool have = false; int64_t best = 0; uint64_t best_n = 0; uint64_t launches = 0; float ms_total = 0;
-    for (long long u0 = 0; u0 < n_units; u0 += c->unit_batch) {
-        const long long nu = std::min(c->unit_batch, n_units - u0);
+    bool have = false; int64_t best = 0; uint64_t best_n = 0;
+    for (long long u0 = 0; u0 < q.n_units; u0 += c->unit_batch) {
+        const long long nu = std::min(c->unit_batch, q.n_units - u0);
+        // (the buffers are grown before ev0: the bracket holds no allocation)
         if (w->d_bitmaps.ensure((size_t)nu * 8192) || w->d_counts.ensure((size_t)nu * sizeof(MinMaxUnit)) || w->h_out.ensure((size_t)nu * sizeof(MinMaxUnit))) return FBGPU_E_NOMEM;
-        EvalOut eo{ nullptr, nullptr, (uint4*)w->d_bitmaps.p, nullptr, FuseReduce{} };
         CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
-        rc = launch_eval(c, w, prog, d_prog, depth, d_shards + u0 / kSlotsPerRow, nu, eo); if (rc) return rc;
+        rc = q.eval(u0, nu); if (rc) return rc;
         const long long grid = std::min<long long>(nu, (long long)c->sm_count * 8);
-        bsi_minmax_kernel<<<(unsigned)grid, kEvalThreads, 0, w->stream>>>(store_ref(c), fv, bit_depth, (const uint4*)w->d_bitmaps.p, d_shards + u0 / kSlotsPerRow, nu, want_max ? 1 : 0, (MinMaxUnit*)w->d_counts.p);
-        CUDA_TRY(cudaGetLastError()); launches += 2;
+        bsi_minmax_kernel<<<(unsigned)grid, kEvalThreads, 0, w->stream>>>(store_ref(c), fv, bit_depth, (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, want_max ? 1 : 0, (MinMaxUnit*)w->d_counts.p);
+        CUDA_TRY(cudaGetLastError()); q.launches++;
         CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
         CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, (size_t)nu * sizeof(MinMaxUnit), cudaMemcpyDeviceToHost, w->stream));
         CUDA_TRY(cudaStreamSynchronize(w->stream));
@@ -1337,11 +1363,10 @@ extern "C" int fbgpu_bsi_minmax(fbgpu_ctx* c, uint32_t index, const fbgpu_op* op
             if (!have || (want_max ? r[u].val > best : r[u].val < best)) { have = true; best = r[u].val; best_n = r[u].cnt; }
             else if (r[u].val == best) best_n += r[u].cnt;
         }
-        float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1); ms_total += ms;
+        q.add_elapsed();
     }
-    bump(c, launches, ms_total);
     if (have) { *out_val = best; *out_count = best_n; }
-    lease.ok = true;
+    q.finish();
     return FBGPU_OK;
 } FBGPU_CATCH
 
@@ -1349,34 +1374,23 @@ extern "C" int fbgpu_bsi_sum(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, 
                              const uint64_t* shards, int64_t n_shards, int64_t* out_sum, uint64_t* out_count) try {
     if (!c || !out_sum || !out_count || n_shards < 0 || (n_shards && !shards) || n_ops < 0 || (n_ops && !ops)) return fail(FBGPU_E_INVALID, "null argument");
     if (bit_depth < 0 || bit_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", bit_depth);
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
+    int rc = begin_query(c, lk); if (rc) return rc;
     *out_sum = 0; *out_count = 0;
-    std::vector<fbgpu_op> full(ops, ops + n_ops);
-    fbgpu_op ex{}; ex.opcode = FBGPU_OP_ROW; ex.field = field; ex.view = view; ex.a = 0;
-    full.push_back(ex);
-    if (n_ops) { fbgpu_op in{}; in.opcode = FBGPU_OP_INTERSECT; in.argc = 2; full.push_back(in); }
-    std::vector<DevOp> prog; int depth = 1;
-    rc = compile_program(c, index, full.data(), (int32_t)full.size(), prog, depth); if (rc) return rc;
+    const std::vector<fbgpu_op> full = and_row(ops, n_ops, field, view, 0);
+    Query q(c); Workspace* w = q.w;
+    rc = q.open(index, full.data(), (int32_t)full.size(), shards, n_shards); if (rc) return rc;
     const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
-    WsLease lease(c); Workspace* w = lease.w;
-    const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, prog, shards, n_shards, &d_prog, &d_shards); if (rc) return rc;
-    const long long n_units = (long long)n_shards * kSlotsPerRow;
     const size_t n_acc = 1 + 2 * (size_t)bit_depth;
     if (w->d_counts.ensure(n_acc * 8) || w->h_out.ensure(n_acc * 8)) return FBGPU_E_NOMEM;
     CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, n_acc * 8, w->stream));
-    uint64_t launches = 0;
     CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
-    for (long long u0 = 0; u0 < n_units; u0 += c->unit_batch) {
-        const long long nu = std::min(c->unit_batch, n_units - u0);
-        if (w->d_bitmaps.ensure((size_t)nu * 8192)) return FBGPU_E_NOMEM;
-        EvalOut eo{ nullptr, nullptr, (uint4*)w->d_bitmaps.p, nullptr, FuseReduce{} };
-        rc = launch_eval(c, w, prog, d_prog, depth, d_shards + u0 / kSlotsPerRow, nu, eo); if (rc) return rc;
+    for (long long u0 = 0; u0 < q.n_units; u0 += c->unit_batch) {
+        const long long nu = std::min(c->unit_batch, q.n_units - u0);
+        rc = q.eval(u0, nu); if (rc) return rc;
         const long long grid = std::min<long long>(nu, (long long)c->sm_count * 8);
-        bsi_sum_kernel<<<(unsigned)grid, kEvalThreads, 0, w->stream>>>(store_ref(c), fv, bit_depth, (const uint4*)w->d_bitmaps.p, d_shards + u0 / kSlotsPerRow, nu, (unsigned long long*)w->d_counts.p);
-        CUDA_TRY(cudaGetLastError()); launches += 2;
+        bsi_sum_kernel<<<(unsigned)grid, kEvalThreads, 0, w->stream>>>(store_ref(c), fv, bit_depth, (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, (unsigned long long*)w->d_counts.p);
+        CUDA_TRY(cudaGetLastError()); q.launches++;
     }
     CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
     CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, n_acc * 8, cudaMemcpyDeviceToHost, w->stream));
@@ -1385,9 +1399,8 @@ extern "C" int fbgpu_bsi_sum(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, 
     uint64_t sum = 0;                                       // wrapping, like the reference's int64 arithmetic
     for (int i = 0; i < bit_depth; i++) sum += (acc[1 + 2 * i] - acc[2 + 2 * i]) << i;
     *out_sum = (int64_t)sum; *out_count = acc[0];
-    float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1);
-    bump(c, launches, ms);
-    lease.ok = true;
+    q.add_elapsed();
+    q.finish();
     return FBGPU_OK;
 } FBGPU_CATCH
 
@@ -1404,25 +1417,16 @@ extern "C" int fbgpu_bsi_select(fbgpu_ctx* c, uint32_t index, const fbgpu_op* op
     if (bit_depth < 0 || bit_depth > 63) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..63", bit_depth);     // the sort key takes depth + 1 bits
     if (n_ranks > FBGPU_SELECT_MAX_RANKS) return fail(FBGPU_E_INVALID, "%d ranks: at most %d per call", n_ranks, FBGPU_SELECT_MAX_RANKS);
     if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_bsi_select is local to one context: order statistics of the ranks' shares do not merge");
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
+    int rc = begin_query(c, lk); if (rc) return rc;
     *out_total = 0;
-    std::vector<uint64_t> uniq(ranks, ranks + n_ranks);     // the device works on distinct ranks (at least one: slot 0 holds the row)
-    std::sort(uniq.begin(), uniq.end());
-    uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
+    const std::vector<uint64_t> uniq = sorted_unique(ranks, n_ranks);     // the device works on distinct ranks (at least one: slot 0 holds the row)
     const int nr = std::max(1, (int)uniq.size());
-    std::vector<fbgpu_op> full(ops, ops + n_ops);           // the row = <filter> ∩ exists, as for Min / Max
-    fbgpu_op ex{}; ex.opcode = FBGPU_OP_ROW; ex.field = field; ex.view = view; ex.a = 0;
-    full.push_back(ex);
-    if (n_ops) { fbgpu_op in{}; in.opcode = FBGPU_OP_INTERSECT; in.argc = 2; full.push_back(in); }
-    std::vector<DevOp> prog; int depth = 1;
-    rc = compile_program(c, index, full.data(), (int32_t)full.size(), prog, depth); if (rc) return rc;
+    const std::vector<fbgpu_op> full = and_row(ops, n_ops, field, view, 0);    // the row = <filter> ∩ exists, as for Min / Max
+    Query q(c); Workspace* w = q.w;
+    rc = q.open(index, full.data(), (int32_t)full.size(), shards, n_shards); if (rc) return rc;
     const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
-    WsLease lease(c); Workspace* w = lease.w;
-    const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, prog, shards, n_shards, &d_prog, &d_shards); if (rc) return rc;
-    const long long n_units = (long long)n_shards * kSlotsPerRow;
+    const long long n_units = q.n_units;
     // d_counts: [SelRank x kSelMaxRanks][buckets kSelMaxRanks x kSelBuckets][total]
     const size_t st_bytes = kSelMaxRanks * sizeof(SelRank), bk_bytes = kSelMaxRanks * kSelBuckets * 8, ctl_bytes = st_bytes + bk_bytes + 8;
     if (w->d_counts.ensure(ctl_bytes) || w->h_out.ensure(ctl_bytes)) return FBGPU_E_NOMEM;
@@ -1437,32 +1441,27 @@ extern "C" int fbgpu_bsi_select(fbgpu_ctx* c, uint32_t index, const fbgpu_op* op
     unsigned long long* d_total = d_buckets + kSelMaxRanks * kSelBuckets;
     uint4* d_cand = (uint4*)w->d_select.p;
     unsigned int* d_live = n_units > 0 ? (unsigned int*)((uint8_t*)w->d_select.p + cand_bytes) : nullptr;
-    uint64_t launches = 0;
     CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
     if (n_units > 0) {
         for (long long u0 = 0; u0 < n_units; u0 += c->unit_batch) {
-            const long long nu = std::min(c->unit_batch, n_units - u0);
-            EvalOut eo{ nullptr, nullptr, d_cand + (size_t)u0 * 512, nullptr, FuseReduce{} };
-            rc = launch_eval(c, w, prog, d_prog, depth, d_shards + u0 / kSlotsPerRow, nu, eo); if (rc) return rc;
-            launches++;
+            rc = q.eval(u0, std::min(c->unit_batch, n_units - u0), false, d_cand + (size_t)u0 * 512); if (rc) return rc;
         }
         const int n_steps = (bit_depth + 1 + kSelDigit - 1) / kSelDigit;
         const long long grid = std::min<long long>(n_units, (long long)c->sm_count * 4);
         for (int s = 0; s < n_steps; s++) {
-            bsi_select_step_kernel<<<(unsigned)grid, kEvalThreads, 0, w->stream>>>(store_ref(c), fv, bit_depth, s, s == n_steps - 1 ? 1 : 0, d_cand, d_shards, n_units, nr,
+            bsi_select_step_kernel<<<(unsigned)grid, kEvalThreads, 0, w->stream>>>(store_ref(c), fv, bit_depth, s, s == n_steps - 1 ? 1 : 0, d_cand, q.d_shards, n_units, nr,
                                                                                    d_state, d_live, d_buckets);
             CUDA_TRY(cudaGetLastError());
             bsi_select_decide_kernel<<<1, 32, 0, w->stream>>>(bit_depth, s, nr, d_state, d_buckets, d_total);
             CUDA_TRY(cudaGetLastError());
-            launches += 2;
+            q.launches += 2;
         }
     }
     CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
     CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, ctl_bytes, cudaMemcpyDeviceToHost, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
-    float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1);
-    bump(c, launches, ms);
-    lease.ok = true;
+    q.add_elapsed();
+    q.finish();
     const SelRank* rs = (const SelRank*)w->h_out.p;
     const uint64_t total = *(const uint64_t*)((const uint8_t*)w->h_out.p + st_bytes + bk_bytes);
     *out_total = total;
@@ -1479,43 +1478,32 @@ extern "C" int fbgpu_bsi_select(fbgpu_ctx* c, uint32_t index, const fbgpu_op* op
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ per-row counts (TopK / TopN ids)
-// evaluates `filter` for shards [s0, s0+ns) into w->d_bitmaps (16 bitmaps per shard)
-static int eval_filter_batch(fbgpu_ctx* c, Workspace* w, const std::vector<DevOp>& prog, int depth, const DevOp* d_prog, const uint64_t* d_shards, int64_t ns) {
-    if (w->d_bitmaps.ensure((size_t)ns * kSlotsPerRow * 8192)) return FBGPU_E_NOMEM;
-    EvalOut eo{ nullptr, nullptr, (uint4*)w->d_bitmaps.p, nullptr, FuseReduce{} };
-    return launch_eval(c, w, prog, d_prog, depth, d_shards, ns * kSlotsPerRow, eo);
-}
-
 static int row_counts_impl(fbgpu_ctx* c, uint32_t index, uint32_t fv, const std::vector<uint64_t>& rows, const fbgpu_op* filter, int32_t n_filter_ops,
                            const uint64_t* shards, int64_t n_shards, std::vector<uint64_t>& counts, bool reduce = true, bool per_shard = false) {
     counts.assign(rows.size() * (per_shard ? (size_t)n_shards : 1), 0);
     if (rows.empty()) return 0;
-    std::vector<DevOp> prog; int depth = 1; int rc;
-    bool have_filter = filter && n_filter_ops > 0;
-    if (have_filter) { rc = compile_program(c, index, filter, n_filter_ops, prog, depth); if (rc) return rc; }
-    WsLease lease(c); Workspace* w = lease.w;
-    const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, prog, shards, n_shards, &d_prog, &d_shards); if (rc) return rc;
+    const bool have_filter = filter && n_filter_ops > 0;
+    Query q(c); Workspace* w = q.w;
+    int rc = have_filter ? q.open(index, filter, n_filter_ops, shards, n_shards) : q.open(shards, n_shards); if (rc) return rc;
     size_t nr = rows.size();
     const size_t n_out = counts.size();                     // nr, or n_shards x nr (per_shard: one row of the matrix per listed shard)
     if (w->d_rows.ensure(nr * 8) || w->d_counts.ensure(n_out * 8) || w->h_out.ensure(n_out * 8)) return FBGPU_E_NOMEM;
     CUDA_TRY(cudaMemcpyAsync(w->d_rows.p, rows.data(), nr * 8, cudaMemcpyHostToDevice, w->stream));
     CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, n_out * 8, w->stream));
     CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
-    uint64_t launches = 0;
     const int64_t batch = have_filter ? c->unit_batch / kSlotsPerRow : n_shards;
     for (int64_t s0 = 0; s0 < n_shards; s0 += batch) {
         int64_t ns = std::min(batch, n_shards - s0);
-        if (have_filter) { rc = eval_filter_batch(c, w, prog, depth, d_prog, d_shards + s0, ns); if (rc) return rc; launches++; }
+        if (have_filter) { rc = q.eval(s0 * kSlotsPerRow, ns * kSlotsPerRow); if (rc) return rc; }
         long long tasks = (long long)ns * (long long)nr;
         long long grid = std::min<long long>((tasks + kPairWarps - 1) / kPairWarps, (long long)c->sm_count * 3);
         if (per_shard)
-            row_count_kernel<true><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, d_shards + s0, ns,
+            row_count_kernel<true><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, q.d_shards + s0, ns,
                 have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p + (size_t)s0 * nr);
         else
-            row_count_kernel<false><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, d_shards + s0, ns,
+            row_count_kernel<false><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, q.d_shards + s0, ns,
                 have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p);
-        CUDA_TRY(cudaGetLastError()); launches++;
+        CUDA_TRY(cudaGetLastError()); q.launches++;
     }
     CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
     // every rank must bring the same row list to the collective: only the explicit-ids form is all-reduced (fbgpu.h)
@@ -1523,9 +1511,8 @@ static int row_counts_impl(fbgpu_ctx* c, uint32_t index, uint32_t fv, const std:
     CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, n_out * 8, cudaMemcpyDeviceToHost, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
     memcpy(counts.data(), w->h_out.p, n_out * 8);
-    float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1);
-    bump(c, launches, ms);
-    lease.ok = true;
+    q.add_elapsed();
+    q.finish();
     return 0;
 }
 
@@ -1533,9 +1520,8 @@ extern "C" int fbgpu_row_counts(fbgpu_ctx* c, uint32_t index, uint32_t field, ui
                                 const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
                                 uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n) try {
     if (!c || !out_counts || n_shards < 0 || (n_shards && !shards) || n_rows < 0) return fail(FBGPU_E_INVALID, "null argument");
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
+    int rc = begin_query(c, lk); if (rc) return rc;
     uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
     std::vector<uint64_t> rows, counts;
     if (row_ids) rows.assign(row_ids, row_ids + n_rows);
@@ -1572,9 +1558,8 @@ extern "C" int fbgpu_row_counts_per_shard(fbgpu_ctx* c, uint32_t index, uint32_t
                                           const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     if (!c || !out_counts || !row_ids || n_rows < 0 || n_shards < 0 || (n_shards && !shards) || n_filter_ops < 0 || (n_filter_ops && !filter)) return fail(FBGPU_E_INVALID, "null argument");
     if (n_rows == 0 || n_shards == 0) return FBGPU_OK;
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
+    int rc = begin_query(c, lk); if (rc) return rc;
     const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
     std::vector<uint64_t> rows(row_ids, row_ids + n_rows), counts;
     // the matrix is produced in blocks of shards so that the device / pinned buffers stay below 512 MiB however many rows are asked for
@@ -1597,21 +1582,21 @@ extern "C" int fbgpu_count_pairs(fbgpu_ctx* c, uint32_t index, uint32_t field_a,
     std::shared_lock<std::shared_mutex> lk;
     int rc = lock_committed(c, lk); if (rc) return rc;
     uint32_t fa = view_id_locked(c, ViewKey{ index, field_a, view_a }, false), fb = view_id_locked(c, ViewKey{ index, field_b, view_b }, false);
-    WsLease lease(c); Workspace* w = lease.w;
-    std::vector<DevOp> none; const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, none, shards, n_shards, &d_prog, &d_shards); if (rc) return rc;
+    Query q(c); Workspace* w = q.w;
+    rc = q.open(shards, n_shards); if (rc) return rc;
     size_t np = (size_t)n_pairs;
     if (w->d_rows.ensure(np * 16) || w->d_counts.ensure(np * 8) || w->h_out.ensure(np * 16)) return FBGPU_E_NOMEM;
     memcpy(w->h_out.p, rows_a, np * 8); memcpy((uint8_t*)w->h_out.p + np * 8, rows_b, np * 8);
     CUDA_TRY(cudaMemcpyAsync(w->d_rows.p, w->h_out.p, np * 16, cudaMemcpyHostToDevice, w->stream));
     CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, np * 8, w->stream));
-    const long long upp = (long long)n_shards * kSlotsPerRow, n_units = upp * n_pairs;
+    const long long upp = q.n_units, n_units = upp * n_pairs;
     CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
     if (n_units > 0) {
         long long grid = std::min<long long>((n_units + kPcWarps - 1) / kPcWarps, (long long)c->sm_count * c->pair_ctas_per_sm);
+        const PairShards ps = pair_shards(shards, n_shards, q.d_shards);
         pair_count_kernel<<<(unsigned)grid, kPcWarps * 32, kPcWarps * 8192, w->stream>>>(store_ref(c), fa, 0, fb, 0, (const uint64_t*)w->d_rows.p, (const uint64_t*)w->d_rows.p + np,
-            upp, contiguous_shards(shards, n_shards) ? nullptr : d_shards, n_shards ? shards[0] : 0, n_units, nullptr, nullptr, (unsigned long long*)w->d_counts.p, FuseReduce{});
-        CUDA_TRY(cudaGetLastError());
+            upp, ps.list, ps.first, n_units, nullptr, nullptr, (unsigned long long*)w->d_counts.p, FuseReduce{});
+        CUDA_TRY(cudaGetLastError()); q.launches++;
     }
     CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
     rc = allreduce_u64(c, w, w->d_counts.p, np); if (rc) return rc;
@@ -1619,9 +1604,8 @@ extern "C" int fbgpu_count_pairs(fbgpu_ctx* c, uint32_t index, uint32_t field_a,
     CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, np * 8, cudaMemcpyDeviceToHost, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
     memcpy(out_counts, w->h_out.p, np * 8);
-    float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1);
-    bump(c, n_units > 0 ? 1 : 0, ms);
-    lease.ok = true;
+    q.add_elapsed();
+    q.finish();
     return FBGPU_OK;
 } FBGPU_CATCH
 
@@ -1635,20 +1619,17 @@ extern "C" int fbgpu_pair_types(fbgpu_ctx* c, uint32_t index, uint32_t field_a, 
     std::shared_lock<std::shared_mutex> lk;
     int rc = lock_committed(c, lk); if (rc) return rc;
     const uint32_t fa = view_id_locked(c, ViewKey{ index, field_a, view_a }, false), fb = view_id_locked(c, ViewKey{ index, field_b, view_b }, false);
-    WsLease lease(c); Workspace* w = lease.w;
-    std::vector<DevOp> none; const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, none, shards, n_shards, &d_prog, &d_shards); if (rc) return rc;
+    Query q(c); Workspace* w = q.w;
+    rc = q.open(shards, n_shards); if (rc) return rc;
     if (w->d_counts.ensure(16 * 8) || w->h_out.ensure(16 * 8)) return FBGPU_E_NOMEM;
     CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, 16 * 8, w->stream));
-    const long long n_units = (long long)n_shards * kSlotsPerRow;
-    const long long grid = std::min<long long>((n_units + 255) / 256, (long long)c->sm_count * 4);
-    pair_types_kernel<<<(unsigned)grid, 256, 0, w->stream>>>(store_ref(c), fa, row_a, fb, row_b, d_shards, n_units, (unsigned long long*)w->d_counts.p);
-    CUDA_TRY(cudaGetLastError());
+    const long long grid = std::min<long long>((q.n_units + 255) / 256, (long long)c->sm_count * 4);
+    pair_types_kernel<<<(unsigned)grid, 256, 0, w->stream>>>(store_ref(c), fa, row_a, fb, row_b, q.d_shards, q.n_units, (unsigned long long*)w->d_counts.p);
+    CUDA_TRY(cudaGetLastError()); q.launches++;
     CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, 16 * 8, cudaMemcpyDeviceToHost, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
     memcpy(out_hist, w->h_out.p, 16 * 8);
-    bump(c, 1, 0.f);
-    lease.ok = true;
+    q.finish();                              // (untimed: last_query_gpu_ms reads 0)
     return FBGPU_OK;
 } FBGPU_CATCH
 
@@ -1694,12 +1675,10 @@ static bool groupby_direct_eligible(fbgpu_ctx* c, uint32_t fvA, uint32_t fvB, co
 
 static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* rowsA, int nA, uint32_t fvB, const uint64_t* rowsB, int nB,
                     const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards, uint64_t* out) {
-    std::vector<DevOp> prog; int depth = 1; int rc;
-    bool have_filter = !filter.empty();
-    if (have_filter) { rc = compile_program(c, index, filter.data(), (int)filter.size(), prog, depth); if (rc) return rc; }
-    WsLease lease(c); Workspace* w = lease.w;
-    const DevOp* d_prog; const uint64_t* d_shards;
-    rc = upload_inputs(w, prog, shards, n_shards, &d_prog, &d_shards); if (rc) return rc;
+    const bool have_filter = !filter.empty();
+    Query q(c); Workspace* w = q.w;
+    int rc = have_filter ? q.open(index, filter.data(), (int)filter.size(), shards, n_shards) : q.open(shards, n_shards); if (rc) return rc;
+    const uint64_t* d_shards = q.d_shards;
     size_t ncnt = (size_t)nA * nB;
     if (w->d_rows.ensure((size_t)(nA + nB) * 8) || w->d_counts.ensure(ncnt * 8) || w->h_out.ensure(ncnt * 8)) return FBGPU_E_NOMEM;
     std::vector<uint64_t> rr(rowsA, rowsA + nA); rr.insert(rr.end(), rowsB, rowsB + nB);
@@ -1707,12 +1686,12 @@ static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* 
     CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, ncnt * 8, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));   // rr is a local
     CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
-    uint64_t launches = 0, fb_units = 0, all_units = 0;
+    uint64_t fb_units = 0, all_units = 0;
     const int64_t batch = have_filter ? c->unit_batch / kSlotsPerRow : n_shards;
     const size_t smem = kGbSlots * 4 + 8192;
     for (int64_t s0 = 0; s0 < n_shards; s0 += batch) {
         int64_t ns = std::min(batch, n_shards - s0);
-        if (have_filter) { rc = eval_filter_batch(c, w, prog, depth, d_prog, d_shards + s0, ns); if (rc) return rc; launches++; }
+        if (have_filter) { rc = q.eval(s0 * kSlotsPerRow, ns * kSlotsPerRow); if (rc) return rc; }
         long long units = (long long)ns * kSlotsPerRow;
         long long grid = std::min<long long>(units, (long long)c->sm_count * 4);
         static const bool gb_cta_only = getenv("FBGPU_GROUPBY_CTA") != nullptr; // round-1 path only: one CTA per unit
@@ -1731,7 +1710,7 @@ static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* 
                 CUDA_TRY(cudaMemsetAsync(d_fb, 0, 4, w->stream));
                 groupby_direct_kernel<<<(unsigned)dgrid, kGdThreads, kGdSmemBytes, w->stream>>>(store_ref(c), fvA, d_ra, na, fvB, (const uint64_t*)w->d_rows.p + nA, nB,
                     d_shards + s0, units, have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, d_cnt, d_fb);
-                CUDA_TRY(cudaGetLastError()); launches++;
+                CUDA_TRY(cudaGetLastError()); q.launches++;
                 CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
                 CUDA_TRY(cudaMemcpyAsync(h_fb, d_fb, 4, cudaMemcpyDeviceToHost, w->stream));
                 CUDA_TRY(cudaStreamSynchronize(w->stream));
@@ -1739,7 +1718,7 @@ static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* 
                 if (n_fb) {
                     groupby_kernel<<<(unsigned)std::min<long long>(n_fb, grid), kGbThreads, smem, w->stream>>>(store_ref(c), fvA, d_ra, na, fvB, (const uint64_t*)w->d_rows.p + nA, nB,
                         d_shards + s0, units, have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, d_cnt, d_fb);
-                    CUDA_TRY(cudaGetLastError()); launches++;
+                    CUDA_TRY(cudaGetLastError()); q.launches++;
                     CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
                 }
                 fb_units += n_fb; all_units += (uint64_t)units;
@@ -1747,7 +1726,7 @@ static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* 
         } else {
             groupby_kernel<<<(unsigned)grid, kGbThreads, smem, w->stream>>>(store_ref(c), fvA, (const uint64_t*)w->d_rows.p, nA, fvB, (const uint64_t*)w->d_rows.p + nA, nB,
                 d_shards + s0, units, have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p, nullptr);
-            CUDA_TRY(cudaGetLastError()); launches++;
+            CUDA_TRY(cudaGetLastError()); q.launches++;
             CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
         }
     }
@@ -1756,10 +1735,9 @@ static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* 
     CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, ncnt * 8, cudaMemcpyDeviceToHost, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
     memcpy(out, w->h_out.p, ncnt * 8);
-    float ms = 0; cudaEventElapsedTime(&ms, w->ev0, w->ev1);
-    bump(c, launches, ms);
+    q.add_elapsed();
     { std::lock_guard<std::mutex> lk2(c->cnt_mu); c->counters.groupby_units += all_units; c->counters.groupby_fallback_units += fb_units; }
-    lease.ok = true;
+    q.finish();
     return 0;
 }
 
@@ -1780,11 +1758,8 @@ static int groupby_rec(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, con
     }
     size_t sub = 1; for (int i = 1; i < nf; i++) sub *= (size_t)n_rows[i];
     for (int r = 0; r < n_rows[0]; r++) {
-        std::vector<fbgpu_op> f2 = filter;
-        fbgpu_op ro{}; ro.opcode = FBGPU_OP_ROW; ro.field = fields[0]; ro.view = views[0]; ro.a = rows[0][r];
-        f2.push_back(ro);
-        if (!filter.empty()) { fbgpu_op in{}; in.opcode = FBGPU_OP_INTERSECT; in.argc = 2; f2.push_back(in); }
-        int rc = groupby_rec(c, index, fields + 1, views + 1, nf - 1, rows + 1, n_rows + 1, f2, shards, n_shards, out + (size_t)r * sub); if (rc) return rc;
+        int rc = groupby_rec(c, index, fields + 1, views + 1, nf - 1, rows + 1, n_rows + 1, and_row(filter.data(), (int32_t)filter.size(), fields[0], views[0], rows[0][r]),
+                             shards, n_shards, out + (size_t)r * sub); if (rc) return rc;
     }
     return 0;
 }
@@ -1792,9 +1767,8 @@ static int groupby_rec(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, con
 extern "C" int fbgpu_groupby(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows,
                              const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     if (!c || !fields || !views || !row_ids_flat || !n_rows || !out_counts || n_fields < 1 || n_fields > 8 || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
-    USE_DEVICE(c);
     std::shared_lock<std::shared_mutex> lk;
-    int rc = lock_committed(c, lk); if (rc) return rc;
+    int rc = begin_query(c, lk); if (rc) return rc;
     std::vector<const uint64_t*> rows(n_fields); const uint64_t* p = row_ids_flat; size_t total = 1;
     for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); rows[i] = p; p += n_rows[i]; total *= (size_t)n_rows[i]; }
     memset(out_counts, 0, total * 8);

@@ -31,7 +31,6 @@ struct fbgpu_node {
     std::vector<std::vector<std::unique_ptr<NodeWorker>>> workers; // [device][k]
     std::vector<std::atomic<uint32_t>> rr;                         // round-robin cursor per device
     uint64_t shard_block = 1;
-    std::atomic<uint64_t> queries{ 0 };
     explicit fbgpu_node(size_t n) : rr(n) {}
     int owner(uint64_t shard) const { return (int)((shard / shard_block) % ctx.size()); }
 };
@@ -104,18 +103,15 @@ extern "C" int fbgpu_node_load_fragments(fbgpu_node* n, uint32_t index, uint32_t
     if (!n || !shards || !buf || !offsets || cnt < 0) return fail(FBGPU_E_INVALID, "null argument");
     // per device: the sub-list of fragments with their own offsets table into the caller's buffer (no payload copy here); a
     // device's batch is all-or-nothing (StoreTxn), devices load concurrently
-    const size_t nd = n->ctx.size();
-    std::vector<std::vector<uint64_t>> sh(nd); std::vector<std::vector<int64_t>> idx(nd);
-    for (int64_t i = 0; i < cnt; i++) { int d = n->owner(shards[i]); sh[d].push_back(shards[i]); idx[d].push_back(i); }
-    std::vector<int> devs; for (size_t d = 0; d < nd; d++) if (!sh[d].empty()) devs.push_back((int)d);
-    return node_fan_out(n, devs, [&](int d) -> int {
+    const NodeSplit sp = node_split(n, shards, cnt);
+    return node_fan_out(n, node_owners(sp), [&](int d) -> int {
         // fragments of one device are generally not adjacent in buf: load them as runs of adjacent fragments
-        const auto& ix = idx[(size_t)d];
+        const auto& ix = sp.pos[(size_t)d];
         for (size_t a = 0; a < ix.size();) {
             size_t b = a + 1; while (b < ix.size() && ix[b] == ix[b - 1] + 1) b++;
             std::vector<uint64_t> off(b - a + 1); const uint64_t base = offsets[ix[a]];
             for (size_t k = a; k <= b; k++) off[k - a] = (k < b ? offsets[ix[k]] : offsets[ix[b - 1] + 1]) - base;
-            int rc = fbgpu_load_fragments(n->ctx[(size_t)d], index, field, view, sh[(size_t)d].data() + a, (int64_t)(b - a), buf + base, off.data()); if (rc) return rc;
+            int rc = fbgpu_load_fragments(n->ctx[(size_t)d], index, field, view, sp.shards[(size_t)d].data() + a, (int64_t)(b - a), buf + base, off.data()); if (rc) return rc;
             a = b;
         }
         return 0;
@@ -155,7 +151,6 @@ extern "C" int fbgpu_node_get_stats(fbgpu_node* n, fbgpu_stats* out) try {
 extern "C" int fbgpu_node_count(fbgpu_node* n, uint32_t index, const fbgpu_op* ops, int32_t n_ops, const uint64_t* shards, int64_t n_shards,
                                 uint64_t* out_total, uint64_t* out_per_shard) try {
     if (!n || !out_total || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "null argument");
-    n->queries.fetch_add(1, std::memory_order_relaxed);
     NodeSplit sp = node_split(n, shards, n_shards);
     std::vector<int> devs = node_owners(sp);
     if (devs.empty()) devs.push_back(0);                 // no shard listed: still validate the program (Intersect() etc. must error)
@@ -185,63 +180,49 @@ extern "C" int fbgpu_node_any(fbgpu_node* n, uint32_t index, const fbgpu_op* ops
     return FBGPU_OK;
 } FBGPU_CATCH
 
-// element-wise sum of per-device u64 vectors into out (out is overwritten)
-static void node_sum(const std::vector<int>& devs, const std::vector<std::vector<uint64_t>>& part, uint64_t* out, size_t len) {
+// runs fn(ctx, its shards, part) on every device that owns listed shards, each filling a zeroed u64 vector of `len`, and writes
+// their element-wise sum to out (overwritten; zeros when no shard is listed)
+template <class F>
+static int node_sum(fbgpu_node* n, const uint64_t* shards, int64_t n_shards, size_t len, uint64_t* out, F fn) {
+    const NodeSplit sp = node_split(n, shards, n_shards);
+    const std::vector<int> devs = node_owners(sp);
+    std::vector<std::vector<uint64_t>> part(n->ctx.size());
+    int rc = node_fan_out(n, devs, [&](int d) {
+        part[(size_t)d].assign(len, 0);
+        return fn(n->ctx[(size_t)d], sp.shards[(size_t)d], part[(size_t)d].data());
+    });
+    if (rc) return rc;
     memset(out, 0, len * 8);
     for (int d : devs) { const uint64_t* p = part[(size_t)d].data(); for (size_t i = 0; i < len; i++) out[i] += p[i]; }
+    return FBGPU_OK;
 }
 
 extern "C" int fbgpu_node_count_pairs(fbgpu_node* n, uint32_t index, uint32_t field_a, uint32_t view_a, const uint64_t* rows_a,
                                       uint32_t field_b, uint32_t view_b, const uint64_t* rows_b, int32_t n_pairs,
                                       const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     if (!n || !rows_a || !rows_b || !out_counts || n_pairs < 0 || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "null argument");
-    n->queries.fetch_add(1, std::memory_order_relaxed);
-    NodeSplit sp = node_split(n, shards, n_shards);
-    std::vector<int> devs = node_owners(sp);
-    std::vector<std::vector<uint64_t>> part(n->ctx.size());
-    int rc = node_fan_out(n, devs, [&](int d) {
-        part[(size_t)d].assign((size_t)n_pairs, 0);
-        return fbgpu_count_pairs(n->ctx[(size_t)d], index, field_a, view_a, rows_a, field_b, view_b, rows_b, n_pairs, sp.shards[(size_t)d].data(), (int64_t)sp.shards[(size_t)d].size(), part[(size_t)d].data());
+    return node_sum(n, shards, n_shards, (size_t)n_pairs, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {
+        return fbgpu_count_pairs(c, index, field_a, view_a, rows_a, field_b, view_b, rows_b, n_pairs, s.data(), (int64_t)s.size(), part);
     });
-    if (rc) return rc;
-    node_sum(devs, part, out_counts, (size_t)n_pairs);
-    return FBGPU_OK;
 } FBGPU_CATCH
 
 // explicit-ids form only (TopN(ids=...), TopK candidates): the reduced vector is what Pairs.Add produces (cache.go:464)
 extern "C" int fbgpu_node_row_counts(fbgpu_node* n, uint32_t index, uint32_t field, uint32_t view, const uint64_t* row_ids, int32_t n_rows,
                                      const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     if (!n || !row_ids || !out_counts || n_rows < 0 || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "null argument");
-    n->queries.fetch_add(1, std::memory_order_relaxed);
-    NodeSplit sp = node_split(n, shards, n_shards);
-    std::vector<int> devs = node_owners(sp);
-    std::vector<std::vector<uint64_t>> part(n->ctx.size());
-    int rc = node_fan_out(n, devs, [&](int d) {
-        part[(size_t)d].assign((size_t)n_rows, 0);
+    return node_sum(n, shards, n_shards, (size_t)n_rows, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {
         int32_t got = 0;
-        return fbgpu_row_counts(n->ctx[(size_t)d], index, field, view, row_ids, n_rows, filter, n_filter_ops, sp.shards[(size_t)d].data(), (int64_t)sp.shards[(size_t)d].size(),
-                                nullptr, part[(size_t)d].data(), n_rows, &got);
+        return fbgpu_row_counts(c, index, field, view, row_ids, n_rows, filter, n_filter_ops, s.data(), (int64_t)s.size(), nullptr, part, n_rows, &got);
     });
-    if (rc) return rc;
-    node_sum(devs, part, out_counts, (size_t)n_rows);
-    return FBGPU_OK;
 } FBGPU_CATCH
 
 extern "C" int fbgpu_node_groupby(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
                                   const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     if (!n || !fields || !views || !row_ids_flat || !n_rows || !out_counts || n_fields < 1 || n_fields > 8 || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
-    n->queries.fetch_add(1, std::memory_order_relaxed);
     size_t total = 1; for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); total *= (size_t)n_rows[i]; }
-    NodeSplit sp = node_split(n, shards, n_shards);
-    std::vector<int> devs = node_owners(sp);
-    std::vector<std::vector<uint64_t>> part(n->ctx.size());
-    int rc = node_fan_out(n, devs, [&](int d) {
-        part[(size_t)d].assign(total, 0);
-        return fbgpu_groupby(n->ctx[(size_t)d], index, fields, views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, sp.shards[(size_t)d].data(), (int64_t)sp.shards[(size_t)d].size(), part[(size_t)d].data());
+    return node_sum(n, shards, n_shards, total, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {     // mergeGroupCounts executor.go:3728
+        return fbgpu_groupby(c, index, fields, views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, s.data(), (int64_t)s.size(), part);
     });
-    if (rc) return rc;
-    node_sum(devs, part, out_counts, total);       // mergeGroupCounts executor.go:3728
-    return FBGPU_OK;
 } FBGPU_CATCH
 
 // Sum / Min / Max of an int field: per-device partials merged as ValCount.Add / Smaller / Larger do (executor.go:8446-8560)
@@ -287,7 +268,6 @@ static inline uint64_t node_rd64(const uint8_t* p) { uint64_t v; memcpy(&v, p, 8
 extern "C" int fbgpu_node_row(fbgpu_node* n, uint32_t index, const fbgpu_op* ops, int32_t n_ops, const uint64_t* shards, int64_t n_shards,
                               uint8_t* out_buf, uint64_t out_cap, uint64_t* out_len, uint64_t* out_count) try {
     if (!n || !out_len || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "null argument");
-    n->queries.fetch_add(1, std::memory_order_relaxed);
     NodeSplit sp = node_split(n, shards, n_shards);
     std::vector<int> devs = node_owners(sp);
     if (devs.empty()) devs.push_back(0);

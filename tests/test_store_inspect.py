@@ -101,10 +101,96 @@ def test_queries_are_refused_without_a_device():
     ctx.load_fragment(0, 1, 0, 0, D.fragment(1, 0, [0, 1], 0.01))
     row = [L.Op(L.OP_ROW, 1, 0, 0, 0, 0, 0, 0)]
     for call in (lambda: ctx.count(0, row, [0]), lambda: ctx.row(0, row, [0]), lambda: ctx.row_counts(0, 1, 0, [0]),
-                 lambda: ctx.count_pairs(0, 1, 0, [0], 1, 0, [1], [0]), lambda: ctx.groupby(0, [1, 1], [0, 0], [[0], [1]], [0])):
+                 lambda: ctx.count_pairs(0, 1, 0, [0], 1, 0, [1], [0]), lambda: ctx.groupby(0, [1, 1], [0, 0], [[0], [1]], [0]),
+                 lambda: ctx.columns(0, row, [0]), lambda: ctx.extract(0, 2, 0, 8, [0], filter_ops=row), lambda: ctx.bsi_sum(0, 2, 0, 8, [0]),
+                 lambda: ctx.bsi_minmax(0, 2, 0, 8, [0], True), lambda: ctx.bsi_select(0, 2, 0, 8, [0], [0]), lambda: ctx.any(0, row, [0]),
+                 lambda: ctx.pair_types(0, 1, 0, 0, 1, 0, 1, [0]), lambda: ctx.row_counts(0, 1, 0, [0], row_ids=[0, 1], filter_ops=row),
+                 lambda: ctx.row_counts_per_shard(0, 1, 0, [0], [0, 1])):
         with pytest.raises(L.FbgpuError) as e:
             call()
         assert e.value.code == L.E_CUDA and "no device" in str(e.value)
+
+
+def test_query_argument_errors_without_a_device():
+    """every query entry point rejects bad arguments with FBGPU_E_INVALID before it looks for a device, so the same table holds
+    on a box without one; fbgpu_row_counts_per_shard answers an empty matrix before the device check"""
+    import ctypes as C
+    ctx = L.Context(L.DEVICE_NONE)
+    node = L.Node([L.DEVICE_NONE, L.DEVICE_NONE], 1)
+    lib, h = ctx.L, ctx.h
+    op = L.ops_array([L.Op(L.OP_ROW, 1, 0, 0, 0, 0, 0, 0)])
+    sh, rows, out = _u64([0]), _u64([0, 1]), _u64([0] * 64)
+    u64, i64, i32 = C.c_uint64(0), C.c_int64(0), C.c_int32(0)
+    p, u, v, w = sh.ctypes.data, C.byref(u64), C.byref(i64), C.byref(i32)
+    null = "null argument"
+    fields, views, nrow = np.ones(9, dtype=np.uint32), np.zeros(9, dtype=np.uint32), np.ones(9, dtype=np.int32)
+    big = np.asarray([65536], dtype=np.int32)
+    cases = [
+        ("count null total", lib.fbgpu_count, (h, 0, op, 1, p, 1, None, None), null),
+        ("count n_shards<0", lib.fbgpu_count, (h, 0, op, 1, p, -1, u, None), null),
+        ("count null shards", lib.fbgpu_count, (h, 0, op, 1, None, 1, u, None), null),
+        ("any null out", lib.fbgpu_any, (h, 0, op, 1, p, 1, None), null),
+        ("any n_shards<0", lib.fbgpu_any, (h, 0, op, 1, p, -1, w), null),
+        ("row null len", lib.fbgpu_row, (h, 0, op, 1, p, 1, None, 0, None, None), null),
+        ("row n_shards<0", lib.fbgpu_row, (h, 0, op, 1, p, -1, None, 0, u, None), null),
+        ("columns null n", lib.fbgpu_columns, (h, 0, op, 1, p, 1, 0, -1, out.ctypes.data, 8, None, None), null),
+        ("columns n_shards<0", lib.fbgpu_columns, (h, 0, op, 1, p, -1, 0, -1, out.ctypes.data, 8, u, None), null),
+        ("columns null cols", lib.fbgpu_columns, (h, 0, op, 1, p, 1, 0, -1, None, 8, u, None), null),
+        ("extract null n", lib.fbgpu_extract, (h, 0, None, 0, 2, 0, 8, p, 1, 0, -1, out.ctypes.data, out.ctypes.data, 8, None, None), null),
+        ("extract n_shards<0", lib.fbgpu_extract, (h, 0, None, 0, 2, 0, 8, p, -1, 0, -1, out.ctypes.data, out.ctypes.data, 8, u, None), null),
+        ("extract null vals", lib.fbgpu_extract, (h, 0, None, 0, 2, 0, 8, p, 1, 0, -1, out.ctypes.data, None, 8, u, None), null),
+        ("extract null ops", lib.fbgpu_extract, (h, 0, None, 1, 2, 0, 8, p, 1, 0, -1, out.ctypes.data, out.ctypes.data, 8, u, None), null),
+        ("extract depth 65", lib.fbgpu_extract, (h, 0, None, 0, 2, 0, 65, p, 1, 0, -1, out.ctypes.data, out.ctypes.data, 8, u, None), "bit depth 65 outside 0..64"),
+        ("minmax null val", lib.fbgpu_bsi_minmax, (h, 0, None, 0, 2, 0, 8, p, 1, 1, None, u), null),
+        ("minmax n_shards<0", lib.fbgpu_bsi_minmax, (h, 0, None, 0, 2, 0, 8, p, -1, 1, v, u), null),
+        ("minmax null ops", lib.fbgpu_bsi_minmax, (h, 0, None, 1, 2, 0, 8, p, 1, 1, v, u), null),
+        ("minmax depth 65", lib.fbgpu_bsi_minmax, (h, 0, None, 0, 2, 0, 65, p, 1, 1, v, u), "bit depth 65 outside 0..64"),
+        ("sum null count", lib.fbgpu_bsi_sum, (h, 0, None, 0, 2, 0, 8, p, 1, v, None), null),
+        ("sum n_shards<0", lib.fbgpu_bsi_sum, (h, 0, None, 0, 2, 0, 8, p, -1, v, u), null),
+        ("sum null ops", lib.fbgpu_bsi_sum, (h, 0, None, 1, 2, 0, 8, p, 1, v, u), null),
+        ("sum depth 65", lib.fbgpu_bsi_sum, (h, 0, None, 0, 2, 0, 65, p, 1, v, u), "bit depth 65 outside 0..64"),
+        ("select null total", lib.fbgpu_bsi_select, (h, 0, None, 0, 2, 0, 8, p, 1, rows.ctypes.data, 1, out.ctypes.data, None, None), null),
+        ("select n_shards<0", lib.fbgpu_bsi_select, (h, 0, None, 0, 2, 0, 8, p, -1, rows.ctypes.data, 1, out.ctypes.data, None, u), null),
+        ("select null ops", lib.fbgpu_bsi_select, (h, 0, None, 1, 2, 0, 8, p, 1, rows.ctypes.data, 1, out.ctypes.data, None, u), null),
+        ("select null ranks", lib.fbgpu_bsi_select, (h, 0, None, 0, 2, 0, 8, p, 1, None, 1, out.ctypes.data, None, u), null),
+        ("select depth 64", lib.fbgpu_bsi_select, (h, 0, None, 0, 2, 0, 64, p, 1, rows.ctypes.data, 1, out.ctypes.data, None, u), "bit depth 64 outside 0..63"),
+        ("select 9 ranks", lib.fbgpu_bsi_select, (h, 0, None, 0, 2, 0, 8, p, 1, out.ctypes.data, 9, out.ctypes.data, None, u), "9 ranks: at most 8 per call"),
+        ("row_counts null out", lib.fbgpu_row_counts, (h, 0, 1, 0, rows.ctypes.data, 2, None, 0, p, 1, None, None, 2, w), null),
+        ("row_counts n_shards<0", lib.fbgpu_row_counts, (h, 0, 1, 0, rows.ctypes.data, 2, None, 0, p, -1, None, out.ctypes.data, 2, w), null),
+        ("row_counts n_rows<0", lib.fbgpu_row_counts, (h, 0, 1, 0, rows.ctypes.data, -1, None, 0, p, 1, None, out.ctypes.data, 2, w), null),
+        ("per_shard null out", lib.fbgpu_row_counts_per_shard, (h, 0, 1, 0, rows.ctypes.data, 2, None, 0, p, 1, None), null),
+        ("per_shard null rows", lib.fbgpu_row_counts_per_shard, (h, 0, 1, 0, None, 2, None, 0, p, 1, out.ctypes.data), null),
+        ("per_shard n_shards<0", lib.fbgpu_row_counts_per_shard, (h, 0, 1, 0, rows.ctypes.data, 2, None, 0, p, -1, out.ctypes.data), null),
+        ("per_shard null ops", lib.fbgpu_row_counts_per_shard, (h, 0, 1, 0, rows.ctypes.data, 2, None, 1, p, 1, out.ctypes.data), null),
+        ("pairs null out", lib.fbgpu_count_pairs, (h, 0, 1, 0, rows.ctypes.data, 1, 0, rows.ctypes.data, 2, p, 1, None), null),
+        ("pairs null rows", lib.fbgpu_count_pairs, (h, 0, 1, 0, None, 1, 0, rows.ctypes.data, 2, p, 1, out.ctypes.data), null),
+        ("pairs n_shards<0", lib.fbgpu_count_pairs, (h, 0, 1, 0, rows.ctypes.data, 1, 0, rows.ctypes.data, 2, p, -1, out.ctypes.data), null),
+        ("pair_types null out", lib.fbgpu_pair_types, (h, 0, 1, 0, 0, 1, 0, 1, p, 1, None), null),
+        ("pair_types n_shards<0", lib.fbgpu_pair_types, (h, 0, 1, 0, 0, 1, 0, 1, p, -1, out.ctypes.data), null),
+        ("groupby null out", lib.fbgpu_groupby, (h, 0, fields.ctypes.data, views.ctypes.data, 2, rows.ctypes.data, nrow.ctypes.data, None, 0, p, 1, None), "bad argument"),
+        ("groupby 0 fields", lib.fbgpu_groupby, (h, 0, fields.ctypes.data, views.ctypes.data, 0, rows.ctypes.data, nrow.ctypes.data, None, 0, p, 1, out.ctypes.data), "bad argument"),
+        ("groupby 9 fields", lib.fbgpu_groupby, (h, 0, fields.ctypes.data, views.ctypes.data, 9, rows.ctypes.data, nrow.ctypes.data, None, 0, p, 1, out.ctypes.data), "bad argument"),
+        ("groupby n_shards<0", lib.fbgpu_groupby, (h, 0, fields.ctypes.data, views.ctypes.data, 2, rows.ctypes.data, nrow.ctypes.data, None, 0, p, -1, out.ctypes.data), "bad argument"),
+        # (the context form checks n_rows after the device check; the node form checks it before fanning out)
+        ("node groupby n_rows 65536", lib.fbgpu_node_groupby, (node.h, 0, fields.ctypes.data, views.ctypes.data, 1, rows.ctypes.data, big.ctypes.data, None, 0, p, 1, out.ctypes.data),
+         "n_rows[0]=65536 out of range"),
+        ("node groupby 9 fields", lib.fbgpu_node_groupby, (node.h, 0, fields.ctypes.data, views.ctypes.data, 9, rows.ctypes.data, nrow.ctypes.data, None, 0, p, 1, out.ctypes.data), "bad argument"),
+        ("node pairs n_pairs<0", lib.fbgpu_node_count_pairs, (node.h, 0, 1, 0, rows.ctypes.data, 1, 0, rows.ctypes.data, -1, p, 1, out.ctypes.data), null),
+        ("node row_counts null ids", lib.fbgpu_node_row_counts, (node.h, 0, 1, 0, None, 2, None, 0, p, 1, out.ctypes.data), null),
+    ]
+    for name, fn, args, msg in cases:
+        rc = fn(*args)
+        assert rc == L.E_INVALID, (name, rc, lib.fbgpu_last_error())
+        assert lib.fbgpu_last_error().decode() == msg, name
+    # an empty matrix is answered before the device check
+    for n_rows, n_shards in ((0, 1), (2, 0)):
+        assert lib.fbgpu_row_counts_per_shard(h, 0, 1, 0, rows.ctypes.data, n_rows, None, 0, p, n_shards, out.ctypes.data) == 0
+    node.close()
+    ctx.close()
+
+
+def _u64(x):
+    return np.ascontiguousarray(np.asarray(x, dtype=np.uint64))
 
 
 def test_rbf_loader_end_to_end():

@@ -1459,3 +1459,62 @@ def test_multi_batch_paths(monkeypatch):
     test_filter_sample_goldens()
     test_topn_cutoffs_random()
     test_row_counts_per_shard_entry_point()
+
+
+def test_launch_and_query_counts(monkeypatch):
+    """kernel_launches / queries of one call to each query entry point, one shard per batch (FBGPU_UNIT_BATCH=16): what
+    bench.py's gpu_launches and the per-call counters report.  Then the two calls that answer an empty request after the device
+    check without committing the pending load."""
+    import ctypes as C
+    import featurebase_b200.datagen as D
+    monkeypatch.setenv("FBGPU_UNIT_BATCH", "16")
+    ctx = L.Context(0)
+    shards = [0, 1, 2]
+    for s in shards:
+        ctx.load_fragment(0, 1, 0, s, D.fragment(1, s, [0, 1, 2, 3], 0.002))
+        ctx.load_fragment(0, 3, 0, s, D.fragment(3, s, [0, 1], 0.02))
+        ctx.load_fragment(0, 2, 0, s, D.fragment(2, s, list(range(10)), 0.002))      # an int field of depth 8: exists, sign, 8 planes
+    ctx.commit()
+    row = lambda f, r: L.Op(L.OP_ROW, f, 0, 0, r, 0, 0, 0)
+    inter = L.Op(L.OP_INTERSECT, 0, 0, 2, 0, 0, 0, 0)
+    union = [row(1, 0), row(1, 1), L.Op(L.OP_UNION, 0, 0, 2, 0, 0, 0, 0)]
+    filt = [row(3, 0)]
+
+    def delta(call):
+        before = ctx.counters()
+        call()
+        after = ctx.counters()
+        return after["kernel_launches"] - before["kernel_launches"], after["queries"] - before["queries"]
+    calls = {
+        "count": lambda: ctx.count(0, [row(1, 0), row(1, 1), inter], shards),
+        "count_eval": lambda: ctx.count(0, union, shards),
+        "any": lambda: ctx.any(0, union, shards),
+        "row": lambda: ctx.row(0, union, shards),
+        "columns": lambda: ctx.columns(0, union, shards),
+        "extract": lambda: ctx.extract(0, 2, 0, 8, shards, filter_ops=filt),
+        "bsi_sum": lambda: ctx.bsi_sum(0, 2, 0, 8, shards, filter_ops=filt),
+        "bsi_minmax": lambda: ctx.bsi_minmax(0, 2, 0, 8, shards, True),
+        "bsi_select": lambda: ctx.bsi_select(0, 2, 0, 8, shards, [0, 3]),
+        "row_counts": lambda: ctx.row_counts(0, 1, 0, shards, row_ids=[0, 1, 2], filter_ops=filt),
+        "count_pairs": lambda: ctx.count_pairs(0, 1, 0, [0, 1], 3, 0, [0, 1], shards),
+        "groupby2": lambda: ctx.groupby(0, [1, 3], [0, 0], [[0, 1, 2], [0, 1]], shards),
+        "groupby3": lambda: ctx.groupby(0, [1, 3, 1], [0, 0, 0], [[0, 1], [0, 1], [2, 3]], shards),
+    }
+    got = {name: delta(call) for name, call in calls.items()}
+    # row / columns: eval + emit per batch; extract: + the value gather; bsi_sum / bsi_minmax: eval + plane kernel per batch;
+    # bsi_select: eval per batch + (step, decide) per 4-bit digit of the 9-bit key; filtered row_counts: eval + count per batch;
+    # GroupBy: groupby_direct_kernel + groupby_kernel for the units it declines (field 3's containers are too large for it),
+    # behind a filter eval per batch for 3 fields, which run one 2-field pass per row of the first field
+    assert got == {"count": (1, 1), "count_eval": (1, 1), "any": (1, 1), "row": (6, 1), "columns": (6, 1), "extract": (9, 1),
+                   "bsi_sum": (6, 1), "bsi_minmax": (6, 1), "bsi_select": (9, 1), "row_counts": (6, 1), "count_pairs": (1, 1),
+                   "groupby2": (2, 1), "groupby3": (18, 2)}, got
+    # a load that is not committed yet: an empty request is answered without committing it
+    ctx.load_fragment(0, 1, 0, 5, D.fragment(1, 5, [0], 0.002))
+    commits = lambda: ctx.stats()["full_commits"] + ctx.stats()["patch_commits"]
+    before, counters = commits(), ctx.counters()
+    one = np.zeros(1, dtype=np.uint64)
+    assert ctx.L.fbgpu_count_pairs(ctx.h, 0, 1, 0, one.ctypes.data, 1, 0, one.ctypes.data, 0, one.ctypes.data, 1, one.ctypes.data) == 0
+    assert ctx.pair_types(0, 1, 0, 0, 1, 0, 1, []).sum() == 0
+    assert commits() == before
+    assert ctx.counters()["queries"] == counters["queries"] and ctx.counters()["kernel_launches"] == counters["kernel_launches"]
+    ctx.close()
