@@ -8,6 +8,8 @@
   config X: fbgpu_columns / fbgpu_extract (device-side column-id and int-value expansion), wall clock; R: fbgpu_row.
   config P: Percentile over config X's 32-bit field, order statistics (fbgpu_bsi_select) against the query-driven bisection
             (only when named in --configs).
+  config V: GroupBy(Rows(a), Rows(v)) with v an int field of 64 / 1000 / 65535 distinct values, fbgpu_groupby_values against the
+            Row(v == value)-per-value composition (only when named in --configs).
 Every point is spot-checked against the CPU oracle on a few shards (the checker, not the thing measured)."""
 import argparse
 import json
@@ -268,6 +270,92 @@ def config_percentile(args, out):
     real.close()
 
 
+class _NoGroupByValues(_KernelMs):
+    """the same proxy without groupby_values: the executor takes the Row(v == value)-per-value composition"""
+
+    def __getattr__(self, name):
+        if name == "groupby_values":
+            raise AttributeError(name)
+        return super().__getattr__(name)
+
+
+def config_groupby_values(args, out):
+    """GroupBy(Rows(a), Rows(v)) over --groupby-shards shards: int fields v holding one of D values (uniform) for each of the first
+    16,384 columns of every shard, D in {64, 1000, 65535}, and a 256-row set field a at 1/256 density per row, without and with a
+    1 % filter row, through the executor.  The device arm (one fbgpu_groupby_values) runs at every D.  The composition arm (one
+    Row(v == value) and one scratch-row load per value, then fbgpu_groupby) runs only for the unfiltered query at D = 64, for
+    --composition-steps steps alternated with the device arm, every one of them reported (no warm-up): it adds D scratch rows to
+    the store every step, so each step is slower than the one before (at 512 shards on an H100: about 97 s, 266 s, 387 s).  Both
+    arms must return the same groups; every result's total must equal Σ_r Count(Row(a=r) ∩ filter ∩ exists(v)).  Progress goes
+    to stderr."""
+    from featurebase_b200 import datagen as D, executor as X
+    S = args.groupby_shards
+    n_cols = 16384
+    shards = np.arange(S, dtype=np.uint64)
+    h = X.Holder()
+    idx = h.create_index("i", track_existence=False)
+    fa, ff = idx.create_field("a"), idx.create_field("f")
+    dvals = (64, 1000, 65535)
+    t0 = time.time()
+    for fld, rows, p in ((fa, range(256), 1 / 256), (ff, [0], 0.01)):
+        bulk = D.fragments(40 + fld.id, shards, list(rows), p)
+        h.ctx.load_fragments(idx.id, fld.id, X.VIEW_STANDARD, shards, bulk.buf, bulk.offsets)
+        h.ctx.commit()
+        del bulk
+    for k, d in enumerate(dvals):
+        f = idx.create_field(f"v{d}", "int", min=0, max=d - 1)
+        for s in range(S):
+            h.ctx.load_fragment(idx.id, f.id, X.VIEW_BSI, s, D.bsi_fragment(50 + k, s, n_cols, f.bit_depth, 0, d - 1))
+        h.ctx.commit()
+    idx.shards.update(range(S))
+    load_s = time.time() - t0
+    print(f"config V: loaded {S} shards in {load_s:.1f}s", file=sys.stderr, flush=True)
+    real = h.ctx
+    from featurebase_b200 import lib as L
+    n_rec = S * n_cols
+    dev = _KernelMs(real)
+    comp = _NoGroupByValues(real)
+    for d in dvals:
+        for q_filter in (False, True):
+            q = f"GroupBy(Rows(a), Rows(v{d})" + (", filter=Row(f=0))" if q_filter else ")")
+            exists = [L.Op(L.OP_ROW, idx.fields[f"v{d}"].id, X.VIEW_BSI, 0, 0, 0, 0, 0)]
+            if q_filter:
+                exists += [L.Op(L.OP_ROW, ff.id, X.VIEW_STANDARD, 0, 0, 0, 0, 0), L.Op(L.OP_INTERSECT, 0, 0, 2, 0, 0, 0, 0)]
+            want = int(real.row_counts(idx.id, fa.id, X.VIEW_STANDARD, list(range(S)), row_ids=list(range(256)), filter_ops=exists).sum())
+            arms = {"device": dev} if d != 64 or q_filter or args.composition_steps < 1 else {"device": dev, "composition": comp}
+            rec = {name: {"wall": [], "kernel_ms": [], "queries": []} for name in arms}
+            res = {}
+            for i in range(1 + args.steps):                  # one warm-up round of the device arm, then alternate the arms
+                for name in (sorted(arms) if i % 2 == 0 else sorted(arms, reverse=True)):
+                    if name == "composition" and len(rec[name]["wall"]) >= args.composition_steps:
+                        continue
+                    h.ctx = arms[name]
+                    q0, arms[name].ms = real.counters()["queries"], 0.0
+                    t1 = time.perf_counter()
+                    r = X.Executor(h).execute("i", q)[0]
+                    wall = (time.perf_counter() - t1) * 1e3
+                    res.setdefault(name, r)
+                    assert r == res[name], (q, name)
+                    print(f"config V: {q} {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                    if i >= 1 or name == "composition":
+                        rec[name]["wall"].append(wall)
+                        rec[name]["kernel_ms"].append(arms[name].ms)
+                        rec[name]["queries"].append(real.counters()["queries"] - q0)
+            h.ctx = real
+            assert all(r == res["device"] for r in res.values()), q
+            assert sum(g[1] for g in res["device"]) == want, (q, want)
+            for name, dd in rec.items():
+                o = {"config": "V", "query": q, "arm": name, "distinct_values": d, "shards": S, "records": n_rec, "groups": len(res[name]),
+                     "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])), "wall_ms_max": float(np.max(dd["wall"])),
+                     "kernel_ms": float(np.median(dd["kernel_ms"])), "queries": int(np.median(dd["queries"])), "steps": args.steps, "load_s": round(load_s, 1),
+                     "kernel": "eval_kernel + groupby_values_kernel" if name == "device" else "eval_kernel (Row(v == value) per value) + groupby kernels",
+                     "note": "median over the timed steps of the executor call (wall clock, Distinct and Rows pre-passes included) and of the summed last_query_gpu_ms of its library queries"}
+                if name == "composition":
+                    o["wall_ms_per_step"], o["steps"] = [round(x, 2) for x in dd["wall"]], len(dd["wall"])
+                out(o)
+    real.close()
+
+
 def config3(args, out, n_rec=10_000_000, nf=4):
     """nf fields are rotated between steps so that the touched planes exceed L2 (the 10 M-record config is 42.5 MB)"""
     from featurebase_b200 import datagen as D, executor as X, pql
@@ -362,6 +450,7 @@ def main():
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--shards", type=int, default=1024)
     ap.add_argument("--groupby-shards", type=int, default=512)
+    ap.add_argument("--composition-steps", type=int, default=1, help="config V: steps of the composition arm (each one slower than the last)")
     ap.add_argument("--generators", default="uniform,clustered")
     ap.add_argument("--batched", action="store_true", help="also time the multi-pair launch (config 5b)")
     ap.add_argument("--densities", default="0.0001,0.001,0.01,0.03,0.0625,0.125,0.25,0.5")
@@ -378,6 +467,8 @@ def main():
             config_extract(args, out)
         elif c == "P":
             config_percentile(args, out)
+        elif c == "V":
+            config_groupby_values(args, out)
         elif c == "3L":     # the same BSI query at 256 shards (268 M records, 1.1 GB of planes): shows the kernel away from the launch-bound regime
             config3(args, out, n_rec=256 * SW, nf=1)
         else:

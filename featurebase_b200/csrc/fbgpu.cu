@@ -1780,6 +1780,86 @@ extern "C" int fbgpu_groupby(fbgpu_ctx* c, uint32_t index, const uint32_t* field
     return groupby_rec(c, index, fields, views, n_fields, rows.data(), n_rows, f, shards, n_shards, out_counts);
 } FBGPU_CATCH
 
+// ------------------------------------------------------------------ GroupBy over the values of an int field
+// the int dimension of fbgpu_groupby_values: field, view, depth and the ascending stored values that are its groups
+struct GvInt { uint32_t field, view; int32_t depth; const int64_t* values; int32_t n_values; };
+
+// the argument checks fbgpu_groupby_values and its node form make before any device is touched
+static int groupby_values_args(const void* handle, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
+                               const int32_t* n_rows, int32_t bit_depth, const int64_t* values, int32_t n_values, const fbgpu_op* filter,
+                               int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts) {
+    if (!handle || !values || !out_counts || n_fields < 0 || n_fields > 7 || (n_fields && (!fields || !views || !row_ids_flat || !n_rows)) ||
+        n_filter_ops < 0 || (n_filter_ops && !filter) || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
+    if (bit_depth < 0 || bit_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", bit_depth);
+    if (n_values < 1 || n_values > 65535) return fail(FBGPU_E_INVALID, "n_values=%d outside 1..65535", n_values);
+    for (int32_t i = 1; i < n_values; i++)
+        if (values[i] <= values[i - 1]) return fail(FBGPU_E_INVALID, "values are not strictly ascending at position %d", i);
+    return 0;
+}
+
+// one groupby_values_kernel pass over the shards: counts[nB or 1][n_values] of consider = filter ∩ exists(v) (∩ Row(b = row))
+static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, uint32_t fvB, const uint64_t* rowsB, int nB, const GvInt& v,
+                               const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards, uint64_t* out) {
+    const std::vector<fbgpu_op> full = and_row(filter.data(), (int32_t)filter.size(), v.field, v.view, 0);
+    Query q(c); Workspace* w = q.w;
+    int rc = q.open(index, full.data(), (int32_t)full.size(), shards, n_shards); if (rc) return rc;
+    const uint32_t fvV = view_id_locked(c, ViewKey{ index, v.field, v.view }, false);
+    const size_t ncnt = (size_t)(rowsB ? nB : 1) * (size_t)v.n_values;
+    if (w->d_rows.ensure(((size_t)nB + (size_t)v.n_values) * 8) || w->d_counts.ensure(ncnt * 8) || w->h_out.ensure(ncnt * 8)) return FBGPU_E_NOMEM;
+    std::vector<uint64_t> in(v.values, v.values + v.n_values);      // [values (as int64) | b rows]
+    if (rowsB) in.insert(in.end(), rowsB, rowsB + nB);
+    CUDA_TRY(cudaMemcpyAsync(w->d_rows.p, in.data(), in.size() * 8, cudaMemcpyHostToDevice, w->stream));
+    CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, ncnt * 8, w->stream));
+    CUDA_TRY(cudaStreamSynchronize(w->stream));   // `in` is a local
+    const long long* d_values = (const long long*)w->d_rows.p;
+    const uint64_t* d_rowsB = rowsB ? (const uint64_t*)w->d_rows.p + v.n_values : nullptr;
+    CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
+    for (long long u0 = 0; u0 < q.n_units; u0 += c->unit_batch) {
+        const long long nu = std::min(c->unit_batch, q.n_units - u0);
+        rc = q.eval(u0, nu); if (rc) return rc;
+        const long long grid = std::min<long long>(nu, (long long)c->sm_count * kGvCtasPerSm);
+        groupby_values_kernel<<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), fvV, v.depth, d_values, v.n_values, fvB, d_rowsB, nB,
+                                                                            (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, (unsigned long long*)w->d_counts.p);
+        CUDA_TRY(cudaGetLastError()); q.launches++;
+    }
+    CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+    rc = allreduce_u64(c, w, w->d_counts.p, ncnt); if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, ncnt * 8, cudaMemcpyDeviceToHost, w->stream));
+    CUDA_TRY(cudaStreamSynchronize(w->stream));
+    memcpy(out, w->h_out.p, ncnt * 8);
+    q.add_elapsed();
+    q.finish();
+    return 0;
+}
+
+// set dimensions beyond the last are peeled into the filter as groupby_rec does; the last one (if any) is the kernel's b
+static int groupby_values_rec(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int nf, const uint64_t* const* rows, const int32_t* n_rows,
+                              const GvInt& v, const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards, uint64_t* out) {
+    if (nf == 0) return groupby_values_leaf(c, index, kNoView, nullptr, 0, v, filter, shards, n_shards, out);
+    if (nf == 1) return groupby_values_leaf(c, index, view_id_locked(c, ViewKey{ index, fields[0], views[0] }, false), rows[0], n_rows[0], v, filter, shards, n_shards, out);
+    size_t sub = (size_t)v.n_values; for (int i = 1; i < nf; i++) sub *= (size_t)n_rows[i];
+    for (int r = 0; r < n_rows[0]; r++) {
+        int rc = groupby_values_rec(c, index, fields + 1, views + 1, nf - 1, rows + 1, n_rows + 1, v, and_row(filter.data(), (int32_t)filter.size(), fields[0], views[0], rows[0][r]),
+                                    shards, n_shards, out + (size_t)r * sub); if (rc) return rc;
+    }
+    return 0;
+}
+
+extern "C" int fbgpu_groupby_values(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
+                                    const int32_t* n_rows, uint32_t vfield, uint32_t vview, int32_t bit_depth, const int64_t* values, int32_t n_values,
+                                    const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
+    int rc = groupby_values_args(c, fields, views, n_fields, row_ids_flat, n_rows, bit_depth, values, n_values, filter, n_filter_ops, shards, n_shards, out_counts);
+    if (rc) return rc;
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    std::vector<const uint64_t*> rows((size_t)n_fields); const uint64_t* p = row_ids_flat; size_t total = (size_t)n_values;
+    for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); rows[(size_t)i] = p; p += n_rows[i]; total *= (size_t)n_rows[i]; }
+    memset(out_counts, 0, total * 8);
+    if (total == 0) return 0;
+    const GvInt v{ vfield, vview, bit_depth, values, n_values };
+    return groupby_values_rec(c, index, fields, views, n_fields, rows.data(), n_rows, v, std::vector<fbgpu_op>(filter, filter + n_filter_ops), shards, n_shards, out_counts);
+} FBGPU_CATCH
+
 // ------------------------------------------------------------------ comm
 extern "C" int fbgpu_comm_unique_id(uint8_t id[FBGPU_NCCL_ID_BYTES]) try {
     if (!nccl_load()) return fail(FBGPU_E_COMM, "libnccl.so.2 not loadable: %s", dlerror());

@@ -1865,6 +1865,146 @@ groupby_direct_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ ro
 }
 
 // ------------------------------------------------------------------------------------------------
+// groupby_values_kernel (fbgpu_groupby_values): GroupBy whose last dimension is the values of an int field, optionally after one
+// set field b — counts[b-row][j] += |{columns of consider ∩ Row(b = b-row) whose stored value is values[j]}|, or counts[j] without
+// b.  consider = filter ∩ exists(v), one 8 KiB bitmap per (shard, slot) unit from eval_kernel.  The groups of an int field are
+// its values (groupByIterator with FieldRow.Value, executor.go:8740-8750); the reference reaches each one through a
+// Row(v == value) plane sweep.  Here one CTA per unit walks the unit in ranges of kGvRange columns, skipping a range without a
+// consider bit, and for each range:
+//   1. assembles every consider column's magnitude (one u64 per column) and sign from the planes, one warp per plane;
+//   2. maps each column's stored value (sign ? -magnitude : magnitude, wrapping like fbgpu_extract) to its position in the
+//      ascending `values` by binary search, kGvNone when absent.  Sign set with magnitude 0 is no value: Row(v == 0) does not
+//      hold such a column;
+//   3. walks b's rows restricted to the range (a warp per row, the rows resolved 32 at a time by the lanes) and adds 1 per
+//      column with a value; without b, the counts of the first kGvHist values are summed in shared memory per unit.
+// Each plane and b-row container is read once per range it meets: a bitmap word by word, a run container from the first
+// interval that reaches the range (intervals are sorted), an array in full, because array payloads may be stored in the
+// bank-striped order of stripe.h, which no search can use.  47 KiB of shared memory: four CTAs per SM.
+// A shard missing the int field's fragment has an empty consider set, one missing b's fragment resolves no b-row: either
+// contributes nothing (executor.go:8769-8772).
+// ------------------------------------------------------------------------------------------------
+constexpr int kGvThreads = 256;
+constexpr int kGvCtasPerSm = 4;
+constexpr uint32_t kGvRange = 4096;                // columns per range
+constexpr int kGvRangeWords = (int)kGvRange / 64;
+constexpr int kGvHist = 1024;
+constexpr uint16_t kGvNone = 0xffff;
+
+// calls f(local column) for every column of [lo, lo + kGvRange) that is in the container and in the range's consider words
+// `cons`; warp-wide (every lane with the same r), the lanes share the work
+template <class F>
+__device__ __forceinline__ void gv_for_each(const Resolved& r, uint32_t lo, const unsigned long long* cons, int lane, F f) {
+    if (r.ptr == nullptr) return;
+    if (r.typ == kBitmap) {
+        const uint64_t* g = reinterpret_cast<const uint64_t*>(r.ptr) + (lo >> 6);
+        for (int i = lane; i < kGvRangeWords; i += 32) {
+            uint64_t v = __ldg(g + i) & cons[i];
+            while (v) { const int b = __ffsll((long long)v) - 1; f((uint32_t)i * 64 + (uint32_t)b); v &= v - 1; }
+        }
+    } else if (r.typ == kArray) {
+        const uint16_t* a = reinterpret_cast<const uint16_t*>(r.ptr);
+        for (uint32_t i = lane; i < r.card; i += 32) {
+            const uint32_t v = (uint32_t)__ldg(a + i) - lo;                 // outside the range: >= kGvRange (unsigned)
+            if (v < kGvRange && ((cons[v >> 6] >> (v & 63)) & 1ull)) f(v);
+        }
+    } else {
+        const uint32_t* r32 = reinterpret_cast<const uint32_t*>(r.ptr);    // {u16 start, u16 last} per interval
+        const uint32_t hi = lo + kGvRange - 1;
+        uint32_t k = 0, e = r.cnt;
+        while (k < e) { const uint32_t m = (k + e) >> 1; if ((__ldg(r32 + m) >> 16) < lo) k = m + 1; else e = m; }
+        for (; k < r.cnt; k++) {
+            const uint32_t iv = __ldg(r32 + k), s0 = iv & 0xffffu, l0 = iv >> 16;
+            if (s0 > hi) break;
+            const uint32_t s = max(s0, lo) - lo, l = min(l0, hi) - lo;
+            for (uint32_t i = (s >> 6) + lane; i <= (l >> 6); i += 32) {
+                uint64_t m = cons[i];
+                if (i == (s >> 6)) m &= ~0ull << (s & 63);
+                if (i == (l >> 6)) m &= ~0ull >> (63 - (l & 63));
+                while (m) { const int b = __ffsll((long long)m) - 1; f(i * 64 + (uint32_t)b); m &= m - 1; }
+            }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kGvThreads, kGvCtasPerSm)
+groupby_values_kernel(StoreRef st, uint32_t fvV, int depth, const long long* __restrict__ values, int n_values,
+                      uint32_t fvB, const uint64_t* __restrict__ rowsB /* null: no set field */, int nB,
+                      const uint4* __restrict__ consider, const uint64_t* __restrict__ shards, long long n_units,
+                      unsigned long long* __restrict__ counts /* [nB or 1][n_values], zeroed by the host */) {
+    __shared__ unsigned long long mag[kGvRange];
+    __shared__ uint16_t vidx[kGvRange];
+    __shared__ uint32_t sign[kGvRange / 32];
+    __shared__ unsigned long long cons[kGvRangeWords];
+    __shared__ Resolved planes[65];                   // sign row, then magnitude bits 0 .. depth - 1
+    __shared__ uint32_t hist[kGvHist];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nwarps = kGvThreads / 32;
+    const int n_hist = rowsB ? 0 : min(n_values, kGvHist);
+    for (long long unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
+        const uint64_t shard = shards[unit >> 4];
+        const int slot = (int)(unit & 15);
+        const uint64_t* cu = reinterpret_cast<const uint64_t*>(consider + (size_t)unit * 512);
+        uint64_t any = 0;
+        for (int i = tid; i < 1024; i += kGvThreads) any |= cu[i];
+        if (!__syncthreads_or(any != 0)) continue;
+        for (int p = tid; p <= depth; p += kGvThreads) planes[p] = resolve(st, fvV, shard, (uint64_t)(p + 1), slot);
+        for (int i = tid; i < n_hist; i += kGvThreads) hist[i] = 0;
+        for (uint32_t lo = 0; lo < kFull; lo += kGvRange) {
+            __syncthreads();                              // the previous range's readers are done; planes / hist are written
+            const uint64_t cw = tid < kGvRangeWords ? cu[(lo >> 6) + tid] : 0;
+            if (tid < kGvRangeWords) cons[tid] = cw;
+            if (!__syncthreads_or(cw != 0)) continue;
+            for (int i = tid; i < (int)kGvRange; i += kGvThreads) mag[i] = 0;
+            for (int i = tid; i < (int)kGvRange / 32; i += kGvThreads) sign[i] = 0;
+            __syncthreads();
+            for (int p = wid; p <= depth; p += nwarps) {
+                const Resolved r = planes[p];
+                if (p == 0) gv_for_each(r, lo, cons, lane, [&](uint32_t v) { atomicOr(&sign[v >> 5], 1u << (v & 31)); });
+                else { const unsigned long long bit = 1ull << (p - 1); gv_for_each(r, lo, cons, lane, [&](uint32_t v) { atomicOr(&mag[v], bit); }); }
+            }
+            __syncthreads();
+            for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
+                uint16_t k = kGvNone;
+                const unsigned long long m = mag[i];
+                const bool neg = (sign[i >> 5] >> (i & 31)) & 1u;
+                if (((cons[i >> 6] >> (i & 63)) & 1ull) && (m || !neg)) {
+                    const long long val = (long long)(neg ? 0ull - m : m);
+                    int a = 0, b = n_values;
+                    while (a < b) { const int h = (a + b) >> 1; if (__ldg(values + h) < val) a = h + 1; else b = h; }
+                    if (a < n_values && __ldg(values + a) == val) k = (uint16_t)a;
+                }
+                vidx[i] = k;
+            }
+            __syncthreads();
+            if (!rowsB) {
+                for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
+                    const uint32_t k = vidx[i];
+                    if (k == kGvNone) continue;
+                    if ((int)k < n_hist) atomicAdd(&hist[k], 1u);
+                    else atomicAdd(&counts[k], 1ull);
+                }
+                continue;
+            }
+            for (int b0 = wid * 32; b0 < nB; b0 += nwarps * 32) {
+                Resolved mine; mine.ptr = nullptr; mine.card = 0; mine.typ = 0; mine.cnt = 0;
+                if (b0 + lane < nB) mine = resolve(st, fvB, shard, rowsB[b0 + lane], slot);
+                const int n = min(32, nB - b0);
+                for (int j = 0; j < n; j++) {
+                    Resolved r;
+                    r.ptr = (const void*)__shfl_sync(0xffffffffu, (unsigned long long)mine.ptr, j);
+                    r.card = __shfl_sync(0xffffffffu, mine.card, j);
+                    const uint32_t meta = __shfl_sync(0xffffffffu, ((uint32_t)mine.typ << 16) | mine.cnt, j);
+                    r.typ = (uint16_t)(meta >> 16); r.cnt = (uint16_t)(meta & 0xffffu);
+                    unsigned long long* row = counts + (size_t)(b0 + j) * (size_t)n_values;
+                    gv_for_each(r, lo, cons, lane, [&](uint32_t v) { const uint32_t k = vidx[v]; if (k != kGvNone) atomicAdd(&row[k], 1ull); });
+                }
+            }
+        }
+        __syncthreads();
+        for (int i = tid; i < n_hist; i += kGvThreads) if (hist[i]) atomicAdd(&counts[i], (unsigned long long)hist[i]);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // arena_gather_kernel (fbgpu_compact): copies containers one by one from the old payload arena into the new one — one warp per
 // container, 16 bytes per lane and step.  Used for fragments that fbgpu_apply_containers left with holes.
 // ------------------------------------------------------------------------------------------------

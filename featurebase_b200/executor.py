@@ -1003,18 +1003,22 @@ class Executor:
                 raise QueryError(f"aggregate {agg.name} is not supported by this mirror")
         if any(len(r) == 0 for r in row_ids):
             return []
-        # what the device groups over: a field's standard view, or — for Rows(f, from=, to=) on a time field — one operand
-        # row per row id holding the union of that row over the covering views (timeFragmentsRowIterator :8755-8768)
-        dev_fields, dev_rows = [], []
-        for f, rows, targs in zip(fields, row_ids, time_args):
-            if targs is not None and not targs:
-                dev_fields.append(f.id)
-                dev_rows.append(rows)
-                continue
-            sf, operands = self._time_rows_as_operands(idx, f, rows, targs or {}, shards)      # (int field: Row(f == value) per value)
-            dev_fields.append(sf.id)
-            dev_rows.append(operands)
-        counts = self.ctx.groupby(idx.id, dev_fields, [VIEW_STANDARD] * len(fields), dev_rows, shards, filter_ops=filt)
+        int_dims = [k for k, f in enumerate(fields) if f.type == "int"]
+        if len(int_dims) == 1 and hasattr(self.ctx, "groupby_values"):
+            counts = self._groupby_int_counts(idx, fields, row_ids, time_args, int_dims[0], filt, shards)
+        else:
+            # what the device groups over: a field's standard view, or — for Rows(f, from=, to=) on a time field — one operand
+            # row per row id holding the union of that row over the covering views (timeFragmentsRowIterator :8755-8768)
+            dev_fields, dev_rows = [], []
+            for f, rows, targs in zip(fields, row_ids, time_args):
+                if targs is not None and not targs:
+                    dev_fields.append(f.id)
+                    dev_rows.append(rows)
+                    continue
+                sf, operands = self._time_rows_as_operands(idx, f, rows, targs or {}, shards)      # (int field: Row(f == value) per value)
+                dev_fields.append(sf.id)
+                dev_rows.append(operands)
+            counts = self.ctx.groupby(idx.id, dev_fields, [VIEW_STANDARD] * len(fields), dev_rows, shards, filter_ops=filt)
         start = self._groupby_start(c, row_ids)
         if start is None:
             return []
@@ -1071,6 +1075,31 @@ class Executor:
             for col, asc in reversed(keys):                       # stable sorts, last key first == sort.Stable on the tuple
                 out.sort(key=lambda g: (g[col] if len(g) > col else 0), reverse=not asc)
         return self._window(c, out)
+
+    GROUPBY_VALUES_MAX = 65535                                    # values per fbgpu_groupby_values call
+
+    def _groupby_int_counts(self, idx, fields, row_ids, time_args, k, filt, shards):
+        """the count tensor of a GroupBy with exactly one int child (child k), from fbgpu_groupby_values: the other children are
+        its set dimensions (a time-range child as operand rows, as above), the int child's values its last dimension, moved
+        back to position k.  No Row(v == value) per value and no scratch rows.  A longer value list than one call takes is
+        split into slices, one call each: a column's value lies in exactly one slice."""
+        dev_fields, dev_rows = [], []
+        for j, (f, rows, targs) in enumerate(zip(fields, row_ids, time_args)):
+            if j == k:
+                continue
+            if not targs:
+                dev_fields.append(f.id)
+                dev_rows.append(rows)
+                continue
+            sf, operands = self._time_rows_as_operands(idx, f, rows, targs, shards)
+            dev_fields.append(sf.id)
+            dev_rows.append(operands)
+        vf = fields[k]
+        stored = [v - vf.base for v in row_ids[k]]                 # values as the planes hold them (value - Base)
+        step = self.GROUPBY_VALUES_MAX
+        parts = [self.ctx.groupby_values(idx.id, dev_fields, [VIEW_STANDARD] * len(dev_fields), dev_rows, vf.id, VIEW_BSI, vf.bit_depth,
+                                         stored[s:s + step], shards, filter_ops=filt) for s in range(0, len(stored), step)]
+        return np.moveaxis(np.concatenate(parts, axis=-1), -1, k)
 
     @staticmethod
     def _window(c, out):                                          # applyLimitAndOffsetToGroupByResult :3441-3459

@@ -48,7 +48,8 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_any", "fbgpu_pair_types", "fbgpu_node_any", "fbgpu_apply_containers", "fbgpu_node_apply_containers",
            "fbgpu_comm_p2p_open_local", "fbgpu_node_init", "fbgpu_node_shutdown", "fbgpu_node_devices", "fbgpu_node_owner", "fbgpu_node_ctx", "fbgpu_node_load_fragment",
            "fbgpu_node_load_fragments", "fbgpu_node_load_rbf_dir", "fbgpu_node_drop_fragment", "fbgpu_node_commit", "fbgpu_node_get_stats", "fbgpu_node_count", "fbgpu_node_row",
-           "fbgpu_node_count_pairs", "fbgpu_node_row_counts", "fbgpu_node_groupby", "fbgpu_node_bsi_sum", "fbgpu_node_bsi_minmax"]
+           "fbgpu_node_count_pairs", "fbgpu_node_row_counts", "fbgpu_node_groupby", "fbgpu_node_bsi_sum", "fbgpu_node_bsi_minmax",
+           "fbgpu_groupby_values", "fbgpu_node_groupby_values"]
 
 
 def lib_path():
@@ -94,6 +95,8 @@ def load():
     L.fbgpu_row_counts.argtypes, L.fbgpu_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp, vp, i32, C.POINTER(i32)], C.c_int
     L.fbgpu_row_counts_per_shard.argtypes, L.fbgpu_row_counts_per_shard.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_groupby.argtypes, L.fbgpu_groupby.restype = [vp, u32, vp, vp, i32, vp, vp, vp, i32, vp, i64, vp], C.c_int
+    L.fbgpu_groupby_values.argtypes = [vp, u32, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i32, vp, i64, vp]
+    L.fbgpu_groupby_values.restype = C.c_int
     L.fbgpu_count_pairs.argtypes, L.fbgpu_count_pairs.restype = [vp, u32, u32, u32, vp, u32, u32, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_comm_unique_id.argtypes, L.fbgpu_comm_unique_id.restype = [vp], C.c_int
     L.fbgpu_comm_init.argtypes, L.fbgpu_comm_init.restype = [vp, i32, i32, vp], C.c_int
@@ -113,7 +116,7 @@ def load():
     L.fbgpu_node_devices.argtypes, L.fbgpu_node_devices.restype = [vp], i32
     L.fbgpu_node_owner.argtypes, L.fbgpu_node_owner.restype = [vp, u64], i32
     L.fbgpu_node_ctx.argtypes, L.fbgpu_node_ctx.restype = [vp, i32], vp
-    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "bsi_sum", "bsi_minmax"):
+    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "bsi_sum", "bsi_minmax"):
         src, dst = getattr(L, "fbgpu_" + name), getattr(L, "fbgpu_node_" + name)
         dst.argtypes, dst.restype = src.argtypes, src.restype
     L.fbgpu_node_row_counts.argtypes, L.fbgpu_node_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
@@ -409,6 +412,24 @@ class Context:
         self._check(self.L.fbgpu_groupby(self.h, index, fl.ctypes.data, vw.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
                                          f, nf, sh.ctypes.data, len(sh), out.ctypes.data))
         return out.reshape([int(x) for x in n_rows])
+
+    def groupby_values(self, index, fields, views, row_ids, vfield, vview, bit_depth, values, shards, filter_ops=None):
+        """GroupBy whose last dimension is the values of an int field (fbgpu_groupby_values): the count tensor
+        [len(row_ids[0])] ... [len(values)] over the set fields' row lists (none is fine) and the int field's strictly ascending
+        stored values (value - Base, 1..65535 of them)"""
+        sh = _u64arr(shards)
+        fl = np.ascontiguousarray(np.asarray(fields, dtype=np.uint32))
+        vw = np.ascontiguousarray(np.asarray(views, dtype=np.uint32))
+        n_rows = np.ascontiguousarray(np.asarray([len(r) for r in row_ids], dtype=np.int32))
+        flat = _u64arr(np.concatenate([np.asarray(r, dtype=np.uint64) for r in row_ids]) if len(row_ids) else [])
+        vals = np.ascontiguousarray(np.asarray(values, dtype=np.int64))
+        shape = [int(x) for x in n_rows] + [len(vals)]
+        out = np.zeros(int(np.prod(shape, dtype=np.int64)), dtype=np.uint64)
+        f = ops_array(filter_ops) if filter_ops else None
+        nf = len(filter_ops) if filter_ops else 0
+        self._check(self.L.fbgpu_groupby_values(self.h, index, fl.ctypes.data, vw.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
+                                                vfield, vview, int(bit_depth), vals.ctypes.data, len(vals), f, nf, sh.ctypes.data, len(sh), out.ctypes.data))
+        return out.reshape(shape)
 
     def rows_payload_bytes(self, index, field, view, shards, row_ids=None):
         sh = _u64arr(shards)

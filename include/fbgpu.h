@@ -260,6 +260,21 @@ int fbgpu_groupby(fbgpu_ctx *ctx, uint32_t index, const uint32_t *fields, const 
                   const fbgpu_op *filter, int32_t n_filter_ops,
                   const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
 
+/* GroupBy whose last dimension is the values of an int field: GroupBy(Rows(f1), ..., Rows(v)) with v an int field, whose groups
+ * are v's values (FieldRow.Value, executor.go:8740-8750), in one device pass instead of one Row(v == value) per value.
+ * fields / views / row_ids_flat / n_rows: n_fields (0..7) set-like dimensions, as for fbgpu_groupby (may be NULL when
+ * n_fields == 0).  vfield / vview / bit_depth (0..64): the int field's BSI view.  values: n_values (1..65535) strictly ascending
+ * stored values (value - bsiGroup.Base, as fbgpu_extract reports them; at depth 64, INT64_MIN is stored as sign + 2^63).
+ * out_counts: the dense tensor [n_rows[0]] ... [n_rows[n_fields-1]] [n_values], row-major, the int dimension last; entry
+ * (i..., j) = |{columns of filter ∩ exists(v) ∩ Row(f1 = r1_i) ∩ ... whose stored value is values[j]}|.  A column whose value is
+ * not listed is counted nowhere, nor is a column stored as sign with magnitude 0 (Row(v == 0) does not hold it).  A shard lacking
+ * the int field's fragment or any set field's fragment contributes nothing (executor.go:8769-8772).  All-reduced over the
+ * communicator. */
+int fbgpu_groupby_values(fbgpu_ctx *ctx, uint32_t index, const uint32_t *fields, const uint32_t *views, int32_t n_fields,
+                         const uint64_t *row_ids_flat, const int32_t *n_rows, uint32_t vfield, uint32_t vview, int32_t bit_depth,
+                         const int64_t *values, int32_t n_values, const fbgpu_op *filter, int32_t n_filter_ops,
+                         const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+
 /* ---- multi-GPU reduce (replaces the HTTP fan-in of mapReduce/remoteExec, executor.go:6392-6533) ----
  * One context (process) per GPU; rank 0 creates the id, every rank joins.  When a communicator is attached,
  * count / row_counts / groupby results are summed with one ncclAllReduce(uint64,sum) on the device before
@@ -325,6 +340,10 @@ int fbgpu_node_row_counts(fbgpu_node *node, uint32_t index, uint32_t field, uint
 int fbgpu_node_groupby(fbgpu_node *node, uint32_t index, const uint32_t *fields, const uint32_t *views, int32_t n_fields,
                        const uint64_t *row_ids_flat, const int32_t *n_rows, const fbgpu_op *filter, int32_t n_filter_ops,
                        const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+int fbgpu_node_groupby_values(fbgpu_node *node, uint32_t index, const uint32_t *fields, const uint32_t *views, int32_t n_fields,
+                              const uint64_t *row_ids_flat, const int32_t *n_rows, uint32_t vfield, uint32_t vview, int32_t bit_depth,
+                              const int64_t *values, int32_t n_values, const fbgpu_op *filter, int32_t n_filter_ops,
+                              const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
 int fbgpu_node_bsi_sum(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                        const uint64_t *shards, int64_t n_shards, int64_t *out_sum, uint64_t *out_count);
 int fbgpu_node_bsi_minmax(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
