@@ -38,7 +38,13 @@ NAMES = ["empty", "full", "firstBitSet", "lastBitSet", "firstBitUnset", "lastBit
 def container(name, typ):
     """explicit-encoding container, like doContainer() (roaring_helpers_test.go:246-257); note the reference's
     run archetypes for odd/even hold 32768 single-value runs"""
-    vals = archetype_values(name)
+    return container_of(archetype_values(name), typ)
+
+
+def container_of(vals, typ):
+    """the sorted unique values `vals` as a container of encoding `typ` (O.ARRAY / O.BITMAP / O.RUN), whatever their number:
+    to_bytes(optimize=False) keeps it as built"""
+    vals = np.asarray(vals, dtype=np.int64)
     if typ == O.ARRAY:
         return O.Container.array(vals)
     if typ == O.BITMAP:
