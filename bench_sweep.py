@@ -10,6 +10,8 @@
             (only when named in --configs).
   config V: GroupBy(Rows(a), Rows(v)) with v an int field of 64 / 1000 / 65535 distinct values, fbgpu_groupby_values against the
             Row(v == value)-per-value composition (only when named in --configs).
+  config T: TopK(f, from=, to=) and GroupBy(Rows(a), Rows(f, from=, to=)) over 48 views of a quantum-YMD field,
+            fbgpu_row_counts_views / fbgpu_groupby_views against the operand-row composition (only when named in --configs).
 Every point is spot-checked against the CPU oracle on a few shards (the checker, not the thing measured)."""
 import argparse
 import json
@@ -356,6 +358,137 @@ def config_groupby_values(args, out):
     real.close()
 
 
+class _NoTimeViews(_KernelMs):
+    """the same proxy without row_counts_views / groupby_views: the executor takes the operand-row composition"""
+
+    def __getattr__(self, name):
+        if name in ("row_counts_views", "groupby_views"):
+            raise AttributeError(name)
+        return super().__getattr__(name)
+
+
+def _array_fragment(v):
+    """Pilosa-roaring bytes of sorted unique values whose containers all hold fewer than 4096 values and are not run-shaped (the
+    random sparse bits of config T): every container an array, encoded without a per-container Python loop"""
+    keys = v >> np.uint64(16)
+    uk, first, cnt = np.unique(keys, return_index=True, return_counts=True)
+    hdr = np.zeros(len(uk), dtype=[("key", "<u8"), ("typ", "<u2"), ("n1", "<u2")])
+    hdr["key"], hdr["typ"], hdr["n1"] = uk, 1, cnt - 1
+    offs = (8 + 16 * len(uk) + 2 * first).astype("<u4")
+    return np.array([12348, len(uk)], dtype="<u4").tobytes() + hdr.tobytes() + offs.tobytes() + (v & np.uint64(0xFFFF)).astype("<u2").tobytes()
+
+
+def _card():
+    """the card's name, power limit and maximum SM clock, read in the same run as the numbers they belong to"""
+    import subprocess
+    try:
+        r = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], stdout=subprocess.PIPE,
+                           stderr=subprocess.DEVNULL, text=True, timeout=30)
+        name, power, clock = [x.strip() for x in r.stdout.strip().splitlines()[0].split(",")]
+        return {"name": name, "power_limit": power, "max_sm_clock": clock}
+    except Exception as e:
+        return {"name": None, "error": f"nvidia-smi unavailable: {e}"}
+
+
+def config_time_views(args, out):
+    """TopK(f, from=, to=) and GroupBy(Rows(a), Rows(f, from=, to=)) over a range of 48 views, without and with a 1 % filter row,
+    through the executor.  f: a quantum-YMD time field of 256 rows over --groupby-shards shards, 64 Ki bits per shard, each at a
+    random column with a timestamp spread uniformly over the 120 days from 2019-01-01 (every bit is in its day, month, year and
+    standard views); a: a 256-row set field at 1/256 density per row.  The device arm (fbgpu_row_counts_views /
+    fbgpu_groupby_views) runs over all shards.  The composition arm (per row, a Row over the views, read back and stored as a row of
+    the scratch field, then one row-count or GroupBy call) re-sends the scratch fragment of every touched shard and commits the
+    store again for every row (about two minutes per query on one shard on an H100): it runs over the first --composition-shards
+    shards, for
+    --composition-steps steps alternated with the device arm over the same shards, every step reported (the scratch field grows
+    with each).  Both arms must return the same result.  Progress goes to stderr."""
+    import datetime
+    from featurebase_b200 import datagen as D, executor as X, lib as L, roaring_io
+    S, R, per_shard, days = args.groupby_shards, 256, 1 << 16, 120
+    shards = np.arange(S, dtype=np.uint64)
+    h = X.Holder()
+    idx = h.create_index("i", track_existence=False)
+    fa, ff, ft = idx.create_field("a"), idx.create_field("c"), idx.create_field("f", "time", quantum="YMD")
+    t0 = time.time()
+    for fld, rows, p in ((fa, range(R), 1 / 256), (ff, [0], 0.01)):
+        bulk = D.fragments(60 + fld.id, shards, list(rows), p)
+        h.ctx.load_fragments(idx.id, fld.id, X.VIEW_STANDARD, shards, bulk.buf, bulk.offsets)
+        del bulk
+    rng = np.random.default_rng(61)
+    day0 = datetime.date(2019, 1, 1)
+    names = [(day0 + datetime.timedelta(days=d)).strftime("%Y%m%d") for d in range(days)]
+    month_of = np.array([int(n[4:6]) for n in names])
+    views = {}                                                   # view name -> [per-shard fragment bytes]
+    for s in range(S):
+        col = rng.integers(0, SW, per_shard, dtype=np.uint64)
+        pos = rng.integers(0, R, per_shard, dtype=np.uint64) * np.uint64(SW) + col
+        day = rng.integers(0, days, per_shard)
+        every = _array_fragment(np.unique(pos))
+        views.setdefault("standard", []).append(every)
+        views.setdefault("standard_2019", []).append(every)
+        for m in sorted(set(month_of.tolist())):
+            views.setdefault("standard_2019%02d" % m, []).append(_array_fragment(np.unique(pos[month_of[day] == m])))
+        order = np.argsort(day, kind="stable")
+        bounds = np.searchsorted(day[order], np.arange(days + 1))
+        for d in range(days):
+            views.setdefault("standard_" + names[d], []).append(_array_fragment(np.unique(pos[order[bounds[d]:bounds[d + 1]]])))
+        if s == 0:
+            assert every == roaring_io.encode(pos)
+    for name, blobs in views.items():
+        vid = X.VIEW_STANDARD if name == "standard" else ft.view_id(name, create=True)
+        offsets = np.concatenate([[0], np.cumsum([len(b) for b in blobs])]).astype(np.uint64)
+        h.ctx.load_fragments(idx.id, ft.id, vid, shards, np.frombuffer(b"".join(blobs), dtype=np.uint8), offsets)
+    del views
+    h.ctx.commit()
+    idx.shards.update(range(S))
+    load_s = time.time() - t0
+    rng_q = "from=2019-01-05T00:00, to=2019-04-20T00:00"
+    n_views = len(X.Executor(h)._time_view_ids(ft, {"from": "2019-01-05T00:00", "to": "2019-04-20T00:00"}))
+    print(f"config T: loaded {S} shards in {load_s:.1f}s; the range covers {n_views} views", file=sys.stderr, flush=True)
+    real = h.ctx
+    card = _card()
+    dev, comp = _KernelMs(real), _NoTimeViews(real)
+    CS = min(S, args.composition_shards)
+    for q in (f"TopK(f, k=10, {rng_q})", f"TopK(f, k=10, {rng_q}, filter=Row(c=0))", f"GroupBy(Rows(a), Rows(f, {rng_q}))",
+              f"GroupBy(Rows(a), Rows(f, {rng_q}), filter=Row(c=0))"):
+        for n_sh, arms in ((S, {"device": dev}), (CS, {"device": dev, "composition": comp})):
+            sh = list(range(n_sh))
+            rec = {name: {"wall": [], "kernel_ms": [], "queries": [], "scratch_bytes": []} for name in arms}
+            res = {}
+            for i in range(1 + args.steps):                  # one warm-up round of the device arm, then alternate the arms
+                for name in (sorted(arms) if i % 2 == 0 else sorted(arms, reverse=True)):
+                    if name == "composition" and len(rec[name]["wall"]) >= args.composition_steps:
+                        continue
+                    h.ctx = arms[name]
+                    q0, arms[name].ms, b0 = real.counters()["queries"], 0.0, real.stats()["payload_bytes"]
+                    t1 = time.perf_counter()
+                    r = X.Executor(h).execute("i", q, sh)[0]
+                    wall = (time.perf_counter() - t1) * 1e3
+                    res.setdefault(name, r)
+                    assert r == res[name], (q, name)
+                    print(f"config T: {q} over {n_sh} shards, {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                    if i >= 1 or name == "composition":
+                        rec[name]["wall"].append(wall)
+                        rec[name]["kernel_ms"].append(arms[name].ms)
+                        rec[name]["queries"].append(real.counters()["queries"] - q0)
+                        rec[name]["scratch_bytes"].append(real.stats()["payload_bytes"] - b0)
+            h.ctx = real
+            assert all(r == res["device"] for r in res.values()), q
+            assert res["device"], q
+            for name, dd in rec.items():
+                o = {"config": "T", "query": q, "arm": name, "gpu": card, "shards": n_sh, "views": n_views, "rows": R, "results": len(res[name]),
+                     "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])), "wall_ms_max": float(np.max(dd["wall"])),
+                     "kernel_ms": float(np.median(dd["kernel_ms"])), "queries": int(np.median(dd["queries"])),
+                     "scratch_bytes": int(np.median(dd["scratch_bytes"])), "steps": len(dd["wall"]), "load_s": round(load_s, 1),
+                     "kernel": "row_count_views_kernel (+ eval_kernel for filters and peeled GroupBy dimensions)" if name == "device"
+                               else "eval_kernel + canonical emission per row, row_count_kernel / groupby kernels over the scratch rows",
+                     "note": "median over the timed steps of the executor call (wall clock, Rows pre-passes included), of the summed "
+                             "last_query_gpu_ms and of the number of its library queries; scratch_bytes: growth of the store's payload bytes"}
+                if name == "composition":
+                    o["wall_ms_per_step"] = [round(x, 2) for x in dd["wall"]]
+                out(o)
+    real.close()
+
+
 def config3(args, out, n_rec=10_000_000, nf=4):
     """nf fields are rotated between steps so that the touched planes exceed L2 (the 10 M-record config is 42.5 MB)"""
     from featurebase_b200 import datagen as D, executor as X, pql
@@ -450,7 +583,8 @@ def main():
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--shards", type=int, default=1024)
     ap.add_argument("--groupby-shards", type=int, default=512)
-    ap.add_argument("--composition-steps", type=int, default=1, help="config V: steps of the composition arm (each one slower than the last)")
+    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T: steps of the composition arm (each one slower than the last)")
+    ap.add_argument("--composition-shards", type=int, default=1, help="config T: shards of the composition arm and of the device arm timed beside it")
     ap.add_argument("--generators", default="uniform,clustered")
     ap.add_argument("--batched", action="store_true", help="also time the multi-pair launch (config 5b)")
     ap.add_argument("--densities", default="0.0001,0.001,0.01,0.03,0.0625,0.125,0.25,0.5")
@@ -469,6 +603,8 @@ def main():
             config_percentile(args, out)
         elif c == "V":
             config_groupby_values(args, out)
+        elif c == "T":
+            config_time_views(args, out)
         elif c == "3L":     # the same BSI query at 256 shards (268 M records, 1.1 GB of planes): shows the kernel away from the launch-bound regime
             config3(args, out, n_rec=256 * SW, nf=1)
         else:

@@ -234,6 +234,7 @@ extern "C" int fbgpu_init(int32_t device_ordinal, fbgpu_ctx** out) try {
     CUDA_TRY(cudaFuncSetAttribute(pair_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPcWarps * 8192));
     CUDA_TRY(cudaFuncSetAttribute(row_count_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
     CUDA_TRY(cudaFuncSetAttribute(row_count_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
+    CUDA_TRY(cudaFuncSetAttribute(row_count_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
     CUDA_TRY(cudaFuncSetAttribute(groupby_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGbSlots * 4 + 8192));
     CUDA_TRY(cudaFuncSetAttribute(groupby_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGdSmemBytes));
     { int nb = 0; if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, groupby_direct_kernel, kGdThreads, kGdSmemBytes) == cudaSuccess && nb > 0) c->gd_ctas_per_sm = nb; }
@@ -1019,13 +1020,17 @@ static std::vector<uint64_t> sorted_unique(const uint64_t* v, int64_t n) {
     return s;
 }
 
-// the program "<ops> ∩ Row(field, view, row)": the row alone when there are no ops
-static std::vector<fbgpu_op> and_row(const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, uint64_t row) {
+// the program "<ops> ∩ Union(Row(field, views[0], row), ..., Row(field, views[n_views - 1], row))": one view's row without the
+// Union, and the row (or union) alone when there are no ops
+static std::vector<fbgpu_op> and_row(const fbgpu_op* ops, int32_t n_ops, uint32_t field, const uint32_t* views, int32_t n_views, uint64_t row) {
     std::vector<fbgpu_op> full(ops, ops + n_ops);
-    fbgpu_op r{}; r.opcode = FBGPU_OP_ROW; r.field = field; r.view = view; r.a = row;
-    full.push_back(r);
+    for (int32_t i = 0; i < n_views; i++) { fbgpu_op r{}; r.opcode = FBGPU_OP_ROW; r.field = field; r.view = views[i]; r.a = row; full.push_back(r); }
+    if (n_views > 1) { fbgpu_op u{}; u.opcode = FBGPU_OP_UNION; u.argc = (uint32_t)n_views; full.push_back(u); }
     if (n_ops) { fbgpu_op in{}; in.opcode = FBGPU_OP_INTERSECT; in.argc = 2; full.push_back(in); }
     return full;
+}
+static std::vector<fbgpu_op> and_row(const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, uint64_t row) {
+    return and_row(ops, n_ops, field, &view, 1, row);
 }
 
 // One query call on a leased workspace: the device program and its operand stack depth, the uploaded program and shard list,
@@ -1478,17 +1483,21 @@ extern "C" int fbgpu_bsi_select(fbgpu_ctx* c, uint32_t index, const fbgpu_op* op
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ per-row counts (TopK / TopN ids)
-static int row_counts_impl(fbgpu_ctx* c, uint32_t index, uint32_t fv, const std::vector<uint64_t>& rows, const fbgpu_op* filter, int32_t n_filter_ops,
+// fvs: the view slots each row is the union over.  One slot: row_count_kernel; several: row_count_views_kernel, whose counts
+// are always summed over the shards (per_shard needs one slot).
+static int row_counts_impl(fbgpu_ctx* c, uint32_t index, const std::vector<uint32_t>& fvs, const std::vector<uint64_t>& rows, const fbgpu_op* filter, int32_t n_filter_ops,
                            const uint64_t* shards, int64_t n_shards, std::vector<uint64_t>& counts, bool reduce = true, bool per_shard = false) {
     counts.assign(rows.size() * (per_shard ? (size_t)n_shards : 1), 0);
     if (rows.empty()) return 0;
     const bool have_filter = filter && n_filter_ops > 0;
     Query q(c); Workspace* w = q.w;
     int rc = have_filter ? q.open(index, filter, n_filter_ops, shards, n_shards) : q.open(shards, n_shards); if (rc) return rc;
-    size_t nr = rows.size();
+    size_t nr = rows.size(), nv = fvs.size();
     const size_t n_out = counts.size();                     // nr, or n_shards x nr (per_shard: one row of the matrix per listed shard)
-    if (w->d_rows.ensure(nr * 8) || w->d_counts.ensure(n_out * 8) || w->h_out.ensure(n_out * 8)) return FBGPU_E_NOMEM;
-    CUDA_TRY(cudaMemcpyAsync(w->d_rows.p, rows.data(), nr * 8, cudaMemcpyHostToDevice, w->stream));
+    if (w->d_rows.ensure(nr * 8 + nv * 4) || w->d_counts.ensure(n_out * 8) || w->h_out.ensure(n_out * 8)) return FBGPU_E_NOMEM;
+    CUDA_TRY(cudaMemcpyAsync(w->d_rows.p, rows.data(), nr * 8, cudaMemcpyHostToDevice, w->stream));       // [rows | view slots]
+    const uint32_t* d_fvs = (const uint32_t*)((const uint64_t*)w->d_rows.p + nr);
+    if (nv > 1) CUDA_TRY(cudaMemcpyAsync((void*)d_fvs, fvs.data(), nv * 4, cudaMemcpyHostToDevice, w->stream));
     CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, n_out * 8, w->stream));
     CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
     const int64_t batch = have_filter ? c->unit_batch / kSlotsPerRow : n_shards;
@@ -1497,7 +1506,11 @@ static int row_counts_impl(fbgpu_ctx* c, uint32_t index, uint32_t fv, const std:
         if (have_filter) { rc = q.eval(s0 * kSlotsPerRow, ns * kSlotsPerRow); if (rc) return rc; }
         long long tasks = (long long)ns * (long long)nr;
         long long grid = std::min<long long>((tasks + kPairWarps - 1) / kPairWarps, (long long)c->sm_count * 3);
-        if (per_shard)
+        const uint32_t fv = fvs[0];
+        if (nv > 1)
+            row_count_views_kernel<<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), d_fvs, (int)nv, (const uint64_t*)w->d_rows.p, (int)nr,
+                q.d_shards + s0, ns, have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p);
+        else if (per_shard)
             row_count_kernel<true><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, q.d_shards + s0, ns,
                 have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p + (size_t)s0 * nr);
         else
@@ -1516,18 +1529,15 @@ static int row_counts_impl(fbgpu_ctx* c, uint32_t index, uint32_t fv, const std:
     return 0;
 }
 
-extern "C" int fbgpu_row_counts(fbgpu_ctx* c, uint32_t index, uint32_t field, uint32_t view, const uint64_t* row_ids, int32_t n_rows,
-                                const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
-                                uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n) try {
-    if (!c || !out_counts || n_shards < 0 || (n_shards && !shards) || n_rows < 0) return fail(FBGPU_E_INVALID, "null argument");
-    std::shared_lock<std::shared_mutex> lk;
-    int rc = begin_query(c, lk); if (rc) return rc;
-    uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
+// fbgpu_row_counts / fbgpu_row_counts_views once the store is locked: the rows are their unions over the view slots fvs
+static int row_counts_query(fbgpu_ctx* c, uint32_t index, const std::vector<uint32_t>& fvs, const uint64_t* row_ids, int32_t n_rows,
+                            const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
+                            uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n) {
     std::vector<uint64_t> rows, counts;
     if (row_ids) rows.assign(row_ids, row_ids + n_rows);
     else {
-        // fragment.rows() (fragment.go:2465-2486): distinct row ids present in the listed shards
-        if (fv != kNoView) for (int64_t s = 0; s < n_shards; s++) {
+        // fragment.rows() (fragment.go:2465-2486): distinct row ids present in the listed shards (of any of the views)
+        for (uint32_t fv : fvs) if (fv != kNoView) for (int64_t s = 0; s < n_shards; s++) {
             const auto& sm = c->shardmaps[fv];
             if (shards[s] >= sm.size() || sm[shards[s]] < 0) continue;
             const HostFrag& f = c->frags[sm[shards[s]]];
@@ -1535,7 +1545,7 @@ extern "C" int fbgpu_row_counts(fbgpu_ctx* c, uint32_t index, uint32_t field, ui
         }
         std::sort(rows.begin(), rows.end()); rows.erase(std::unique(rows.begin(), rows.end()), rows.end());
     }
-    rc = row_counts_impl(c, index, fv, rows, filter, n_filter_ops, shards, n_shards, counts, row_ids != nullptr); if (rc) return rc;
+    int rc = row_counts_impl(c, index, fvs, rows, filter, n_filter_ops, shards, n_shards, counts, row_ids != nullptr); if (rc) return rc;
     if (row_ids) {
         if (cap < n_rows) return fail(FBGPU_E_NOSPACE, "cap %d < n_rows %d", cap, n_rows);
         for (int32_t i = 0; i < n_rows; i++) { out_counts[i] = counts[i]; if (out_row_ids) out_row_ids[i] = rows[i]; }
@@ -1551,6 +1561,49 @@ extern "C" int fbgpu_row_counts(fbgpu_ctx* c, uint32_t index, uint32_t field, ui
     if (order.size() > (size_t)std::max(cap, 0)) return fail(FBGPU_E_NOSPACE, "%zu rows have a non-zero count, cap is %d", order.size(), cap);
     for (size_t i = 0; i < order.size(); i++) { if (out_row_ids) out_row_ids[i] = rows[order[i]]; out_counts[i] = counts[order[i]]; }
     return FBGPU_OK;
+}
+
+extern "C" int fbgpu_row_counts(fbgpu_ctx* c, uint32_t index, uint32_t field, uint32_t view, const uint64_t* row_ids, int32_t n_rows,
+                                const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
+                                uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n) try {
+    if (!c || !out_counts || n_shards < 0 || (n_shards && !shards) || n_rows < 0) return fail(FBGPU_E_INVALID, "null argument");
+    std::shared_lock<std::shared_mutex> lk;
+    int rc = begin_query(c, lk); if (rc) return rc;
+    const std::vector<uint32_t> fvs{ view_id_locked(c, ViewKey{ index, field, view }, false) };
+    return row_counts_query(c, index, fvs, row_ids, n_rows, filter, n_filter_ops, shards, n_shards, out_row_ids, out_counts, cap, out_n);
+} FBGPU_CATCH
+
+// the argument checks fbgpu_row_counts_views and its node form make before any device is touched
+static int row_counts_views_args(const void* handle, const uint32_t* views, int32_t n_views, int32_t n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
+                                 const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts) {
+    if (!handle || !views || !out_counts || n_rows < 0 || n_filter_ops < 0 || (n_filter_ops && !filter) || n_shards < 0 || (n_shards && !shards))
+        return fail(FBGPU_E_INVALID, "bad argument");
+    if (n_views < 1) return fail(FBGPU_E_INVALID, "n_views=%d < 1", n_views);
+    return 0;
+}
+
+// the view slots of (index, field, views[i]) that exist, each once: a view never loaded, or listed twice, adds nothing to a
+// union.  {kNoView} when none exists, so that every row counts 0.
+static std::vector<uint32_t> view_slots(fbgpu_ctx* c, uint32_t index, uint32_t field, const uint32_t* views, int32_t n_views) {
+    std::vector<uint32_t> fvs;
+    for (int32_t i = 0; i < n_views; i++) { const uint32_t fv = view_id_locked(c, ViewKey{ index, field, views[i] }, false); if (fv != kNoView) fvs.push_back(fv); }
+    std::sort(fvs.begin(), fvs.end()); fvs.erase(std::unique(fvs.begin(), fvs.end()), fvs.end());
+    if (fvs.empty()) fvs.push_back(kNoView);
+    return fvs;
+}
+
+// TopK / Rows of a time field with from= / to=: fbgpu_row_counts with each row taken as its union over the covering views.
+// executeTopKShardTime (executor.go:2506-2533) counts a row over the mergerator of the views' fragments (:2570), and
+// executeRowsShard (:4107-4127) merges the row ids of every covering view; both in one pass over the shards here.
+extern "C" int fbgpu_row_counts_views(fbgpu_ctx* c, uint32_t index, uint32_t field, const uint32_t* views, int32_t n_views,
+                                      const uint64_t* row_ids, int32_t n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
+                                      const uint64_t* shards, int64_t n_shards, uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n) try {
+    int rc = row_counts_views_args(c, views, n_views, n_rows, filter, n_filter_ops, shards, n_shards, out_counts); if (rc) return rc;
+    if (n_views == 1) return fbgpu_row_counts(c, index, field, views[0], row_ids, n_rows, filter, n_filter_ops, shards, n_shards, out_row_ids, out_counts, cap, out_n);
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    return row_counts_query(c, index, view_slots(c, index, field, views, n_views), row_ids, n_rows, filter, n_filter_ops, shards, n_shards,
+                            out_row_ids, out_counts, cap, out_n);
 } FBGPU_CATCH
 
 // per-shard counts of explicit rows: out_counts[s * n_rows + i] = |Row(row_ids[i]) [∩ filter]| in shards[s]
@@ -1560,7 +1613,7 @@ extern "C" int fbgpu_row_counts_per_shard(fbgpu_ctx* c, uint32_t index, uint32_t
     if (n_rows == 0 || n_shards == 0) return FBGPU_OK;
     std::shared_lock<std::shared_mutex> lk;
     int rc = begin_query(c, lk); if (rc) return rc;
-    const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
+    const std::vector<uint32_t> fv{ view_id_locked(c, ViewKey{ index, field, view }, false) };
     std::vector<uint64_t> rows(row_ids, row_ids + n_rows), counts;
     // the matrix is produced in blocks of shards so that the device / pinned buffers stay below 512 MiB however many rows are asked for
     const int64_t block = std::max<int64_t>(1, (int64_t)((64ull << 20) / (uint64_t)n_rows));
@@ -1741,27 +1794,43 @@ static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* 
     return 0;
 }
 
-// n-field GroupBy: peel the leading field on the host, folding Row(f0=r) into the filter (groupByIterator keeps
-// the same prefix intersections per level, executor.go:8829-8835,8861-8867)
-static int groupby_rec(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int nf, const uint64_t* const* rows, const int32_t* n_rows,
-                       std::vector<fbgpu_op> filter, const uint64_t* shards, int64_t n_shards, uint64_t* out) {
+// one GroupBy dimension: the listed rows of `field`, each taken as its union over views[0..n_views)
+struct GbDim { uint32_t field; const uint32_t* views; int32_t n_views; const uint64_t* rows; int32_t n_rows; };
+
+// n-field GroupBy: peel the leading field on the host, folding Row(f0=r) — over several views, the union of those rows — into
+// the filter (groupByIterator keeps the same prefix intersections per level, executor.go:8829-8835,8861-8867).  The last
+// dimension is counted by the row-count kernels, two single-view last dimensions by groupby2.
+static int groupby_rec(fbgpu_ctx* c, uint32_t index, const GbDim* d, int nf, std::vector<fbgpu_op> filter, const uint64_t* shards, int64_t n_shards, uint64_t* out) {
     if (nf == 1) {
-        uint32_t fv = view_id_locked(c, ViewKey{ index, fields[0], views[0] }, false);
-        std::vector<uint64_t> r(rows[0], rows[0] + n_rows[0]), counts;
-        int rc = row_counts_impl(c, index, fv, r, filter.empty() ? nullptr : filter.data(), (int)filter.size(), shards, n_shards, counts); if (rc) return rc;
+        std::vector<uint64_t> r(d[0].rows, d[0].rows + d[0].n_rows), counts;
+        int rc = row_counts_impl(c, index, view_slots(c, index, d[0].field, d[0].views, d[0].n_views), r, filter.empty() ? nullptr : filter.data(), (int)filter.size(),
+                                 shards, n_shards, counts); if (rc) return rc;
         memcpy(out, counts.data(), counts.size() * 8);
         return 0;
     }
-    if (nf == 2) {
-        uint32_t fa = view_id_locked(c, ViewKey{ index, fields[0], views[0] }, false), fb = view_id_locked(c, ViewKey{ index, fields[1], views[1] }, false);
-        return groupby2(c, index, fa, rows[0], n_rows[0], fb, rows[1], n_rows[1], filter, shards, n_shards, out);
+    if (nf == 2 && d[0].n_views == 1 && d[1].n_views == 1) {
+        uint32_t fa = view_id_locked(c, ViewKey{ index, d[0].field, d[0].views[0] }, false), fb = view_id_locked(c, ViewKey{ index, d[1].field, d[1].views[0] }, false);
+        return groupby2(c, index, fa, d[0].rows, d[0].n_rows, fb, d[1].rows, d[1].n_rows, filter, shards, n_shards, out);
     }
-    size_t sub = 1; for (int i = 1; i < nf; i++) sub *= (size_t)n_rows[i];
-    for (int r = 0; r < n_rows[0]; r++) {
-        int rc = groupby_rec(c, index, fields + 1, views + 1, nf - 1, rows + 1, n_rows + 1, and_row(filter.data(), (int32_t)filter.size(), fields[0], views[0], rows[0][r]),
+    size_t sub = 1; for (int i = 1; i < nf; i++) sub *= (size_t)d[i].n_rows;
+    for (int r = 0; r < d[0].n_rows; r++) {
+        int rc = groupby_rec(c, index, d + 1, nf - 1, and_row(filter.data(), (int32_t)filter.size(), d[0].field, d[0].views, d[0].n_views, d[0].rows[r]),
                              shards, n_shards, out + (size_t)r * sub); if (rc) return rc;
     }
     return 0;
+}
+
+// fbgpu_groupby / fbgpu_groupby_views once the arguments are checked and the store is locked
+static int groupby_dims(fbgpu_ctx* c, uint32_t index, const std::vector<GbDim>& dims, const fbgpu_op* filter, int32_t n_filter_ops,
+                        const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) {
+    size_t total = 1; for (const GbDim& d : dims) total *= (size_t)d.n_rows;
+    memset(out_counts, 0, total * 8);
+    if (total == 0) return 0;
+    // executor.go:8769-8772: the kernels treat a shard with a missing fragment as contributing nothing; for the
+    // row_counts path (n_fields == 1) a missing fragment naturally yields zeros.  For n_fields >= 3 the peeled
+    // fields enter through the filter, which is empty on shards without that fragment.
+    std::vector<fbgpu_op> f(filter, filter + (filter ? n_filter_ops : 0));
+    return groupby_rec(c, index, dims.data(), (int)dims.size(), f, shards, n_shards, out_counts);
 }
 
 extern "C" int fbgpu_groupby(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows,
@@ -1769,15 +1838,40 @@ extern "C" int fbgpu_groupby(fbgpu_ctx* c, uint32_t index, const uint32_t* field
     if (!c || !fields || !views || !row_ids_flat || !n_rows || !out_counts || n_fields < 1 || n_fields > 8 || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
     std::shared_lock<std::shared_mutex> lk;
     int rc = begin_query(c, lk); if (rc) return rc;
-    std::vector<const uint64_t*> rows(n_fields); const uint64_t* p = row_ids_flat; size_t total = 1;
-    for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); rows[i] = p; p += n_rows[i]; total *= (size_t)n_rows[i]; }
-    memset(out_counts, 0, total * 8);
-    if (total == 0) return 0;
-    // executor.go:8769-8772: the kernels treat a shard with a missing fragment as contributing nothing; for the
-    // row_counts path (n_fields == 1) a missing fragment naturally yields zeros.  For n_fields >= 3 the peeled
-    // fields enter through the filter, which is empty on shards without that fragment.
-    std::vector<fbgpu_op> f(filter, filter + (filter ? n_filter_ops : 0));
-    return groupby_rec(c, index, fields, views, n_fields, rows.data(), n_rows, f, shards, n_shards, out_counts);
+    std::vector<GbDim> dims((size_t)n_fields); const uint64_t* p = row_ids_flat;
+    for (int i = 0; i < n_fields; i++) {
+        if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]);
+        dims[(size_t)i] = GbDim{ fields[i], views + i, 1, p, n_rows[i] }; p += n_rows[i];
+    }
+    return groupby_dims(c, index, dims, filter, n_filter_ops, shards, n_shards, out_counts);
+} FBGPU_CATCH
+
+// the argument checks fbgpu_groupby_views and its node form make before any device is touched
+static int groupby_views_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                              const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
+                              const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts) {
+    if (!handle || !fields || !views_flat || !n_views || !row_ids_flat || !n_rows || !out_counts || n_filter_ops < 0 || (n_filter_ops && !filter) ||
+        n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
+    if (n_fields < 1 || n_fields > 8) return fail(FBGPU_E_INVALID, "n_fields=%d outside 1..8", n_fields);
+    for (int i = 0; i < n_fields; i++) {
+        if (n_views[i] < 1) return fail(FBGPU_E_INVALID, "n_views[%d]=%d < 1", i, n_views[i]);
+        if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]);
+    }
+    return 0;
+}
+
+// GroupBy(Rows(f1, from=, to=), ...): fbgpu_groupby with dimension i's rows taken as their unions over n_views[i] views
+// (timeFragmentsRowIterator, executor.go:8755-8768)
+extern "C" int fbgpu_groupby_views(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                   const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
+                                   const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
+    int rc = groupby_views_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards, out_counts);
+    if (rc) return rc;
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    std::vector<GbDim> dims((size_t)n_fields); const uint32_t* v = views_flat; const uint64_t* p = row_ids_flat;
+    for (int i = 0; i < n_fields; i++) { dims[(size_t)i] = GbDim{ fields[i], v, n_views[i], p, n_rows[i] }; v += n_views[i]; p += n_rows[i]; }
+    return groupby_dims(c, index, dims, filter, n_filter_ops, shards, n_shards, out_counts);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ GroupBy over the values of an int field

@@ -6,6 +6,7 @@
 //   pair_count_kernel  one warp per container pair: fused Intersect+Count for Count(Intersect(Row,Row))
 //                      (replaces roaring.intersectionCount's 9 type-pair kernels, roaring.go:4477-4614).
 //   row_count_kernel   one warp per (shard,row): per-row |row ∩ filter| (doTopK executor.go:2705, fragment.top).
+//   row_count_views_kernel  the same with each row taken as its union over several views (time fields, from= / to=).
 //   groupby_kernel     one CTA per (shard, slot): column-keyed join of two fields' rows (groupByIterator :8617).
 //   canon_*            canonical (optimize()) container emission for Row results (roaring.go:3412-3461).
 #pragma once
@@ -985,6 +986,117 @@ row_count_kernel(StoreRef st, uint32_t fv, const uint64_t* __restrict__ row_ids,
             else acc += warp_count_vs_global_bitmap(a, reinterpret_cast<const uint32_t*>(filter_bitmaps + ((size_t)si * 16 + s) * 512), bm, lane);
         }
         if (lane == 0 && acc) { if (kPerShard) out_counts[(size_t)si * n_rows + ri] = acc; else atomicAdd(&out_counts[ri], acc); }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Per-row counts of a row taken as its union over several views (TopK / Rows of a time field with from= / to=:
+// executeTopKShardTime executor.go:2506-2533 counts each row over the mergerator of the covering views, :2570).  One warp
+// per (shard, requested row), as row_count_kernel, with the same 8 KiB shared bitmap per warp and the same optional
+// per-unit filter bitmaps.  For every slot the lanes resolve the row's container in the listed views, 32 views per round:
+// a slot with one container is counted as row_count_kernel counts it; with two or more, each container is OR-ed into the
+// warp's bitmap as it is found (bitmap words, array bit scatters, run range fills), and the bitmap (∩ the filter) is
+// counted and cleared.  Every container is read once, and a container listed twice only sets its bits twice.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ Resolved shfl_resolved(const Resolved& r, int src) {
+    Resolved a;
+    a.ptr = (const void*)__shfl_sync(0xffffffffu, (unsigned long long)r.ptr, src);
+    a.card = __shfl_sync(0xffffffffu, r.card, src);
+    const uint32_t meta = __shfl_sync(0xffffffffu, ((uint32_t)r.typ << 16) | r.cnt, src);
+    a.typ = meta >> 16; a.cnt = meta & 0xffff;
+    return a;
+}
+
+// the bits of [s, l] OR-ed into the shared bitmap at shared address sb
+__device__ __forceinline__ void smem_fill_range(uint32_t sb, uint32_t s, uint32_t l) {
+    const uint32_t ws = s >> 5, wl = l >> 5, ms = 0xffffffffu << (s & 31), ml = 0xffffffffu >> (31 - (l & 31));
+    if (ws == wl) { red_or_at(sb + 4 * ws, ms & ml); return; }
+    red_or_at(sb + 4 * ws, ms);
+    for (uint32_t k = ws + 1; k < wl; k++) red_or_at(sb + 4 * k, 0xffffffffu);
+    red_or_at(sb + 4 * wl, ml);
+}
+
+// OR one container into the warp's bitmap (bm, at shared address sb); the caller separates two containers by __syncwarp()
+__device__ __noinline__ void warp_or_container(Resolved a, uint32_t* bm, uint32_t sb, int lane) {
+    if (a.typ == kArray) {                                    // element order is irrelevant: bank-striped arrays need nothing special
+        const uint4* a4 = reinterpret_cast<const uint4*>(a.ptr);
+        const uint32_t n8 = (a.card + 7) >> 3;
+        for (uint32_t i = lane; i < n8; i += 32) scatter_chunk_sb<0>(sb, ldg_nc(a4 + i), i * 8, a.card);      // (tail padded with the last element)
+    } else if (a.typ == kBitmap) {                            // lane L owns words 4L.. of every 512-byte stride: no atomics
+        const uint4* g = reinterpret_cast<const uint4*>(a.ptr);
+        uint4* b4 = reinterpret_cast<uint4*>(bm);
+#pragma unroll 4
+        for (int i = lane; i < 512; i += 32) b4[i] = or4(b4[i], ldg_nc(g + i));
+    } else {
+        const uint32_t* r32 = reinterpret_cast<const uint32_t*>(a.ptr);
+        if (a.cnt >= 32) {                                    // many runs: one lane per run
+            for (uint32_t i = lane; i < a.cnt; i += 32) { const uint32_t v = __ldg(r32 + i); smem_fill_range(sb, v & 0xffffu, v >> 16); }
+        } else {                                              // few, possibly long runs: the warp fills each run's words together
+            for (uint32_t i = 0; i < a.cnt; i++) {
+                const uint32_t v = __ldg(r32 + i), s0 = v & 0xffffu, l0 = v >> 16;
+                for (uint32_t w = (s0 >> 5) + lane; w <= (l0 >> 5); w += 32) {
+                    uint32_t m = 0xffffffffu;
+                    if (w == (s0 >> 5)) m &= 0xffffffffu << (s0 & 31);
+                    if (w == (l0 >> 5)) m &= 0xffffffffu >> (31 - (l0 & 31));
+                    red_or_at(sb + 4 * w, m);
+                }
+            }
+        }
+    }
+}
+
+// |bitmap| or |bitmap ∩ fb| (fb: the unit's filter bitmap, or null), reduced over the warp; leaves the bitmap all zero
+__device__ __forceinline__ uint32_t warp_count_and_clear(uint32_t* bm, const uint32_t* fb, int lane) {
+    uint4* b4 = reinterpret_cast<uint4*>(bm);
+    const uint4* f4 = reinterpret_cast<const uint4*>(fb);
+    uint32_t c = 0;
+#pragma unroll 4
+    for (int i = lane; i < 512; i += 32) { const uint4 x = b4[i]; c += popc4(fb ? and4(x, f4[i]) : x); b4[i] = make_uint4(0, 0, 0, 0); }
+    return __reduce_add_sync(0xffffffffu, c);
+}
+
+__global__ void __launch_bounds__(kPairWarps * 32)
+row_count_views_kernel(StoreRef st, const uint32_t* __restrict__ fvs, int n_views, const uint64_t* __restrict__ row_ids, int n_rows,
+                       const uint64_t* __restrict__ shards, long long n_shards,
+                       const uint4* __restrict__ filter_bitmaps /* [n_shards*16][512] or null */,
+                       unsigned long long* out_counts /* [n_rows] */) {
+    extern __shared__ __align__(128) uint32_t smem32[];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    uint32_t* bm = smem32 + wid * 2048;
+    {   uint4* b4 = reinterpret_cast<uint4*>(bm);          // the only full clear: every count leaves the bitmap all zero again
+#pragma unroll 4
+        for (int i = lane; i < 512; i += 32) b4[i] = make_uint4(0, 0, 0, 0); }
+    __syncwarp();
+    uint32_t sb = (uint32_t)__cvta_generic_to_shared(bm);
+    pin_base(sb);
+    const long long n_tasks = n_shards * (long long)n_rows;
+    const long long stride = (long long)gridDim.x * kPairWarps;
+    for (long long t = (long long)blockIdx.x * kPairWarps + wid; t < n_tasks; t += stride) {
+        const long long si = t / n_rows; const int ri = (int)(t - si * n_rows);
+        const uint64_t shard = shards[si], row = row_ids[ri];
+        unsigned long long acc = 0;
+        for (int s = 0; s < kSlotsPerRow; s++) {
+            Resolved first; first.ptr = nullptr; first.card = 0; first.typ = 0; first.cnt = 0;
+            int found = 0;                                    // (warp-uniform) 0, 1: `first` only, 2: merged into the bitmap
+            for (int v0 = 0; v0 < n_views; v0 += 32) {
+                Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
+                if (v0 + lane < n_views) r = resolve(st, fvs[v0 + lane], shard, row, s);
+                unsigned present = __ballot_sync(0xffffffffu, r.ptr != nullptr);
+                while (present) {
+                    const int l = __ffs(present) - 1; present &= present - 1;
+                    const Resolved a = shfl_resolved(r, l);
+                    if (found == 0) { first = a; found = 1; continue; }
+                    if (found == 1) { warp_or_container(first, bm, sb, lane); __syncwarp(); found = 2; }
+                    warp_or_container(a, bm, sb, lane);
+                    __syncwarp();
+                }
+            }
+            if (found == 0) continue;
+            const uint32_t* fb = filter_bitmaps ? reinterpret_cast<const uint32_t*>(filter_bitmaps + ((size_t)si * 16 + s) * 512) : nullptr;
+            if (found == 1) acc += fb ? warp_count_vs_global_bitmap(first, fb, bm, lane) : first.card;
+            else { acc += warp_count_and_clear(bm, fb, lane); __syncwarp(); }
+        }
+        if (lane == 0 && acc) atomicAdd(&out_counts[ri], acc);
     }
 }
 

@@ -216,6 +216,27 @@ extern "C" int fbgpu_node_row_counts(fbgpu_node* n, uint32_t index, uint32_t fie
     });
 } FBGPU_CATCH
 
+extern "C" int fbgpu_node_row_counts_views(fbgpu_node* n, uint32_t index, uint32_t field, const uint32_t* views, int32_t n_views, const uint64_t* row_ids, int32_t n_rows,
+                                           const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
+    int rc = row_counts_views_args(n, views, n_views, n_rows, filter, n_filter_ops, shards, n_shards, out_counts); if (rc) return rc;
+    if (!row_ids) return fail(FBGPU_E_INVALID, "bad argument");
+    return node_sum(n, shards, n_shards, (size_t)n_rows, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {
+        int32_t got = 0;
+        return fbgpu_row_counts_views(c, index, field, views, n_views, row_ids, n_rows, filter, n_filter_ops, s.data(), (int64_t)s.size(), nullptr, part, n_rows, &got);
+    });
+} FBGPU_CATCH
+
+extern "C" int fbgpu_node_groupby_views(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                        const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
+                                        const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
+    int rc = groupby_views_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards, out_counts);
+    if (rc) return rc;
+    size_t total = 1; for (int i = 0; i < n_fields; i++) total *= (size_t)n_rows[i];
+    return node_sum(n, shards, n_shards, total, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {     // mergeGroupCounts executor.go:3728
+        return fbgpu_groupby_views(c, index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, s.data(), (int64_t)s.size(), part);
+    });
+} FBGPU_CATCH
+
 extern "C" int fbgpu_node_groupby(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
                                   const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     if (!n || !fields || !views || !row_ids_flat || !n_rows || !out_counts || n_fields < 1 || n_fields > 8 || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");

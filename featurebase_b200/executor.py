@@ -611,8 +611,15 @@ class Executor:
         filt = c.args.get("filter")
         filt = self._bitmap_call(idx, filt) if isinstance(filt, pql.Call) else None
         targs = {a: c.args[a] for a in ("from", "to") if a in c.args} if f.quantum else {}
-        if targs:                                                # executeTopKShardTime :2506-2533 / mergerator :2570: a row is the union of
-            rows = self._rows(idx, pql.Call("Rows", {"_field": f.name, **targs}), shards)      # itself over the covering views
+        if targs and hasattr(self.ctx, "row_counts_views"):     # executeTopKShardTime :2506-2533 / mergerator :2570: a row is the union of
+            views = self._time_view_ids(f, targs)                # itself over the covering views, counted in one library call
+            if not views:
+                return []
+            rid, cnt = self.ctx.row_counts_views(idx.id, f.id, views, shards, filter_ops=filt)
+            pairs = [(int(i), int(n)) for i, n in zip(rid, cnt)]
+            return pairs[:k] if k else pairs
+        if targs:
+            rows = self._rows(idx, pql.Call("Rows", {"_field": f.name, **targs}), shards)
             if not rows:
                 return []
             sf, operands = self._time_rows_as_operands(idx, f, rows, targs, shards)
@@ -626,7 +633,10 @@ class Executor:
     def _time_rows_as_operands(self, idx, f, rows, targs, shards):
         """Rows of a time field restricted to from= / to=, made addressable by the single-view kernels: each row's union over
         the covering views (timeFragmentsRowIterator :8755-8768, mergerator :2570) is evaluated once and stored as an operand
-        row of the scratch field.  Returns (scratch field, operand row ids in the order of `rows`)."""
+        row of the scratch field.  Returns (scratch field, operand row ids in the order of `rows`).  TopK, Rows and GroupBy
+        count such rows with row_counts_views / groupby_views instead where the context has them; this remains for a GroupBy that
+        also has an int child (the groupby_values path), a GroupBy with two or more int children, and contexts without those
+        calls."""
         operands = []
         for r in rows:
             data, _ = self.ctx.row(idx.id, self._bitmap_call(idx, pql.Call("Row", {f.name: r, **targs})), shards)
@@ -652,13 +662,18 @@ class Executor:
             filt = [L.Op(L.OP_ROW, ef.id, VIEW_STANDARD, 0, erow, 0, 0, 0)]
             shards = [s for s in shards if s == col // SHARD_WIDTH]
         views = [VIEW_BSI if f.type == "int" else VIEW_STANDARD]
-        if f.quantum and ("from" in c.args or "to" in c.args):    # executeRowsShard :4107-4127: the rows of every covering view, merged
+        timed = f.quantum and ("from" in c.args or "to" in c.args)
+        if timed:                                                # executeRowsShard :4107-4127: the rows of every covering view, merged
             views = self._time_view_ids(f, c.args)
-        out = set()
-        for v in views:
-            rid, _ = self.ctx.row_counts(idx.id, f.id, v, shards, filter_ops=filt)
-            out.update(int(r) for r in rid)
-        out = sorted(out)
+        if timed and views and hasattr(self.ctx, "row_counts_views"):       # (in one library call)
+            rid, _ = self.ctx.row_counts_views(idx.id, f.id, views, shards, filter_ops=filt)
+            out = sorted(int(r) for r in rid)
+        else:
+            out = set()
+            for v in views:
+                rid, _ = self.ctx.row_counts(idx.id, f.id, v, shards, filter_ops=filt)
+                out.update(int(r) for r in rid)
+            out = sorted(out)
         if "in" in c.args:
             keep = {int(r) for r in c.args["in"]}
             out = [r for r in out if r in keep]
@@ -1006,6 +1021,10 @@ class Executor:
         int_dims = [k for k, f in enumerate(fields) if f.type == "int"]
         if len(int_dims) == 1 and hasattr(self.ctx, "groupby_values"):
             counts = self._groupby_int_counts(idx, fields, row_ids, time_args, int_dims[0], filt, shards)
+        elif not int_dims and any(time_args) and hasattr(self.ctx, "groupby_views"):
+            # a Rows(f, from=, to=) child groups by its rows' unions over the covering views, in the same call as the other children
+            views = [self._time_view_ids(f, targs) if targs else [VIEW_STANDARD] for f, targs in zip(fields, time_args)]
+            counts = self.ctx.groupby_views(idx.id, [f.id for f in fields], views, row_ids, shards, filter_ops=filt)
         else:
             # what the device groups over: a field's standard view, or — for Rows(f, from=, to=) on a time field — one operand
             # row per row id holding the union of that row over the covering views (timeFragmentsRowIterator :8755-8768)

@@ -49,7 +49,8 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_comm_p2p_open_local", "fbgpu_node_init", "fbgpu_node_shutdown", "fbgpu_node_devices", "fbgpu_node_owner", "fbgpu_node_ctx", "fbgpu_node_load_fragment",
            "fbgpu_node_load_fragments", "fbgpu_node_load_rbf_dir", "fbgpu_node_drop_fragment", "fbgpu_node_commit", "fbgpu_node_get_stats", "fbgpu_node_count", "fbgpu_node_row",
            "fbgpu_node_count_pairs", "fbgpu_node_row_counts", "fbgpu_node_groupby", "fbgpu_node_bsi_sum", "fbgpu_node_bsi_minmax",
-           "fbgpu_groupby_values", "fbgpu_node_groupby_values"]
+           "fbgpu_groupby_values", "fbgpu_node_groupby_values", "fbgpu_row_counts_views", "fbgpu_node_row_counts_views", "fbgpu_groupby_views",
+           "fbgpu_node_groupby_views"]
 
 
 def lib_path():
@@ -97,6 +98,9 @@ def load():
     L.fbgpu_groupby.argtypes, L.fbgpu_groupby.restype = [vp, u32, vp, vp, i32, vp, vp, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_groupby_values.argtypes = [vp, u32, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i32, vp, i64, vp]
     L.fbgpu_groupby_values.restype = C.c_int
+    L.fbgpu_row_counts_views.argtypes = [vp, u32, u32, vp, i32, vp, i32, vp, i32, vp, i64, vp, vp, i32, C.POINTER(i32)]
+    L.fbgpu_row_counts_views.restype = C.c_int
+    L.fbgpu_groupby_views.argtypes, L.fbgpu_groupby_views.restype = [vp, u32, vp, vp, vp, i32, vp, vp, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_count_pairs.argtypes, L.fbgpu_count_pairs.restype = [vp, u32, u32, u32, vp, u32, u32, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_comm_unique_id.argtypes, L.fbgpu_comm_unique_id.restype = [vp], C.c_int
     L.fbgpu_comm_init.argtypes, L.fbgpu_comm_init.restype = [vp, i32, i32, vp], C.c_int
@@ -116,10 +120,11 @@ def load():
     L.fbgpu_node_devices.argtypes, L.fbgpu_node_devices.restype = [vp], i32
     L.fbgpu_node_owner.argtypes, L.fbgpu_node_owner.restype = [vp, u64], i32
     L.fbgpu_node_ctx.argtypes, L.fbgpu_node_ctx.restype = [vp, i32], vp
-    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "bsi_sum", "bsi_minmax"):
+    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "bsi_sum", "bsi_minmax"):
         src, dst = getattr(L, "fbgpu_" + name), getattr(L, "fbgpu_node_" + name)
         dst.argtypes, dst.restype = src.argtypes, src.restype
     L.fbgpu_node_row_counts.argtypes, L.fbgpu_node_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
+    L.fbgpu_node_row_counts_views.argtypes, L.fbgpu_node_row_counts_views.restype = [vp, u32, u32, vp, i32, vp, i32, vp, i32, vp, i64, vp], C.c_int
     _LIB = L
     return L
 
@@ -383,6 +388,30 @@ class Context:
             self._check(rc)
             return rid[: n.value], out[: n.value]
 
+    def row_counts_views(self, index, field, views, shards, row_ids=None, filter_ops=None, cap=1 << 20):
+        """row_counts with each row taken as its union over `views` (fbgpu_row_counts_views: TopK / Rows with from= / to=)"""
+        sh = _u64arr(shards)
+        vw = np.ascontiguousarray(np.asarray(views, dtype=np.uint32))
+        f = ops_array(filter_ops) if filter_ops else None
+        nf = len(filter_ops) if filter_ops else 0
+        n = C.c_int32(0)
+        if row_ids is not None:
+            ids = _u64arr(row_ids)
+            out = np.zeros(len(ids), dtype=np.uint64)
+            self._check(self.L.fbgpu_row_counts_views(self.h, index, field, vw.ctypes.data, len(vw), ids.ctypes.data, len(ids), f, nf, sh.ctypes.data, len(sh),
+                                                      None, out.ctypes.data, len(ids), C.byref(n)))
+            return out
+        cap = min(cap, 1 << 16)
+        while True:                                  # the library reports how many rows there are when the buffers are too small
+            rid, out = np.zeros(cap, dtype=np.uint64), np.zeros(cap, dtype=np.uint64)
+            rc = self.L.fbgpu_row_counts_views(self.h, index, field, vw.ctypes.data, len(vw), None, 0, f, nf, sh.ctypes.data, len(sh),
+                                               rid.ctypes.data, out.ctypes.data, cap, C.byref(n))
+            if rc == E_NOSPACE and n.value > cap:
+                cap = n.value
+                continue
+            self._check(rc)
+            return rid[: n.value], out[: n.value]
+
     def row_counts_per_shard(self, index, field, view, shards, row_ids, filter_ops=None):
         """[len(shards), len(row_ids)] matrix of per-shard counts (fbgpu_row_counts_per_shard)"""
         sh, ids = _u64arr(shards), _u64arr(row_ids)
@@ -411,6 +440,22 @@ class Context:
         nf = len(filter_ops) if filter_ops else 0
         self._check(self.L.fbgpu_groupby(self.h, index, fl.ctypes.data, vw.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
                                          f, nf, sh.ctypes.data, len(sh), out.ctypes.data))
+        return out.reshape([int(x) for x in n_rows])
+
+    def groupby_views(self, index, fields, views, row_ids, shards, filter_ops=None):
+        """groupby with dimension i's rows taken as their unions over the views listed in views[i] (fbgpu_groupby_views:
+        GroupBy over Rows(f, from=, to=) children)"""
+        sh = _u64arr(shards)
+        fl = np.ascontiguousarray(np.asarray(fields, dtype=np.uint32))
+        vw = np.ascontiguousarray(np.concatenate([np.asarray(v, dtype=np.uint32) for v in views]))
+        n_views = np.ascontiguousarray(np.asarray([len(v) for v in views], dtype=np.int32))
+        n_rows = np.ascontiguousarray(np.asarray([len(r) for r in row_ids], dtype=np.int32))
+        flat = _u64arr(np.concatenate([np.asarray(r, dtype=np.uint64) for r in row_ids]))
+        out = np.zeros(int(np.prod(n_rows.astype(np.int64))), dtype=np.uint64)
+        f = ops_array(filter_ops) if filter_ops else None
+        nf = len(filter_ops) if filter_ops else 0
+        self._check(self.L.fbgpu_groupby_views(self.h, index, fl.ctypes.data, vw.ctypes.data, n_views.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
+                                               f, nf, sh.ctypes.data, len(sh), out.ctypes.data))
         return out.reshape([int(x) for x in n_rows])
 
     def groupby_values(self, index, fields, views, row_ids, vfield, vview, bit_depth, values, shards, filter_ops=None):
@@ -527,6 +572,17 @@ class Node(Context):
         out = np.zeros(len(ids), dtype=np.uint64)
         self._check(self.L.fbgpu_node_row_counts(self.h, index, field, view, ids.ctypes.data, len(ids), f, len(filter_ops) if filter_ops else 0,
                                                  sh.ctypes.data, len(sh), out.ctypes.data))
+        return out
+
+    def row_counts_views(self, index, field, views, shards, row_ids=None, filter_ops=None, cap=1 << 20):
+        if row_ids is None:
+            raise NotImplementedError("fbgpu_node_row_counts_views takes explicit row ids")
+        sh, ids = _u64arr(shards), _u64arr(row_ids)
+        vw = np.ascontiguousarray(np.asarray(views, dtype=np.uint32))
+        f = ops_array(filter_ops) if filter_ops else None
+        out = np.zeros(len(ids), dtype=np.uint64)
+        self._check(self.L.fbgpu_node_row_counts_views(self.h, index, field, vw.ctypes.data, len(vw), ids.ctypes.data, len(ids), f,
+                                                       len(filter_ops) if filter_ops else 0, sh.ctypes.data, len(sh), out.ctypes.data))
         return out
 
 

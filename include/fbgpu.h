@@ -234,6 +234,18 @@ int fbgpu_row_counts(fbgpu_ctx *ctx, uint32_t index, uint32_t field, uint32_t vi
 int fbgpu_row_counts_per_shard(fbgpu_ctx *ctx, uint32_t index, uint32_t field, uint32_t view,
                                const uint64_t *row_ids, int32_t n_rows, const fbgpu_op *filter, int32_t n_filter_ops,
                                const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+/* fbgpu_row_counts with each row taken as its union over n_views (>= 1, any number) views of the field: the counts of TopK(f,
+ * from=, to=) and the row ids of Rows(f, from=, to=) on a time field, whose covering views are listed in `views`
+ * (executeTopKShardTime executor.go:2506-2533 over the mergerator :2570; executeRowsShard :4107-4127).
+ * count(r) = |(∪_v Row(field = r) in view v) [∩ filter]|.  row_ids != NULL: out_counts[i] for row_ids[i], all-reduced over the
+ * communicator.  row_ids == NULL: the candidates are the row ids with a container in at least one listed view in at least one
+ * listed shard; the rows with count > 0 are written sorted by (count desc, row id asc), with fbgpu_row_counts' FBGPU_E_NOSPACE /
+ * *out_n contract, not all-reduced.  A view never loaded, or without a fragment in a shard, contributes nothing there; a view
+ * listed twice counts once.  n_views == 1 is fbgpu_row_counts. */
+int fbgpu_row_counts_views(fbgpu_ctx *ctx, uint32_t index, uint32_t field, const uint32_t *views, int32_t n_views,
+                           const uint64_t *row_ids, int32_t n_rows, const fbgpu_op *filter, int32_t n_filter_ops,
+                           const uint64_t *shards, int64_t n_shards,
+                           uint64_t *out_row_ids, uint64_t *out_counts, int32_t cap, int32_t *out_n);
 
 /* Many fused Intersect+Count pairs in ONE launch: out_counts[i] = |Row(field_a = rows_a[i]) ∩ Row(field_b = rows_b[i])| over
  * the shards — the inner loop of fragment.top with a plain-row Src (count = Src.intersectionCount(row) per candidate
@@ -259,6 +271,15 @@ int fbgpu_groupby(fbgpu_ctx *ctx, uint32_t index, const uint32_t *fields, const 
                   const uint64_t *row_ids_flat, const int32_t *n_rows,
                   const fbgpu_op *filter, int32_t n_filter_ops,
                   const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+/* fbgpu_groupby with dimension i's rows taken as their unions over n_views[i] (>= 1) views of fields[i]: GroupBy(Rows(f,
+ * from=, to=), ...) on time fields (timeFragmentsRowIterator executor.go:8755-8768).  The views of all dimensions are listed
+ * one dimension after the other in views_flat.  Same dense output tensor (rightmost fastest) and all-reduce as fbgpu_groupby;
+ * with every n_views[i] == 1 the result is fbgpu_groupby's.  A shard lacking a dimension's fragment in every listed view
+ * contributes nothing.  Argument errors (n_fields outside 1..8, n_views[i] < 1, n_rows[i] outside 0..65535, null pointers)
+ * are reported before the device check. */
+int fbgpu_groupby_views(fbgpu_ctx *ctx, uint32_t index, const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views,
+                        int32_t n_fields, const uint64_t *row_ids_flat, const int32_t *n_rows,
+                        const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
 
 /* GroupBy whose last dimension is the values of an int field: GroupBy(Rows(f1), ..., Rows(v)) with v an int field, whose groups
  * are v's values (FieldRow.Value, executor.go:8740-8750), in one device pass instead of one Row(v == value) per value.
@@ -337,6 +358,12 @@ int fbgpu_node_count_pairs(fbgpu_node *node, uint32_t index, uint32_t field_a, u
                            const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
 int fbgpu_node_row_counts(fbgpu_node *node, uint32_t index, uint32_t field, uint32_t view, const uint64_t *row_ids, int32_t n_rows,
                           const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+int fbgpu_node_row_counts_views(fbgpu_node *node, uint32_t index, uint32_t field, const uint32_t *views, int32_t n_views,
+                                const uint64_t *row_ids, int32_t n_rows, const fbgpu_op *filter, int32_t n_filter_ops,
+                                const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+int fbgpu_node_groupby_views(fbgpu_node *node, uint32_t index, const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views,
+                             int32_t n_fields, const uint64_t *row_ids_flat, const int32_t *n_rows,
+                             const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
 int fbgpu_node_groupby(fbgpu_node *node, uint32_t index, const uint32_t *fields, const uint32_t *views, int32_t n_fields,
                        const uint64_t *row_ids_flat, const int32_t *n_rows, const fbgpu_op *filter, int32_t n_filter_ops,
                        const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
