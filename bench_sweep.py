@@ -12,6 +12,8 @@
             Row(v == value)-per-value composition (only when named in --configs).
   config T: TopK(f, from=, to=) and GroupBy(Rows(a), Rows(f, from=, to=)) over 48 views of a quantum-YMD field,
             fbgpu_row_counts_views / fbgpu_groupby_views against the operand-row composition (only when named in --configs).
+  config M: GroupBy(Rows(a), Rows(v), Rows(w)) and GroupBy(Rows(t, from=, to=), Rows(v)) with int fields of 8 / 64 / 256
+            distinct values each, fbgpu_groupby_mixed against the composition (only when named in --configs).
 Every point is spot-checked against the CPU oracle on a few shards (the checker, not the thing measured)."""
 import argparse
 import json
@@ -273,10 +275,10 @@ def config_percentile(args, out):
 
 
 class _NoGroupByValues(_KernelMs):
-    """the same proxy without groupby_values: the executor takes the Row(v == value)-per-value composition"""
+    """the same proxy without groupby_values / groupby_mixed: the executor takes the Row(v == value)-per-value composition"""
 
     def __getattr__(self, name):
-        if name == "groupby_values":
+        if name in ("groupby_values", "groupby_mixed"):
             raise AttributeError(name)
         return super().__getattr__(name)
 
@@ -390,35 +392,20 @@ def _card():
         return {"name": None, "error": f"nvidia-smi unavailable: {e}"}
 
 
-def config_time_views(args, out):
-    """TopK(f, from=, to=) and GroupBy(Rows(a), Rows(f, from=, to=)) over a range of 48 views, without and with a 1 % filter row,
-    through the executor.  f: a quantum-YMD time field of 256 rows over --groupby-shards shards, 64 Ki bits per shard, each at a
-    random column with a timestamp spread uniformly over the 120 days from 2019-01-01 (every bit is in its day, month, year and
-    standard views); a: a 256-row set field at 1/256 density per row.  The device arm (fbgpu_row_counts_views /
-    fbgpu_groupby_views) runs over all shards.  The composition arm (per row, a Row over the views, read back and stored as a row of
-    the scratch field, then one row-count or GroupBy call) re-sends the scratch fragment of every touched shard and commits the
-    store again for every row (about two minutes per query on one shard on an H100): it runs over the first --composition-shards
-    shards, for
-    --composition-steps steps alternated with the device arm over the same shards, every step reported (the scratch field grows
-    with each).  Both arms must return the same result.  Progress goes to stderr."""
+TIME_RANGE = "from=2019-01-05T00:00, to=2019-04-20T00:00"       # configs T and M: 48 views of a quantum-YMD field
+
+
+def _load_time_field(h, idx, ft, shards, R, per_shard, days):
+    """config T's time field: R rows, per_shard bits per shard, each at a random column with a timestamp spread uniformly over
+    `days` days from 2019-01-01, in its day, month, year and standard views"""
     import datetime
-    from featurebase_b200 import datagen as D, executor as X, lib as L, roaring_io
-    S, R, per_shard, days = args.groupby_shards, 256, 1 << 16, 120
-    shards = np.arange(S, dtype=np.uint64)
-    h = X.Holder()
-    idx = h.create_index("i", track_existence=False)
-    fa, ff, ft = idx.create_field("a"), idx.create_field("c"), idx.create_field("f", "time", quantum="YMD")
-    t0 = time.time()
-    for fld, rows, p in ((fa, range(R), 1 / 256), (ff, [0], 0.01)):
-        bulk = D.fragments(60 + fld.id, shards, list(rows), p)
-        h.ctx.load_fragments(idx.id, fld.id, X.VIEW_STANDARD, shards, bulk.buf, bulk.offsets)
-        del bulk
+    from featurebase_b200 import executor as X, roaring_io
     rng = np.random.default_rng(61)
     day0 = datetime.date(2019, 1, 1)
     names = [(day0 + datetime.timedelta(days=d)).strftime("%Y%m%d") for d in range(days)]
     month_of = np.array([int(n[4:6]) for n in names])
     views = {}                                                   # view name -> [per-shard fragment bytes]
-    for s in range(S):
+    for s in range(len(shards)):
         col = rng.integers(0, SW, per_shard, dtype=np.uint64)
         pos = rng.integers(0, R, per_shard, dtype=np.uint64) * np.uint64(SW) + col
         day = rng.integers(0, days, per_shard)
@@ -438,10 +425,35 @@ def config_time_views(args, out):
         offsets = np.concatenate([[0], np.cumsum([len(b) for b in blobs])]).astype(np.uint64)
         h.ctx.load_fragments(idx.id, ft.id, vid, shards, np.frombuffer(b"".join(blobs), dtype=np.uint8), offsets)
     del views
+
+
+def config_time_views(args, out):
+    """TopK(f, from=, to=) and GroupBy(Rows(a), Rows(f, from=, to=)) over a range of 48 views, without and with a 1 % filter row,
+    through the executor.  f: a quantum-YMD time field of 256 rows over --groupby-shards shards, 64 Ki bits per shard, each at a
+    random column with a timestamp spread uniformly over the 120 days from 2019-01-01 (every bit is in its day, month, year and
+    standard views); a: a 256-row set field at 1/256 density per row.  The device arm (fbgpu_row_counts_views /
+    fbgpu_groupby_views) runs over all shards.  The composition arm (per row, a Row over the views, read back and stored as a row of
+    the scratch field, then one row-count or GroupBy call) re-sends the scratch fragment of every touched shard and commits the
+    store again for every row (about two minutes per query on one shard on an H100): it runs over the first --composition-shards
+    shards, for
+    --composition-steps steps alternated with the device arm over the same shards, every step reported (the scratch field grows
+    with each).  Both arms must return the same result.  Progress goes to stderr."""
+    from featurebase_b200 import datagen as D, executor as X, lib as L
+    S, R, per_shard, days = args.groupby_shards, 256, 1 << 16, 120
+    shards = np.arange(S, dtype=np.uint64)
+    h = X.Holder()
+    idx = h.create_index("i", track_existence=False)
+    fa, ff, ft = idx.create_field("a"), idx.create_field("c"), idx.create_field("f", "time", quantum="YMD")
+    t0 = time.time()
+    for fld, rows, p in ((fa, range(R), 1 / 256), (ff, [0], 0.01)):
+        bulk = D.fragments(60 + fld.id, shards, list(rows), p)
+        h.ctx.load_fragments(idx.id, fld.id, X.VIEW_STANDARD, shards, bulk.buf, bulk.offsets)
+        del bulk
+    _load_time_field(h, idx, ft, shards, R, per_shard, days)
     h.ctx.commit()
     idx.shards.update(range(S))
     load_s = time.time() - t0
-    rng_q = "from=2019-01-05T00:00, to=2019-04-20T00:00"
+    rng_q = TIME_RANGE
     n_views = len(X.Executor(h)._time_view_ids(ft, {"from": "2019-01-05T00:00", "to": "2019-04-20T00:00"}))
     print(f"config T: loaded {S} shards in {load_s:.1f}s; the range covers {n_views} views", file=sys.stderr, flush=True)
     real = h.ctx
@@ -486,6 +498,97 @@ def config_time_views(args, out):
                 if name == "composition":
                     o["wall_ms_per_step"] = [round(x, 2) for x in dd["wall"]]
                 out(o)
+    real.close()
+
+
+def config_groupby_mixed(args, out):
+    """GroupBy(Rows(a), Rows(v), Rows(w)) and GroupBy(Rows(t, from=, to=), Rows(v)) over --groupby-shards shards, without and with
+    a 1 % filter row, through the executor.  v and w: int fields holding one of D values (uniform) for each of the first 16,384
+    columns of every shard, D x D in {8 x 8, 64 x 64, 256 x 256} (256 x 256 groups exceed one call's 65,535 and take two
+    calls); a: a 256-row set field at 1/256 density per row; t: config T's quantum-YMD field (256 rows) over config T's range of
+    48 views.  The device arm (fbgpu_groupby_mixed) runs over all shards at every D.  The composition arm (one Row per value and
+    per time row, each read back and stored as a row of the scratch field, then fbgpu_groupby) runs over the first
+    --composition-shards shards at D = 8 without the filter, for --composition-steps steps alternated with the device arm over
+    the same shards: it stores D + D (or 256 time rows + D) scratch rows per step and is slower at every step.  Both arms must
+    return the same groups; every device result's total must equal Σ_r Count(Row(a=r) or Row(t=r) ∩ filter ∩ exists(v) (∩
+    exists(w))).  Progress goes to stderr."""
+    from featurebase_b200 import datagen as D, executor as X, lib as L
+    S, R, n_cols = args.groupby_shards, 256, 16384
+    shards = np.arange(S, dtype=np.uint64)
+    h = X.Holder()
+    idx = h.create_index("i", track_existence=False)
+    fa, ff, ft = idx.create_field("a"), idx.create_field("c"), idx.create_field("t", "time", quantum="YMD")
+    dvals = (8, 64, 256)
+    t0 = time.time()
+    for fld, rows, p in ((fa, range(R), 1 / 256), (ff, [0], 0.01)):
+        bulk = D.fragments(70 + fld.id, shards, list(rows), p)
+        h.ctx.load_fragments(idx.id, fld.id, X.VIEW_STANDARD, shards, bulk.buf, bulk.offsets)
+        del bulk
+    _load_time_field(h, idx, ft, shards, R, 1 << 16, 120)
+    for k, d in enumerate(dvals):
+        for name in ("v", "w"):
+            f = idx.create_field(f"{name}{d}", "int", min=0, max=d - 1)
+            for s in range(S):
+                h.ctx.load_fragment(idx.id, f.id, X.VIEW_BSI, s, D.bsi_fragment(80 + 2 * k + (name == "w"), s, n_cols, f.bit_depth, 0, d - 1))
+    h.ctx.commit()
+    idx.shards.update(range(S))
+    load_s = time.time() - t0
+    tviews = X.Executor(h)._time_view_ids(ft, {"from": "2019-01-05T00:00", "to": "2019-04-20T00:00"})
+    print(f"config M: loaded {S} shards in {load_s:.1f}s", file=sys.stderr, flush=True)
+    real = h.ctx
+    card = _card()
+    dev, comp = _KernelMs(real), _NoGroupByValues(real)
+    CS = min(S, args.composition_shards)
+    op = lambda code, field=0, view=0, argc=0: L.Op(code, field, view, argc, 0, 0, 0, 0)
+    for d in dvals:
+        v, w = idx.fields[f"v{d}"], idx.fields[f"w{d}"]
+        for q_time in (False, True):
+            for q_filter in (False, True):
+                q = (f"GroupBy(Rows(t, {TIME_RANGE}), Rows(v{d})" if q_time else f"GroupBy(Rows(a), Rows(v{d}), Rows(w{d})") + (", filter=Row(c=0))" if q_filter else ")")
+                exists = [op(L.OP_ROW, v.id, X.VIEW_BSI)] + ([] if q_time else [op(L.OP_ROW, w.id, X.VIEW_BSI), op(L.OP_INTERSECT, argc=2)])
+                if q_filter:
+                    exists += [op(L.OP_ROW, ff.id), op(L.OP_INTERSECT, argc=2)]
+                runs = [(S, {"device": dev})]
+                if d == dvals[0] and not q_filter and args.composition_steps > 0:
+                    runs.append((CS, {"device": dev, "composition": comp}))
+                for n_sh, arms in runs:
+                    sh = list(range(n_sh))
+                    if q_time:
+                        want = int(real.row_counts_views(idx.id, ft.id, tviews, sh, row_ids=list(range(R)), filter_ops=exists).sum())
+                    else:
+                        want = int(real.row_counts(idx.id, fa.id, X.VIEW_STANDARD, sh, row_ids=list(range(R)), filter_ops=exists).sum())
+                    rec = {name: {"wall": [], "kernel_ms": [], "queries": []} for name in arms}
+                    res = {}
+                    for i in range(1 + args.steps):          # one warm-up round of the device arm, then alternate the arms
+                        for name in (sorted(arms) if i % 2 == 0 else sorted(arms, reverse=True)):
+                            if name == "composition" and len(rec[name]["wall"]) >= args.composition_steps:
+                                continue
+                            h.ctx = arms[name]
+                            q0, arms[name].ms = real.counters()["queries"], 0.0
+                            t1 = time.perf_counter()
+                            r = X.Executor(h).execute("i", q, sh)[0]
+                            wall = (time.perf_counter() - t1) * 1e3
+                            res.setdefault(name, r)
+                            assert r == res[name], (q, name)
+                            print(f"config M: {q} over {n_sh} shards, {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                            if i >= 1 or name == "composition":
+                                rec[name]["wall"].append(wall)
+                                rec[name]["kernel_ms"].append(arms[name].ms)
+                                rec[name]["queries"].append(real.counters()["queries"] - q0)
+                    h.ctx = real
+                    assert all(r == res["device"] for r in res.values()), q
+                    assert sum(g[1] for g in res["device"]) == want > 0, (q, want)
+                    for name, dd in rec.items():
+                        o = {"config": "M", "query": q, "arm": name, "gpu": card, "distinct_values": [d] if q_time else [d, d], "shards": n_sh,
+                             "groups": len(res[name]), "equal_to_composition": ("composition" in res) or None,
+                             "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])), "wall_ms_max": float(np.max(dd["wall"])),
+                             "kernel_ms": float(np.median(dd["kernel_ms"])), "queries": int(np.median(dd["queries"])), "steps": len(dd["wall"]), "load_s": round(load_s, 1),
+                             "kernel": "eval_kernel + groupby_values_kernel" if name == "device" else "eval_kernel (a Row per value / time row) + groupby kernels",
+                             "note": "median over the timed steps of the executor call (wall clock, Distinct and Rows pre-passes included), of the summed "
+                                     "last_query_gpu_ms and of the number of its library queries"}
+                        if name == "composition":
+                            o["wall_ms_per_step"] = [round(x, 2) for x in dd["wall"]]
+                        out(o)
     real.close()
 
 
@@ -583,8 +686,8 @@ def main():
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--shards", type=int, default=1024)
     ap.add_argument("--groupby-shards", type=int, default=512)
-    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T: steps of the composition arm (each one slower than the last)")
-    ap.add_argument("--composition-shards", type=int, default=1, help="config T: shards of the composition arm and of the device arm timed beside it")
+    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M: steps of the composition arm (each one slower than the last)")
+    ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M: shards of the composition arm and of the device arm timed beside it")
     ap.add_argument("--generators", default="uniform,clustered")
     ap.add_argument("--batched", action="store_true", help="also time the multi-pair launch (config 5b)")
     ap.add_argument("--densities", default="0.0001,0.001,0.01,0.03,0.0625,0.125,0.25,0.5")
@@ -605,6 +708,8 @@ def main():
             config_groupby_values(args, out)
         elif c == "T":
             config_time_views(args, out)
+        elif c == "M":
+            config_groupby_mixed(args, out)
         elif c == "3L":     # the same BSI query at 256 shards (268 M records, 1.1 GB of planes): shows the kernel away from the launch-bound regime
             config3(args, out, n_rec=256 * SW, nf=1)
         else:

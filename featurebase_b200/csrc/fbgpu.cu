@@ -1874,8 +1874,8 @@ extern "C" int fbgpu_groupby_views(fbgpu_ctx* c, uint32_t index, const uint32_t*
     return groupby_dims(c, index, dims, filter, n_filter_ops, shards, n_shards, out_counts);
 } FBGPU_CATCH
 
-// ------------------------------------------------------------------ GroupBy over the values of an int field
-// the int dimension of fbgpu_groupby_values: field, view, depth and the ascending stored values that are its groups
+// ------------------------------------------------------------------ GroupBy over the values of int fields
+// one int dimension of fbgpu_groupby_values / fbgpu_groupby_mixed: field, BSI view, depth and the ascending stored values that are its groups
 struct GvInt { uint32_t field, view; int32_t depth; const int64_t* values; int32_t n_values; };
 
 // the argument checks fbgpu_groupby_values and its node form make before any device is touched
@@ -1891,28 +1891,71 @@ static int groupby_values_args(const void* handle, const uint32_t* fields, const
     return 0;
 }
 
-// one groupby_values_kernel pass over the shards: counts[nB or 1][n_values] of consider = filter ∩ exists(v) (∩ Row(b = row))
-static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, uint32_t fvB, const uint64_t* rowsB, int nB, const GvInt& v,
+// the argument checks fbgpu_groupby_mixed and its node form make before any device is touched (n_rows is checked after it)
+static int groupby_mixed_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                              const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews,
+                              const int32_t* bit_depths, int32_t n_ints, const int64_t* values_flat, const int32_t* n_values,
+                              const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts) {
+    if (!handle || !vfields || !vviews || !bit_depths || !values_flat || !n_values || !out_counts ||
+        (n_fields > 0 && (!fields || !views_flat || !n_views || !row_ids_flat || !n_rows)) ||
+        n_filter_ops < 0 || (n_filter_ops && !filter) || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
+    if (n_fields < 0 || n_fields > 7) return fail(FBGPU_E_INVALID, "n_fields=%d outside 0..7", n_fields);
+    if (n_ints < 1 || n_ints > kGvMaxInts) return fail(FBGPU_E_INVALID, "n_ints=%d outside 1..%d", n_ints, kGvMaxInts);
+    if (n_fields + n_ints > 8) return fail(FBGPU_E_INVALID, "n_fields + n_ints = %d exceeds 8", n_fields + n_ints);
+    for (int32_t i = 0; i < n_fields; i++)
+        if (n_views[i] < 1) return fail(FBGPU_E_INVALID, "n_views[%d]=%d < 1", i, n_views[i]);
+    const int64_t* vals = values_flat;
+    double groups = 1;
+    for (int32_t k = 0; k < n_ints; k++) {
+        if (bit_depths[k] < 0 || bit_depths[k] > 64) return fail(FBGPU_E_INVALID, "bit_depths[%d]=%d outside 0..64", k, bit_depths[k]);
+        if (n_values[k] < 1 || n_values[k] > 65535) return fail(FBGPU_E_INVALID, "n_values[%d]=%d outside 1..65535", k, n_values[k]);
+        for (int32_t i = 1; i < n_values[k]; i++)
+            if (vals[i] <= vals[i - 1]) return fail(FBGPU_E_INVALID, "values[%d] are not strictly ascending at position %d", k, i);
+        vals += n_values[k];
+        groups *= n_values[k];
+    }
+    if (groups > 65535) return fail(FBGPU_E_INVALID, "product of n_values %.0f exceeds 65535", groups);
+    return 0;
+}
+
+// one groupby_values_kernel pass over the shards: counts[nB or 1][groups] of consider = filter ∩ exists(v_1) ∩ ... (∩ Row(b = row))
+static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* null: no set dimension */, const std::vector<GvInt>& v,
                                const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards, uint64_t* out) {
-    const std::vector<fbgpu_op> full = and_row(filter.data(), (int32_t)filter.size(), v.field, v.view, 0);
+    std::vector<fbgpu_op> full = filter;
+    for (const GvInt& x : v) full = and_row(full.data(), (int32_t)full.size(), x.field, x.view, 0);
     Query q(c); Workspace* w = q.w;
     int rc = q.open(index, full.data(), (int32_t)full.size(), shards, n_shards); if (rc) return rc;
-    const uint32_t fvV = view_id_locked(c, ViewKey{ index, v.field, v.view }, false);
-    const size_t ncnt = (size_t)(rowsB ? nB : 1) * (size_t)v.n_values;
-    if (w->d_rows.ensure(((size_t)nB + (size_t)v.n_values) * 8) || w->d_counts.ensure(ncnt * 8) || w->h_out.ensure(ncnt * 8)) return FBGPU_E_NOMEM;
-    std::vector<uint64_t> in(v.values, v.values + v.n_values);      // [values (as int64) | b rows]
-    if (rowsB) in.insert(in.end(), rowsB, rowsB + nB);
+    GvInts k{};
+    k.n = (int)v.size(); k.n_groups = 1;
+    std::vector<uint64_t> in;                                        // [values (as int64) | b rows | b view slots (u32)]
+    for (int i = 0; i < k.n; i++) {
+        k.fv[i] = view_id_locked(c, ViewKey{ index, v[(size_t)i].field, v[(size_t)i].view }, false);
+        k.depth[i] = v[(size_t)i].depth; k.off[i] = (int)in.size(); k.n_values[i] = v[(size_t)i].n_values;
+        k.n_groups *= v[(size_t)i].n_values;
+        in.insert(in.end(), v[(size_t)i].values, v[(size_t)i].values + v[(size_t)i].n_values);
+    }
+    const size_t n_vals = in.size();
+    const int nB = b ? b->n_rows : 0;
+    const std::vector<uint32_t> fvsB = b ? view_slots(c, index, b->field, b->views, b->n_views) : std::vector<uint32_t>{ kNoView };
+    const size_t nvB = fvsB.size();
+    if (b) in.insert(in.end(), b->rows, b->rows + nB);
+    const size_t n_in = in.size();
+    if (nvB > 1) in.resize(n_in + (nvB + 1) / 2);
+    if (nvB > 1) memcpy(in.data() + n_in, fvsB.data(), nvB * 4);
+    const size_t ncnt = (size_t)(b ? nB : 1) * (size_t)k.n_groups;
+    if (w->d_rows.ensure(in.size() * 8) || w->d_counts.ensure(ncnt * 8) || w->h_out.ensure(ncnt * 8)) return FBGPU_E_NOMEM;
     CUDA_TRY(cudaMemcpyAsync(w->d_rows.p, in.data(), in.size() * 8, cudaMemcpyHostToDevice, w->stream));
     CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, ncnt * 8, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));   // `in` is a local
     const long long* d_values = (const long long*)w->d_rows.p;
-    const uint64_t* d_rowsB = rowsB ? (const uint64_t*)w->d_rows.p + v.n_values : nullptr;
+    const uint64_t* d_rowsB = b ? (const uint64_t*)w->d_rows.p + n_vals : nullptr;
+    const uint32_t* d_fvsB = nvB > 1 ? (const uint32_t*)((const uint64_t*)w->d_rows.p + n_in) : nullptr;
     CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
     for (long long u0 = 0; u0 < q.n_units; u0 += c->unit_batch) {
         const long long nu = std::min(c->unit_batch, q.n_units - u0);
         rc = q.eval(u0, nu); if (rc) return rc;
         const long long grid = std::min<long long>(nu, (long long)c->sm_count * kGvCtasPerSm);
-        groupby_values_kernel<<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), fvV, v.depth, d_values, v.n_values, fvB, d_rowsB, nB,
+        groupby_values_kernel<<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB,
                                                                             (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, (unsigned long long*)w->d_counts.p);
         CUDA_TRY(cudaGetLastError()); q.launches++;
     }
@@ -1926,17 +1969,35 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, uint32_t fvB, const
     return 0;
 }
 
-// set dimensions beyond the last are peeled into the filter as groupby_rec does; the last one (if any) is the kernel's b
-static int groupby_values_rec(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int nf, const uint64_t* const* rows, const int32_t* n_rows,
-                              const GvInt& v, const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards, uint64_t* out) {
-    if (nf == 0) return groupby_values_leaf(c, index, kNoView, nullptr, 0, v, filter, shards, n_shards, out);
-    if (nf == 1) return groupby_values_leaf(c, index, view_id_locked(c, ViewKey{ index, fields[0], views[0] }, false), rows[0], n_rows[0], v, filter, shards, n_shards, out);
-    size_t sub = (size_t)v.n_values; for (int i = 1; i < nf; i++) sub *= (size_t)n_rows[i];
-    for (int r = 0; r < n_rows[0]; r++) {
-        int rc = groupby_values_rec(c, index, fields + 1, views + 1, nf - 1, rows + 1, n_rows + 1, v, and_row(filter.data(), (int32_t)filter.size(), fields[0], views[0], rows[0][r]),
+// set dimensions before the last are peeled into the filter as groupby_rec does (a multi-view one as the union of its row over
+// the views); the last one (if any) is the kernel's b
+static int groupby_values_rec(fbgpu_ctx* c, uint32_t index, const GbDim* d, int nf, const std::vector<GvInt>& v, const std::vector<fbgpu_op>& filter,
+                              const uint64_t* shards, int64_t n_shards, uint64_t* out) {
+    if (nf <= 1) return groupby_values_leaf(c, index, nf ? d : nullptr, v, filter, shards, n_shards, out);
+    size_t sub = 1; for (const GvInt& x : v) sub *= (size_t)x.n_values;
+    for (int i = 1; i < nf; i++) sub *= (size_t)d[i].n_rows;
+    for (int r = 0; r < d[0].n_rows; r++) {
+        int rc = groupby_values_rec(c, index, d + 1, nf - 1, v, and_row(filter.data(), (int32_t)filter.size(), d[0].field, d[0].views, d[0].n_views, d[0].rows[r]),
                                     shards, n_shards, out + (size_t)r * sub); if (rc) return rc;
     }
     return 0;
+}
+
+// fbgpu_groupby_values / fbgpu_groupby_mixed once the arguments but n_rows are checked: the set dimensions' rows are laid out
+// from row_ids_flat, the output zeroed, the store locked
+static int groupby_values_query(fbgpu_ctx* c, uint32_t index, std::vector<GbDim>& dims, const uint64_t* row_ids_flat, const std::vector<GvInt>& v,
+                                const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) {
+    std::shared_lock<std::shared_mutex> lk;
+    int rc = begin_query(c, lk); if (rc) return rc;
+    const uint64_t* p = row_ids_flat; size_t total = 1;
+    for (const GvInt& x : v) total *= (size_t)x.n_values;
+    for (size_t i = 0; i < dims.size(); i++) {
+        if (dims[i].n_rows < 0 || dims[i].n_rows > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", (int)i, dims[i].n_rows);
+        dims[i].rows = p; p += dims[i].n_rows; total *= (size_t)dims[i].n_rows;
+    }
+    memset(out_counts, 0, total * 8);
+    if (total == 0) return 0;
+    return groupby_values_rec(c, index, dims.data(), (int)dims.size(), v, std::vector<fbgpu_op>(filter, filter + n_filter_ops), shards, n_shards, out_counts);
 }
 
 extern "C" int fbgpu_groupby_values(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
@@ -1944,14 +2005,25 @@ extern "C" int fbgpu_groupby_values(fbgpu_ctx* c, uint32_t index, const uint32_t
                                     const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     int rc = groupby_values_args(c, fields, views, n_fields, row_ids_flat, n_rows, bit_depth, values, n_values, filter, n_filter_ops, shards, n_shards, out_counts);
     if (rc) return rc;
-    std::shared_lock<std::shared_mutex> lk;
-    rc = begin_query(c, lk); if (rc) return rc;
-    std::vector<const uint64_t*> rows((size_t)n_fields); const uint64_t* p = row_ids_flat; size_t total = (size_t)n_values;
-    for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); rows[(size_t)i] = p; p += n_rows[i]; total *= (size_t)n_rows[i]; }
-    memset(out_counts, 0, total * 8);
-    if (total == 0) return 0;
-    const GvInt v{ vfield, vview, bit_depth, values, n_values };
-    return groupby_values_rec(c, index, fields, views, n_fields, rows.data(), n_rows, v, std::vector<fbgpu_op>(filter, filter + n_filter_ops), shards, n_shards, out_counts);
+    std::vector<GbDim> dims((size_t)n_fields);
+    for (int i = 0; i < n_fields; i++) dims[(size_t)i] = GbDim{ fields[i], views + i, 1, nullptr, n_rows[i] };
+    return groupby_values_query(c, index, dims, row_ids_flat, { GvInt{ vfield, vview, bit_depth, values, n_values } }, filter, n_filter_ops, shards, n_shards, out_counts);
+} FBGPU_CATCH
+
+// GroupBy(Rows(f1), ..., Rows(v1), Rows(v2), ...) with set dimensions (each row a union over views, as fbgpu_groupby_views) and
+// one or more int dimensions: fbgpu_groupby_values generalised; with one int field and single views it is that call
+extern "C" int fbgpu_groupby_mixed(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                   const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews, const int32_t* bit_depths,
+                                   int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, const fbgpu_op* filter, int32_t n_filter_ops,
+                                   const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
+    int rc = groupby_mixed_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
+                                filter, n_filter_ops, shards, n_shards, out_counts);
+    if (rc) return rc;
+    std::vector<GbDim> dims((size_t)n_fields); const uint32_t* vw = views_flat;
+    for (int i = 0; i < n_fields; i++) { dims[(size_t)i] = GbDim{ fields[i], vw, n_views[i], nullptr, n_rows[i] }; vw += n_views[i]; }
+    std::vector<GvInt> ints((size_t)n_ints); const int64_t* vals = values_flat;
+    for (int k = 0; k < n_ints; k++) { ints[(size_t)k] = GvInt{ vfields[k], vviews[k], bit_depths[k], vals, n_values[k] }; vals += n_values[k]; }
+    return groupby_values_query(c, index, dims, row_ids_flat, ints, filter, n_filter_ops, shards, n_shards, out_counts);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ comm

@@ -1977,23 +1977,30 @@ groupby_direct_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ ro
 }
 
 // ------------------------------------------------------------------------------------------------
-// groupby_values_kernel (fbgpu_groupby_values): GroupBy whose last dimension is the values of an int field, optionally after one
-// set field b — counts[b-row][j] += |{columns of consider ∩ Row(b = b-row) whose stored value is values[j]}|, or counts[j] without
-// b.  consider = filter ∩ exists(v), one 8 KiB bitmap per (shard, slot) unit from eval_kernel.  The groups of an int field are
-// its values (groupByIterator with FieldRow.Value, executor.go:8740-8750); the reference reaches each one through a
-// Row(v == value) plane sweep.  Here one CTA per unit walks the unit in ranges of kGvRange columns, skipping a range without a
-// consider bit, and for each range:
-//   1. assembles every consider column's magnitude (one u64 per column) and sign from the planes, one warp per plane;
-//   2. maps each column's stored value (sign ? -magnitude : magnitude, wrapping like fbgpu_extract) to its position in the
-//      ascending `values` by binary search, kGvNone when absent.  Sign set with magnitude 0 is no value: Row(v == 0) does not
-//      hold such a column;
-//   3. walks b's rows restricted to the range (a warp per row, the rows resolved 32 at a time by the lanes) and adds 1 per
-//      column with a value; without b, the counts of the first kGvHist values are summed in shared memory per unit.
-// Each plane and b-row container is read once per range it meets: a bitmap word by word, a run container from the first
-// interval that reaches the range (intervals are sorted), an array in full, because array payloads may be stored in the
-// bank-striped order of stripe.h, which no search can use.  47 KiB of shared memory: four CTAs per SM.
-// A shard missing the int field's fragment has an empty consider set, one missing b's fragment resolves no b-row: either
-// contributes nothing (executor.go:8769-8772).
+// groupby_values_kernel (fbgpu_groupby_values, fbgpu_groupby_mixed): GroupBy whose trailing dimensions are the values of one
+// to eight int fields, optionally after one set field b — counts[b-row][g] += |{columns of consider ∩ Row(b = b-row) whose
+// stored values are those of group g}|, or counts[g] without b, where g is the row-major index (rightmost fastest) of one listed
+// value per int field.  consider = filter ∩ exists(v_1) ∩ ... ∩ exists(v_K), one 8 KiB bitmap per (shard, slot) unit from
+// eval_kernel.  The groups of an int field are its values (groupByIterator with FieldRow.Value, executor.go:8740-8750); the
+// reference reaches each one through a Row(v == value) plane sweep.  Here one CTA per unit walks the unit in ranges of kGvRange
+// columns, skipping a range without a consider bit, and for each range:
+//   1. for each int field k in turn, assembles every consider column's magnitude (one u64 per column) and sign from v_k's
+//      planes, one warp per plane; maps the column's stored value (sign ? -magnitude : magnitude, wrapping like fbgpu_extract)
+//      to its position j_k in v_k's ascending value list by binary search, and folds it into the column's 16-bit group index,
+//      g = g * n_values[k] + j_k, or kGvNone as soon as one field's value is not listed.  Sign set with magnitude 0 is no
+//      value: Row(v == 0) does not hold such a column;
+//   2. walks b's rows restricted to the range and adds 1 per column with a group.  With one view a warp per row walks the
+//      row's container (the rows resolved 32 at a time by the lanes).  With several, a warp per row ORs the row's range from
+//      every view into a warp-private 64-word bitmap laid over mag[] (dead once the group indices are made) and counts its
+//      bits ∩ cons, so a column in two views counts once (the per-warp view merge of row_count_views_kernel);
+//      without b, the counts of the first kGvHist groups are summed in shared memory per unit.
+// The int fields' planes are resolved once per unit when they fit the kGvPlanes-entry table together (two 64-bit fields do),
+// otherwise each field's planes once per range.  Each plane and b-row container is read once per range it meets: a bitmap
+// word by word, a run container from the first interval that reaches the range (intervals are sorted), an array in full,
+// because array payloads may be stored in the bank-striped order of stripe.h, which no search can use.  48 KiB of static
+// shared memory: four CTAs per SM.
+// A shard missing an int field's fragment has an empty consider set, one missing b's fragment in every view resolves no
+// b-row: either contributes nothing (executor.go:8769-8772).
 // ------------------------------------------------------------------------------------------------
 constexpr int kGvThreads = 256;
 constexpr int kGvCtasPerSm = 4;
@@ -2001,23 +2008,32 @@ constexpr uint32_t kGvRange = 4096;                // columns per range
 constexpr int kGvRangeWords = (int)kGvRange / 64;
 constexpr int kGvHist = 1024;
 constexpr uint16_t kGvNone = 0xffff;
+constexpr int kGvMaxInts = 8;
+constexpr int kGvPlanes = 184;                     // plane table entries: what 48 KiB of static shared memory leaves
 
-// calls f(local column) for every column of [lo, lo + kGvRange) that is in the container and in the range's consider words
-// `cons`; warp-wide (every lane with the same r), the lanes share the work
-template <class F>
-__device__ __forceinline__ void gv_for_each(const Resolved& r, uint32_t lo, const unsigned long long* cons, int lane, F f) {
+// the int dimensions of one launch, passed by value
+struct GvInts {
+    int n;                                         // 1..kGvMaxInts
+    int n_groups;                                  // product of n_values, <= 65535: group indices are 16-bit
+    uint32_t fv[kGvMaxInts];                       // BSI view slots
+    int depth[kGvMaxInts];
+    int off[kGvMaxInts];                           // dimension k's ascending stored values: values[off[k] .. off[k] + n_values[k])
+    int n_values[kGvMaxInts];
+};
+
+// calls w(word, bits) with the container's bits in the 64-bit words of [lo, lo + kGvRange) (word 0 .. kGvRangeWords - 1; an
+// array reports one bit per call); warp-wide (every lane with the same r), the lanes share the work
+template <class W>
+__device__ __forceinline__ void gv_for_each_word(const Resolved& r, uint32_t lo, int lane, W w) {
     if (r.ptr == nullptr) return;
     if (r.typ == kBitmap) {
         const uint64_t* g = reinterpret_cast<const uint64_t*>(r.ptr) + (lo >> 6);
-        for (int i = lane; i < kGvRangeWords; i += 32) {
-            uint64_t v = __ldg(g + i) & cons[i];
-            while (v) { const int b = __ffsll((long long)v) - 1; f((uint32_t)i * 64 + (uint32_t)b); v &= v - 1; }
-        }
+        for (int i = lane; i < kGvRangeWords; i += 32) w((uint32_t)i, (uint64_t)__ldg(g + i));
     } else if (r.typ == kArray) {
         const uint16_t* a = reinterpret_cast<const uint16_t*>(r.ptr);
         for (uint32_t i = lane; i < r.card; i += 32) {
             const uint32_t v = (uint32_t)__ldg(a + i) - lo;                 // outside the range: >= kGvRange (unsigned)
-            if (v < kGvRange && ((cons[v >> 6] >> (v & 63)) & 1ull)) f(v);
+            if (v < kGvRange) w(v >> 6, 1ull << (v & 63));
         }
     } else {
         const uint32_t* r32 = reinterpret_cast<const uint32_t*>(r.ptr);    // {u16 start, u16 last} per interval
@@ -2029,28 +2045,42 @@ __device__ __forceinline__ void gv_for_each(const Resolved& r, uint32_t lo, cons
             if (s0 > hi) break;
             const uint32_t s = max(s0, lo) - lo, l = min(l0, hi) - lo;
             for (uint32_t i = (s >> 6) + lane; i <= (l >> 6); i += 32) {
-                uint64_t m = cons[i];
+                uint64_t m = ~0ull;
                 if (i == (s >> 6)) m &= ~0ull << (s & 63);
                 if (i == (l >> 6)) m &= ~0ull >> (63 - (l & 63));
-                while (m) { const int b = __ffsll((long long)m) - 1; f(i * 64 + (uint32_t)b); m &= m - 1; }
+                w(i, m);
             }
         }
     }
 }
 
+// calls f(local column) for every column of [lo, lo + kGvRange) that is in the container and in the range's consider words
+// `cons`; warp-wide, as gv_for_each_word
+template <class F>
+__device__ __forceinline__ void gv_for_each(const Resolved& r, uint32_t lo, const unsigned long long* cons, int lane, F f) {
+    gv_for_each_word(r, lo, lane, [&](uint32_t i, uint64_t m) {
+        m &= cons[i];
+        while (m) { const int b = __ffsll((long long)m) - 1; f(i * 64 + (uint32_t)b); m &= m - 1; }
+    });
+}
+
 __global__ void __launch_bounds__(kGvThreads, kGvCtasPerSm)
-groupby_values_kernel(StoreRef st, uint32_t fvV, int depth, const long long* __restrict__ values, int n_values,
-                      uint32_t fvB, const uint64_t* __restrict__ rowsB /* null: no set field */, int nB,
+groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__ values,
+                      const uint64_t* __restrict__ rowsB /* null: no set field */, int nB,
+                      uint32_t fvB, const uint32_t* __restrict__ fvsB /* nvB > 1: b's view slots, each row taken as its union */, int nvB,
                       const uint4* __restrict__ consider, const uint64_t* __restrict__ shards, long long n_units,
-                      unsigned long long* __restrict__ counts /* [nB or 1][n_values], zeroed by the host */) {
-    __shared__ unsigned long long mag[kGvRange];
-    __shared__ uint16_t vidx[kGvRange];
+                      unsigned long long* __restrict__ counts /* [nB or 1][v.n_groups], zeroed by the host */) {
+    __shared__ unsigned long long mag[kGvRange];      // (with a multi-view b, the warps' row bitmaps once the groups are made)
+    __shared__ uint16_t vidx[kGvRange];               // group index per column
     __shared__ uint32_t sign[kGvRange / 32];
     __shared__ unsigned long long cons[kGvRangeWords];
-    __shared__ Resolved planes[65];                   // sign row, then magnitude bits 0 .. depth - 1
+    __shared__ Resolved planes[kGvPlanes];            // per int field: sign row, then magnitude bits 0 .. depth - 1
     __shared__ uint32_t hist[kGvHist];
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nwarps = kGvThreads / 32;
-    const int n_hist = rowsB ? 0 : min(n_values, kGvHist);
+    const int n_hist = rowsB ? 0 : min(v.n_groups, kGvHist);
+    int n_planes = 0;
+    for (int k = 0; k < v.n; k++) n_planes += v.depth[k] + 1;
+    const bool unit_planes = n_planes <= kGvPlanes;   // else every field's planes are resolved per range, at table entry 0
     for (long long unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
         const uint64_t shard = shards[unit >> 4];
         const int slot = (int)(unit & 15);
@@ -2058,41 +2088,80 @@ groupby_values_kernel(StoreRef st, uint32_t fvV, int depth, const long long* __r
         uint64_t any = 0;
         for (int i = tid; i < 1024; i += kGvThreads) any |= cu[i];
         if (!__syncthreads_or(any != 0)) continue;
-        for (int p = tid; p <= depth; p += kGvThreads) planes[p] = resolve(st, fvV, shard, (uint64_t)(p + 1), slot);
+        if (unit_planes)
+            for (int k = 0, base = 0; k < v.n; base += v.depth[k] + 1, k++)
+                for (int p = tid; p <= v.depth[k]; p += kGvThreads) planes[base + p] = resolve(st, v.fv[k], shard, (uint64_t)(p + 1), slot);
         for (int i = tid; i < n_hist; i += kGvThreads) hist[i] = 0;
         for (uint32_t lo = 0; lo < kFull; lo += kGvRange) {
             __syncthreads();                              // the previous range's readers are done; planes / hist are written
             const uint64_t cw = tid < kGvRangeWords ? cu[(lo >> 6) + tid] : 0;
             if (tid < kGvRangeWords) cons[tid] = cw;
             if (!__syncthreads_or(cw != 0)) continue;
-            for (int i = tid; i < (int)kGvRange; i += kGvThreads) mag[i] = 0;
-            for (int i = tid; i < (int)kGvRange / 32; i += kGvThreads) sign[i] = 0;
-            __syncthreads();
-            for (int p = wid; p <= depth; p += nwarps) {
-                const Resolved r = planes[p];
-                if (p == 0) gv_for_each(r, lo, cons, lane, [&](uint32_t v) { atomicOr(&sign[v >> 5], 1u << (v & 31)); });
-                else { const unsigned long long bit = 1ull << (p - 1); gv_for_each(r, lo, cons, lane, [&](uint32_t v) { atomicOr(&mag[v], bit); }); }
-            }
-            __syncthreads();
-            for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
-                uint16_t k = kGvNone;
-                const unsigned long long m = mag[i];
-                const bool neg = (sign[i >> 5] >> (i & 31)) & 1u;
-                if (((cons[i >> 6] >> (i & 63)) & 1ull) && (m || !neg)) {
-                    const long long val = (long long)(neg ? 0ull - m : m);
-                    int a = 0, b = n_values;
-                    while (a < b) { const int h = (a + b) >> 1; if (__ldg(values + h) < val) a = h + 1; else b = h; }
-                    if (a < n_values && __ldg(values + a) == val) k = (uint16_t)a;
+            for (int k = 0, base = 0; k < v.n; k++) {
+                const int depth = v.depth[k];
+                if (!unit_planes) for (int p = tid; p <= depth; p += kGvThreads) planes[p] = resolve(st, v.fv[k], shard, (uint64_t)(p + 1), slot);
+                for (int i = tid; i < (int)kGvRange; i += kGvThreads) mag[i] = 0;
+                for (int i = tid; i < (int)kGvRange / 32; i += kGvThreads) sign[i] = 0;
+                __syncthreads();
+                for (int p = wid; p <= depth; p += nwarps) {
+                    const Resolved r = planes[base + p];
+                    if (p == 0) gv_for_each(r, lo, cons, lane, [&](uint32_t c) { atomicOr(&sign[c >> 5], 1u << (c & 31)); });
+                    else { const unsigned long long bit = 1ull << (p - 1); gv_for_each(r, lo, cons, lane, [&](uint32_t c) { atomicOr(&mag[c], bit); }); }
                 }
-                vidx[i] = k;
+                __syncthreads();
+                const long long* vals = values + v.off[k];
+                const int nv = v.n_values[k];
+                for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
+                    uint32_t g = k ? (uint32_t)vidx[i] : (((cons[i >> 6] >> (i & 63)) & 1ull) ? 0u : (uint32_t)kGvNone);
+                    if (g != kGvNone) {
+                        const unsigned long long m = mag[i];
+                        const bool neg = (sign[i >> 5] >> (i & 31)) & 1u;
+                        uint32_t j = kGvNone;
+                        if (m || !neg) {
+                            const long long val = (long long)(neg ? 0ull - m : m);
+                            int a = 0, b = nv;
+                            while (a < b) { const int h = (a + b) >> 1; if (__ldg(vals + h) < val) a = h + 1; else b = h; }
+                            if (a < nv && __ldg(vals + a) == val) j = (uint32_t)a;
+                        }
+                        g = j == kGvNone ? (uint32_t)kGvNone : g * (uint32_t)nv + j;
+                    }
+                    vidx[i] = (uint16_t)g;
+                }
+                __syncthreads();                          // (mag / sign / planes are read no more)
+                if (unit_planes) base += depth + 1;
             }
-            __syncthreads();
             if (!rowsB) {
                 for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
                     const uint32_t k = vidx[i];
                     if (k == kGvNone) continue;
                     if ((int)k < n_hist) atomicAdd(&hist[k], 1u);
                     else atomicAdd(&counts[k], 1ull);
+                }
+                continue;
+            }
+            if (nvB > 1) {
+                unsigned long long* bm = mag + wid * kGvRangeWords;          // this warp's row bitmap
+                for (int i = lane; i < kGvRangeWords; i += 32) bm[i] = 0;
+                __syncwarp();
+                for (int br = wid; br < nB; br += nwarps) {
+                    const uint64_t row = rowsB[br];
+                    for (int v0 = 0; v0 < nvB; v0 += 32) {
+                        Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
+                        if (v0 + lane < nvB) r = resolve(st, fvsB[v0 + lane], shard, row, slot);
+                        unsigned present = __ballot_sync(0xffffffffu, r.ptr != nullptr);
+                        while (present) {
+                            const int l = __ffs(present) - 1; present &= present - 1;
+                            gv_for_each_word(shfl_resolved(r, l), lo, lane, [&](uint32_t i, uint64_t m) { atomicOr(&bm[i], m); });
+                        }
+                    }
+                    __syncwarp();
+                    unsigned long long* crow = counts + (size_t)br * (size_t)v.n_groups;
+                    for (int i = lane; i < kGvRangeWords; i += 32) {
+                        uint64_t m = bm[i] & cons[i];
+                        bm[i] = 0;
+                        while (m) { const int t = __ffsll((long long)m) - 1; const uint32_t g = vidx[i * 64 + t]; if (g != kGvNone) atomicAdd(&crow[g], 1ull); m &= m - 1; }
+                    }
+                    __syncwarp();
                 }
                 continue;
             }
@@ -2106,8 +2175,8 @@ groupby_values_kernel(StoreRef st, uint32_t fvV, int depth, const long long* __r
                     r.card = __shfl_sync(0xffffffffu, mine.card, j);
                     const uint32_t meta = __shfl_sync(0xffffffffu, ((uint32_t)mine.typ << 16) | mine.cnt, j);
                     r.typ = (uint16_t)(meta >> 16); r.cnt = (uint16_t)(meta & 0xffffu);
-                    unsigned long long* row = counts + (size_t)(b0 + j) * (size_t)n_values;
-                    gv_for_each(r, lo, cons, lane, [&](uint32_t v) { const uint32_t k = vidx[v]; if (k != kGvNone) atomicAdd(&row[k], 1ull); });
+                    unsigned long long* row = counts + (size_t)(b0 + j) * (size_t)v.n_groups;
+                    gv_for_each(r, lo, cons, lane, [&](uint32_t c) { const uint32_t k = vidx[c]; if (k != kGvNone) atomicAdd(&row[k], 1ull); });
                 }
             }
         }

@@ -8,6 +8,7 @@ post-order fbgpu_op program and hands the whole shard batch to libfbgpu (one C-A
 In a real integration this layer stays in Go (INTEGRATION.md); it exists here because the Go toolchain is absent
 and the parity tests should read like the reference's executor tests.  All reference cites are executor.go unless
 noted."""
+import itertools
 import math
 
 import numpy as np
@@ -634,9 +635,8 @@ class Executor:
         """Rows of a time field restricted to from= / to=, made addressable by the single-view kernels: each row's union over
         the covering views (timeFragmentsRowIterator :8755-8768, mergerator :2570) is evaluated once and stored as an operand
         row of the scratch field.  Returns (scratch field, operand row ids in the order of `rows`).  TopK, Rows and GroupBy
-        count such rows with row_counts_views / groupby_views instead where the context has them; this remains for a GroupBy that
-        also has an int child (the groupby_values path), a GroupBy with two or more int children, and contexts without those
-        calls."""
+        count such rows with row_counts_views / groupby_views / groupby_mixed instead where the context has them; this remains for
+        contexts without those calls."""
         operands = []
         for r in rows:
             data, _ = self.ctx.row(idx.id, self._bitmap_call(idx, pql.Call("Row", {f.name: r, **targs})), shards)
@@ -1019,8 +1019,8 @@ class Executor:
         if any(len(r) == 0 for r in row_ids):
             return []
         int_dims = [k for k, f in enumerate(fields) if f.type == "int"]
-        if len(int_dims) == 1 and hasattr(self.ctx, "groupby_values"):
-            counts = self._groupby_int_counts(idx, fields, row_ids, time_args, int_dims[0], filt, shards)
+        if int_dims and hasattr(self.ctx, "groupby_mixed"):
+            counts = self._groupby_int_counts(idx, fields, row_ids, time_args, int_dims, filt, shards)
         elif not int_dims and any(time_args) and hasattr(self.ctx, "groupby_views"):
             # a Rows(f, from=, to=) child groups by its rows' unions over the covering views, in the same call as the other children
             views = [self._time_view_ids(f, targs) if targs else [VIEW_STANDARD] for f, targs in zip(fields, time_args)]
@@ -1095,30 +1095,28 @@ class Executor:
                 out.sort(key=lambda g: (g[col] if len(g) > col else 0), reverse=not asc)
         return self._window(c, out)
 
-    GROUPBY_VALUES_MAX = 65535                                    # values per fbgpu_groupby_values call
+    GROUPBY_MIXED_MAX = 65535                                     # groups (product of the int children's value counts) per fbgpu_groupby_mixed call
 
-    def _groupby_int_counts(self, idx, fields, row_ids, time_args, k, filt, shards):
-        """the count tensor of a GroupBy with exactly one int child (child k), from fbgpu_groupby_values: the other children are
-        its set dimensions (a time-range child as operand rows, as above), the int child's values its last dimension, moved
-        back to position k.  No Row(v == value) per value and no scratch rows.  A longer value list than one call takes is
-        split into slices, one call each: a column's value lies in exactly one slice."""
-        dev_fields, dev_rows = [], []
-        for j, (f, rows, targs) in enumerate(zip(fields, row_ids, time_args)):
-            if j == k:
-                continue
-            if not targs:
-                dev_fields.append(f.id)
-                dev_rows.append(rows)
-                continue
-            sf, operands = self._time_rows_as_operands(idx, f, rows, targs, shards)
-            dev_fields.append(sf.id)
-            dev_rows.append(operands)
-        vf = fields[k]
-        stored = [v - vf.base for v in row_ids[k]]                 # values as the planes hold them (value - Base)
-        step = self.GROUPBY_VALUES_MAX
-        parts = [self.ctx.groupby_values(idx.id, dev_fields, [VIEW_STANDARD] * len(dev_fields), dev_rows, vf.id, VIEW_BSI, vf.bit_depth,
-                                         stored[s:s + step], shards, filter_ops=filt) for s in range(0, len(stored), step)]
-        return np.moveaxis(np.concatenate(parts, axis=-1), -1, k)
+    def _groupby_int_counts(self, idx, fields, row_ids, time_args, int_dims, filt, shards):
+        """the count tensor of a GroupBy with int children (positions int_dims), from fbgpu_groupby_mixed: the other children are
+        its set dimensions (a time-range child with its covering views), the int children's values its trailing dimensions,
+        moved back to the children's order.  No Row(v == value) per value and no scratch rows.  When the value lists' product
+        exceeds GROUPBY_MIXED_MAX, each int child's list is cut into slices whose product fits and every combination of slices
+        is one call: a column's value lies in exactly one slice per field, so the pieces tile the tensor."""
+        set_k = [j for j in range(len(fields)) if j not in int_dims]
+        set_dims = [(fields[j].id, self._time_view_ids(fields[j], time_args[j]) if time_args[j] else [VIEW_STANDARD], row_ids[j]) for j in set_k]
+        stored = [[v - fields[k].base for v in row_ids[k]] for k in int_dims]      # values as the planes hold them (value - Base)
+        step, room = [], self.GROUPBY_MIXED_MAX
+        for vals in stored:
+            step.append(max(1, min(len(vals), room)))
+            room //= step[-1]
+        counts = np.zeros([len(row_ids[j]) for j in set_k] + [len(v) for v in stored], dtype=np.uint64)
+        for starts in itertools.product(*[range(0, len(v), n) for v, n in zip(stored, step)]):
+            cut = [slice(s, s + n) for s, n in zip(starts, step)]
+            int_part = [(fields[k].id, VIEW_BSI, fields[k].bit_depth, v[c]) for k, v, c in zip(int_dims, stored, cut)]
+            counts[(Ellipsis, *cut)] = self.ctx.groupby_mixed(idx.id, set_dims, int_part, shards, filter_ops=filt)
+        order = set_k + list(int_dims)
+        return np.transpose(counts, [order.index(j) for j in range(len(fields))])
 
     @staticmethod
     def _window(c, out):                                          # applyLimitAndOffsetToGroupByResult :3441-3459

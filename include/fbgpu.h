@@ -295,6 +295,26 @@ int fbgpu_groupby_values(fbgpu_ctx *ctx, uint32_t index, const uint32_t *fields,
                          const uint64_t *row_ids_flat, const int32_t *n_rows, uint32_t vfield, uint32_t vview, int32_t bit_depth,
                          const int64_t *values, int32_t n_values, const fbgpu_op *filter, int32_t n_filter_ops,
                          const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+/* GroupBy over set dimensions and one or more int dimensions in one device call: GroupBy(Rows(a), Rows(v), Rows(w)) (SQL GROUP BY
+ * int_a, int_b) or GroupBy(Rows(t, from=, to=), Rows(v)).
+ * fields / views_flat / n_views / row_ids_flat / n_rows: n_fields (0..7) set dimensions, as for fbgpu_groupby_views: dimension i
+ * has n_views[i] >= 1 views and n_rows[i] (0..65535) rows, each row its union over those views (may be NULL when n_fields == 0).
+ * vfields / vviews / bit_depths / values_flat / n_values: n_ints (1..8, n_fields + n_ints <= 8) int dimensions, each a BSI view of
+ * depth 0..64 with n_values[k] (1..65535) strictly ascending stored values (as for fbgpu_groupby_values), listed one dimension
+ * after the other in values_flat; the product of the n_values is at most 65535.
+ * out_counts: the dense tensor [n_rows[0]] ... [n_rows[n_fields-1]] [n_values[0]] ... [n_values[n_ints-1]], row-major, set
+ * dimensions first, rightmost fastest.  A column is counted in a cell when it is in the filter, in every set row of the cell, in
+ * exists(v_k) of every int field and its stored value of every v_k is the listed one; sign with magnitude 0 is no value.  A shard
+ * lacking any int field's fragment, or a set dimension's fragment in every listed view, contributes nothing.  All-reduced over
+ * the communicator.  With n_ints == 1 and every n_views[i] == 1 the result is fbgpu_groupby_values'.  Argument errors other than
+ * n_rows are reported before the device check; a counts workspace (rows of the last set dimension x groups x 8 bytes) that
+ * cannot be allocated gives FBGPU_E_NOMEM. */
+int fbgpu_groupby_mixed(fbgpu_ctx *ctx, uint32_t index,
+                        const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                        const uint64_t *row_ids_flat, const int32_t *n_rows,
+                        const uint32_t *vfields, const uint32_t *vviews, const int32_t *bit_depths, int32_t n_ints,
+                        const int64_t *values_flat, const int32_t *n_values,
+                        const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
 
 /* ---- multi-GPU reduce (replaces the HTTP fan-in of mapReduce/remoteExec, executor.go:6392-6533) ----
  * One context (process) per GPU; rank 0 creates the id, every rank joins.  When a communicator is attached,
@@ -371,6 +391,12 @@ int fbgpu_node_groupby_values(fbgpu_node *node, uint32_t index, const uint32_t *
                               const uint64_t *row_ids_flat, const int32_t *n_rows, uint32_t vfield, uint32_t vview, int32_t bit_depth,
                               const int64_t *values, int32_t n_values, const fbgpu_op *filter, int32_t n_filter_ops,
                               const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+int fbgpu_node_groupby_mixed(fbgpu_node *node, uint32_t index,
+                             const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                             const uint64_t *row_ids_flat, const int32_t *n_rows,
+                             const uint32_t *vfields, const uint32_t *vviews, const int32_t *bit_depths, int32_t n_ints,
+                             const int64_t *values_flat, const int32_t *n_values,
+                             const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
 int fbgpu_node_bsi_sum(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                        const uint64_t *shards, int64_t n_shards, int64_t *out_sum, uint64_t *out_count);
 int fbgpu_node_bsi_minmax(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
