@@ -1891,16 +1891,18 @@ static int groupby_values_args(const void* handle, const uint32_t* fields, const
     return 0;
 }
 
-// the argument checks fbgpu_groupby_mixed and its node form make before any device is touched (n_rows is checked after it)
+// the argument checks fbgpu_groupby_mixed and its node form make before any device is touched (n_rows is checked after it);
+// fbgpu_groupby_sum's dimensions are the same but for the bounds: 0..8 set and 0..8 int dimensions, the int arrays may then be NULL
 static int groupby_mixed_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
                               const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews,
                               const int32_t* bit_depths, int32_t n_ints, const int64_t* values_flat, const int32_t* n_values,
-                              const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts) {
-    if (!handle || !vfields || !vviews || !bit_depths || !values_flat || !n_values || !out_counts ||
+                              const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts,
+                              int32_t min_ints = 1, int32_t max_fields = 7) {
+    if (!handle || ((min_ints || n_ints) && (!vfields || !vviews || !bit_depths || !values_flat || !n_values)) || !out_counts ||
         (n_fields > 0 && (!fields || !views_flat || !n_views || !row_ids_flat || !n_rows)) ||
         n_filter_ops < 0 || (n_filter_ops && !filter) || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
-    if (n_fields < 0 || n_fields > 7) return fail(FBGPU_E_INVALID, "n_fields=%d outside 0..7", n_fields);
-    if (n_ints < 1 || n_ints > kGvMaxInts) return fail(FBGPU_E_INVALID, "n_ints=%d outside 1..%d", n_ints, kGvMaxInts);
+    if (n_fields < 0 || n_fields > max_fields) return fail(FBGPU_E_INVALID, "n_fields=%d outside 0..%d", n_fields, max_fields);
+    if (n_ints < min_ints || n_ints > kGvMaxInts) return fail(FBGPU_E_INVALID, "n_ints=%d outside %d..%d", n_ints, min_ints, kGvMaxInts);
     if (n_fields + n_ints > 8) return fail(FBGPU_E_INVALID, "n_fields + n_ints = %d exceeds 8", n_fields + n_ints);
     for (int32_t i = 0; i < n_fields; i++)
         if (n_views[i] < 1) return fail(FBGPU_E_INVALID, "n_views[%d]=%d < 1", i, n_views[i]);
@@ -1918,11 +1920,29 @@ static int groupby_mixed_args(const void* handle, const uint32_t* fields, const 
     return 0;
 }
 
-// one groupby_values_kernel pass over the shards: counts[nB or 1][groups] of consider = filter ∩ exists(v_1) ∩ ... (∩ Row(b = row))
+// the argument checks fbgpu_groupby_sum and its node form make before any device is touched (n_rows is checked after it)
+static int groupby_sum_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                            const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews,
+                            const int32_t* bit_depths, int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, int32_t a_depth,
+                            const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts,
+                            const int64_t* out_sums) {
+    if (!out_sums) return fail(FBGPU_E_INVALID, "bad argument");
+    int rc = groupby_mixed_args(handle, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat,
+                                n_values, filter, n_filter_ops, shards, n_shards, out_counts, 0, 8);
+    if (rc) return rc;
+    if (n_fields + n_ints < 1) return fail(FBGPU_E_INVALID, "no dimension: n_fields + n_ints = 0");
+    if (a_depth < 0 || a_depth > 64) return fail(FBGPU_E_INVALID, "a_depth=%d outside 0..64", a_depth);
+    return 0;
+}
+
+// one groupby_values_kernel pass over the shards: counts[nB or 1][groups] of consider = filter ∩ exists(v_1) ∩ ... (∩ Row(b = row));
+// with an aggregate x, consider also ∩ exists(x) and sums[nB or 1][groups] the columns' stored values of x
 static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* null: no set dimension */, const std::vector<GvInt>& v,
-                               const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards, uint64_t* out) {
+                               const GvInt* x /* null: counts only */, const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards,
+                               uint64_t* out, uint64_t* out_sums) {
     std::vector<fbgpu_op> full = filter;
-    for (const GvInt& x : v) full = and_row(full.data(), (int32_t)full.size(), x.field, x.view, 0);
+    for (const GvInt& f : v) full = and_row(full.data(), (int32_t)full.size(), f.field, f.view, 0);
+    if (x) full = and_row(full.data(), (int32_t)full.size(), x->field, x->view, 0);
     Query q(c); Workspace* w = q.w;
     int rc = q.open(index, full.data(), (int32_t)full.size(), shards, n_shards); if (rc) return rc;
     GvInts k{};
@@ -1935,6 +1955,7 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
         in.insert(in.end(), v[(size_t)i].values, v[(size_t)i].values + v[(size_t)i].n_values);
     }
     const size_t n_vals = in.size();
+    const uint32_t fvX = x ? view_id_locked(c, ViewKey{ index, x->field, x->view }, false) : kNoView;
     const int nB = b ? b->n_rows : 0;
     const std::vector<uint32_t> fvsB = b ? view_slots(c, index, b->field, b->views, b->n_views) : std::vector<uint32_t>{ kNoView };
     const size_t nvB = fvsB.size();
@@ -1943,9 +1964,10 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
     if (nvB > 1) in.resize(n_in + (nvB + 1) / 2);
     if (nvB > 1) memcpy(in.data() + n_in, fvsB.data(), nvB * 4);
     const size_t ncnt = (size_t)(b ? nB : 1) * (size_t)k.n_groups;
-    if (w->d_rows.ensure(in.size() * 8) || w->d_counts.ensure(ncnt * 8) || w->h_out.ensure(ncnt * 8)) return FBGPU_E_NOMEM;
+    const size_t nout = x ? 2 * ncnt : ncnt;                         // [counts | sums]
+    if (w->d_rows.ensure(in.size() * 8) || w->d_counts.ensure(nout * 8) || w->h_out.ensure(nout * 8)) return FBGPU_E_NOMEM;
     CUDA_TRY(cudaMemcpyAsync(w->d_rows.p, in.data(), in.size() * 8, cudaMemcpyHostToDevice, w->stream));
-    CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, ncnt * 8, w->stream));
+    CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, nout * 8, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));   // `in` is a local
     const long long* d_values = (const long long*)w->d_rows.p;
     const uint64_t* d_rowsB = b ? (const uint64_t*)w->d_rows.p + n_vals : nullptr;
@@ -1955,15 +1977,22 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
         const long long nu = std::min(c->unit_batch, q.n_units - u0);
         rc = q.eval(u0, nu); if (rc) return rc;
         const long long grid = std::min<long long>(nu, (long long)c->sm_count * kGvCtasPerSm);
-        groupby_values_kernel<<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB,
-                                                                            (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, (unsigned long long*)w->d_counts.p);
+        unsigned long long* d_counts = (unsigned long long*)w->d_counts.p;
+        if (x)
+            groupby_values_kernel<true><<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB,
+                                                                                    (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, d_counts,
+                                                                                    fvX, x->depth, d_counts + ncnt);
+        else
+            groupby_values_kernel<false><<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB,
+                                                                                     (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, d_counts);
         CUDA_TRY(cudaGetLastError()); q.launches++;
     }
     CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
-    rc = allreduce_u64(c, w, w->d_counts.p, ncnt); if (rc) return rc;
-    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, ncnt * 8, cudaMemcpyDeviceToHost, w->stream));
+    rc = allreduce_u64(c, w, w->d_counts.p, nout); if (rc) return rc;           // a wrapping int64 sum is a u64 sum
+    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, nout * 8, cudaMemcpyDeviceToHost, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
     memcpy(out, w->h_out.p, ncnt * 8);
+    if (x) memcpy(out_sums, (const uint64_t*)w->h_out.p + ncnt, ncnt * 8);
     q.add_elapsed();
     q.finish();
     return 0;
@@ -1971,33 +2000,36 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
 
 // set dimensions before the last are peeled into the filter as groupby_rec does (a multi-view one as the union of its row over
 // the views); the last one (if any) is the kernel's b
-static int groupby_values_rec(fbgpu_ctx* c, uint32_t index, const GbDim* d, int nf, const std::vector<GvInt>& v, const std::vector<fbgpu_op>& filter,
-                              const uint64_t* shards, int64_t n_shards, uint64_t* out) {
-    if (nf <= 1) return groupby_values_leaf(c, index, nf ? d : nullptr, v, filter, shards, n_shards, out);
-    size_t sub = 1; for (const GvInt& x : v) sub *= (size_t)x.n_values;
+static int groupby_values_rec(fbgpu_ctx* c, uint32_t index, const GbDim* d, int nf, const std::vector<GvInt>& v, const GvInt* x,
+                              const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards, uint64_t* out, uint64_t* out_sums) {
+    if (nf <= 1) return groupby_values_leaf(c, index, nf ? d : nullptr, v, x, filter, shards, n_shards, out, out_sums);
+    size_t sub = 1; for (const GvInt& f : v) sub *= (size_t)f.n_values;
     for (int i = 1; i < nf; i++) sub *= (size_t)d[i].n_rows;
     for (int r = 0; r < d[0].n_rows; r++) {
-        int rc = groupby_values_rec(c, index, d + 1, nf - 1, v, and_row(filter.data(), (int32_t)filter.size(), d[0].field, d[0].views, d[0].n_views, d[0].rows[r]),
-                                    shards, n_shards, out + (size_t)r * sub); if (rc) return rc;
+        int rc = groupby_values_rec(c, index, d + 1, nf - 1, v, x, and_row(filter.data(), (int32_t)filter.size(), d[0].field, d[0].views, d[0].n_views, d[0].rows[r]),
+                                    shards, n_shards, out + (size_t)r * sub, x ? out_sums + (size_t)r * sub : nullptr); if (rc) return rc;
     }
     return 0;
 }
 
-// fbgpu_groupby_values / fbgpu_groupby_mixed once the arguments but n_rows are checked: the set dimensions' rows are laid out
-// from row_ids_flat, the output zeroed, the store locked
+// fbgpu_groupby_values / fbgpu_groupby_mixed / fbgpu_groupby_sum once the arguments but n_rows are checked: the set dimensions'
+// rows are laid out from row_ids_flat, the outputs zeroed, the store locked
 static int groupby_values_query(fbgpu_ctx* c, uint32_t index, std::vector<GbDim>& dims, const uint64_t* row_ids_flat, const std::vector<GvInt>& v,
-                                const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) {
+                                const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts,
+                                const GvInt* x = nullptr, int64_t* out_sums = nullptr) {
     std::shared_lock<std::shared_mutex> lk;
     int rc = begin_query(c, lk); if (rc) return rc;
     const uint64_t* p = row_ids_flat; size_t total = 1;
-    for (const GvInt& x : v) total *= (size_t)x.n_values;
+    for (const GvInt& f : v) total *= (size_t)f.n_values;
     for (size_t i = 0; i < dims.size(); i++) {
         if (dims[i].n_rows < 0 || dims[i].n_rows > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", (int)i, dims[i].n_rows);
         dims[i].rows = p; p += dims[i].n_rows; total *= (size_t)dims[i].n_rows;
     }
     memset(out_counts, 0, total * 8);
+    if (x) memset(out_sums, 0, total * 8);
     if (total == 0) return 0;
-    return groupby_values_rec(c, index, dims.data(), (int)dims.size(), v, std::vector<fbgpu_op>(filter, filter + n_filter_ops), shards, n_shards, out_counts);
+    return groupby_values_rec(c, index, dims.data(), (int)dims.size(), v, x, std::vector<fbgpu_op>(filter, filter + n_filter_ops), shards, n_shards,
+                              out_counts, (uint64_t*)out_sums);
 }
 
 extern "C" int fbgpu_groupby_values(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
@@ -2024,6 +2056,23 @@ extern "C" int fbgpu_groupby_mixed(fbgpu_ctx* c, uint32_t index, const uint32_t*
     std::vector<GvInt> ints((size_t)n_ints); const int64_t* vals = values_flat;
     for (int k = 0; k < n_ints; k++) { ints[(size_t)k] = GvInt{ vfields[k], vviews[k], bit_depths[k], vals, n_values[k] }; vals += n_values[k]; }
     return groupby_values_query(c, index, dims, row_ids_flat, ints, filter, n_filter_ops, shards, n_shards, out_counts);
+} FBGPU_CATCH
+
+// GroupBy(..., aggregate=Sum(field=x)): fbgpu_groupby_mixed's dimensions (none of them int is fine) with, per cell, the number of
+// columns holding a value of x and the sum of their stored values: fbgpu_bsi_sum under filter ∩ the cell's rows, for every cell
+extern "C" int fbgpu_groupby_sum(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                 const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews, const int32_t* bit_depths,
+                                 int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, uint32_t afield, uint32_t aview, int32_t a_depth,
+                                 const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts, int64_t* out_sums) try {
+    int rc = groupby_sum_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values, a_depth,
+                              filter, n_filter_ops, shards, n_shards, out_counts, out_sums);
+    if (rc) return rc;
+    std::vector<GbDim> dims((size_t)n_fields); const uint32_t* vw = views_flat;
+    for (int i = 0; i < n_fields; i++) { dims[(size_t)i] = GbDim{ fields[i], vw, n_views[i], nullptr, n_rows[i] }; vw += n_views[i]; }
+    std::vector<GvInt> ints((size_t)n_ints); const int64_t* vals = values_flat;
+    for (int k = 0; k < n_ints; k++) { ints[(size_t)k] = GvInt{ vfields[k], vviews[k], bit_depths[k], vals, n_values[k] }; vals += n_values[k]; }
+    const GvInt x{ afield, aview, a_depth, nullptr, 0 };
+    return groupby_values_query(c, index, dims, row_ids_flat, ints, filter, n_filter_ops, shards, n_shards, out_counts, &x, out_sums);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ comm

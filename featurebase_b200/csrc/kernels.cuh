@@ -2001,6 +2001,12 @@ groupby_direct_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ ro
 // shared memory: four CTAs per SM.
 // A shard missing an int field's fragment has an empty consider set, one missing b's fragment in every view resolves no
 // b-row: either contributes nothing (executor.go:8769-8772).
+// kSum (fbgpu_groupby_sum, GroupBy(..., aggregate=Sum(field=x))): consider also holds exists(x), and there may be no int
+// field (every consider column is then in group 0).  Once the group indices are made, x's magnitude and sign are assembled
+// the same way into mag / sign and each column's stored value (wrapping int64, sign with magnitude 0 is 0) left in mag; every
+// counted (b-row, column) adds 1 to counts and the value to sums, each lane or thread running one total per group until the
+// group changes.  x's planes follow the int fields' in the table.  The multi-view b bitmaps move to hist (eight warps x 64
+// words, as 32-bit halves), which is unused whenever b is present; without b there is no shared histogram.
 // ------------------------------------------------------------------------------------------------
 constexpr int kGvThreads = 256;
 constexpr int kGvCtasPerSm = 4;
@@ -2064,12 +2070,28 @@ __device__ __forceinline__ void gv_for_each(const Resolved& r, uint32_t lo, cons
     });
 }
 
+// kSum: one (count, sum) total per group, added to the output when the caller's column walk reaches another group and at its end
+struct GvTotal {
+    uint32_t g = kGvNone;
+    unsigned long long n = 0, s = 0;
+    __device__ __forceinline__ void flush(unsigned long long* counts, unsigned long long* sums) {
+        if (n) { atomicAdd(&counts[g], n); atomicAdd(&sums[g], s); n = 0; s = 0; }
+    }
+    __device__ __forceinline__ void add(uint32_t k, unsigned long long val, unsigned long long* counts, unsigned long long* sums) {
+        if (k != g) { flush(counts, sums); g = k; }
+        n++; s += val;
+    }
+};
+
+template <bool kSum>
 __global__ void __launch_bounds__(kGvThreads, kGvCtasPerSm)
 groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__ values,
                       const uint64_t* __restrict__ rowsB /* null: no set field */, int nB,
                       uint32_t fvB, const uint32_t* __restrict__ fvsB /* nvB > 1: b's view slots, each row taken as its union */, int nvB,
                       const uint4* __restrict__ consider, const uint64_t* __restrict__ shards, long long n_units,
-                      unsigned long long* __restrict__ counts /* [nB or 1][v.n_groups], zeroed by the host */) {
+                      unsigned long long* __restrict__ counts /* [nB or 1][v.n_groups], zeroed by the host */,
+                      uint32_t fvX = 0, int depthX = 0 /* kSum: the aggregate field's BSI view slot and depth */,
+                      unsigned long long* __restrict__ sums = nullptr /* kSum: shaped as counts, zeroed by the host */) {
     __shared__ unsigned long long mag[kGvRange];      // (with a multi-view b, the warps' row bitmaps once the groups are made)
     __shared__ uint16_t vidx[kGvRange];               // group index per column
     __shared__ uint32_t sign[kGvRange / 32];
@@ -2077,8 +2099,8 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
     __shared__ Resolved planes[kGvPlanes];            // per int field: sign row, then magnitude bits 0 .. depth - 1
     __shared__ uint32_t hist[kGvHist];
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nwarps = kGvThreads / 32;
-    const int n_hist = rowsB ? 0 : min(v.n_groups, kGvHist);
-    int n_planes = 0;
+    const int n_hist = (kSum || rowsB) ? 0 : min(v.n_groups, kGvHist);
+    int n_planes = kSum ? depthX + 1 : 0;
     for (int k = 0; k < v.n; k++) n_planes += v.depth[k] + 1;
     const bool unit_planes = n_planes <= kGvPlanes;   // else every field's planes are resolved per range, at table entry 0
     for (long long unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
@@ -2091,6 +2113,9 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
         if (unit_planes)
             for (int k = 0, base = 0; k < v.n; base += v.depth[k] + 1, k++)
                 for (int p = tid; p <= v.depth[k]; p += kGvThreads) planes[base + p] = resolve(st, v.fv[k], shard, (uint64_t)(p + 1), slot);
+        if constexpr (kSum)
+            if (unit_planes)
+                for (int p = tid; p <= depthX; p += kGvThreads) planes[n_planes - depthX - 1 + p] = resolve(st, fvX, shard, (uint64_t)(p + 1), slot);
         for (int i = tid; i < n_hist; i += kGvThreads) hist[i] = 0;
         for (uint32_t lo = 0; lo < kFull; lo += kGvRange) {
             __syncthreads();                              // the previous range's readers are done; planes / hist are written
@@ -2130,16 +2155,75 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                 __syncthreads();                          // (mag / sign / planes are read no more)
                 if (unit_planes) base += depth + 1;
             }
+            if constexpr (kSum) {                         // the aggregate's stored value per column, into mag
+                if (v.n == 0)
+                    for (int i = tid; i < (int)kGvRange; i += kGvThreads) vidx[i] = ((cons[i >> 6] >> (i & 63)) & 1ull) ? 0 : kGvNone;
+                const int base = unit_planes ? n_planes - depthX - 1 : 0;
+                if (!unit_planes) for (int p = tid; p <= depthX; p += kGvThreads) planes[p] = resolve(st, fvX, shard, (uint64_t)(p + 1), slot);
+                for (int i = tid; i < (int)kGvRange; i += kGvThreads) mag[i] = 0;
+                for (int i = tid; i < (int)kGvRange / 32; i += kGvThreads) sign[i] = 0;
+                __syncthreads();
+                for (int p = wid; p <= depthX; p += nwarps) {
+                    const Resolved r = planes[base + p];
+                    if (p == 0) gv_for_each(r, lo, cons, lane, [&](uint32_t c) { atomicOr(&sign[c >> 5], 1u << (c & 31)); });
+                    else { const unsigned long long bit = 1ull << (p - 1); gv_for_each(r, lo, cons, lane, [&](uint32_t c) { atomicOr(&mag[c], bit); }); }
+                }
+                __syncthreads();
+                for (int i = tid; i < (int)kGvRange; i += kGvThreads)
+                    if ((sign[i >> 5] >> (i & 31)) & 1u) mag[i] = 0ull - mag[i];      // wrapping: sign + 2^63 is INT64_MIN
+                __syncthreads();
+            }
             if (!rowsB) {
-                for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
-                    const uint32_t k = vidx[i];
-                    if (k == kGvNone) continue;
-                    if ((int)k < n_hist) atomicAdd(&hist[k], 1u);
-                    else atomicAdd(&counts[k], 1ull);
+                if constexpr (kSum) {
+                    GvTotal t;
+                    for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
+                        const uint32_t k = vidx[i];
+                        if (k != kGvNone) t.add(k, mag[i], counts, sums);
+                    }
+                    t.flush(counts, sums);
+                } else {
+                    for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
+                        const uint32_t k = vidx[i];
+                        if (k == kGvNone) continue;
+                        if ((int)k < n_hist) atomicAdd(&hist[k], 1u);
+                        else atomicAdd(&counts[k], 1ull);
+                    }
                 }
                 continue;
             }
-            if (nvB > 1) {
+            if (kSum && nvB > 1) {
+                uint32_t* bm = hist + wid * 2 * kGvRangeWords;              // this warp's row bitmap, word i as halves 2i, 2i + 1
+                for (int i = lane; i < 2 * kGvRangeWords; i += 32) bm[i] = 0;
+                __syncwarp();
+                for (int br = wid; br < nB; br += nwarps) {
+                    const uint64_t row = rowsB[br];
+                    for (int v0 = 0; v0 < nvB; v0 += 32) {
+                        Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
+                        if (v0 + lane < nvB) r = resolve(st, fvsB[v0 + lane], shard, row, slot);
+                        unsigned present = __ballot_sync(0xffffffffu, r.ptr != nullptr);
+                        while (present) {
+                            const int l = __ffs(present) - 1; present &= present - 1;
+                            gv_for_each_word(shfl_resolved(r, l), lo, lane, [&](uint32_t i, uint64_t m) {
+                                if ((uint32_t)m) atomicOr(&bm[2 * i], (uint32_t)m);
+                                if (m >> 32) atomicOr(&bm[2 * i + 1], (uint32_t)(m >> 32));
+                            });
+                        }
+                    }
+                    __syncwarp();
+                    unsigned long long* crow = counts + (size_t)br * (size_t)v.n_groups;
+                    unsigned long long* srow = sums + (size_t)br * (size_t)v.n_groups;
+                    GvTotal t;
+                    for (int i = lane; i < kGvRangeWords; i += 32) {
+                        uint64_t m = ((uint64_t)bm[2 * i] | ((uint64_t)bm[2 * i + 1] << 32)) & cons[i];
+                        bm[2 * i] = 0; bm[2 * i + 1] = 0;
+                        while (m) { const int b = __ffsll((long long)m) - 1; const uint32_t g = vidx[i * 64 + b]; if (g != kGvNone) t.add(g, mag[i * 64 + b], crow, srow); m &= m - 1; }
+                    }
+                    t.flush(crow, srow);
+                    __syncwarp();
+                }
+                continue;
+            }
+            if (!kSum && nvB > 1) {
                 unsigned long long* bm = mag + wid * kGvRangeWords;          // this warp's row bitmap
                 for (int i = lane; i < kGvRangeWords; i += 32) bm[i] = 0;
                 __syncwarp();
@@ -2176,7 +2260,14 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                     const uint32_t meta = __shfl_sync(0xffffffffu, ((uint32_t)mine.typ << 16) | mine.cnt, j);
                     r.typ = (uint16_t)(meta >> 16); r.cnt = (uint16_t)(meta & 0xffffu);
                     unsigned long long* row = counts + (size_t)(b0 + j) * (size_t)v.n_groups;
-                    gv_for_each(r, lo, cons, lane, [&](uint32_t c) { const uint32_t k = vidx[c]; if (k != kGvNone) atomicAdd(&row[k], 1ull); });
+                    if constexpr (kSum) {
+                        unsigned long long* srow = sums + (size_t)(b0 + j) * (size_t)v.n_groups;
+                        GvTotal t;
+                        gv_for_each(r, lo, cons, lane, [&](uint32_t c) { const uint32_t k = vidx[c]; if (k != kGvNone) t.add(k, mag[c], row, srow); });
+                        t.flush(row, srow);
+                    } else {
+                        gv_for_each(r, lo, cons, lane, [&](uint32_t c) { const uint32_t k = vidx[c]; if (k != kGvNone) atomicAdd(&row[k], 1ull); });
+                    }
                 }
             }
         }

@@ -273,6 +273,26 @@ extern "C" int fbgpu_node_groupby_mixed(fbgpu_node* n, uint32_t index, const uin
     });
 } FBGPU_CATCH
 
+extern "C" int fbgpu_node_groupby_sum(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                      const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews, const int32_t* bit_depths,
+                                      int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, uint32_t afield, uint32_t aview, int32_t a_depth,
+                                      const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts, int64_t* out_sums) try {
+    int rc = groupby_sum_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values, a_depth,
+                              filter, n_filter_ops, shards, n_shards, out_counts, out_sums);
+    if (rc) return rc;
+    size_t total = 1; for (int k = 0; k < n_ints; k++) total *= (size_t)n_values[k];
+    for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); total *= (size_t)n_rows[i]; }
+    std::vector<uint64_t> both(2 * total);                                     // [counts | sums]: wrapping int64 sums add as u64
+    rc = node_sum(n, shards, n_shards, 2 * total, both.data(), [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {
+        return fbgpu_groupby_sum(c, index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
+                                 afield, aview, a_depth, filter, n_filter_ops, s.data(), (int64_t)s.size(), part, (int64_t*)(part + total));
+    });
+    if (rc) return rc;
+    memcpy(out_counts, both.data(), total * 8);
+    memcpy(out_sums, both.data() + total, total * 8);
+    return FBGPU_OK;
+} FBGPU_CATCH
+
 // Sum / Min / Max of an int field: per-device partials merged as ValCount.Add / Smaller / Larger do (executor.go:8446-8560)
 extern "C" int fbgpu_node_bsi_sum(fbgpu_node* n, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                                   const uint64_t* shards, int64_t n_shards, int64_t* out_sum, uint64_t* out_count) try {

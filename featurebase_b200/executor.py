@@ -984,7 +984,8 @@ class Executor:
 
     # ------------------------------------------------------------------ GroupBy (executeGroupBy :3176)
     def _groupby(self, idx, c, shards):
-        """The device returns the dense count tensor over the children's row lists; everything after it is the host-side
+        """The device returns the dense count tensor over the children's row lists (with aggregate=Sum over an int field, the
+        counts of columns holding a value and their sums, from the same call); everything after it is the host-side
         post-processing executeGroupBy does in Go: previous (iterator start, newGroupByIterator :8779-8826), aggregate=Sum
         (groupByIterator.Next :8893-8911: Count becomes the number of columns holding a value), having (:3388-3406),
         sort (:3130-3162, 3408-3414), offset / limit (:3441-3459).  Results: (group, count) or (group, count, agg)."""
@@ -1019,8 +1020,15 @@ class Executor:
         if any(len(r) == 0 for r in row_ids):
             return []
         int_dims = [k for k, f in enumerate(fields) if f.type == "int"]
-        if int_dims and hasattr(self.ctx, "groupby_mixed"):
-            counts = self._groupby_int_counts(idx, fields, row_ids, time_args, int_dims, filt, shards)
+        sum_f = None                                              # Sum over an int field: counts and sums from one device call
+        if isinstance(agg, pql.Call) and hasattr(self.ctx, "groupby_sum"):
+            f = idx.fields.get(agg.args.get("field", agg.args.get("_field")))
+            if f is not None and f.type == "int":                 # otherwise the per-group Sum below raises or finds no values
+                sum_f = f
+        if sum_f is not None:
+            counts, sums = self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, filt, shards, agg=sum_f)
+        elif int_dims and hasattr(self.ctx, "groupby_mixed"):
+            counts, = self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, filt, shards)
         elif not int_dims and any(time_args) and hasattr(self.ctx, "groupby_views"):
             # a Rows(f, from=, to=) child groups by its rows' unions over the covering views, in the same call as the other children
             views = [self._time_view_ids(f, targs) if targs else [VIEW_STANDARD] for f, targs in zip(fields, time_args)]
@@ -1050,7 +1058,10 @@ class Executor:
                 continue
             ix = np.unravel_index(int(flat), counts.shape)
             group = [(f.name, row_ids[k][int(i)]) for k, (f, i) in enumerate(zip(fields, ix))]
-            if isinstance(agg, pql.Call):
+            if sum_f is not None:                                 # counts here: columns of the group holding a value of the field
+                n = int(counts[ix])
+                out.append((group, n, _i64(int(sums[ix]) + n * sum_f.base)))      # executeSumCountShard :2203-2206
+            elif isinstance(agg, pql.Call):
                 rows = [pql.Call("Row", {name: rid, **(targs or {})}) for (name, rid), targs in zip(group, time_args)]
                 if isinstance(filt_call, pql.Call):
                     rows.append(filt_call)
@@ -1095,14 +1106,15 @@ class Executor:
                 out.sort(key=lambda g: (g[col] if len(g) > col else 0), reverse=not asc)
         return self._window(c, out)
 
-    GROUPBY_MIXED_MAX = 65535                                     # groups (product of the int children's value counts) per fbgpu_groupby_mixed call
+    GROUPBY_MIXED_MAX = 65535                                     # groups (product of the int children's value counts) per fbgpu_groupby_mixed / _sum call
 
-    def _groupby_int_counts(self, idx, fields, row_ids, time_args, int_dims, filt, shards):
-        """the count tensor of a GroupBy with int children (positions int_dims), from fbgpu_groupby_mixed: the other children are
-        its set dimensions (a time-range child with its covering views), the int children's values its trailing dimensions,
-        moved back to the children's order.  No Row(v == value) per value and no scratch rows.  When the value lists' product
-        exceeds GROUPBY_MIXED_MAX, each int child's list is cut into slices whose product fits and every combination of slices
-        is one call: a column's value lies in exactly one slice per field, so the pieces tile the tensor."""
+    def _groupby_tensors(self, idx, fields, row_ids, time_args, int_dims, filt, shards, agg=None):
+        """[counts] of a GroupBy with int children (positions int_dims), from fbgpu_groupby_mixed, or with agg (the int field of
+        aggregate=Sum) [counts, sums] from fbgpu_groupby_sum, where int_dims may be empty: the other children are the set
+        dimensions (a time-range child with its covering views), the int children's values the trailing dimensions, moved back
+        to the children's order.  No Row(v == value) per value and no scratch rows.  When the value lists' product exceeds
+        GROUPBY_MIXED_MAX, each int child's list is cut into slices whose product fits and every combination of slices is one
+        call: a column's value lies in exactly one slice per field, so the pieces tile the tensors."""
         set_k = [j for j in range(len(fields)) if j not in int_dims]
         set_dims = [(fields[j].id, self._time_view_ids(fields[j], time_args[j]) if time_args[j] else [VIEW_STANDARD], row_ids[j]) for j in set_k]
         stored = [[v - fields[k].base for v in row_ids[k]] for k in int_dims]      # values as the planes hold them (value - Base)
@@ -1110,13 +1122,19 @@ class Executor:
         for vals in stored:
             step.append(max(1, min(len(vals), room)))
             room //= step[-1]
-        counts = np.zeros([len(row_ids[j]) for j in set_k] + [len(v) for v in stored], dtype=np.uint64)
+        shape = [len(row_ids[j]) for j in set_k] + [len(v) for v in stored]
+        outs = [np.zeros(shape, dtype=np.uint64)] + ([np.zeros(shape, dtype=np.int64)] if agg is not None else [])
         for starts in itertools.product(*[range(0, len(v), n) for v, n in zip(stored, step)]):
             cut = [slice(s, s + n) for s, n in zip(starts, step)]
             int_part = [(fields[k].id, VIEW_BSI, fields[k].bit_depth, v[c]) for k, v, c in zip(int_dims, stored, cut)]
-            counts[(Ellipsis, *cut)] = self.ctx.groupby_mixed(idx.id, set_dims, int_part, shards, filter_ops=filt)
+            if agg is None:
+                got = [self.ctx.groupby_mixed(idx.id, set_dims, int_part, shards, filter_ops=filt)]
+            else:
+                got = self.ctx.groupby_sum(idx.id, set_dims, int_part, (agg.id, VIEW_BSI, agg.bit_depth), shards, filter_ops=filt)
+            for o, g in zip(outs, got):
+                o[(Ellipsis, *cut)] = g
         order = set_k + list(int_dims)
-        return np.transpose(counts, [order.index(j) for j in range(len(fields))])
+        return [np.transpose(o, [order.index(j) for j in range(len(fields))]) for o in outs]
 
     @staticmethod
     def _window(c, out):                                          # applyLimitAndOffsetToGroupByResult :3441-3459

@@ -50,7 +50,7 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_node_load_fragments", "fbgpu_node_load_rbf_dir", "fbgpu_node_drop_fragment", "fbgpu_node_commit", "fbgpu_node_get_stats", "fbgpu_node_count", "fbgpu_node_row",
            "fbgpu_node_count_pairs", "fbgpu_node_row_counts", "fbgpu_node_groupby", "fbgpu_node_bsi_sum", "fbgpu_node_bsi_minmax",
            "fbgpu_groupby_values", "fbgpu_node_groupby_values", "fbgpu_row_counts_views", "fbgpu_node_row_counts_views", "fbgpu_groupby_views",
-           "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed"]
+           "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum"]
 
 
 def lib_path():
@@ -103,6 +103,8 @@ def load():
     L.fbgpu_groupby_views.argtypes, L.fbgpu_groupby_views.restype = [vp, u32, vp, vp, vp, i32, vp, vp, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_groupby_mixed.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, i32, vp, i64, vp]
     L.fbgpu_groupby_mixed.restype = C.c_int
+    L.fbgpu_groupby_sum.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i64, vp, vp]
+    L.fbgpu_groupby_sum.restype = C.c_int
     L.fbgpu_count_pairs.argtypes, L.fbgpu_count_pairs.restype = [vp, u32, u32, u32, vp, u32, u32, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_comm_unique_id.argtypes, L.fbgpu_comm_unique_id.restype = [vp], C.c_int
     L.fbgpu_comm_init.argtypes, L.fbgpu_comm_init.restype = [vp, i32, i32, vp], C.c_int
@@ -122,7 +124,7 @@ def load():
     L.fbgpu_node_devices.argtypes, L.fbgpu_node_devices.restype = [vp], i32
     L.fbgpu_node_owner.argtypes, L.fbgpu_node_owner.restype = [vp, u64], i32
     L.fbgpu_node_ctx.argtypes, L.fbgpu_node_ctx.restype = [vp, i32], vp
-    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "bsi_sum", "bsi_minmax"):
+    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "groupby_sum", "bsi_sum", "bsi_minmax"):
         src, dst = getattr(L, "fbgpu_" + name), getattr(L, "fbgpu_node_" + name)
         dst.argtypes, dst.restype = src.argtypes, src.restype
     L.fbgpu_node_row_counts.argtypes, L.fbgpu_node_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
@@ -502,6 +504,32 @@ class Context:
                                                vf.ctypes.data, vv.ctypes.data, depths.ctypes.data, len(vf), vals.ctypes.data, n_values.ctypes.data,
                                                f, nf, sh.ctypes.data, len(sh), out.ctypes.data))
         return out.reshape(shape)
+
+    def groupby_sum(self, index, set_dims, int_dims, agg, shards, filter_ops=None):
+        """GroupBy(..., aggregate=Sum(field=x)) in one call (fbgpu_groupby_sum).  set_dims and int_dims as for groupby_mixed, but
+        0..8 of each (at least one dimension in all); agg: (field, BSI view, bit depth) of x.  Returns (counts, sums), tensors of
+        groupby_mixed's shape: per cell the number of columns holding a value of x and the wrapping int64 sum of their stored
+        values (value - Base)."""
+        sh = _u64arr(shards)
+        fl = np.ascontiguousarray(np.asarray([d[0] for d in set_dims], dtype=np.uint32))
+        vw = np.ascontiguousarray(np.asarray([v for d in set_dims for v in d[1]], dtype=np.uint32))
+        n_views = np.ascontiguousarray(np.asarray([len(d[1]) for d in set_dims], dtype=np.int32))
+        n_rows = np.ascontiguousarray(np.asarray([len(d[2]) for d in set_dims], dtype=np.int32))
+        flat = _u64arr([r for d in set_dims for r in d[2]])
+        vf = np.ascontiguousarray(np.asarray([d[0] for d in int_dims], dtype=np.uint32))
+        vv = np.ascontiguousarray(np.asarray([d[1] for d in int_dims], dtype=np.uint32))
+        depths = np.ascontiguousarray(np.asarray([int(d[2]) for d in int_dims], dtype=np.int32))
+        n_values = np.ascontiguousarray(np.asarray([len(d[3]) for d in int_dims], dtype=np.int32))
+        vals = np.ascontiguousarray(np.asarray([int(x) for d in int_dims for x in d[3]], dtype=np.int64))
+        shape = [int(x) for x in n_rows] + [int(x) for x in n_values]
+        counts = np.zeros(int(np.prod(shape, dtype=np.int64)), dtype=np.uint64)
+        sums = np.zeros(counts.size, dtype=np.int64)
+        f = ops_array(filter_ops) if filter_ops else None
+        nf = len(filter_ops) if filter_ops else 0
+        self._check(self.L.fbgpu_groupby_sum(self.h, index, fl.ctypes.data, vw.ctypes.data, n_views.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
+                                             vf.ctypes.data, vv.ctypes.data, depths.ctypes.data, len(vf), vals.ctypes.data, n_values.ctypes.data,
+                                             int(agg[0]), int(agg[1]), int(agg[2]), f, nf, sh.ctypes.data, len(sh), counts.ctypes.data, sums.ctypes.data))
+        return counts.reshape(shape), sums.reshape(shape)
 
     def rows_payload_bytes(self, index, field, view, shards, row_ids=None):
         sh = _u64arr(shards)

@@ -315,6 +315,22 @@ int fbgpu_groupby_mixed(fbgpu_ctx *ctx, uint32_t index,
                         const uint32_t *vfields, const uint32_t *vviews, const int32_t *bit_depths, int32_t n_ints,
                         const int64_t *values_flat, const int32_t *n_values,
                         const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+/* GroupBy(..., aggregate=Sum(field=x)) in one device call (SQL SELECT a, SUM(x) ... GROUP BY a).
+ * The dimensions are fbgpu_groupby_mixed's, except that n_fields is 0..8 and n_ints 0..8 with 1 <= n_fields + n_ints <= 8 (with
+ * n_ints == 0 the int arrays may be NULL).  afield / aview / a_depth (0..64): the aggregate's BSI view and its depth.
+ * out_counts / out_sums: tensors of fbgpu_groupby_mixed's shape and layout.  Per cell, out_counts = |cell ∩ filter ∩ exists(x)|
+ * and out_sums = the sum of those columns' stored values of x (value - Base) in wrapping int64: for every cell the pair
+ * fbgpu_bsi_sum returns under the filter `filter ∩ the cell's rows` (sign with magnitude 0 counts, with value 0; the caller adds
+ * count x Base).  A shard lacking x's fragment contributes nothing; missing set or int fragments as for fbgpu_groupby_mixed.
+ * Both tensors are all-reduced over the communicator as u64 sums.  Argument errors other than n_rows are reported before the
+ * device check; a workspace (rows of the last set dimension x groups x 16 bytes) that cannot be allocated gives FBGPU_E_NOMEM. */
+int fbgpu_groupby_sum(fbgpu_ctx *ctx, uint32_t index,
+                      const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                      const uint64_t *row_ids_flat, const int32_t *n_rows,
+                      const uint32_t *vfields, const uint32_t *vviews, const int32_t *bit_depths, int32_t n_ints,
+                      const int64_t *values_flat, const int32_t *n_values, uint32_t afield, uint32_t aview, int32_t a_depth,
+                      const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards,
+                      uint64_t *out_counts, int64_t *out_sums);
 
 /* ---- multi-GPU reduce (replaces the HTTP fan-in of mapReduce/remoteExec, executor.go:6392-6533) ----
  * One context (process) per GPU; rank 0 creates the id, every rank joins.  When a communicator is attached,
@@ -397,6 +413,13 @@ int fbgpu_node_groupby_mixed(fbgpu_node *node, uint32_t index,
                              const uint32_t *vfields, const uint32_t *vviews, const int32_t *bit_depths, int32_t n_ints,
                              const int64_t *values_flat, const int32_t *n_values,
                              const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+int fbgpu_node_groupby_sum(fbgpu_node *node, uint32_t index,
+                           const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                           const uint64_t *row_ids_flat, const int32_t *n_rows,
+                           const uint32_t *vfields, const uint32_t *vviews, const int32_t *bit_depths, int32_t n_ints,
+                           const int64_t *values_flat, const int32_t *n_values, uint32_t afield, uint32_t aview, int32_t a_depth,
+                           const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards,
+                           uint64_t *out_counts, int64_t *out_sums);
 int fbgpu_node_bsi_sum(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                        const uint64_t *shards, int64_t n_shards, int64_t *out_sum, uint64_t *out_count);
 int fbgpu_node_bsi_minmax(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
