@@ -16,6 +16,8 @@
             distinct values each, fbgpu_groupby_mixed against the composition (only when named in --configs).
   config S: GroupBy(Rows(a), aggregate=Sum(field=v)), the same with Rows(b) or Rows(w) beside a, fbgpu_groupby_sum against the
             Sum-per-group composition (only when named in --configs).
+  config D: GroupBy(Rows(a), aggregate=Count(Distinct(field=v))), the same with Rows(w) or Rows(b) beside a, on config S's data,
+            fbgpu_groupby_distinct against the Distinct-per-group composition (only when named in --configs).
 Every point is spot-checked against the CPU oracle on a few shards (the checker, not the thing measured)."""
 import argparse
 import json
@@ -603,16 +605,20 @@ class _NoGroupBySum(_KernelMs):
         return super().__getattr__(name)
 
 
-def config_groupby_sum(args, out):
-    """GroupBy(Rows(a), aggregate=Sum(field=v)), GroupBy(Rows(a), Rows(b), aggregate=Sum(field=v)) and GroupBy(Rows(a), Rows(w),
-    aggregate=Sum(field=v)) over --groupby-shards shards, without and with a 1 % filter row, through the executor.  Config V / M's
-    data shape: a and b are 256-row set fields at 1/256 density per row; w (64 distinct values) and v (values in ±2^20, 21 bits)
-    are int fields holding a value for each of the first 16,384 columns of every shard.  The device arm (one fbgpu_groupby_sum)
-    runs over all shards.  The composition arm (the group counts on the device, then one Sum(Intersect(rows, filter)) library
-    query per non-empty group) runs over the first --composition-shards shards, for --composition-steps steps alternated with the
-    device arm over the same shards.  Both arms must return the same groups; every device result's total count must equal
-    Σ_r Count(Row(a=r) ∩ filter ∩ exists(v) (∩ exists(w))).  Progress goes to stderr."""
-    from featurebase_b200 import datagen as D, executor as X, lib as L
+class _NoGroupByDistinct(_KernelMs):
+    """the same proxy without groupby_distinct: the executor counts the groups on the device, then runs one Distinct per group"""
+
+    def __getattr__(self, name):
+        if name == "groupby_distinct":
+            raise AttributeError(name)
+        return super().__getattr__(name)
+
+
+def _config_s_world(args, tag):
+    """config S's data over --groupby-shards shards: a and b are 256-row set fields at 1/256 density per row, c a 1 % filter row;
+    w (64 distinct values) and v (values in ±2^20, 21 bits) are int fields holding a value for each of the first 16,384 columns
+    of every shard.  Returns (holder, index, fields a, b, c, w, v, load seconds)."""
+    from featurebase_b200 import datagen as D, executor as X
     S, R, n_cols, dw = args.groupby_shards, 256, 16384, 64
     shards = np.arange(S, dtype=np.uint64)
     h = X.Holder()
@@ -631,7 +637,20 @@ def config_groupby_sum(args, out):
     h.ctx.commit()
     idx.shards.update(range(S))
     load_s = time.time() - t0
-    print(f"config S: loaded {S} shards in {load_s:.1f}s", file=sys.stderr, flush=True)
+    print(f"config {tag}: loaded {S} shards in {load_s:.1f}s", file=sys.stderr, flush=True)
+    return h, idx, fa, fb, ff, fw, fv, load_s
+
+
+def config_groupby_sum(args, out):
+    """GroupBy(Rows(a), aggregate=Sum(field=v)), GroupBy(Rows(a), Rows(b), aggregate=Sum(field=v)) and GroupBy(Rows(a), Rows(w),
+    aggregate=Sum(field=v)) over --groupby-shards shards (_config_s_world), without and with a 1 % filter row, through the
+    executor.  The device arm (one fbgpu_groupby_sum) runs over all shards.  The composition arm (the group counts on the device,
+    then one Sum(Intersect(rows, filter)) library query per non-empty group) runs over the first --composition-shards shards, for
+    --composition-steps steps alternated with the device arm over the same shards.  Both arms must return the same groups; every
+    device result's total count must equal Σ_r Count(Row(a=r) ∩ filter ∩ exists(v) (∩ exists(w))).  Progress goes to stderr."""
+    from featurebase_b200 import executor as X, lib as L
+    S, R = args.groupby_shards, 256
+    h, idx, fa, fb, ff, fw, fv, load_s = _config_s_world(args, "S")
     real = h.ctx
     card = _card()
     dev, comp = _KernelMs(real), _NoGroupBySum(real)
@@ -675,6 +694,70 @@ def config_groupby_sum(args, out):
                          "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])), "wall_ms_max": float(np.max(dd["wall"])),
                          "kernel_ms": float(np.median(dd["kernel_ms"])), "queries": int(np.median(dd["queries"])), "steps": len(dd["wall"]), "load_s": round(load_s, 1),
                          "kernel": "eval_kernel + groupby_values_kernel<true>" if name == "device" else "eval_kernel + groupby kernels, then eval_kernel + bsi_sum_kernel per group",
+                         "note": "median over the timed steps of the executor call (wall clock, Rows / Distinct pre-passes included), of the summed "
+                                 "last_query_gpu_ms and of the number of its library queries"}
+                    if name == "composition":
+                        o["wall_ms_per_step"] = [round(x, 2) for x in dd["wall"]]
+                    out(o)
+    real.close()
+
+
+def config_groupby_distinct(args, out):
+    """GroupBy(Rows(a), aggregate=Count(Distinct(field=v))), the same with Rows(w) and then Rows(b) beside a, over config S's data
+    (_config_s_world), without and with a 1 % filter row, through the executor.  The device arm (one Distinct for v's values,
+    then fbgpu_groupby_distinct, sliced by GROUPBY_DISTINCT_BITS) runs over all shards.  The composition arm (the group counts on
+    the device, then one Distinct(Intersect(rows, filter), field=v) library query per group) runs over the first
+    --composition-shards shards, for --composition-steps steps alternated with the device arm over the same shards.  Both arms
+    must return the same groups, every distinct count lies in 0 .. the group's count, and without b (a and w partition the
+    columns) the counts add up to Σ_r Count(Row(a=r) ∩ filter).  Progress goes to stderr."""
+    from featurebase_b200 import executor as X, lib as L
+    S, R = args.groupby_shards, 256
+    h, idx, fa, fb, ff, fw, fv, load_s = _config_s_world(args, "D")
+    real = h.ctx
+    card = _card()
+    dev, comp = _KernelMs(real), _NoGroupByDistinct(real)
+    CS = min(S, args.composition_shards)
+    op = lambda code, field=0, view=0, argc=0: L.Op(code, field, view, argc, 0, 0, 0, 0)
+    for second in ("", "Rows(w), ", "Rows(b), "):
+        for q_filter in (False, True):
+            q = f"GroupBy(Rows(a), {second}aggregate=Count(Distinct(field=v))" + (", filter=Row(c=0))" if q_filter else ")")
+            need = [op(L.OP_ROW, fw.id, X.VIEW_BSI)] if "w" in second else []
+            if q_filter:
+                need += [op(L.OP_ROW, ff.id)] + ([op(L.OP_INTERSECT, argc=2)] if "w" in second else [])
+            runs = [(S, {"device": dev})] + ([(CS, {"device": dev, "composition": comp})] if args.composition_steps > 0 else [])
+            for n_sh, arms in runs:
+                sh = list(range(n_sh))
+                want = int(real.row_counts(idx.id, fa.id, X.VIEW_STANDARD, sh, row_ids=list(range(R)), filter_ops=need or None).sum())
+                rec = {name: {"wall": [], "kernel_ms": [], "queries": []} for name in arms}
+                res = {}
+                for i in range(1 + args.steps):              # one warm-up round of the device arm, then alternate the arms
+                    for name in (sorted(arms) if i % 2 == 0 else sorted(arms, reverse=True)):
+                        if name == "composition" and len(rec[name]["wall"]) >= args.composition_steps:
+                            continue
+                        h.ctx = arms[name]
+                        q0, arms[name].ms = real.counters()["queries"], 0.0
+                        t1 = time.perf_counter()
+                        r = X.Executor(h).execute("i", q, sh)[0]
+                        wall = (time.perf_counter() - t1) * 1e3
+                        res.setdefault(name, r)
+                        assert r == res[name], (q, name)
+                        print(f"config D: {q} over {n_sh} shards, {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                        if i >= 1 or name == "composition":
+                            rec[name]["wall"].append(wall)
+                            rec[name]["kernel_ms"].append(arms[name].ms)
+                            rec[name]["queries"].append(real.counters()["queries"] - q0)
+                h.ctx = real
+                assert all(r == res["device"] for r in res.values()), q
+                assert all(0 <= g[2] <= g[1] for g in res["device"]) and any(g[2] for g in res["device"]), q
+                if "b" not in second:
+                    assert sum(g[1] for g in res["device"]) == want > 0, (q, want)
+                for name, dd in rec.items():
+                    o = {"config": "D", "query": q, "arm": name, "gpu": card, "shards": n_sh, "groups": len(res[name]),
+                         "equal_to_composition": ("composition" in res) or None,
+                         "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])), "wall_ms_max": float(np.max(dd["wall"])),
+                         "kernel_ms": float(np.median(dd["kernel_ms"])), "queries": int(np.median(dd["queries"])), "steps": len(dd["wall"]), "load_s": round(load_s, 1),
+                         "kernel": ("eval_kernel + groupby kernels, extract_values_kernel once, groupby_values_kernel<GvAgg::kDistinct> + gv_popcount_kernel"
+                                    if name == "device" else "eval_kernel + groupby kernels, then eval_kernel + extract_values_kernel per group"),
                          "note": "median over the timed steps of the executor call (wall clock, Rows / Distinct pre-passes included), of the summed "
                                  "last_query_gpu_ms and of the number of its library queries"}
                     if name == "composition":
@@ -777,8 +860,8 @@ def main():
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--shards", type=int, default=1024)
     ap.add_argument("--groupby-shards", type=int, default=512)
-    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S: steps of the composition arm")
-    ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S: shards of the composition arm and of the device arm timed beside it")
+    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D: steps of the composition arm")
+    ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S, D: shards of the composition arm and of the device arm timed beside it")
     ap.add_argument("--generators", default="uniform,clustered")
     ap.add_argument("--batched", action="store_true", help="also time the multi-pair launch (config 5b)")
     ap.add_argument("--densities", default="0.0001,0.001,0.01,0.03,0.0625,0.125,0.25,0.5")
@@ -803,6 +886,8 @@ def main():
             config_groupby_mixed(args, out)
         elif c == "S":
             config_groupby_sum(args, out)
+        elif c == "D":
+            config_groupby_distinct(args, out)
         elif c == "3L":     # the same BSI query at 256 shards (268 M records, 1.1 GB of planes): shows the kernel away from the launch-bound regime
             config3(args, out, n_rec=256 * SW, nf=1)
         else:

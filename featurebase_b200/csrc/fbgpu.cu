@@ -146,6 +146,7 @@ struct Workspace {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     DevBuf d_in, d_counts, d_bitmaps, d_info, d_emit_units, d_emit, d_rows, d_aux;
     DevBuf d_select;                     // fbgpu_bsi_select: per-rank candidate bitmaps of every unit of the call
+    DevBuf d_present;                    // fbgpu_groupby_distinct: one leaf's presence bitset, (cell, listed value of x) -> present
     PinBuf h_in, h_out;
     bool busy = false;
 };
@@ -251,7 +252,7 @@ extern "C" void fbgpu_shutdown(fbgpu_ctx* c) {
     cudaDeviceSynchronize();
     if (c->comm && nccl_load()) g_nccl.CommDestroy(c->comm);
     for (auto& w : c->wss) {
-        for (DevBuf* b : { &w->d_in, &w->d_counts, &w->d_bitmaps, &w->d_info, &w->d_emit_units, &w->d_emit, &w->d_rows, &w->d_aux, &w->d_select }) b->release();
+        for (DevBuf* b : { &w->d_in, &w->d_counts, &w->d_bitmaps, &w->d_info, &w->d_emit_units, &w->d_emit, &w->d_rows, &w->d_aux, &w->d_select, &w->d_present }) b->release();
         w->h_in.release(); w->h_out.release();
         if (w->ev0) cudaEventDestroy(w->ev0);
         if (w->ev1) cudaEventDestroy(w->ev1);
@@ -1875,7 +1876,8 @@ extern "C" int fbgpu_groupby_views(fbgpu_ctx* c, uint32_t index, const uint32_t*
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ GroupBy over the values of int fields
-// one int dimension of fbgpu_groupby_values / fbgpu_groupby_mixed: field, BSI view, depth and the ascending stored values that are its groups
+// one int dimension of fbgpu_groupby_values / fbgpu_groupby_mixed: field, BSI view, depth and the ascending stored values that are its groups.
+// As the aggregate field x: values is null for Sum, and for Count(Distinct) the ascending stored values whose presence is counted
 struct GvInt { uint32_t field, view; int32_t depth; const int64_t* values; int32_t n_values; };
 
 // the argument checks fbgpu_groupby_values and its node form make before any device is touched
@@ -1935,8 +1937,28 @@ static int groupby_sum_args(const void* handle, const uint32_t* fields, const ui
     return 0;
 }
 
+// the argument checks fbgpu_groupby_distinct makes before any device is touched (n_rows is checked after it)
+static int groupby_distinct_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                 const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews,
+                                 const int32_t* bit_depths, int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, int32_t x_depth,
+                                 const int64_t* x_values, int32_t n_x, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards,
+                                 int64_t n_shards, const uint64_t* out_distinct) {
+    if (!x_values) return fail(FBGPU_E_INVALID, "bad argument");
+    int rc = groupby_mixed_args(handle, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat,
+                                n_values, filter, n_filter_ops, shards, n_shards, out_distinct, 0, 8);
+    if (rc) return rc;
+    if (n_fields + n_ints < 1) return fail(FBGPU_E_INVALID, "no dimension: n_fields + n_ints = 0");
+    if (x_depth < 0 || x_depth > 64) return fail(FBGPU_E_INVALID, "x_depth=%d outside 0..64", x_depth);
+    if (n_x < 1) return fail(FBGPU_E_INVALID, "n_x=%d < 1", n_x);
+    for (int32_t i = 1; i < n_x; i++)
+        if (x_values[i] <= x_values[i - 1]) return fail(FBGPU_E_INVALID, "x_values are not strictly ascending at position %d", i);
+    return 0;
+}
+
 // one groupby_values_kernel pass over the shards: counts[nB or 1][groups] of consider = filter ∩ exists(v_1) ∩ ... (∩ Row(b = row));
-// with an aggregate x, consider also ∩ exists(x) and sums[nB or 1][groups] the columns' stored values of x
+// with an aggregate x, consider also ∩ exists(x) and sums[nB or 1][groups] the columns' stored values of x (Sum), or out[nB or 1]
+// [groups] the number of x's listed values present in the cell (Count(Distinct): x->values set, out_sums null).  The presence
+// bitset stays on the device; only the per-cell counts come back
 static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* null: no set dimension */, const std::vector<GvInt>& v,
                                const GvInt* x /* null: counts only */, const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards,
                                uint64_t* out, uint64_t* out_sums) {
@@ -1947,13 +1969,16 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
     int rc = q.open(index, full.data(), (int32_t)full.size(), shards, n_shards); if (rc) return rc;
     GvInts k{};
     k.n = (int)v.size(); k.n_groups = 1;
-    std::vector<uint64_t> in;                                        // [values (as int64) | b rows | b view slots (u32)]
+    std::vector<uint64_t> in;                                        // [values (as int64) | x's values | b rows | b view slots (u32)]
     for (int i = 0; i < k.n; i++) {
         k.fv[i] = view_id_locked(c, ViewKey{ index, v[(size_t)i].field, v[(size_t)i].view }, false);
         k.depth[i] = v[(size_t)i].depth; k.off[i] = (int)in.size(); k.n_values[i] = v[(size_t)i].n_values;
         k.n_groups *= v[(size_t)i].n_values;
         in.insert(in.end(), v[(size_t)i].values, v[(size_t)i].values + v[(size_t)i].n_values);
     }
+    const bool distinct = x && x->values;
+    const size_t x_off = in.size();
+    if (distinct) in.insert(in.end(), x->values, x->values + x->n_values);
     const size_t n_vals = in.size();
     const uint32_t fvX = x ? view_id_locked(c, ViewKey{ index, x->field, x->view }, false) : kNoView;
     const int nB = b ? b->n_rows : 0;
@@ -1964,10 +1989,13 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
     if (nvB > 1) in.resize(n_in + (nvB + 1) / 2);
     if (nvB > 1) memcpy(in.data() + n_in, fvsB.data(), nvB * 4);
     const size_t ncnt = (size_t)(b ? nB : 1) * (size_t)k.n_groups;
-    const size_t nout = x ? 2 * ncnt : ncnt;                         // [counts | sums]
+    const size_t nout = x && !distinct ? 2 * ncnt : ncnt;            // [counts | sums], or the distinct counts
+    const size_t xwords = distinct ? ((size_t)x->n_values + 63) / 64 : 0;       // presence words per cell
+    if (distinct && w->d_present.ensure(ncnt * xwords * 8)) return FBGPU_E_NOMEM;
     if (w->d_rows.ensure(in.size() * 8) || w->d_counts.ensure(nout * 8) || w->h_out.ensure(nout * 8)) return FBGPU_E_NOMEM;
     CUDA_TRY(cudaMemcpyAsync(w->d_rows.p, in.data(), in.size() * 8, cudaMemcpyHostToDevice, w->stream));
     CUDA_TRY(cudaMemsetAsync(w->d_counts.p, 0, nout * 8, w->stream));
+    if (distinct) CUDA_TRY(cudaMemsetAsync(w->d_present.p, 0, ncnt * xwords * 8, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));   // `in` is a local
     const long long* d_values = (const long long*)w->d_rows.p;
     const uint64_t* d_rowsB = b ? (const uint64_t*)w->d_rows.p + n_vals : nullptr;
@@ -1978,13 +2006,23 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
         rc = q.eval(u0, nu); if (rc) return rc;
         const long long grid = std::min<long long>(nu, (long long)c->sm_count * kGvCtasPerSm);
         unsigned long long* d_counts = (unsigned long long*)w->d_counts.p;
-        if (x)
-            groupby_values_kernel<true><<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB,
-                                                                                    (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, d_counts,
-                                                                                    fvX, x->depth, d_counts + ncnt);
+        if (distinct)
+            groupby_values_kernel<GvAgg::kDistinct><<<(unsigned)grid, kGvThreads, 0, w->stream>>>(
+                store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB, (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, d_counts,
+                fvX, x->depth, nullptr, d_values + x_off, x->n_values, (unsigned long long*)w->d_present.p);
+        else if (x)
+            groupby_values_kernel<GvAgg::kSum><<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB,
+                                                                                           (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, d_counts,
+                                                                                           fvX, x->depth, d_counts + ncnt);
         else
-            groupby_values_kernel<false><<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB,
-                                                                                     (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, d_counts);
+            groupby_values_kernel<GvAgg::kCount><<<(unsigned)grid, kGvThreads, 0, w->stream>>>(store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB,
+                                                                                             (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, d_counts);
+        CUDA_TRY(cudaGetLastError()); q.launches++;
+    }
+    if (distinct) {                                                  // every batch has marked the bitset: count each cell's bits
+        const long long grid = std::min<long long>(((long long)ncnt + 7) / 8, (long long)c->sm_count * 8);
+        gv_popcount_kernel<<<(unsigned)grid, 256, 0, w->stream>>>((const unsigned long long*)w->d_present.p, (long long)xwords, (long long)ncnt,
+                                                                  (unsigned long long*)w->d_counts.p);
         CUDA_TRY(cudaGetLastError()); q.launches++;
     }
     CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
@@ -1992,7 +2030,7 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
     CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_counts.p, nout * 8, cudaMemcpyDeviceToHost, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
     memcpy(out, w->h_out.p, ncnt * 8);
-    if (x) memcpy(out_sums, (const uint64_t*)w->h_out.p + ncnt, ncnt * 8);
+    if (x && !distinct) memcpy(out_sums, (const uint64_t*)w->h_out.p + ncnt, ncnt * 8);
     q.add_elapsed();
     q.finish();
     return 0;
@@ -2007,13 +2045,13 @@ static int groupby_values_rec(fbgpu_ctx* c, uint32_t index, const GbDim* d, int 
     for (int i = 1; i < nf; i++) sub *= (size_t)d[i].n_rows;
     for (int r = 0; r < d[0].n_rows; r++) {
         int rc = groupby_values_rec(c, index, d + 1, nf - 1, v, x, and_row(filter.data(), (int32_t)filter.size(), d[0].field, d[0].views, d[0].n_views, d[0].rows[r]),
-                                    shards, n_shards, out + (size_t)r * sub, x ? out_sums + (size_t)r * sub : nullptr); if (rc) return rc;
+                                    shards, n_shards, out + (size_t)r * sub, out_sums ? out_sums + (size_t)r * sub : nullptr); if (rc) return rc;
     }
     return 0;
 }
 
-// fbgpu_groupby_values / fbgpu_groupby_mixed / fbgpu_groupby_sum once the arguments but n_rows are checked: the set dimensions'
-// rows are laid out from row_ids_flat, the outputs zeroed, the store locked
+// fbgpu_groupby_values / fbgpu_groupby_mixed / fbgpu_groupby_sum / fbgpu_groupby_distinct once the arguments but n_rows are
+// checked: the set dimensions' rows are laid out from row_ids_flat, the outputs zeroed, the store locked
 static int groupby_values_query(fbgpu_ctx* c, uint32_t index, std::vector<GbDim>& dims, const uint64_t* row_ids_flat, const std::vector<GvInt>& v,
                                 const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts,
                                 const GvInt* x = nullptr, int64_t* out_sums = nullptr) {
@@ -2026,7 +2064,7 @@ static int groupby_values_query(fbgpu_ctx* c, uint32_t index, std::vector<GbDim>
         dims[i].rows = p; p += dims[i].n_rows; total *= (size_t)dims[i].n_rows;
     }
     memset(out_counts, 0, total * 8);
-    if (x) memset(out_sums, 0, total * 8);
+    if (out_sums) memset(out_sums, 0, total * 8);
     if (total == 0) return 0;
     return groupby_values_rec(c, index, dims.data(), (int)dims.size(), v, x, std::vector<fbgpu_op>(filter, filter + n_filter_ops), shards, n_shards,
                               out_counts, (uint64_t*)out_sums);
@@ -2073,6 +2111,26 @@ extern "C" int fbgpu_groupby_sum(fbgpu_ctx* c, uint32_t index, const uint32_t* f
     for (int k = 0; k < n_ints; k++) { ints[(size_t)k] = GvInt{ vfields[k], vviews[k], bit_depths[k], vals, n_values[k] }; vals += n_values[k]; }
     const GvInt x{ afield, aview, a_depth, nullptr, 0 };
     return groupby_values_query(c, index, dims, row_ids_flat, ints, filter, n_filter_ops, shards, n_shards, out_counts, &x, out_sums);
+} FBGPU_CATCH
+
+// GroupBy(..., aggregate=Count(Distinct(field=x))): fbgpu_groupby_sum's dimensions with, per cell, how many of x's listed stored
+// values some column of filter ∩ the cell's rows holds.  Local to one context: distinct sets merge by union, which the u64 sum
+// the ranks' tensors are reduced with is not
+extern "C" int fbgpu_groupby_distinct(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                      const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews, const int32_t* bit_depths,
+                                      int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, uint32_t xfield, uint32_t xview, int32_t x_depth,
+                                      const int64_t* x_values, int32_t n_x, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
+                                      uint64_t* out_distinct) try {
+    int rc = groupby_distinct_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
+                                   x_depth, x_values, n_x, filter, n_filter_ops, shards, n_shards, out_distinct);
+    if (rc) return rc;
+    if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_groupby_distinct is local to one context: distinct sets of the ranks merge by union, not by sum");
+    std::vector<GbDim> dims((size_t)n_fields); const uint32_t* vw = views_flat;
+    for (int i = 0; i < n_fields; i++) { dims[(size_t)i] = GbDim{ fields[i], vw, n_views[i], nullptr, n_rows[i] }; vw += n_views[i]; }
+    std::vector<GvInt> ints((size_t)n_ints); const int64_t* vals = values_flat;
+    for (int k = 0; k < n_ints; k++) { ints[(size_t)k] = GvInt{ vfields[k], vviews[k], bit_depths[k], vals, n_values[k] }; vals += n_values[k]; }
+    const GvInt x{ xfield, xview, x_depth, x_values, n_x };
+    return groupby_values_query(c, index, dims, row_ids_flat, ints, filter, n_filter_ops, shards, n_shards, out_distinct, &x);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ comm

@@ -2007,6 +2007,11 @@ groupby_direct_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ ro
 // counted (b-row, column) adds 1 to counts and the value to sums, each lane or thread running one total per group until the
 // group changes.  x's planes follow the int fields' in the table.  The multi-view b bitmaps move to hist (eight warps x 64
 // words, as 32-bit halves), which is unused whenever b is present; without b there is no shared histogram.
+// kDistinct (fbgpu_groupby_distinct, GroupBy(..., aggregate=Count(Distinct(field=x)))): consider, x's planes and the stored
+// value per column as for kSum; the value is then binary-searched in x's ascending list xvals[0 .. nX) and its position j
+// (or kGvNoPos) left in mag.  Every counted (b-row, column) with a group and a position sets bit j of its cell's row of
+// `present` (cells of ceil(nX / 64) words, 64-bit indexed) with atomicOr, a lane skipping the bit it set last;
+// gv_popcount_kernel then counts each cell's bits.
 // ------------------------------------------------------------------------------------------------
 constexpr int kGvThreads = 256;
 constexpr int kGvCtasPerSm = 4;
@@ -2016,6 +2021,9 @@ constexpr int kGvHist = 1024;
 constexpr uint16_t kGvNone = 0xffff;
 constexpr int kGvMaxInts = 8;
 constexpr int kGvPlanes = 184;                     // plane table entries: what 48 KiB of static shared memory leaves
+constexpr unsigned long long kGvNoPos = ~0ull;     // kDistinct: the column's value of x is not listed
+
+enum class GvAgg { kCount, kSum, kDistinct };      // what groupby_values_kernel adds up per cell
 
 // the int dimensions of one launch, passed by value
 struct GvInts {
@@ -2083,7 +2091,18 @@ struct GvTotal {
     }
 };
 
-template <bool kSum>
+// kDistinct: bits per cell of the presence bitset, whole 64-bit words
+__device__ __forceinline__ unsigned long long gv_cell_bits(int nX) { return (((unsigned long long)nX + 63) >> 6) << 6; }
+
+// kDistinct: sets bit `bit` of the presence bitset, unless this lane set that bit last
+struct GvMark {
+    unsigned long long last = ~0ull;
+    __device__ __forceinline__ void mark(unsigned long long* present, unsigned long long bit) {
+        if (bit != last) { atomicOr(&present[bit >> 6], 1ull << (bit & 63)); last = bit; }
+    }
+};
+
+template <GvAgg kAgg>
 __global__ void __launch_bounds__(kGvThreads, kGvCtasPerSm)
 groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__ values,
                       const uint64_t* __restrict__ rowsB /* null: no set field */, int nB,
@@ -2091,7 +2110,10 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                       const uint4* __restrict__ consider, const uint64_t* __restrict__ shards, long long n_units,
                       unsigned long long* __restrict__ counts /* [nB or 1][v.n_groups], zeroed by the host */,
                       uint32_t fvX = 0, int depthX = 0 /* kSum: the aggregate field's BSI view slot and depth */,
-                      unsigned long long* __restrict__ sums = nullptr /* kSum: shaped as counts, zeroed by the host */) {
+                      unsigned long long* __restrict__ sums = nullptr /* kSum: shaped as counts, zeroed by the host */,
+                      const long long* __restrict__ xvals = nullptr, int nX = 0 /* kDistinct: x's ascending stored values */,
+                      unsigned long long* __restrict__ present = nullptr /* kDistinct: [nB or 1][v.n_groups][ceil(nX / 64)] words, zeroed */) {
+    constexpr bool kSum = kAgg == GvAgg::kSum, kDistinct = kAgg == GvAgg::kDistinct, kX = kSum || kDistinct;
     __shared__ unsigned long long mag[kGvRange];      // (with a multi-view b, the warps' row bitmaps once the groups are made)
     __shared__ uint16_t vidx[kGvRange];               // group index per column
     __shared__ uint32_t sign[kGvRange / 32];
@@ -2099,8 +2121,8 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
     __shared__ Resolved planes[kGvPlanes];            // per int field: sign row, then magnitude bits 0 .. depth - 1
     __shared__ uint32_t hist[kGvHist];
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nwarps = kGvThreads / 32;
-    const int n_hist = (kSum || rowsB) ? 0 : min(v.n_groups, kGvHist);
-    int n_planes = kSum ? depthX + 1 : 0;
+    const int n_hist = (kX || rowsB) ? 0 : min(v.n_groups, kGvHist);
+    int n_planes = kX ? depthX + 1 : 0;
     for (int k = 0; k < v.n; k++) n_planes += v.depth[k] + 1;
     const bool unit_planes = n_planes <= kGvPlanes;   // else every field's planes are resolved per range, at table entry 0
     for (long long unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
@@ -2113,7 +2135,7 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
         if (unit_planes)
             for (int k = 0, base = 0; k < v.n; base += v.depth[k] + 1, k++)
                 for (int p = tid; p <= v.depth[k]; p += kGvThreads) planes[base + p] = resolve(st, v.fv[k], shard, (uint64_t)(p + 1), slot);
-        if constexpr (kSum)
+        if constexpr (kX)
             if (unit_planes)
                 for (int p = tid; p <= depthX; p += kGvThreads) planes[n_planes - depthX - 1 + p] = resolve(st, fvX, shard, (uint64_t)(p + 1), slot);
         for (int i = tid; i < n_hist; i += kGvThreads) hist[i] = 0;
@@ -2155,7 +2177,7 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                 __syncthreads();                          // (mag / sign / planes are read no more)
                 if (unit_planes) base += depth + 1;
             }
-            if constexpr (kSum) {                         // the aggregate's stored value per column, into mag
+            if constexpr (kX) {                           // the aggregate's stored value (kDistinct: its position) per column, into mag
                 if (v.n == 0)
                     for (int i = tid; i < (int)kGvRange; i += kGvThreads) vidx[i] = ((cons[i >> 6] >> (i & 63)) & 1ull) ? 0 : kGvNone;
                 const int base = unit_planes ? n_planes - depthX - 1 : 0;
@@ -2169,8 +2191,22 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                     else { const unsigned long long bit = 1ull << (p - 1); gv_for_each(r, lo, cons, lane, [&](uint32_t c) { atomicOr(&mag[c], bit); }); }
                 }
                 __syncthreads();
-                for (int i = tid; i < (int)kGvRange; i += kGvThreads)
-                    if ((sign[i >> 5] >> (i & 31)) & 1u) mag[i] = 0ull - mag[i];      // wrapping: sign + 2^63 is INT64_MIN
+                if constexpr (kSum) {
+                    for (int i = tid; i < (int)kGvRange; i += kGvThreads)
+                        if ((sign[i >> 5] >> (i & 31)) & 1u) mag[i] = 0ull - mag[i];      // wrapping: sign + 2^63 is INT64_MIN
+                } else {
+                    for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
+                        unsigned long long j = kGvNoPos;
+                        if (vidx[i] != kGvNone) {
+                            const unsigned long long m = mag[i];
+                            const long long val = (long long)(((sign[i >> 5] >> (i & 31)) & 1u) ? 0ull - m : m);
+                            int a = 0, b = nX;
+                            while (a < b) { const int h = (int)(((unsigned)a + (unsigned)b) >> 1); if (__ldg(xvals + h) < val) a = h + 1; else b = h; }
+                            if (a < nX && __ldg(xvals + a) == val) j = (unsigned long long)a;
+                        }
+                        mag[i] = j;
+                    }
+                }
                 __syncthreads();
             }
             if (!rowsB) {
@@ -2181,6 +2217,13 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                         if (k != kGvNone) t.add(k, mag[i], counts, sums);
                     }
                     t.flush(counts, sums);
+                } else if constexpr (kDistinct) {
+                    GvMark mk;
+                    const unsigned long long xbits = gv_cell_bits(nX);
+                    for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
+                        const uint32_t k = vidx[i];
+                        if (k != kGvNone && mag[i] != kGvNoPos) mk.mark(present, (unsigned long long)k * xbits + mag[i]);
+                    }
                 } else {
                     for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
                         const uint32_t k = vidx[i];
@@ -2191,7 +2234,7 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                 }
                 continue;
             }
-            if (kSum && nvB > 1) {
+            if (kX && nvB > 1) {
                 uint32_t* bm = hist + wid * 2 * kGvRangeWords;              // this warp's row bitmap, word i as halves 2i, 2i + 1
                 for (int i = lane; i < 2 * kGvRangeWords; i += 32) bm[i] = 0;
                 __syncwarp();
@@ -2210,20 +2253,34 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                         }
                     }
                     __syncwarp();
-                    unsigned long long* crow = counts + (size_t)br * (size_t)v.n_groups;
-                    unsigned long long* srow = sums + (size_t)br * (size_t)v.n_groups;
-                    GvTotal t;
-                    for (int i = lane; i < kGvRangeWords; i += 32) {
-                        uint64_t m = ((uint64_t)bm[2 * i] | ((uint64_t)bm[2 * i + 1] << 32)) & cons[i];
-                        bm[2 * i] = 0; bm[2 * i + 1] = 0;
-                        while (m) { const int b = __ffsll((long long)m) - 1; const uint32_t g = vidx[i * 64 + b]; if (g != kGvNone) t.add(g, mag[i * 64 + b], crow, srow); m &= m - 1; }
+                    if constexpr (kSum) {
+                        unsigned long long* crow = counts + (size_t)br * (size_t)v.n_groups;
+                        unsigned long long* srow = sums + (size_t)br * (size_t)v.n_groups;
+                        GvTotal t;
+                        for (int i = lane; i < kGvRangeWords; i += 32) {
+                            uint64_t m = ((uint64_t)bm[2 * i] | ((uint64_t)bm[2 * i + 1] << 32)) & cons[i];
+                            bm[2 * i] = 0; bm[2 * i + 1] = 0;
+                            while (m) { const int b = __ffsll((long long)m) - 1; const uint32_t g = vidx[i * 64 + b]; if (g != kGvNone) t.add(g, mag[i * 64 + b], crow, srow); m &= m - 1; }
+                        }
+                        t.flush(crow, srow);
+                    } else {
+                        const unsigned long long xbits = gv_cell_bits(nX), rbit = (unsigned long long)br * (unsigned long long)v.n_groups * xbits;
+                        GvMark mk;
+                        for (int i = lane; i < kGvRangeWords; i += 32) {
+                            uint64_t m = ((uint64_t)bm[2 * i] | ((uint64_t)bm[2 * i + 1] << 32)) & cons[i];
+                            bm[2 * i] = 0; bm[2 * i + 1] = 0;
+                            while (m) {
+                                const int b = __ffsll((long long)m) - 1; const uint32_t g = vidx[i * 64 + b]; const unsigned long long j = mag[i * 64 + b];
+                                if (g != kGvNone && j != kGvNoPos) mk.mark(present, rbit + (unsigned long long)g * xbits + j);
+                                m &= m - 1;
+                            }
+                        }
                     }
-                    t.flush(crow, srow);
                     __syncwarp();
                 }
                 continue;
             }
-            if (!kSum && nvB > 1) {
+            if (!kX && nvB > 1) {
                 unsigned long long* bm = mag + wid * kGvRangeWords;          // this warp's row bitmap
                 for (int i = lane; i < kGvRangeWords; i += 32) bm[i] = 0;
                 __syncwarp();
@@ -2265,6 +2322,13 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                         GvTotal t;
                         gv_for_each(r, lo, cons, lane, [&](uint32_t c) { const uint32_t k = vidx[c]; if (k != kGvNone) t.add(k, mag[c], row, srow); });
                         t.flush(row, srow);
+                    } else if constexpr (kDistinct) {
+                        const unsigned long long xbits = gv_cell_bits(nX), rbit = (unsigned long long)(b0 + j) * (unsigned long long)v.n_groups * xbits;
+                        GvMark mk;
+                        gv_for_each(r, lo, cons, lane, [&](uint32_t c) {
+                            const uint32_t k = vidx[c]; const unsigned long long jx = mag[c];
+                            if (k != kGvNone && jx != kGvNoPos) mk.mark(present, rbit + (unsigned long long)k * xbits + jx);
+                        });
                     } else {
                         gv_for_each(r, lo, cons, lane, [&](uint32_t c) { const uint32_t k = vidx[c]; if (k != kGvNone) atomicAdd(&row[k], 1ull); });
                     }
@@ -2273,6 +2337,21 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
         }
         __syncthreads();
         for (int i = tid; i < n_hist; i += kGvThreads) if (hist[i]) atomicAdd(&counts[i], (unsigned long long)hist[i]);
+    }
+}
+
+// gv_popcount_kernel (fbgpu_groupby_distinct): out[cell] = the number of bits set in the cell's `words` words of groupby_values_kernel
+// <kDistinct>'s presence bitset; one warp per cell, the lanes striding its words
+__global__ void __launch_bounds__(256)
+gv_popcount_kernel(const unsigned long long* __restrict__ present, long long words, long long n_cells, unsigned long long* __restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long cell = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; cell < n_cells; cell += warps) {
+        const unsigned long long* w = present + cell * words;
+        unsigned long long n = 0;
+        for (long long i = lane; i < words; i += 32) n += (unsigned long long)__popcll(w[i]);
+        for (int o = 16; o; o >>= 1) n += __shfl_down_sync(0xffffffffu, n, o);
+        if (lane == 0) out[cell] = n;
     }
 }
 

@@ -985,7 +985,8 @@ class Executor:
     # ------------------------------------------------------------------ GroupBy (executeGroupBy :3176)
     def _groupby(self, idx, c, shards):
         """The device returns the dense count tensor over the children's row lists (with aggregate=Sum over an int field, the
-        counts of columns holding a value and their sums, from the same call); everything after it is the host-side
+        counts of columns holding a value and their sums, from the same call; with aggregate=Count(Distinct) over an int field,
+        the distinct counts from one more call after one Distinct for the field's values); everything after it is the host-side
         post-processing executeGroupBy does in Go: previous (iterator start, newGroupByIterator :8779-8826), aggregate=Sum
         (groupByIterator.Next :8893-8911: Count becomes the number of columns holding a value), having (:3388-3406),
         sort (:3130-3162, 3408-3414), offset / limit (:3441-3459).  Results: (group, count) or (group, count, agg)."""
@@ -1049,6 +1050,11 @@ class Executor:
         start = self._groupby_start(c, row_ids)
         if start is None:
             return []
+        dist = None                                               # Count(Distinct) over an int field of this index: per-cell counts
+        if distinct_agg and hasattr(self.ctx, "groupby_distinct") and "index" not in agg_distinct.args and counts.any():
+            f = idx.fields.get(agg_distinct.args.get("field", agg_distinct.args.get("_field")))
+            if f is not None and f.type == "int":                 # otherwise the per-group Distinct below raises or counts rows
+                dist = self._groupby_distinct(idx, fields, row_ids, time_args, int_dims, filt_call, agg_distinct, f, counts.shape, shards)
         has_sort, has_having = "sort" in c.args, isinstance(c.args.get("having"), pql.Call)
         limit = c.args.get("limit") if not (has_sort or has_having) else None       # :3196-3212: no early limit when sorting / filtering
         out = []
@@ -1070,11 +1076,13 @@ class Executor:
                 if vc.count == 0:
                     continue                                      # ret.Count == 0 => skipped (:8913-8919)
                 out.append((group, vc.count, vc.val))
+            elif dist is not None:
+                out.append((group, int(counts[ix]), int(dist[ix])))   # a distinct count of 0 is kept (:3343-3385)
             else:
                 out.append((group, int(counts[ix])))
             if limit and len(out) >= limit and "offset" not in c.args:
                 break
-        if distinct_agg:
+        if distinct_agg and dist is None:
             if not (has_sort or has_having):                      # limits first: the aggregate is expensive per group (:3327-3335)
                 out = self._window(c, out)
             for k, (group, n) in enumerate(out):                  # Count(Distinct(Intersect(group rows, filter, Distinct's child), field=..)) :3343-3385
@@ -1106,15 +1114,41 @@ class Executor:
                 out.sort(key=lambda g: (g[col] if len(g) > col else 0), reverse=not asc)
         return self._window(c, out)
 
-    GROUPBY_MIXED_MAX = 65535                                     # groups (product of the int children's value counts) per fbgpu_groupby_mixed / _sum call
+    GROUPBY_MIXED_MAX = 65535                                     # groups (product of the int children's value counts) per fbgpu_groupby_mixed / _sum / _distinct call
+    # presence bits ((rows of the last set child, or 1) x groups x listed values of x) per fbgpu_groupby_distinct call: 256 MiB
+    # of device workspace.  A choice that bounds the workspace, not a measured optimum.
+    GROUPBY_DISTINCT_BITS = 1 << 31
 
-    def _groupby_tensors(self, idx, fields, row_ids, time_args, int_dims, filt, shards, agg=None):
+    def _groupby_distinct(self, idx, fields, row_ids, time_args, int_dims, filt_call, agg_distinct, xf, shape, shards):
+        """the Count(Distinct(field=xf)) tensor of a GroupBy (shape: the count tensor's), or None when the context answers
+        FBGPU_E_COMM or has no such call (a node): the composition runs instead.  x's listed values are its stored values under
+        filter ∩ Distinct's child (one Distinct, as the int children's lists are made); the device then counts, per cell, those
+        present under filter ∩ Distinct's child ∩ the cell's rows."""
+        parts = [x for x in (filt_call, *agg_distinct.children[:1]) if isinstance(x, pql.Call)]
+        both = (parts[0] if len(parts) == 1 else pql.Call("Intersect", {}, parts)) if parts else None
+        ops = self._bitmap_call(idx, both) if both is not None else None
+        _, vals, _ = self.ctx.extract(idx.id, xf.id, VIEW_BSI, xf.bit_depth, shards, filter_ops=ops)
+        xs = np.unique(np.asarray(vals, dtype=np.int64))
+        if len(xs) == 0:
+            return np.zeros(shape, dtype=np.uint64)
+        try:
+            return self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, ops, shards, distinct=(xf, xs))[0]
+        except NotImplementedError:
+            return None
+        except L.FbgpuError as e:
+            if e.code != L.E_COMM:
+                raise
+            return None
+
+    def _groupby_tensors(self, idx, fields, row_ids, time_args, int_dims, filt, shards, agg=None, distinct=None):
         """[counts] of a GroupBy with int children (positions int_dims), from fbgpu_groupby_mixed, or with agg (the int field of
-        aggregate=Sum) [counts, sums] from fbgpu_groupby_sum, where int_dims may be empty: the other children are the set
-        dimensions (a time-range child with its covering views), the int children's values the trailing dimensions, moved back
-        to the children's order.  No Row(v == value) per value and no scratch rows.  When the value lists' product exceeds
-        GROUPBY_MIXED_MAX, each int child's list is cut into slices whose product fits and every combination of slices is one
-        call: a column's value lies in exactly one slice per field, so the pieces tile the tensors."""
+        aggregate=Sum) [counts, sums] from fbgpu_groupby_sum, or with distinct = (x, its listed stored values) [distinct counts]
+        from fbgpu_groupby_distinct, where int_dims may be empty: the other children are the set dimensions (a time-range child
+        with its covering views), the int children's values the trailing dimensions, moved back to the children's order.  No
+        Row(v == value) per value and no scratch rows.  When the value lists' product exceeds GROUPBY_MIXED_MAX, each int child's
+        list is cut into slices whose product fits and every combination of slices is one call: a column's value lies in exactly
+        one slice per field, so the pieces tile the tensors.  x's list is cut so that each call's presence bits stay within
+        GROUPBY_DISTINCT_BITS; the slices are disjoint, so their distinct counts add up per cell."""
         set_k = [j for j in range(len(fields)) if j not in int_dims]
         set_dims = [(fields[j].id, self._time_view_ids(fields[j], time_args[j]) if time_args[j] else [VIEW_STANDARD], row_ids[j]) for j in set_k]
         stored = [[v - fields[k].base for v in row_ids[k]] for k in int_dims]      # values as the planes hold them (value - Base)
@@ -1124,15 +1158,24 @@ class Executor:
             room //= step[-1]
         shape = [len(row_ids[j]) for j in set_k] + [len(v) for v in stored]
         outs = [np.zeros(shape, dtype=np.uint64)] + ([np.zeros(shape, dtype=np.int64)] if agg is not None else [])
+        x_cuts = [None]
+        if distinct is not None:
+            xf, xs = distinct
+            per_value = (len(row_ids[set_k[-1]]) if set_k else 1) * int(np.prod(step, dtype=np.int64))    # bits per listed value
+            x_step = max(1, self.GROUPBY_DISTINCT_BITS // per_value)
+            x_cuts = [xs[s:s + x_step] for s in range(0, len(xs), x_step)]
         for starts in itertools.product(*[range(0, len(v), n) for v, n in zip(stored, step)]):
             cut = [slice(s, s + n) for s, n in zip(starts, step)]
             int_part = [(fields[k].id, VIEW_BSI, fields[k].bit_depth, v[c]) for k, v, c in zip(int_dims, stored, cut)]
-            if agg is None:
-                got = [self.ctx.groupby_mixed(idx.id, set_dims, int_part, shards, filter_ops=filt)]
-            else:
-                got = self.ctx.groupby_sum(idx.id, set_dims, int_part, (agg.id, VIEW_BSI, agg.bit_depth), shards, filter_ops=filt)
-            for o, g in zip(outs, got):
-                o[(Ellipsis, *cut)] = g
+            for xc in x_cuts:
+                if distinct is not None:
+                    got = [self.ctx.groupby_distinct(idx.id, set_dims, int_part, (xf.id, VIEW_BSI, xf.bit_depth, xc), shards, filter_ops=filt)]
+                elif agg is None:
+                    got = [self.ctx.groupby_mixed(idx.id, set_dims, int_part, shards, filter_ops=filt)]
+                else:
+                    got = self.ctx.groupby_sum(idx.id, set_dims, int_part, (agg.id, VIEW_BSI, agg.bit_depth), shards, filter_ops=filt)
+                for o, g in zip(outs, got):
+                    o[(Ellipsis, *cut)] += g
         order = set_k + list(int_dims)
         return [np.transpose(o, [order.index(j) for j in range(len(fields))]) for o in outs]
 

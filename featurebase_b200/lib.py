@@ -50,7 +50,8 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_node_load_fragments", "fbgpu_node_load_rbf_dir", "fbgpu_node_drop_fragment", "fbgpu_node_commit", "fbgpu_node_get_stats", "fbgpu_node_count", "fbgpu_node_row",
            "fbgpu_node_count_pairs", "fbgpu_node_row_counts", "fbgpu_node_groupby", "fbgpu_node_bsi_sum", "fbgpu_node_bsi_minmax",
            "fbgpu_groupby_values", "fbgpu_node_groupby_values", "fbgpu_row_counts_views", "fbgpu_node_row_counts_views", "fbgpu_groupby_views",
-           "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum"]
+           "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum",
+           "fbgpu_groupby_distinct"]
 
 
 def lib_path():
@@ -105,6 +106,8 @@ def load():
     L.fbgpu_groupby_mixed.restype = C.c_int
     L.fbgpu_groupby_sum.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i64, vp, vp]
     L.fbgpu_groupby_sum.restype = C.c_int
+    L.fbgpu_groupby_distinct.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i32, vp, i64, vp]
+    L.fbgpu_groupby_distinct.restype = C.c_int
     L.fbgpu_count_pairs.argtypes, L.fbgpu_count_pairs.restype = [vp, u32, u32, u32, vp, u32, u32, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_comm_unique_id.argtypes, L.fbgpu_comm_unique_id.restype = [vp], C.c_int
     L.fbgpu_comm_init.argtypes, L.fbgpu_comm_init.restype = [vp, i32, i32, vp], C.c_int
@@ -531,6 +534,32 @@ class Context:
                                              int(agg[0]), int(agg[1]), int(agg[2]), f, nf, sh.ctypes.data, len(sh), counts.ctypes.data, sums.ctypes.data))
         return counts.reshape(shape), sums.reshape(shape)
 
+    def groupby_distinct(self, index, set_dims, int_dims, x, shards, filter_ops=None):
+        """GroupBy(..., aggregate=Count(Distinct(field=x))) in one call (fbgpu_groupby_distinct).  set_dims and int_dims as for
+        groupby_sum; x: (field, BSI view, bit depth, ascending stored values).  Returns a uint64 tensor of groupby_mixed's shape:
+        per cell the number of x's listed values that some column of filter ∩ the cell's rows holds."""
+        sh = _u64arr(shards)
+        fl = np.ascontiguousarray(np.asarray([d[0] for d in set_dims], dtype=np.uint32))
+        vw = np.ascontiguousarray(np.asarray([v for d in set_dims for v in d[1]], dtype=np.uint32))
+        n_views = np.ascontiguousarray(np.asarray([len(d[1]) for d in set_dims], dtype=np.int32))
+        n_rows = np.ascontiguousarray(np.asarray([len(d[2]) for d in set_dims], dtype=np.int32))
+        flat = _u64arr([r for d in set_dims for r in d[2]])
+        vf = np.ascontiguousarray(np.asarray([d[0] for d in int_dims], dtype=np.uint32))
+        vv = np.ascontiguousarray(np.asarray([d[1] for d in int_dims], dtype=np.uint32))
+        depths = np.ascontiguousarray(np.asarray([int(d[2]) for d in int_dims], dtype=np.int32))
+        n_values = np.ascontiguousarray(np.asarray([len(d[3]) for d in int_dims], dtype=np.int32))
+        vals = np.ascontiguousarray(np.asarray([int(v) for d in int_dims for v in d[3]], dtype=np.int64))
+        xv = np.ascontiguousarray(np.asarray(x[3], dtype=np.int64))
+        shape = [int(v) for v in n_rows] + [int(v) for v in n_values]
+        out = np.zeros(int(np.prod(shape, dtype=np.int64)), dtype=np.uint64)
+        f = ops_array(filter_ops) if filter_ops else None
+        nf = len(filter_ops) if filter_ops else 0
+        self._check(self.L.fbgpu_groupby_distinct(self.h, index, fl.ctypes.data, vw.ctypes.data, n_views.ctypes.data, len(fl), flat.ctypes.data,
+                                                  n_rows.ctypes.data, vf.ctypes.data, vv.ctypes.data, depths.ctypes.data, len(vf), vals.ctypes.data,
+                                                  n_values.ctypes.data, int(x[0]), int(x[1]), int(x[2]), xv.ctypes.data, len(xv), f, nf,
+                                                  sh.ctypes.data, len(sh), out.ctypes.data))
+        return out.reshape(shape)
+
     def rows_payload_bytes(self, index, field, view, shards, row_ids=None):
         sh = _u64arr(shards)
         pay, nc = C.c_uint64(0), C.c_uint64(0)
@@ -618,6 +647,9 @@ class Node(Context):
 
     def bsi_select(self, index, field, view, bit_depth, shards, ranks, filter_ops=None):
         raise NotImplementedError("fbgpu_bsi_select has no node form: order statistics of the devices' shares do not merge")
+
+    def groupby_distinct(self, index, set_dims, int_dims, x, shards, filter_ops=None):
+        raise NotImplementedError("fbgpu_groupby_distinct has no node form: the devices' distinct sets merge by union, not by sum")
 
     def row_counts(self, index, field, view, shards, row_ids=None, filter_ops=None, cap=1 << 20):
         if row_ids is None:

@@ -331,6 +331,25 @@ int fbgpu_groupby_sum(fbgpu_ctx *ctx, uint32_t index,
                       const int64_t *values_flat, const int32_t *n_values, uint32_t afield, uint32_t aview, int32_t a_depth,
                       const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards,
                       uint64_t *out_counts, int64_t *out_sums);
+/* GroupBy(..., aggregate=Count(Distinct(field=x))) in one device call (SQL SELECT a, COUNT(DISTINCT x) ... GROUP BY a).
+ * The dimensions are fbgpu_groupby_sum's.  xfield / xview / x_depth (0..64): x's BSI view and its depth; x_values: n_x >= 1
+ * strictly ascending stored values (value - Base) as fbgpu_extract reports them.  out_distinct: a tensor of
+ * fbgpu_groupby_mixed's shape and layout.  Per cell, the number of listed x_values[j] that at least one column of
+ * filter ∩ the cell's rows ∩ exists(x) holds as its stored value of x: the listed values among fbgpu_extract(x)'s values under
+ * `filter ∩ the cell's rows`.  x's sign with magnitude 0 is the value 0 (as in fbgpu_extract), the int dimensions' is no
+ * value (as in fbgpu_groupby_mixed); a column whose x value is not listed counts nowhere.  A shard lacking x's fragment
+ * contributes nothing; missing set or int fragments as for fbgpu_groupby_mixed.  Argument errors other than n_rows are
+ * reported before the device check; a presence workspace (rows of the last set dimension, or 1) x groups x ceil(n_x / 64)
+ * x 8 bytes that cannot be allocated gives FBGPU_E_NOMEM.  A context with a communicator attached returns FBGPU_E_COMM:
+ * distinct sets merge by union, not by the u64 sum the other GroupBy tensors are all-reduced with. */
+int fbgpu_groupby_distinct(fbgpu_ctx *ctx, uint32_t index,
+                           const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                           const uint64_t *row_ids_flat, const int32_t *n_rows,
+                           const uint32_t *vfields, const uint32_t *vviews, const int32_t *bit_depths, int32_t n_ints,
+                           const int64_t *values_flat, const int32_t *n_values,
+                           uint32_t xfield, uint32_t xview, int32_t x_depth, const int64_t *x_values, int32_t n_x,
+                           const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards,
+                           uint64_t *out_distinct);
 
 /* ---- multi-GPU reduce (replaces the HTTP fan-in of mapReduce/remoteExec, executor.go:6392-6533) ----
  * One context (process) per GPU; rank 0 creates the id, every rank joins.  When a communicator is attached,

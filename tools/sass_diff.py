@@ -3,7 +3,8 @@
     python tools/sass_diff.py <commit>         # e.g. the last commit whose library was parity-tested and timed on an H100
 Builds that commit's csrc/ in a scratch directory with the same nvcc line, dumps both libraries with cuobjdump -sass and
 compares the instruction streams per kernel (addresses and encodings stripped; template arguments that did not exist yet
-or no longer exist are matched by kernel name: an untemplated kernel and its <false> instantiation).  Kernels of the old
+or no longer exist are matched by kernel name: an untemplated kernel and its <false> instantiation, and groupby_values_kernel's
+<GvAgg(0)> / <GvAgg(1)> (count only / Sum) and the <false> / <true> of the bool template they replaced).  Kernels of the old
 build that the new one lacks are reported DELETED.  No GPU needed.  A kernel reported IDENTICAL is, bit for bit in its
 instructions, the one that was parity-tested and timed on the device."""
 import os
@@ -32,13 +33,23 @@ def kernels(path):
     return res
 
 
+ENUM_AS_BOOL = {"LNS_5GvAggE0": "Lb0", "LNS_5GvAggE1": "Lb1"}      # GvAgg::kCount / kSum took the place of <false> / <true>
+
+
 def short(name):
-    m = re.match(r"_ZN5fbgpu\d+([a-z_0-9]+?)(I(Lb[01])E)?E", name)
+    """(kernel name, template argument) with the argument as mangled: Lb0 / Lb1 for a bool, LNS_<n><Enum>E<value> for an enum"""
+    m = re.match(r"_ZN5fbgpu\d+([a-z_0-9]+?)(I(Lb[01]|LNS_\d+\w+?E\d+)E)?E", name)
     return (m.group(1), m.group(3) or "") if m else (name, "")
 
 
 def label(name, targ):
-    return name + ("<%s>" % ("true" if targ == "Lb1" else "false") if targ else "")
+    m = re.match(r"LNS_\d+(\w+?)E(\d+)$", targ)
+    return name + ("<%s(%s)>" % m.groups() if m else "<%s>" % ("true" if targ == "Lb1" else "false") if targ else "")
+
+
+def same_arg(a, b):
+    a, b = ENUM_AS_BOOL.get(a, a), ENUM_AS_BOOL.get(b, b)
+    return a == b or {a, b} <= {"", "Lb0"}
 
 
 def main():
@@ -56,7 +67,7 @@ def main():
     for k, v in b.items():
         name, targ = short(k)
         cands = by_name.get(name, [])
-        hit = [x for x in cands if x[0] == targ] or [x for x in cands if {x[0], targ} <= {"", "Lb0"}]
+        hit = [x for x in cands if x[0] == targ] or [x for x in cands if same_arg(x[0], targ)]
         if not hit:
             print(f"NEW        {label(name, targ):28s} {len(v):5d} instructions")
         else:
