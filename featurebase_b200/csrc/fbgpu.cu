@@ -1798,54 +1798,13 @@ static int groupby2(fbgpu_ctx* c, uint32_t index, uint32_t fvA, const uint64_t* 
 // one GroupBy dimension: the listed rows of `field`, each taken as its union over views[0..n_views)
 struct GbDim { uint32_t field; const uint32_t* views; int32_t n_views; const uint64_t* rows; int32_t n_rows; };
 
-// n-field GroupBy: peel the leading field on the host, folding Row(f0=r) — over several views, the union of those rows — into
-// the filter (groupByIterator keeps the same prefix intersections per level, executor.go:8829-8835,8861-8867).  The last
-// dimension is counted by the row-count kernels, two single-view last dimensions by groupby2.
-static int groupby_rec(fbgpu_ctx* c, uint32_t index, const GbDim* d, int nf, std::vector<fbgpu_op> filter, const uint64_t* shards, int64_t n_shards, uint64_t* out) {
-    if (nf == 1) {
-        std::vector<uint64_t> r(d[0].rows, d[0].rows + d[0].n_rows), counts;
-        int rc = row_counts_impl(c, index, view_slots(c, index, d[0].field, d[0].views, d[0].n_views), r, filter.empty() ? nullptr : filter.data(), (int)filter.size(),
-                                 shards, n_shards, counts); if (rc) return rc;
-        memcpy(out, counts.data(), counts.size() * 8);
-        return 0;
-    }
-    if (nf == 2 && d[0].n_views == 1 && d[1].n_views == 1) {
-        uint32_t fa = view_id_locked(c, ViewKey{ index, d[0].field, d[0].views[0] }, false), fb = view_id_locked(c, ViewKey{ index, d[1].field, d[1].views[0] }, false);
-        return groupby2(c, index, fa, d[0].rows, d[0].n_rows, fb, d[1].rows, d[1].n_rows, filter, shards, n_shards, out);
-    }
-    size_t sub = 1; for (int i = 1; i < nf; i++) sub *= (size_t)d[i].n_rows;
-    for (int r = 0; r < d[0].n_rows; r++) {
-        int rc = groupby_rec(c, index, d + 1, nf - 1, and_row(filter.data(), (int32_t)filter.size(), d[0].field, d[0].views, d[0].n_views, d[0].rows[r]),
-                             shards, n_shards, out + (size_t)r * sub); if (rc) return rc;
-    }
+// the argument checks fbgpu_groupby and its node form make before any device is touched (the context form checks n_rows after it)
+static int groupby_args(const void* handle, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows,
+                        const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts) {
+    if (!handle || !fields || !views || !row_ids_flat || !n_rows || !out_counts || n_fields < 1 || n_fields > 8 || n_filter_ops < 0 || (n_filter_ops && !filter) ||
+        n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
     return 0;
 }
-
-// fbgpu_groupby / fbgpu_groupby_views once the arguments are checked and the store is locked
-static int groupby_dims(fbgpu_ctx* c, uint32_t index, const std::vector<GbDim>& dims, const fbgpu_op* filter, int32_t n_filter_ops,
-                        const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) {
-    size_t total = 1; for (const GbDim& d : dims) total *= (size_t)d.n_rows;
-    memset(out_counts, 0, total * 8);
-    if (total == 0) return 0;
-    // executor.go:8769-8772: the kernels treat a shard with a missing fragment as contributing nothing; for the
-    // row_counts path (n_fields == 1) a missing fragment naturally yields zeros.  For n_fields >= 3 the peeled
-    // fields enter through the filter, which is empty on shards without that fragment.
-    std::vector<fbgpu_op> f(filter, filter + (filter ? n_filter_ops : 0));
-    return groupby_rec(c, index, dims.data(), (int)dims.size(), f, shards, n_shards, out_counts);
-}
-
-extern "C" int fbgpu_groupby(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows,
-                             const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
-    if (!c || !fields || !views || !row_ids_flat || !n_rows || !out_counts || n_fields < 1 || n_fields > 8 || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
-    std::shared_lock<std::shared_mutex> lk;
-    int rc = begin_query(c, lk); if (rc) return rc;
-    std::vector<GbDim> dims((size_t)n_fields); const uint64_t* p = row_ids_flat;
-    for (int i = 0; i < n_fields; i++) {
-        if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]);
-        dims[(size_t)i] = GbDim{ fields[i], views + i, 1, p, n_rows[i] }; p += n_rows[i];
-    }
-    return groupby_dims(c, index, dims, filter, n_filter_ops, shards, n_shards, out_counts);
-} FBGPU_CATCH
 
 // the argument checks fbgpu_groupby_views and its node form make before any device is touched
 static int groupby_views_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
@@ -1860,20 +1819,6 @@ static int groupby_views_args(const void* handle, const uint32_t* fields, const 
     }
     return 0;
 }
-
-// GroupBy(Rows(f1, from=, to=), ...): fbgpu_groupby with dimension i's rows taken as their unions over n_views[i] views
-// (timeFragmentsRowIterator, executor.go:8755-8768)
-extern "C" int fbgpu_groupby_views(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
-                                   const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
-                                   const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
-    int rc = groupby_views_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards, out_counts);
-    if (rc) return rc;
-    std::shared_lock<std::shared_mutex> lk;
-    rc = begin_query(c, lk); if (rc) return rc;
-    std::vector<GbDim> dims((size_t)n_fields); const uint32_t* v = views_flat; const uint64_t* p = row_ids_flat;
-    for (int i = 0; i < n_fields; i++) { dims[(size_t)i] = GbDim{ fields[i], v, n_views[i], p, n_rows[i] }; v += n_views[i]; p += n_rows[i]; }
-    return groupby_dims(c, index, dims, filter, n_filter_ops, shards, n_shards, out_counts);
-} FBGPU_CATCH
 
 // ------------------------------------------------------------------ GroupBy over the values of int fields
 // one int dimension of fbgpu_groupby_values / fbgpu_groupby_mixed: field, BSI view, depth and the ascending stored values that are its groups.
@@ -1922,36 +1867,20 @@ static int groupby_mixed_args(const void* handle, const uint32_t* fields, const 
     return 0;
 }
 
-// the argument checks fbgpu_groupby_sum and its node form make before any device is touched (n_rows is checked after it)
-static int groupby_sum_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+// the argument checks fbgpu_groupby_sum and fbgpu_groupby_distinct (and the node form of Sum) make before any device is touched
+// (n_rows is checked after it): agg_array is out_sums of Sum, x_values of Count(Distinct), the aggregate field's depth is named
+// depth_name in the message.  Count(Distinct) checks its x_values next
+static int groupby_agg_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
                             const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews,
-                            const int32_t* bit_depths, int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, int32_t a_depth,
-                            const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts,
-                            const int64_t* out_sums) {
-    if (!out_sums) return fail(FBGPU_E_INVALID, "bad argument");
+                            const int32_t* bit_depths, int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, const void* agg_array,
+                            const char* depth_name, int32_t depth, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards,
+                            int64_t n_shards, const uint64_t* out_counts) {
+    if (!agg_array) return fail(FBGPU_E_INVALID, "bad argument");
     int rc = groupby_mixed_args(handle, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat,
                                 n_values, filter, n_filter_ops, shards, n_shards, out_counts, 0, 8);
     if (rc) return rc;
     if (n_fields + n_ints < 1) return fail(FBGPU_E_INVALID, "no dimension: n_fields + n_ints = 0");
-    if (a_depth < 0 || a_depth > 64) return fail(FBGPU_E_INVALID, "a_depth=%d outside 0..64", a_depth);
-    return 0;
-}
-
-// the argument checks fbgpu_groupby_distinct makes before any device is touched (n_rows is checked after it)
-static int groupby_distinct_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
-                                 const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews,
-                                 const int32_t* bit_depths, int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, int32_t x_depth,
-                                 const int64_t* x_values, int32_t n_x, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards,
-                                 int64_t n_shards, const uint64_t* out_distinct) {
-    if (!x_values) return fail(FBGPU_E_INVALID, "bad argument");
-    int rc = groupby_mixed_args(handle, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat,
-                                n_values, filter, n_filter_ops, shards, n_shards, out_distinct, 0, 8);
-    if (rc) return rc;
-    if (n_fields + n_ints < 1) return fail(FBGPU_E_INVALID, "no dimension: n_fields + n_ints = 0");
-    if (x_depth < 0 || x_depth > 64) return fail(FBGPU_E_INVALID, "x_depth=%d outside 0..64", x_depth);
-    if (n_x < 1) return fail(FBGPU_E_INVALID, "n_x=%d < 1", n_x);
-    for (int32_t i = 1; i < n_x; i++)
-        if (x_values[i] <= x_values[i - 1]) return fail(FBGPU_E_INVALID, "x_values are not strictly ascending at position %d", i);
+    if (depth < 0 || depth > 64) return fail(FBGPU_E_INVALID, "%s=%d outside 0..64", depth_name, depth);
     return 0;
 }
 
@@ -2036,48 +1965,122 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
     return 0;
 }
 
-// set dimensions before the last are peeled into the filter as groupby_rec does (a multi-view one as the union of its row over
-// the views); the last one (if any) is the kernel's b
-static int groupby_values_rec(fbgpu_ctx* c, uint32_t index, const GbDim* d, int nf, const std::vector<GvInt>& v, const GvInt* x,
-                              const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards, uint64_t* out, uint64_t* out_sums) {
-    if (nf <= 1) return groupby_values_leaf(c, index, nf ? d : nullptr, v, x, filter, shards, n_shards, out, out_sums);
-    size_t sub = 1; for (const GvInt& f : v) sub *= (size_t)f.n_values;
+// ------------------------------------------------------------------ one GroupBy request: every GroupBy entry point
+// The tensor's axes are the set dimensions, then the int dimensions.  Per cell: the number of columns of filter ∩ the cell's rows
+// (∩ exists(x) with an aggregate), and with agg kSum the sum of x's stored values behind it, or with kDistinct, in place of the
+// count, how many of x.values the cell holds
+struct GbRequest {
+    std::vector<GbDim> dims;
+    std::vector<GvInt> ints;
+    GvAgg agg; GvInt x;                                             // (x unused for kCount)
+    const fbgpu_op* filter; int32_t n_filter_ops;
+    const uint64_t* shards; int64_t n_shards;
+    int check_rows() const {
+        for (size_t i = 0; i < dims.size(); i++)
+            if (dims[i].n_rows < 0 || dims[i].n_rows > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", (int)i, dims[i].n_rows);
+        return 0;
+    }
+    size_t cells() const {
+        size_t n = 1;
+        for (const GbDim& d : dims) n *= (size_t)d.n_rows;
+        for (const GvInt& v : ints) n *= (size_t)v.n_values;
+        return n;
+    }
+    size_t out_len() const { return agg == GvAgg::kSum ? 2 * cells() : cells(); }     // Sum: [counts | sums]
+};
+
+// the set dimensions of the ABI's flat arrays: dimension i has n_views[i] views (one when n_views is null) and n_rows[i] rows
+static std::vector<GbDim> gb_set_dims(const uint32_t* fields, const uint32_t* views, const int32_t* n_views, int32_t n_fields,
+                                      const uint64_t* row_ids_flat, const int32_t* n_rows) {
+    std::vector<GbDim> dims((size_t)n_fields);
+    for (int i = 0; i < n_fields; i++) {
+        const int32_t nv = n_views ? n_views[i] : 1;
+        dims[(size_t)i] = GbDim{ fields[i], views, nv, row_ids_flat, n_rows[i] };
+        views += nv; row_ids_flat += n_rows[i];
+    }
+    return dims;
+}
+
+// the int dimensions of the ABI's flat arrays: dimension k has n_values[k] values
+static std::vector<GvInt> gb_int_dims(const uint32_t* vfields, const uint32_t* vviews, const int32_t* bit_depths, int32_t n_ints,
+                                      const int64_t* values_flat, const int32_t* n_values) {
+    std::vector<GvInt> ints((size_t)n_ints);
+    for (int k = 0; k < n_ints; k++) { ints[(size_t)k] = GvInt{ vfields[k], vviews[k], bit_depths[k], values_flat, n_values[k] }; values_flat += n_values[k]; }
+    return ints;
+}
+
+// Peel the leading set dimension on the host, folding Row(f0=r) — over several views, the union of those rows — into the filter
+// (groupByIterator keeps the same prefix intersections per level, executor.go:8829-8835,8861-8867), down to a leaf.  Counts over
+// set dimensions alone: the last dimension by the row-count kernels, two single-view last dimensions by groupby2.  Otherwise one
+// groupby_values_leaf pass once at most one set dimension (the kernel's b) is left
+static int groupby_rec(fbgpu_ctx* c, uint32_t index, const GbRequest& q, const GbDim* d, int nf, const std::vector<fbgpu_op>& filter,
+                       uint64_t* out, uint64_t* out_sums) {
+    if (q.ints.empty() && q.agg == GvAgg::kCount) {
+        if (nf == 1) {
+            std::vector<uint64_t> r(d[0].rows, d[0].rows + d[0].n_rows), counts;
+            int rc = row_counts_impl(c, index, view_slots(c, index, d[0].field, d[0].views, d[0].n_views), r, filter.empty() ? nullptr : filter.data(), (int)filter.size(),
+                                     q.shards, q.n_shards, counts); if (rc) return rc;
+            memcpy(out, counts.data(), counts.size() * 8);
+            return 0;
+        }
+        if (nf == 2 && d[0].n_views == 1 && d[1].n_views == 1) {
+            uint32_t fa = view_id_locked(c, ViewKey{ index, d[0].field, d[0].views[0] }, false), fb = view_id_locked(c, ViewKey{ index, d[1].field, d[1].views[0] }, false);
+            return groupby2(c, index, fa, d[0].rows, d[0].n_rows, fb, d[1].rows, d[1].n_rows, filter, q.shards, q.n_shards, out);
+        }
+    } else if (nf <= 1) {
+        return groupby_values_leaf(c, index, nf ? d : nullptr, q.ints, q.agg == GvAgg::kCount ? nullptr : &q.x, filter, q.shards, q.n_shards, out, out_sums);
+    }
+    size_t sub = 1; for (const GvInt& f : q.ints) sub *= (size_t)f.n_values;
     for (int i = 1; i < nf; i++) sub *= (size_t)d[i].n_rows;
     for (int r = 0; r < d[0].n_rows; r++) {
-        int rc = groupby_values_rec(c, index, d + 1, nf - 1, v, x, and_row(filter.data(), (int32_t)filter.size(), d[0].field, d[0].views, d[0].n_views, d[0].rows[r]),
-                                    shards, n_shards, out + (size_t)r * sub, out_sums ? out_sums + (size_t)r * sub : nullptr); if (rc) return rc;
+        int rc = groupby_rec(c, index, q, d + 1, nf - 1, and_row(filter.data(), (int32_t)filter.size(), d[0].field, d[0].views, d[0].n_views, d[0].rows[r]),
+                             out + (size_t)r * sub, out_sums ? out_sums + (size_t)r * sub : nullptr); if (rc) return rc;
     }
     return 0;
 }
 
-// fbgpu_groupby_values / fbgpu_groupby_mixed / fbgpu_groupby_sum / fbgpu_groupby_distinct once the arguments but n_rows are
-// checked: the set dimensions' rows are laid out from row_ids_flat, the outputs zeroed, the store locked
-static int groupby_values_query(fbgpu_ctx* c, uint32_t index, std::vector<GbDim>& dims, const uint64_t* row_ids_flat, const std::vector<GvInt>& v,
-                                const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts,
-                                const GvInt* x = nullptr, int64_t* out_sums = nullptr) {
+// a GroupBy entry point once its arguments but n_rows are checked: the store locked, the outputs zeroed, the peel.  (Its own
+// catch serves the node forms, which run it on their worker threads.)
+static int groupby_run(fbgpu_ctx* c, uint32_t index, const GbRequest& q, uint64_t* out_counts, int64_t* out_sums = nullptr) try {
     std::shared_lock<std::shared_mutex> lk;
     int rc = begin_query(c, lk); if (rc) return rc;
-    const uint64_t* p = row_ids_flat; size_t total = 1;
-    for (const GvInt& f : v) total *= (size_t)f.n_values;
-    for (size_t i = 0; i < dims.size(); i++) {
-        if (dims[i].n_rows < 0 || dims[i].n_rows > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", (int)i, dims[i].n_rows);
-        dims[i].rows = p; p += dims[i].n_rows; total *= (size_t)dims[i].n_rows;
-    }
-    memset(out_counts, 0, total * 8);
-    if (out_sums) memset(out_sums, 0, total * 8);
-    if (total == 0) return 0;
-    return groupby_values_rec(c, index, dims.data(), (int)dims.size(), v, x, std::vector<fbgpu_op>(filter, filter + n_filter_ops), shards, n_shards,
-                              out_counts, (uint64_t*)out_sums);
-}
+    rc = q.check_rows(); if (rc) return rc;
+    const size_t cells = q.cells();
+    memset(out_counts, 0, cells * 8);
+    if (out_sums) memset(out_sums, 0, cells * 8);
+    if (cells == 0) return 0;
+    // executor.go:8769-8772: the kernels treat a shard with a missing fragment as contributing nothing; for the row_counts
+    // leaf a missing fragment naturally yields zeros.  Peeled dimensions enter through the filter, which is empty on shards
+    // without that fragment.
+    return groupby_rec(c, index, q, q.dims.data(), (int)q.dims.size(), std::vector<fbgpu_op>(q.filter, q.filter + q.n_filter_ops), out_counts, (uint64_t*)out_sums);
+} FBGPU_CATCH
+
+extern "C" int fbgpu_groupby(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows,
+                             const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
+    int rc = groupby_args(c, fields, views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards, out_counts);
+    if (rc) return rc;
+    return groupby_run(c, index, GbRequest{ gb_set_dims(fields, views, nullptr, n_fields, row_ids_flat, n_rows), {}, GvAgg::kCount, {},
+                                            filter, n_filter_ops, shards, n_shards }, out_counts);
+} FBGPU_CATCH
+
+// GroupBy(Rows(f1, from=, to=), ...): fbgpu_groupby with dimension i's rows taken as their unions over n_views[i] views
+// (timeFragmentsRowIterator, executor.go:8755-8768)
+extern "C" int fbgpu_groupby_views(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                   const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
+                                   const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
+    int rc = groupby_views_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards, out_counts);
+    if (rc) return rc;
+    return groupby_run(c, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows), {}, GvAgg::kCount, {},
+                                            filter, n_filter_ops, shards, n_shards }, out_counts);
+} FBGPU_CATCH
 
 extern "C" int fbgpu_groupby_values(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
                                     const int32_t* n_rows, uint32_t vfield, uint32_t vview, int32_t bit_depth, const int64_t* values, int32_t n_values,
                                     const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     int rc = groupby_values_args(c, fields, views, n_fields, row_ids_flat, n_rows, bit_depth, values, n_values, filter, n_filter_ops, shards, n_shards, out_counts);
     if (rc) return rc;
-    std::vector<GbDim> dims((size_t)n_fields);
-    for (int i = 0; i < n_fields; i++) dims[(size_t)i] = GbDim{ fields[i], views + i, 1, nullptr, n_rows[i] };
-    return groupby_values_query(c, index, dims, row_ids_flat, { GvInt{ vfield, vview, bit_depth, values, n_values } }, filter, n_filter_ops, shards, n_shards, out_counts);
+    return groupby_run(c, index, GbRequest{ gb_set_dims(fields, views, nullptr, n_fields, row_ids_flat, n_rows), gb_int_dims(&vfield, &vview, &bit_depth, 1, values, &n_values),
+                                            GvAgg::kCount, {}, filter, n_filter_ops, shards, n_shards }, out_counts);
 } FBGPU_CATCH
 
 // GroupBy(Rows(f1), ..., Rows(v1), Rows(v2), ...) with set dimensions (each row a union over views, as fbgpu_groupby_views) and
@@ -2089,11 +2092,9 @@ extern "C" int fbgpu_groupby_mixed(fbgpu_ctx* c, uint32_t index, const uint32_t*
     int rc = groupby_mixed_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
                                 filter, n_filter_ops, shards, n_shards, out_counts);
     if (rc) return rc;
-    std::vector<GbDim> dims((size_t)n_fields); const uint32_t* vw = views_flat;
-    for (int i = 0; i < n_fields; i++) { dims[(size_t)i] = GbDim{ fields[i], vw, n_views[i], nullptr, n_rows[i] }; vw += n_views[i]; }
-    std::vector<GvInt> ints((size_t)n_ints); const int64_t* vals = values_flat;
-    for (int k = 0; k < n_ints; k++) { ints[(size_t)k] = GvInt{ vfields[k], vviews[k], bit_depths[k], vals, n_values[k] }; vals += n_values[k]; }
-    return groupby_values_query(c, index, dims, row_ids_flat, ints, filter, n_filter_ops, shards, n_shards, out_counts);
+    return groupby_run(c, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows),
+                                            gb_int_dims(vfields, vviews, bit_depths, n_ints, values_flat, n_values), GvAgg::kCount, {},
+                                            filter, n_filter_ops, shards, n_shards }, out_counts);
 } FBGPU_CATCH
 
 // GroupBy(..., aggregate=Sum(field=x)): fbgpu_groupby_mixed's dimensions (none of them int is fine) with, per cell, the number of
@@ -2102,15 +2103,12 @@ extern "C" int fbgpu_groupby_sum(fbgpu_ctx* c, uint32_t index, const uint32_t* f
                                  const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews, const int32_t* bit_depths,
                                  int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, uint32_t afield, uint32_t aview, int32_t a_depth,
                                  const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts, int64_t* out_sums) try {
-    int rc = groupby_sum_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values, a_depth,
-                              filter, n_filter_ops, shards, n_shards, out_counts, out_sums);
+    int rc = groupby_agg_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
+                              out_sums, "a_depth", a_depth, filter, n_filter_ops, shards, n_shards, out_counts);
     if (rc) return rc;
-    std::vector<GbDim> dims((size_t)n_fields); const uint32_t* vw = views_flat;
-    for (int i = 0; i < n_fields; i++) { dims[(size_t)i] = GbDim{ fields[i], vw, n_views[i], nullptr, n_rows[i] }; vw += n_views[i]; }
-    std::vector<GvInt> ints((size_t)n_ints); const int64_t* vals = values_flat;
-    for (int k = 0; k < n_ints; k++) { ints[(size_t)k] = GvInt{ vfields[k], vviews[k], bit_depths[k], vals, n_values[k] }; vals += n_values[k]; }
-    const GvInt x{ afield, aview, a_depth, nullptr, 0 };
-    return groupby_values_query(c, index, dims, row_ids_flat, ints, filter, n_filter_ops, shards, n_shards, out_counts, &x, out_sums);
+    return groupby_run(c, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows),
+                                            gb_int_dims(vfields, vviews, bit_depths, n_ints, values_flat, n_values), GvAgg::kSum, GvInt{ afield, aview, a_depth, nullptr, 0 },
+                                            filter, n_filter_ops, shards, n_shards }, out_counts, out_sums);
 } FBGPU_CATCH
 
 // GroupBy(..., aggregate=Count(Distinct(field=x))): fbgpu_groupby_sum's dimensions with, per cell, how many of x's listed stored
@@ -2121,16 +2119,16 @@ extern "C" int fbgpu_groupby_distinct(fbgpu_ctx* c, uint32_t index, const uint32
                                       int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, uint32_t xfield, uint32_t xview, int32_t x_depth,
                                       const int64_t* x_values, int32_t n_x, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
                                       uint64_t* out_distinct) try {
-    int rc = groupby_distinct_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
-                                   x_depth, x_values, n_x, filter, n_filter_ops, shards, n_shards, out_distinct);
+    int rc = groupby_agg_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
+                              x_values, "x_depth", x_depth, filter, n_filter_ops, shards, n_shards, out_distinct);
     if (rc) return rc;
+    if (n_x < 1) return fail(FBGPU_E_INVALID, "n_x=%d < 1", n_x);
+    for (int32_t i = 1; i < n_x; i++)
+        if (x_values[i] <= x_values[i - 1]) return fail(FBGPU_E_INVALID, "x_values are not strictly ascending at position %d", i);
     if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_groupby_distinct is local to one context: distinct sets of the ranks merge by union, not by sum");
-    std::vector<GbDim> dims((size_t)n_fields); const uint32_t* vw = views_flat;
-    for (int i = 0; i < n_fields; i++) { dims[(size_t)i] = GbDim{ fields[i], vw, n_views[i], nullptr, n_rows[i] }; vw += n_views[i]; }
-    std::vector<GvInt> ints((size_t)n_ints); const int64_t* vals = values_flat;
-    for (int k = 0; k < n_ints; k++) { ints[(size_t)k] = GvInt{ vfields[k], vviews[k], bit_depths[k], vals, n_values[k] }; vals += n_values[k]; }
-    const GvInt x{ xfield, xview, x_depth, x_values, n_x };
-    return groupby_values_query(c, index, dims, row_ids_flat, ints, filter, n_filter_ops, shards, n_shards, out_distinct, &x);
+    return groupby_run(c, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows),
+                                            gb_int_dims(vfields, vviews, bit_depths, n_ints, values_flat, n_values), GvAgg::kDistinct,
+                                            GvInt{ xfield, xview, x_depth, x_values, n_x }, filter, n_filter_ops, shards, n_shards }, out_distinct);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ comm

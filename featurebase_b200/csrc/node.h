@@ -226,24 +226,36 @@ extern "C" int fbgpu_node_row_counts_views(fbgpu_node* n, uint32_t index, uint32
     });
 } FBGPU_CATCH
 
+// a GroupBy node form once its arguments but n_rows are checked: n_rows checked before the fan-out, the request run on each device
+// over its own shards, the tensors added up (mergeGroupCounts executor.go:3728; Sum's [counts | sums]: wrapping int64 sums add as u64)
+static int node_groupby(fbgpu_node* n, uint32_t index, const GbRequest& q, uint64_t* out_counts, int64_t* out_sums = nullptr) {
+    int rc = q.check_rows(); if (rc) return rc;
+    const size_t cells = q.cells();
+    std::vector<uint64_t> both(out_sums ? q.out_len() : 0);
+    rc = node_sum(n, q.shards, q.n_shards, q.out_len(), out_sums ? both.data() : out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {
+        GbRequest qd = q; qd.shards = s.data(); qd.n_shards = (int64_t)s.size();
+        return groupby_run(c, index, qd, part, out_sums ? (int64_t*)(part + cells) : nullptr);
+    });
+    if (rc || !out_sums) return rc;
+    memcpy(out_counts, both.data(), cells * 8);
+    memcpy(out_sums, both.data() + cells, cells * 8);
+    return FBGPU_OK;
+}
+
 extern "C" int fbgpu_node_groupby_views(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
                                         const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
                                         const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     int rc = groupby_views_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards, out_counts);
     if (rc) return rc;
-    size_t total = 1; for (int i = 0; i < n_fields; i++) total *= (size_t)n_rows[i];
-    return node_sum(n, shards, n_shards, total, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {     // mergeGroupCounts executor.go:3728
-        return fbgpu_groupby_views(c, index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, s.data(), (int64_t)s.size(), part);
-    });
+    return node_groupby(n, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows), {}, GvAgg::kCount, {},
+                                             filter, n_filter_ops, shards, n_shards }, out_counts);
 } FBGPU_CATCH
 
 extern "C" int fbgpu_node_groupby(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
                                   const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
-    if (!n || !fields || !views || !row_ids_flat || !n_rows || !out_counts || n_fields < 1 || n_fields > 8 || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
-    size_t total = 1; for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); total *= (size_t)n_rows[i]; }
-    return node_sum(n, shards, n_shards, total, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {     // mergeGroupCounts executor.go:3728
-        return fbgpu_groupby(c, index, fields, views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, s.data(), (int64_t)s.size(), part);
-    });
+    int rc = groupby_args(n, fields, views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards, out_counts); if (rc) return rc;
+    return node_groupby(n, index, GbRequest{ gb_set_dims(fields, views, nullptr, n_fields, row_ids_flat, n_rows), {}, GvAgg::kCount, {},
+                                             filter, n_filter_ops, shards, n_shards }, out_counts);
 } FBGPU_CATCH
 
 extern "C" int fbgpu_node_groupby_values(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
@@ -251,11 +263,8 @@ extern "C" int fbgpu_node_groupby_values(fbgpu_node* n, uint32_t index, const ui
                                          const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts) try {
     int rc = groupby_values_args(n, fields, views, n_fields, row_ids_flat, n_rows, bit_depth, values, n_values, filter, n_filter_ops, shards, n_shards, out_counts);
     if (rc) return rc;
-    size_t total = (size_t)n_values; for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); total *= (size_t)n_rows[i]; }
-    return node_sum(n, shards, n_shards, total, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {     // the per-device counts add up
-        return fbgpu_groupby_values(c, index, fields, views, n_fields, row_ids_flat, n_rows, vfield, vview, bit_depth, values, n_values, filter, n_filter_ops,
-                                    s.data(), (int64_t)s.size(), part);
-    });
+    return node_groupby(n, index, GbRequest{ gb_set_dims(fields, views, nullptr, n_fields, row_ids_flat, n_rows), gb_int_dims(&vfield, &vview, &bit_depth, 1, values, &n_values),
+                                             GvAgg::kCount, {}, filter, n_filter_ops, shards, n_shards }, out_counts);
 } FBGPU_CATCH
 
 extern "C" int fbgpu_node_groupby_mixed(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
@@ -265,32 +274,21 @@ extern "C" int fbgpu_node_groupby_mixed(fbgpu_node* n, uint32_t index, const uin
     int rc = groupby_mixed_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
                                 filter, n_filter_ops, shards, n_shards, out_counts);
     if (rc) return rc;
-    size_t total = 1; for (int k = 0; k < n_ints; k++) total *= (size_t)n_values[k];
-    for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); total *= (size_t)n_rows[i]; }
-    return node_sum(n, shards, n_shards, total, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {     // the per-device counts add up
-        return fbgpu_groupby_mixed(c, index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
-                                   filter, n_filter_ops, s.data(), (int64_t)s.size(), part);
-    });
+    return node_groupby(n, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows),
+                                             gb_int_dims(vfields, vviews, bit_depths, n_ints, values_flat, n_values), GvAgg::kCount, {},
+                                             filter, n_filter_ops, shards, n_shards }, out_counts);
 } FBGPU_CATCH
 
 extern "C" int fbgpu_node_groupby_sum(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
                                       const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews, const int32_t* bit_depths,
                                       int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, uint32_t afield, uint32_t aview, int32_t a_depth,
                                       const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t* out_counts, int64_t* out_sums) try {
-    int rc = groupby_sum_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values, a_depth,
-                              filter, n_filter_ops, shards, n_shards, out_counts, out_sums);
+    int rc = groupby_agg_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
+                              out_sums, "a_depth", a_depth, filter, n_filter_ops, shards, n_shards, out_counts);
     if (rc) return rc;
-    size_t total = 1; for (int k = 0; k < n_ints; k++) total *= (size_t)n_values[k];
-    for (int i = 0; i < n_fields; i++) { if (n_rows[i] < 0 || n_rows[i] > 65535) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d out of range", i, n_rows[i]); total *= (size_t)n_rows[i]; }
-    std::vector<uint64_t> both(2 * total);                                     // [counts | sums]: wrapping int64 sums add as u64
-    rc = node_sum(n, shards, n_shards, 2 * total, both.data(), [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {
-        return fbgpu_groupby_sum(c, index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
-                                 afield, aview, a_depth, filter, n_filter_ops, s.data(), (int64_t)s.size(), part, (int64_t*)(part + total));
-    });
-    if (rc) return rc;
-    memcpy(out_counts, both.data(), total * 8);
-    memcpy(out_sums, both.data() + total, total * 8);
-    return FBGPU_OK;
+    return node_groupby(n, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows),
+                                             gb_int_dims(vfields, vviews, bit_depths, n_ints, values_flat, n_values), GvAgg::kSum, GvInt{ afield, aview, a_depth, nullptr, 0 },
+                                             filter, n_filter_ops, shards, n_shards }, out_counts, out_sums);
 } FBGPU_CATCH
 
 // Sum / Min / Max of an int field: per-device partials merged as ValCount.Add / Smaller / Larger do (executor.go:8446-8560)

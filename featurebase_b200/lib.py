@@ -3,6 +3,7 @@ a call fails, an exception is raised."""
 import ctypes as C
 import os
 import threading
+import types
 
 import numpy as np
 
@@ -149,6 +150,28 @@ def ops_array(ops):
     for i, o in enumerate(ops):
         arr[i] = o
     return arr
+
+
+def _groupby_args(set_dims, int_dims, shards, filter_ops):
+    """the arguments of the fbgpu_groupby* calls: set_dims [(field, views, row ids)], int_dims [(field, BSI view, bit depth,
+    stored values)] -> their flat arrays (as addresses; the namespace keeps the arrays alive), counts, the filter program and
+    shards, and the result tensor's shape, set dimensions first"""
+    keep = []
+
+    def addr(parts, dtype, flat=False):
+        a = np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=dtype) for p in parts]) if flat and len(parts) else np.asarray(parts, dtype=dtype))
+        keep.append(a)
+        return a.ctypes.data
+    sh = _u64arr(shards)
+    keep.append(sh)
+    return types.SimpleNamespace(
+        keep=keep, shape=[len(d[2]) for d in set_dims] + [len(d[3]) for d in int_dims], n_fields=len(set_dims), n_ints=len(int_dims),
+        fields=addr([d[0] for d in set_dims], np.uint32), views=addr([d[1] for d in set_dims], np.uint32, True),
+        n_views=addr([len(d[1]) for d in set_dims], np.int32), rows=addr([d[2] for d in set_dims], np.uint64, True),
+        n_rows=addr([len(d[2]) for d in set_dims], np.int32), vfields=addr([d[0] for d in int_dims], np.uint32),
+        vviews=addr([d[1] for d in int_dims], np.uint32), depths=addr([int(d[2]) for d in int_dims], np.int32),
+        values=addr([d[3] for d in int_dims], np.int64, True), n_values=addr([len(d[3]) for d in int_dims], np.int32),
+        filter=ops_array(filter_ops) if filter_ops else None, n_filter=len(filter_ops) if filter_ops else 0, shards=sh.ctypes.data, n_shards=len(sh))
 
 
 class Context:
@@ -437,128 +460,64 @@ class Context:
         return out
 
     def groupby(self, index, fields, views, row_ids, shards, filter_ops=None):
-        sh = _u64arr(shards)
-        fl = np.ascontiguousarray(np.asarray(fields, dtype=np.uint32))
-        vw = np.ascontiguousarray(np.asarray(views, dtype=np.uint32))
-        n_rows = np.ascontiguousarray(np.asarray([len(r) for r in row_ids], dtype=np.int32))
-        flat = _u64arr(np.concatenate([np.asarray(r, dtype=np.uint64) for r in row_ids]))
-        out = np.zeros(int(np.prod(n_rows.astype(np.int64))), dtype=np.uint64)
-        f = ops_array(filter_ops) if filter_ops else None
-        nf = len(filter_ops) if filter_ops else 0
-        self._check(self.L.fbgpu_groupby(self.h, index, fl.ctypes.data, vw.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
-                                         f, nf, sh.ctypes.data, len(sh), out.ctypes.data))
-        return out.reshape([int(x) for x in n_rows])
+        g = _groupby_args([(f, [v], r) for f, v, r in zip(fields, views, row_ids)], [], shards, filter_ops)
+        out = np.zeros(g.shape, dtype=np.uint64)
+        self._check(self.L.fbgpu_groupby(self.h, index, g.fields, g.views, g.n_fields, g.rows, g.n_rows, g.filter, g.n_filter, g.shards, g.n_shards, out.ctypes.data))
+        return out
 
     def groupby_views(self, index, fields, views, row_ids, shards, filter_ops=None):
         """groupby with dimension i's rows taken as their unions over the views listed in views[i] (fbgpu_groupby_views:
         GroupBy over Rows(f, from=, to=) children)"""
-        sh = _u64arr(shards)
-        fl = np.ascontiguousarray(np.asarray(fields, dtype=np.uint32))
-        vw = np.ascontiguousarray(np.concatenate([np.asarray(v, dtype=np.uint32) for v in views]))
-        n_views = np.ascontiguousarray(np.asarray([len(v) for v in views], dtype=np.int32))
-        n_rows = np.ascontiguousarray(np.asarray([len(r) for r in row_ids], dtype=np.int32))
-        flat = _u64arr(np.concatenate([np.asarray(r, dtype=np.uint64) for r in row_ids]))
-        out = np.zeros(int(np.prod(n_rows.astype(np.int64))), dtype=np.uint64)
-        f = ops_array(filter_ops) if filter_ops else None
-        nf = len(filter_ops) if filter_ops else 0
-        self._check(self.L.fbgpu_groupby_views(self.h, index, fl.ctypes.data, vw.ctypes.data, n_views.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
-                                               f, nf, sh.ctypes.data, len(sh), out.ctypes.data))
-        return out.reshape([int(x) for x in n_rows])
+        g = _groupby_args(list(zip(fields, views, row_ids)), [], shards, filter_ops)
+        out = np.zeros(g.shape, dtype=np.uint64)
+        self._check(self.L.fbgpu_groupby_views(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, g.filter, g.n_filter,
+                                               g.shards, g.n_shards, out.ctypes.data))
+        return out
 
     def groupby_values(self, index, fields, views, row_ids, vfield, vview, bit_depth, values, shards, filter_ops=None):
         """GroupBy whose last dimension is the values of an int field (fbgpu_groupby_values): the count tensor
         [len(row_ids[0])] ... [len(values)] over the set fields' row lists (none is fine) and the int field's strictly ascending
         stored values (value - Base, 1..65535 of them)"""
-        sh = _u64arr(shards)
-        fl = np.ascontiguousarray(np.asarray(fields, dtype=np.uint32))
-        vw = np.ascontiguousarray(np.asarray(views, dtype=np.uint32))
-        n_rows = np.ascontiguousarray(np.asarray([len(r) for r in row_ids], dtype=np.int32))
-        flat = _u64arr(np.concatenate([np.asarray(r, dtype=np.uint64) for r in row_ids]) if len(row_ids) else [])
-        vals = np.ascontiguousarray(np.asarray(values, dtype=np.int64))
-        shape = [int(x) for x in n_rows] + [len(vals)]
-        out = np.zeros(int(np.prod(shape, dtype=np.int64)), dtype=np.uint64)
-        f = ops_array(filter_ops) if filter_ops else None
-        nf = len(filter_ops) if filter_ops else 0
-        self._check(self.L.fbgpu_groupby_values(self.h, index, fl.ctypes.data, vw.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
-                                                vfield, vview, int(bit_depth), vals.ctypes.data, len(vals), f, nf, sh.ctypes.data, len(sh), out.ctypes.data))
-        return out.reshape(shape)
+        g = _groupby_args([(f, [v], r) for f, v, r in zip(fields, views, row_ids)], [(vfield, vview, bit_depth, values)], shards, filter_ops)
+        out = np.zeros(g.shape, dtype=np.uint64)
+        self._check(self.L.fbgpu_groupby_values(self.h, index, g.fields, g.views, g.n_fields, g.rows, g.n_rows, vfield, vview, int(bit_depth), g.values, len(values),
+                                                g.filter, g.n_filter, g.shards, g.n_shards, out.ctypes.data))
+        return out
 
     def groupby_mixed(self, index, set_dims, int_dims, shards, filter_ops=None):
         """GroupBy over set and int dimensions in one call (fbgpu_groupby_mixed).  set_dims: [(field, views, row ids)], each row
         taken as its union over the views (none is fine); int_dims: [(field, BSI view, bit depth, strictly ascending stored
         values)], 1..8 of them, the product of their value counts at most 65535.  Returns the count tensor
         [len(rows_0)] ... [len(values_0)] ..., set dimensions first."""
-        sh = _u64arr(shards)
-        fl = np.ascontiguousarray(np.asarray([d[0] for d in set_dims], dtype=np.uint32))
-        vw = np.ascontiguousarray(np.asarray([v for d in set_dims for v in d[1]], dtype=np.uint32))
-        n_views = np.ascontiguousarray(np.asarray([len(d[1]) for d in set_dims], dtype=np.int32))
-        n_rows = np.ascontiguousarray(np.asarray([len(d[2]) for d in set_dims], dtype=np.int32))
-        flat = _u64arr([r for d in set_dims for r in d[2]])
-        vf = np.ascontiguousarray(np.asarray([d[0] for d in int_dims], dtype=np.uint32))
-        vv = np.ascontiguousarray(np.asarray([d[1] for d in int_dims], dtype=np.uint32))
-        depths = np.ascontiguousarray(np.asarray([int(d[2]) for d in int_dims], dtype=np.int32))
-        n_values = np.ascontiguousarray(np.asarray([len(d[3]) for d in int_dims], dtype=np.int32))
-        vals = np.ascontiguousarray(np.asarray([int(x) for d in int_dims for x in d[3]], dtype=np.int64))
-        shape = [int(x) for x in n_rows] + [int(x) for x in n_values]
-        out = np.zeros(int(np.prod(shape, dtype=np.int64)), dtype=np.uint64)
-        f = ops_array(filter_ops) if filter_ops else None
-        nf = len(filter_ops) if filter_ops else 0
-        self._check(self.L.fbgpu_groupby_mixed(self.h, index, fl.ctypes.data, vw.ctypes.data, n_views.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
-                                               vf.ctypes.data, vv.ctypes.data, depths.ctypes.data, len(vf), vals.ctypes.data, n_values.ctypes.data,
-                                               f, nf, sh.ctypes.data, len(sh), out.ctypes.data))
-        return out.reshape(shape)
+        g = _groupby_args(set_dims, int_dims, shards, filter_ops)
+        out = np.zeros(g.shape, dtype=np.uint64)
+        self._check(self.L.fbgpu_groupby_mixed(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, g.vfields, g.vviews, g.depths, g.n_ints,
+                                               g.values, g.n_values, g.filter, g.n_filter, g.shards, g.n_shards, out.ctypes.data))
+        return out
 
     def groupby_sum(self, index, set_dims, int_dims, agg, shards, filter_ops=None):
         """GroupBy(..., aggregate=Sum(field=x)) in one call (fbgpu_groupby_sum).  set_dims and int_dims as for groupby_mixed, but
         0..8 of each (at least one dimension in all); agg: (field, BSI view, bit depth) of x.  Returns (counts, sums), tensors of
         groupby_mixed's shape: per cell the number of columns holding a value of x and the wrapping int64 sum of their stored
         values (value - Base)."""
-        sh = _u64arr(shards)
-        fl = np.ascontiguousarray(np.asarray([d[0] for d in set_dims], dtype=np.uint32))
-        vw = np.ascontiguousarray(np.asarray([v for d in set_dims for v in d[1]], dtype=np.uint32))
-        n_views = np.ascontiguousarray(np.asarray([len(d[1]) for d in set_dims], dtype=np.int32))
-        n_rows = np.ascontiguousarray(np.asarray([len(d[2]) for d in set_dims], dtype=np.int32))
-        flat = _u64arr([r for d in set_dims for r in d[2]])
-        vf = np.ascontiguousarray(np.asarray([d[0] for d in int_dims], dtype=np.uint32))
-        vv = np.ascontiguousarray(np.asarray([d[1] for d in int_dims], dtype=np.uint32))
-        depths = np.ascontiguousarray(np.asarray([int(d[2]) for d in int_dims], dtype=np.int32))
-        n_values = np.ascontiguousarray(np.asarray([len(d[3]) for d in int_dims], dtype=np.int32))
-        vals = np.ascontiguousarray(np.asarray([int(x) for d in int_dims for x in d[3]], dtype=np.int64))
-        shape = [int(x) for x in n_rows] + [int(x) for x in n_values]
-        counts = np.zeros(int(np.prod(shape, dtype=np.int64)), dtype=np.uint64)
-        sums = np.zeros(counts.size, dtype=np.int64)
-        f = ops_array(filter_ops) if filter_ops else None
-        nf = len(filter_ops) if filter_ops else 0
-        self._check(self.L.fbgpu_groupby_sum(self.h, index, fl.ctypes.data, vw.ctypes.data, n_views.ctypes.data, len(fl), flat.ctypes.data, n_rows.ctypes.data,
-                                             vf.ctypes.data, vv.ctypes.data, depths.ctypes.data, len(vf), vals.ctypes.data, n_values.ctypes.data,
-                                             int(agg[0]), int(agg[1]), int(agg[2]), f, nf, sh.ctypes.data, len(sh), counts.ctypes.data, sums.ctypes.data))
-        return counts.reshape(shape), sums.reshape(shape)
+        g = _groupby_args(set_dims, int_dims, shards, filter_ops)
+        counts, sums = np.zeros(g.shape, dtype=np.uint64), np.zeros(g.shape, dtype=np.int64)
+        self._check(self.L.fbgpu_groupby_sum(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, g.vfields, g.vviews, g.depths, g.n_ints,
+                                             g.values, g.n_values, int(agg[0]), int(agg[1]), int(agg[2]), g.filter, g.n_filter, g.shards, g.n_shards,
+                                             counts.ctypes.data, sums.ctypes.data))
+        return counts, sums
 
     def groupby_distinct(self, index, set_dims, int_dims, x, shards, filter_ops=None):
         """GroupBy(..., aggregate=Count(Distinct(field=x))) in one call (fbgpu_groupby_distinct).  set_dims and int_dims as for
         groupby_sum; x: (field, BSI view, bit depth, ascending stored values).  Returns a uint64 tensor of groupby_mixed's shape:
         per cell the number of x's listed values that some column of filter ∩ the cell's rows holds."""
-        sh = _u64arr(shards)
-        fl = np.ascontiguousarray(np.asarray([d[0] for d in set_dims], dtype=np.uint32))
-        vw = np.ascontiguousarray(np.asarray([v for d in set_dims for v in d[1]], dtype=np.uint32))
-        n_views = np.ascontiguousarray(np.asarray([len(d[1]) for d in set_dims], dtype=np.int32))
-        n_rows = np.ascontiguousarray(np.asarray([len(d[2]) for d in set_dims], dtype=np.int32))
-        flat = _u64arr([r for d in set_dims for r in d[2]])
-        vf = np.ascontiguousarray(np.asarray([d[0] for d in int_dims], dtype=np.uint32))
-        vv = np.ascontiguousarray(np.asarray([d[1] for d in int_dims], dtype=np.uint32))
-        depths = np.ascontiguousarray(np.asarray([int(d[2]) for d in int_dims], dtype=np.int32))
-        n_values = np.ascontiguousarray(np.asarray([len(d[3]) for d in int_dims], dtype=np.int32))
-        vals = np.ascontiguousarray(np.asarray([int(v) for d in int_dims for v in d[3]], dtype=np.int64))
+        g = _groupby_args(set_dims, int_dims, shards, filter_ops)
         xv = np.ascontiguousarray(np.asarray(x[3], dtype=np.int64))
-        shape = [int(v) for v in n_rows] + [int(v) for v in n_values]
-        out = np.zeros(int(np.prod(shape, dtype=np.int64)), dtype=np.uint64)
-        f = ops_array(filter_ops) if filter_ops else None
-        nf = len(filter_ops) if filter_ops else 0
-        self._check(self.L.fbgpu_groupby_distinct(self.h, index, fl.ctypes.data, vw.ctypes.data, n_views.ctypes.data, len(fl), flat.ctypes.data,
-                                                  n_rows.ctypes.data, vf.ctypes.data, vv.ctypes.data, depths.ctypes.data, len(vf), vals.ctypes.data,
-                                                  n_values.ctypes.data, int(x[0]), int(x[1]), int(x[2]), xv.ctypes.data, len(xv), f, nf,
-                                                  sh.ctypes.data, len(sh), out.ctypes.data))
-        return out.reshape(shape)
+        out = np.zeros(g.shape, dtype=np.uint64)
+        self._check(self.L.fbgpu_groupby_distinct(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, g.vfields, g.vviews, g.depths,
+                                                  g.n_ints, g.values, g.n_values, int(x[0]), int(x[1]), int(x[2]), xv.ctypes.data, len(xv), g.filter, g.n_filter,
+                                                  g.shards, g.n_shards, out.ctypes.data))
+        return out
 
     def rows_payload_bytes(self, index, field, view, shards, row_ids=None):
         sh = _u64arr(shards)

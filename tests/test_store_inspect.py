@@ -171,10 +171,16 @@ def test_query_argument_errors_without_a_device():
         ("groupby 0 fields", lib.fbgpu_groupby, (h, 0, fields.ctypes.data, views.ctypes.data, 0, rows.ctypes.data, nrow.ctypes.data, None, 0, p, 1, out.ctypes.data), "bad argument"),
         ("groupby 9 fields", lib.fbgpu_groupby, (h, 0, fields.ctypes.data, views.ctypes.data, 9, rows.ctypes.data, nrow.ctypes.data, None, 0, p, 1, out.ctypes.data), "bad argument"),
         ("groupby n_shards<0", lib.fbgpu_groupby, (h, 0, fields.ctypes.data, views.ctypes.data, 2, rows.ctypes.data, nrow.ctypes.data, None, 0, p, -1, out.ctypes.data), "bad argument"),
+        ("groupby n_filter_ops<0", lib.fbgpu_groupby, (h, 0, fields.ctypes.data, views.ctypes.data, 2, rows.ctypes.data, nrow.ctypes.data, op, -1, p, 1, out.ctypes.data), "bad argument"),
+        ("groupby null filter", lib.fbgpu_groupby, (h, 0, fields.ctypes.data, views.ctypes.data, 2, rows.ctypes.data, nrow.ctypes.data, None, 1, p, 1, out.ctypes.data), "bad argument"),
         # (the context form checks n_rows after the device check; the node form checks it before fanning out)
         ("node groupby n_rows 65536", lib.fbgpu_node_groupby, (node.h, 0, fields.ctypes.data, views.ctypes.data, 1, rows.ctypes.data, big.ctypes.data, None, 0, p, 1, out.ctypes.data),
          "n_rows[0]=65536 out of range"),
         ("node groupby 9 fields", lib.fbgpu_node_groupby, (node.h, 0, fields.ctypes.data, views.ctypes.data, 9, rows.ctypes.data, nrow.ctypes.data, None, 0, p, 1, out.ctypes.data), "bad argument"),
+        ("node groupby n_filter_ops<0", lib.fbgpu_node_groupby, (node.h, 0, fields.ctypes.data, views.ctypes.data, 2, rows.ctypes.data, nrow.ctypes.data, op, -1, p, 1, out.ctypes.data),
+         "bad argument"),
+        ("node groupby null filter", lib.fbgpu_node_groupby, (node.h, 0, fields.ctypes.data, views.ctypes.data, 2, rows.ctypes.data, nrow.ctypes.data, None, 1, p, 1, out.ctypes.data),
+         "bad argument"),
         ("node pairs n_pairs<0", lib.fbgpu_node_count_pairs, (node.h, 0, 1, 0, rows.ctypes.data, 1, 0, rows.ctypes.data, -1, p, 1, out.ctypes.data), null),
         ("node row_counts null ids", lib.fbgpu_node_row_counts, (node.h, 0, 1, 0, None, 2, None, 0, p, 1, out.ctypes.data), null),
     ]

@@ -1472,6 +1472,7 @@ def test_launch_and_query_counts(monkeypatch):
     shards = [0, 1, 2]
     for s in shards:
         ctx.load_fragment(0, 1, 0, s, D.fragment(1, s, [0, 1, 2, 3], 0.002))
+        ctx.load_fragment(0, 1, 1, s, D.fragment(4, s, [0, 1, 2, 3], 0.002))          # a second (time) view of field 1
         ctx.load_fragment(0, 3, 0, s, D.fragment(3, s, [0, 1], 0.02))
         ctx.load_fragment(0, 2, 0, s, D.fragment(2, s, list(range(10)), 0.002))      # an int field of depth 8: exists, sign, 8 planes
     ctx.commit()
@@ -1499,15 +1500,23 @@ def test_launch_and_query_counts(monkeypatch):
         "count_pairs": lambda: ctx.count_pairs(0, 1, 0, [0, 1], 3, 0, [0, 1], shards),
         "groupby2": lambda: ctx.groupby(0, [1, 3], [0, 0], [[0, 1, 2], [0, 1]], shards),
         "groupby3": lambda: ctx.groupby(0, [1, 3, 1], [0, 0, 0], [[0, 1], [0, 1], [2, 3]], shards),
+        "groupby_views": lambda: ctx.groupby_views(0, [1, 3], [[0, 1], [0]], [[0, 1, 2], [0, 1]], shards),
+        "groupby_values": lambda: ctx.groupby_values(0, [1], [0], [[0, 1]], 2, 0, 8, [1, 5, 9], shards),
+        "groupby_mixed": lambda: ctx.groupby_mixed(0, [(1, [0], [0, 1]), (3, [0], [0, 1])], [(2, 0, 8, [1, 5, 9])], shards),
+        "groupby_sum": lambda: ctx.groupby_sum(0, [(1, [0], [0, 1])], [], (2, 0, 8), shards, filter_ops=filt),
+        "groupby_distinct": lambda: ctx.groupby_distinct(0, [(3, [0], [0, 1])], [], (2, 0, 8, [1, 5, 9]), shards),
     }
     got = {name: delta(call) for name, call in calls.items()}
     # row / columns: eval + emit per batch; extract: + the value gather; bsi_sum / bsi_minmax: eval + plane kernel per batch;
     # bsi_select: eval per batch + (step, decide) per 4-bit digit of the 9-bit key; filtered row_counts: eval + count per batch;
     # GroupBy: groupby_direct_kernel + groupby_kernel for the units it declines (field 3's containers are too large for it),
-    # behind a filter eval per batch for 3 fields, which run one 2-field pass per row of the first field
+    # behind a filter eval per batch for 3 fields, which run one 2-field pass per row of the first field; a multi-view first
+    # dimension is peeled too, one filtered row count per row.  Int dimensions or an aggregate: eval + groupby_values_kernel per
+    # batch, one query per row of every set dimension but the last; Count(Distinct) adds the popcount
     assert got == {"count": (1, 1), "count_eval": (1, 1), "any": (1, 1), "row": (6, 1), "columns": (6, 1), "extract": (9, 1),
                    "bsi_sum": (6, 1), "bsi_minmax": (6, 1), "bsi_select": (9, 1), "row_counts": (6, 1), "count_pairs": (1, 1),
-                   "groupby2": (2, 1), "groupby3": (18, 2)}, got
+                   "groupby2": (2, 1), "groupby3": (18, 2), "groupby_views": (18, 3), "groupby_values": (6, 1), "groupby_mixed": (12, 2),
+                   "groupby_sum": (6, 1), "groupby_distinct": (7, 1)}, got
     # a load that is not committed yet: an empty request is answered without committing it
     ctx.load_fragment(0, 1, 0, 5, D.fragment(1, 5, [0], 0.002))
     commits = lambda: ctx.stats()["full_commits"] + ctx.stats()["patch_commits"]
