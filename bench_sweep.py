@@ -18,6 +18,8 @@
             Sum-per-group composition (only when named in --configs).
   config D: GroupBy(Rows(a), aggregate=Count(Distinct(field=v))), the same with Rows(w) or Rows(b) beside a, on config S's data,
             fbgpu_groupby_distinct against the Distinct-per-group composition (only when named in --configs).
+  config N: TopN(f, Row(src=0), tanimotoThreshold=50) and TopN(f, Row(src=0), threshold=100) over --topn-rows rows of varied
+            cardinality, fbgpu_topn_cutoffs against the per-shard count-matrix composition (only when named in --configs).
 Every point is spot-checked against the CPU oracle on a few shards (the checker, not the thing measured)."""
 import argparse
 import json
@@ -766,6 +768,92 @@ def config_groupby_distinct(args, out):
     real.close()
 
 
+class _NoTopnCutoffs(_KernelMs):
+    """the same proxy without topn_cutoffs: the executor fetches per-shard count matrices and applies the cut-offs on the host"""
+
+    def __getattr__(self, name):
+        if name == "topn_cutoffs":
+            raise AttributeError(name)
+        return super().__getattr__(name)
+
+
+def config_topn_cutoffs(args, out):
+    """TopN(f, Row(src=0), tanimotoThreshold=50) and TopN(f, Row(src=0), threshold=100) through the executor.  f is a set field of
+    --topn-rows rows in each of --topn-shards shards; Src (row 0 of src) holds 400 random columns of slot 0 per shard.  Half of
+    f's rows take each of Src's columns with a probability drawn per row from 0.5..1 plus up to 40 other columns, so their
+    Tanimoto coefficient straddles 50; the other half hold 1..300 random columns.  The device arm (fbgpu_topn_cutoffs) runs over
+    all shards; the composition arm (fbgpu_count per shard, two fbgpu_row_counts_per_shard matrices, the cut-offs in a Python
+    loop over (shard, row)) over the first --composition-shards shards, for --composition-steps steps alternated with the device
+    arm over the same shards.  Both arms must return the same pairs, and between 5 % and 95 % of the rows must survive each
+    cut-off, so that neither rule is trivially all-pass or all-fail.  Progress goes to stderr."""
+    from featurebase_b200 import executor as X, roaring_io
+    S, R, n_src = args.topn_shards, args.topn_rows, 400
+    h = X.Holder()
+    idx = h.create_index("i", track_existence=False)
+    idx.create_field("f")
+    idx.create_field("src")
+    t0 = time.perf_counter()
+    rng = np.random.default_rng(2026)
+    for s in range(S):
+        src = np.sort(rng.choice(1 << 16, n_src, replace=False)).astype(np.uint64)
+        h.import_roaring("i", "src", X.VIEW_STANDARD, s, roaring_io.encode(src))
+        half = R // 2
+        take = rng.random((half, n_src)) < rng.uniform(0.5, 1.0, size=(half, 1))
+        rr, cc = np.nonzero(take)
+        n_extra = rng.integers(0, 41, size=half)
+        er = np.repeat(np.arange(half), n_extra)
+        n_rand = rng.integers(1, 301, size=R - half)
+        qr = half + np.repeat(np.arange(R - half), n_rand)
+        rows = np.concatenate([rr, er, qr]).astype(np.uint64)
+        cols = np.concatenate([src[cc], rng.integers(0, 1 << 16, size=len(er) + len(qr)).astype(np.uint64)])
+        h.import_roaring("i", "f", X.VIEW_STANDARD, s, roaring_io.encode(rows * np.uint64(SW) + cols))
+        print(f"config N: shard {s} loaded, {time.perf_counter() - t0:.1f} s", file=sys.stderr, flush=True)
+    h.ctx.commit()
+    load_s = time.perf_counter() - t0
+    real = h.ctx
+    card = _card()
+    dev, comp = _KernelMs(real), _NoTopnCutoffs(real)
+    CS = min(S, args.composition_shards)
+    for q in ("TopN(f, Row(src=0), tanimotoThreshold=50)", "TopN(f, Row(src=0), threshold=100)"):
+        runs = [(S, {"device": dev})] + ([(CS, {"device": dev, "composition": comp})] if args.composition_steps > 0 else [])
+        for n_sh, arms in runs:
+            sh = list(range(n_sh))
+            rec = {name: {"wall": [], "kernel_ms": [], "queries": []} for name in arms}
+            res = {}
+            for i in range(1 + args.steps):                  # one warm-up round of the device arm, then alternate the arms
+                for name in (sorted(arms) if i % 2 == 0 else sorted(arms, reverse=True)):
+                    if name == "composition" and len(rec[name]["wall"]) >= args.composition_steps:
+                        continue
+                    h.ctx = arms[name]
+                    q0, arms[name].ms = real.counters()["queries"], 0.0
+                    t1 = time.perf_counter()
+                    r = X.Executor(h).execute("i", q, sh)[0]
+                    wall = (time.perf_counter() - t1) * 1e3
+                    res.setdefault(name, r)
+                    assert r == res[name], (q, name)
+                    print(f"config N: {q} over {n_sh} shards, {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                    if i >= 1 or name == "composition":
+                        rec[name]["wall"].append(wall)
+                        rec[name]["kernel_ms"].append(arms[name].ms)
+                        rec[name]["queries"].append(real.counters()["queries"] - q0)
+            h.ctx = real
+            assert all(r == res["device"] for r in res.values()), q
+            assert 0.05 * R < len(res["device"]) < 0.95 * R, (q, len(res["device"]), R)
+            for name, dd in rec.items():
+                o = {"config": "N", "query": q, "arm": name, "gpu": card, "shards": n_sh, "rows": R, "pairs": len(res[name]),
+                     "equal_to_composition": ("composition" in res) or None,
+                     "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])), "wall_ms_max": float(np.max(dd["wall"])),
+                     "kernel_ms": float(np.median(dd["kernel_ms"])), "queries": int(np.median(dd["queries"])), "steps": len(dd["wall"]), "load_s": round(load_s, 1),
+                     "kernel": ("eval_kernel + row_count_kernel<RcOut::kCutoff>" if name == "device"
+                                else "row_count_kernel (candidates), eval_kernel (Src counts), row_count_kernel<RcOut::kPerShard> x 2, host loop"),
+                     "note": "median over the timed steps of the executor call (wall clock), of the summed last_query_gpu_ms and of the "
+                             "number of its library queries"}
+                if name == "composition":
+                    o["wall_ms_per_step"] = [round(x, 2) for x in dd["wall"]]
+                out(o)
+    real.close()
+
+
 def config3(args, out, n_rec=10_000_000, nf=4):
     """nf fields are rotated between steps so that the touched planes exceed L2 (the 10 M-record config is 42.5 MB)"""
     from featurebase_b200 import datagen as D, executor as X, pql
@@ -860,8 +948,10 @@ def main():
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--shards", type=int, default=1024)
     ap.add_argument("--groupby-shards", type=int, default=512)
-    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D: steps of the composition arm")
-    ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S, D: shards of the composition arm and of the device arm timed beside it")
+    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D, N: steps of the composition arm")
+    ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S, D, N: shards of the composition arm and of the device arm timed beside it")
+    ap.add_argument("--topn-rows", type=int, default=1 << 14, help="config N: rows of the TopN field")
+    ap.add_argument("--topn-shards", type=int, default=16, help="config N: shards (the fragments are encoded in Python: ~5 s per shard)")
     ap.add_argument("--generators", default="uniform,clustered")
     ap.add_argument("--batched", action="store_true", help="also time the multi-pair launch (config 5b)")
     ap.add_argument("--densities", default="0.0001,0.001,0.01,0.03,0.0625,0.125,0.25,0.5")
@@ -888,6 +978,8 @@ def main():
             config_groupby_sum(args, out)
         elif c == "D":
             config_groupby_distinct(args, out)
+        elif c == "N":
+            config_topn_cutoffs(args, out)
         elif c == "3L":     # the same BSI query at 256 shards (268 M records, 1.1 GB of planes): shows the kernel away from the launch-bound regime
             config3(args, out, n_rec=256 * SW, nf=1)
         else:

@@ -233,8 +233,9 @@ extern "C" int fbgpu_init(int32_t device_ordinal, fbgpu_ctx** out) try {
     // opt in to large dynamic shared memory once
     CUDA_TRY(cudaFuncSetAttribute(eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 17 * 8192));
     CUDA_TRY(cudaFuncSetAttribute(pair_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPcWarps * 8192));
-    CUDA_TRY(cudaFuncSetAttribute(row_count_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
-    CUDA_TRY(cudaFuncSetAttribute(row_count_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
+    CUDA_TRY(cudaFuncSetAttribute(row_count_kernel<RcOut::kSummed>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
+    CUDA_TRY(cudaFuncSetAttribute(row_count_kernel<RcOut::kPerShard>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
+    CUDA_TRY(cudaFuncSetAttribute(row_count_kernel<RcOut::kCutoff>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
     CUDA_TRY(cudaFuncSetAttribute(row_count_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairWarps * 8192));
     CUDA_TRY(cudaFuncSetAttribute(groupby_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGbSlots * 4 + 8192));
     CUDA_TRY(cudaFuncSetAttribute(groupby_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGdSmemBytes));
@@ -1485,9 +1486,11 @@ extern "C" int fbgpu_bsi_select(fbgpu_ctx* c, uint32_t index, const fbgpu_op* op
 
 // ------------------------------------------------------------------ per-row counts (TopK / TopN ids)
 // fvs: the view slots each row is the union over.  One slot: row_count_kernel; several: row_count_views_kernel, whose counts
-// are always summed over the shards (per_shard needs one slot).
+// are always summed over the shards (per_shard and cut need one slot).  cut: TopN's per-shard cut-offs with `filter` as the Src
+// (row_count_kernel<kCutoff>, which gets the Src units' {N, runs} from the evaluation pass; cut->info is not read).
 static int row_counts_impl(fbgpu_ctx* c, uint32_t index, const std::vector<uint32_t>& fvs, const std::vector<uint64_t>& rows, const fbgpu_op* filter, int32_t n_filter_ops,
-                           const uint64_t* shards, int64_t n_shards, std::vector<uint64_t>& counts, bool reduce = true, bool per_shard = false) {
+                           const uint64_t* shards, int64_t n_shards, std::vector<uint64_t>& counts, bool reduce = true, bool per_shard = false,
+                           const RcCut* cut = nullptr) {
     counts.assign(rows.size() * (per_shard ? (size_t)n_shards : 1), 0);
     if (rows.empty()) return 0;
     const bool have_filter = filter && n_filter_ops > 0;
@@ -1504,7 +1507,7 @@ static int row_counts_impl(fbgpu_ctx* c, uint32_t index, const std::vector<uint3
     const int64_t batch = have_filter ? c->unit_batch / kSlotsPerRow : n_shards;
     for (int64_t s0 = 0; s0 < n_shards; s0 += batch) {
         int64_t ns = std::min(batch, n_shards - s0);
-        if (have_filter) { rc = q.eval(s0 * kSlotsPerRow, ns * kSlotsPerRow); if (rc) return rc; }
+        if (have_filter) { rc = q.eval(s0 * kSlotsPerRow, ns * kSlotsPerRow, cut != nullptr); if (rc) return rc; }
         long long tasks = (long long)ns * (long long)nr;
         long long grid = std::min<long long>((tasks + kPairWarps - 1) / kPairWarps, (long long)c->sm_count * 3);
         const uint32_t fv = fvs[0];
@@ -1512,11 +1515,15 @@ static int row_counts_impl(fbgpu_ctx* c, uint32_t index, const std::vector<uint3
             row_count_views_kernel<<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), d_fvs, (int)nv, (const uint64_t*)w->d_rows.p, (int)nr,
                 q.d_shards + s0, ns, have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p);
         else if (per_shard)
-            row_count_kernel<true><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, q.d_shards + s0, ns,
-                have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p + (size_t)s0 * nr);
+            row_count_kernel<RcOut::kPerShard><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, q.d_shards + s0, ns,
+                have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p + (size_t)s0 * nr, RcCut{});
+        else if (cut)
+            row_count_kernel<RcOut::kCutoff><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, q.d_shards + s0, ns,
+                have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p,
+                RcCut{ have_filter ? (const uint2*)w->d_info.p : nullptr, cut->min_threshold, cut->tanimoto });
         else
-            row_count_kernel<false><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, q.d_shards + s0, ns,
-                have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p);
+            row_count_kernel<RcOut::kSummed><<<(unsigned)grid, kPairWarps * 32, kPairWarps * 8192, w->stream>>>(store_ref(c), fv, (const uint64_t*)w->d_rows.p, (int)nr, q.d_shards + s0, ns,
+                have_filter ? (const uint4*)w->d_bitmaps.p : nullptr, (unsigned long long*)w->d_counts.p, RcCut{});
         CUDA_TRY(cudaGetLastError()); q.launches++;
     }
     CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
@@ -1530,11 +1537,13 @@ static int row_counts_impl(fbgpu_ctx* c, uint32_t index, const std::vector<uint3
     return 0;
 }
 
-// fbgpu_row_counts / fbgpu_row_counts_views once the store is locked: the rows are their unions over the view slots fvs
-static int row_counts_query(fbgpu_ctx* c, uint32_t index, const std::vector<uint32_t>& fvs, const uint64_t* row_ids, int32_t n_rows,
-                            const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
-                            uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n) {
-    std::vector<uint64_t> rows, counts;
+// The counts of fbgpu_row_counts / fbgpu_row_counts_views / fbgpu_topn_cutoffs once the store is locked, the rows being their
+// unions over the view slots fvs.  row_ids != NULL: rows = row_ids, counts[i] theirs, all-reduced.  row_ids == NULL: the rows of
+// the listed shards with a non-zero count and their counts, in no particular order, not all-reduced.
+static int row_counts_run(fbgpu_ctx* c, uint32_t index, const std::vector<uint32_t>& fvs, const uint64_t* row_ids, int32_t n_rows,
+                          const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
+                          std::vector<uint64_t>& rows, std::vector<uint64_t>& counts, const RcCut* cut = nullptr) {
+    rows.clear();
     if (row_ids) rows.assign(row_ids, row_ids + n_rows);
     else {
         // fragment.rows() (fragment.go:2465-2486): distinct row ids present in the listed shards (of any of the views)
@@ -1546,15 +1555,19 @@ static int row_counts_query(fbgpu_ctx* c, uint32_t index, const std::vector<uint
         }
         std::sort(rows.begin(), rows.end()); rows.erase(std::unique(rows.begin(), rows.end()), rows.end());
     }
-    int rc = row_counts_impl(c, index, fvs, rows, filter, n_filter_ops, shards, n_shards, counts, row_ids != nullptr); if (rc) return rc;
-    if (row_ids) {
-        if (cap < n_rows) return fail(FBGPU_E_NOSPACE, "cap %d < n_rows %d", cap, n_rows);
-        for (int32_t i = 0; i < n_rows; i++) { out_counts[i] = counts[i]; if (out_row_ids) out_row_ids[i] = rows[i]; }
-        if (out_n) *out_n = n_rows;
-        return FBGPU_OK;
+    int rc = row_counts_impl(c, index, fvs, rows, filter, n_filter_ops, shards, n_shards, counts, row_ids != nullptr, false, cut); if (rc) return rc;
+    if (!row_ids) {
+        size_t k = 0;
+        for (size_t i = 0; i < rows.size(); i++) if (counts[i]) { rows[k] = rows[i]; counts[k++] = counts[i]; }
+        rows.resize(k); counts.resize(k);
     }
-    std::vector<size_t> order;
-    for (size_t i = 0; i < rows.size(); i++) if (counts[i]) order.push_back(i);
+    return 0;
+}
+
+// the all-rows form's output: every (row, count) sorted by (count desc, row id asc), or none
+static int write_sorted_rows(const std::vector<uint64_t>& rows, const std::vector<uint64_t>& counts, uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n) {
+    std::vector<size_t> order(rows.size());
+    for (size_t i = 0; i < rows.size(); i++) order[i] = i;
     std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return counts[a] != counts[b] ? counts[a] > counts[b] : rows[a] < rows[b]; });
     // all rows with a non-zero count, or none: a silently truncated list would make Rows() / the TopN candidate set incomplete
     // (ADVICE r1).  *out_n always receives the number of rows there are, so the caller can size its buffers and call again.
@@ -1562,6 +1575,21 @@ static int row_counts_query(fbgpu_ctx* c, uint32_t index, const std::vector<uint
     if (order.size() > (size_t)std::max(cap, 0)) return fail(FBGPU_E_NOSPACE, "%zu rows have a non-zero count, cap is %d", order.size(), cap);
     for (size_t i = 0; i < order.size(); i++) { if (out_row_ids) out_row_ids[i] = rows[order[i]]; out_counts[i] = counts[order[i]]; }
     return FBGPU_OK;
+}
+
+// fbgpu_row_counts / fbgpu_row_counts_views / fbgpu_topn_cutoffs once the store is locked: row_counts_run, then the output form
+static int row_counts_query(fbgpu_ctx* c, uint32_t index, const std::vector<uint32_t>& fvs, const uint64_t* row_ids, int32_t n_rows,
+                            const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
+                            uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n, const RcCut* cut = nullptr) {
+    std::vector<uint64_t> rows, counts;
+    int rc = row_counts_run(c, index, fvs, row_ids, n_rows, filter, n_filter_ops, shards, n_shards, rows, counts, cut); if (rc) return rc;
+    if (row_ids) {
+        if (cap < n_rows) return fail(FBGPU_E_NOSPACE, "cap %d < n_rows %d", cap, n_rows);
+        for (int32_t i = 0; i < n_rows; i++) { out_counts[i] = counts[i]; if (out_row_ids) out_row_ids[i] = rows[i]; }
+        if (out_n) *out_n = n_rows;
+        return FBGPU_OK;
+    }
+    return write_sorted_rows(rows, counts, out_row_ids, out_counts, cap, out_n);
 }
 
 extern "C" int fbgpu_row_counts(fbgpu_ctx* c, uint32_t index, uint32_t field, uint32_t view, const uint64_t* row_ids, int32_t n_rows,
@@ -1624,6 +1652,28 @@ extern "C" int fbgpu_row_counts_per_shard(fbgpu_ctx* c, uint32_t index, uint32_t
         memcpy(out_counts + (size_t)s0 * n_rows, counts.data(), counts.size() * 8);
     }
     return FBGPU_OK;
+} FBGPU_CATCH
+
+// the argument checks fbgpu_topn_cutoffs and its node form make before any device is touched
+static int topn_cutoffs_args(const void* handle, int32_t n_rows, const fbgpu_op* src, int32_t n_src_ops, uint32_t tanimoto_threshold,
+                             const uint64_t* shards, int64_t n_shards, const uint64_t* out_counts) {
+    if (!handle || !out_counts || n_rows < 0 || n_src_ops < 0 || (n_src_ops && !src) || n_shards < 0 || (n_shards && !shards))
+        return fail(FBGPU_E_INVALID, "bad argument");
+    if (tanimoto_threshold > 100) return fail(FBGPU_E_INVALID, "tanimoto_threshold=%u > 100", tanimoto_threshold);
+    return 0;
+}
+
+// TopN(f, Src, threshold= / tanimotoThreshold=): fragment.top's per-shard cut-offs (fragment.go:1329-1388) and the sum over the
+// shards of what passes (executeTopNShards executor.go:2831-2866), in one pass over the shards
+extern "C" int fbgpu_topn_cutoffs(fbgpu_ctx* c, uint32_t index, uint32_t field, uint32_t view, const uint64_t* row_ids, int32_t n_rows,
+                                  const fbgpu_op* src, int32_t n_src_ops, uint64_t min_threshold, uint32_t tanimoto_threshold,
+                                  const uint64_t* shards, int64_t n_shards, uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n) try {
+    int rc = topn_cutoffs_args(c, n_rows, src, n_src_ops, tanimoto_threshold, shards, n_shards, out_counts); if (rc) return rc;
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    const std::vector<uint32_t> fvs{ view_id_locked(c, ViewKey{ index, field, view }, false) };
+    const RcCut cut{ nullptr, min_threshold, tanimoto_threshold };
+    return row_counts_query(c, index, fvs, row_ids, n_rows, src, n_src_ops, shards, n_shards, out_row_ids, out_counts, cap, out_n, &cut);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ many fused Intersect+Count pairs in one launch

@@ -954,14 +954,37 @@ __device__ __forceinline__ uint32_t warp_count_vs_global_bitmap(Resolved a, cons
     return __reduce_add_sync(0xffffffffu, c);
 }
 
-// kPerShard: out_counts is the [n_shards][n_rows] matrix of per-shard counts (what fragment.top's per-shard cut-offs need,
-// fragment.go:1329-1388) instead of the [n_rows] vector summed over the shards; every (shard, row) task then owns its slot.
-template <bool kPerShard>
+// What row_count_kernel writes.  kSummed: the [n_rows] vector of counts summed over the shards.  kPerShard: the
+// [n_shards][n_rows] matrix of per-shard counts; every (shard, row) task then owns its slot.  kCutoff: the [n_rows] vector of
+// the counts that pass fragment.top's per-shard cut-off (fragment.go:1329-1388) summed over the shards, which is what Pairs.Add
+// makes of the shards' answers (executeTopNShards executor.go:2831-2866).
+enum class RcOut { kSummed, kPerShard, kCutoff };
+
+// kCutoff's inputs.  info: the {N, runs} of the filter (Src) units the evaluation pass wrote, [n_shards*16], or null without a Src.
+struct RcCut { const uint2* info; unsigned long long min_threshold; uint32_t tanimoto; };
+
+// fragment.top's rule for one (shard, row) pair of a cache holding every row, without N-truncation: cnt = |row|, count =
+// |row ∩ Src| (cnt without a Src), src_count = |Src|; returns the count that is kept, or 0.  The products are uint64 and the
+// comparisons double, as in Go (IEEE round-to-nearest division: the library is built without fast math).
+__device__ __forceinline__ unsigned long long topn_cutoff(unsigned long long cnt, unsigned long long count, unsigned long long src_count,
+                                                          bool have_src, const RcCut& cut) {
+    if (cut.tanimoto > 0 && have_src) {
+        const unsigned long long t = cut.tanimoto;
+        if (cnt == 0 || (double)cnt <= (double)(src_count * t) / 100 || (double)cnt >= (double)(src_count * 100) / (double)t) return 0;
+        // Go's ceil(x) <= t, for the integer t: x <= t, the same comparison on the same double x
+        if (count == 0 || (double)(count * 100) / (double)(cnt + src_count - count) <= (double)t) return 0;
+        return count;
+    }
+    const unsigned long long m = cut.min_threshold > 0 ? cut.min_threshold : 1;
+    return cnt < m || count < m ? 0 : count;
+}
+
+template <RcOut kOut>
 __global__ void __launch_bounds__(kPairWarps * 32)
 row_count_kernel(StoreRef st, uint32_t fv, const uint64_t* __restrict__ row_ids, int n_rows,
                  const uint64_t* __restrict__ shards, long long n_shards,
                  const uint4* __restrict__ filter_bitmaps /* [n_shards*16][512] or null */,
-                 unsigned long long* out_counts /* [n_rows], or [n_shards][n_rows] */) {
+                 unsigned long long* out_counts /* [n_rows], or [n_shards][n_rows] */, RcCut cut) {
     extern __shared__ __align__(128) uint32_t smem32[];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     uint32_t* bm = smem32 + wid * 2048;
@@ -974,7 +997,7 @@ row_count_kernel(StoreRef st, uint32_t fv, const uint64_t* __restrict__ row_ids,
         Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
         if (lane < 16) r = resolve(st, fv, shard, row, lane);
         unsigned present = __ballot_sync(0xffffffffu, r.ptr != nullptr);
-        unsigned long long acc = 0;
+        unsigned long long acc = 0, cnt = 0;
         while (present) {
             int s = __ffs(present) - 1; present &= present - 1;
             Resolved a;
@@ -982,10 +1005,17 @@ row_count_kernel(StoreRef st, uint32_t fv, const uint64_t* __restrict__ row_ids,
             a.card = __shfl_sync(0xffffffffu, r.card, s);
             uint32_t meta = __shfl_sync(0xffffffffu, ((uint32_t)r.typ << 16) | r.cnt, s);
             a.typ = meta >> 16; a.cnt = meta & 0xffff;
+            if (kOut == RcOut::kCutoff) cnt += a.card;
             if (!filter_bitmaps) acc += a.card;
             else acc += warp_count_vs_global_bitmap(a, reinterpret_cast<const uint32_t*>(filter_bitmaps + ((size_t)si * 16 + s) * 512), bm, lane);
         }
-        if (lane == 0 && acc) { if (kPerShard) out_counts[(size_t)si * n_rows + ri] = acc; else atomicAdd(&out_counts[ri], acc); }
+        if (kOut == RcOut::kCutoff) {
+            if (cnt == 0) continue;                         // (warp-uniform) the row is absent from the shard: fragment.top never sees it
+            // |Src| in the shard: the sum of its 16 units' N, which the evaluation pass wrote beside the bitmaps
+            uint32_t sc = cut.info && lane < 16 ? cut.info[(size_t)si * 16 + lane].x : 0u;
+            sc = __reduce_add_sync(0xffffffffu, sc);
+            if (lane == 0) { const unsigned long long kept = topn_cutoff(cnt, acc, sc, cut.info != nullptr, cut); if (kept) atomicAdd(&out_counts[ri], kept); }
+        } else if (lane == 0 && acc) { if (kOut == RcOut::kPerShard) out_counts[(size_t)si * n_rows + ri] = acc; else atomicAdd(&out_counts[ri], acc); }
     }
 }
 

@@ -226,6 +226,49 @@ extern "C" int fbgpu_node_row_counts_views(fbgpu_node* n, uint32_t index, uint32
     });
 } FBGPU_CATCH
 
+// Explicit ids: the devices' vectors are summed.  All rows: each device's (row, total) list, merged by row id with the totals
+// summed, then sorted under fbgpu_row_counts' NOSPACE contract.  Both are exact: a shard lives on one device, and a row's total is
+// a sum over shards.
+extern "C" int fbgpu_node_topn_cutoffs(fbgpu_node* n, uint32_t index, uint32_t field, uint32_t view, const uint64_t* row_ids, int32_t n_rows,
+                                       const fbgpu_op* src, int32_t n_src_ops, uint64_t min_threshold, uint32_t tanimoto_threshold,
+                                       const uint64_t* shards, int64_t n_shards, uint64_t* out_row_ids, uint64_t* out_counts, int32_t cap, int32_t* out_n) try {
+    int rc = topn_cutoffs_args(n, n_rows, src, n_src_ops, tanimoto_threshold, shards, n_shards, out_counts); if (rc) return rc;
+    if (row_ids) {
+        rc = node_sum(n, shards, n_shards, (size_t)n_rows, out_counts, [&](fbgpu_ctx* c, const std::vector<uint64_t>& s, uint64_t* part) {
+            int32_t got = 0;
+            return fbgpu_topn_cutoffs(c, index, field, view, row_ids, n_rows, src, n_src_ops, min_threshold, tanimoto_threshold, s.data(), (int64_t)s.size(),
+                                      nullptr, part, n_rows, &got);
+        });
+        if (rc) return rc;
+        if (cap < n_rows) return fail(FBGPU_E_NOSPACE, "cap %d < n_rows %d", cap, n_rows);
+        if (out_row_ids) memcpy(out_row_ids, row_ids, (size_t)n_rows * 8);
+        if (out_n) *out_n = n_rows;
+        return FBGPU_OK;
+    }
+    const NodeSplit sp = node_split(n, shards, n_shards);
+    const std::vector<int> devs = node_owners(sp);
+    std::vector<std::vector<uint64_t>> rows(n->ctx.size()), totals(n->ctx.size());
+    rc = node_fan_out(n, devs, [&](int d) {
+        fbgpu_ctx* c = n->ctx[(size_t)d];
+        const auto& s = sp.shards[(size_t)d];
+        std::shared_lock<std::shared_mutex> lk;
+        int r = begin_query(c, lk); if (r) return r;
+        const std::vector<uint32_t> fvs{ view_id_locked(c, ViewKey{ index, field, view }, false) };
+        const RcCut cut{ nullptr, min_threshold, tanimoto_threshold };
+        return row_counts_run(c, index, fvs, nullptr, 0, src, n_src_ops, s.data(), (int64_t)s.size(), rows[(size_t)d], totals[(size_t)d], &cut);
+    });
+    if (rc) return rc;
+    std::vector<std::pair<uint64_t, uint64_t>> all;
+    for (int d : devs) for (size_t i = 0; i < rows[(size_t)d].size(); i++) all.emplace_back(rows[(size_t)d][i], totals[(size_t)d][i]);
+    std::sort(all.begin(), all.end());
+    std::vector<uint64_t> mr, mt;
+    for (const auto& p : all) {
+        if (!mr.empty() && mr.back() == p.first) mt.back() += p.second;
+        else { mr.push_back(p.first); mt.push_back(p.second); }
+    }
+    return write_sorted_rows(mr, mt, out_row_ids, out_counts, cap, out_n);
+} FBGPU_CATCH
+
 // a GroupBy node form once its arguments but n_rows are checked: n_rows checked before the fan-out, the request run on each device
 // over its own shards, the tensors added up (mergeGroupCounts executor.go:3728; Sum's [counts | sums]: wrapping int64 sums add as u64)
 static int node_groupby(fbgpu_node* n, uint32_t index, const GbRequest& q, uint64_t* out_counts, int64_t* out_sums = nullptr) {

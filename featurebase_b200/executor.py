@@ -574,7 +574,16 @@ class Executor:
         :1329-1338,1351-1356,1378-1383) — and only what passes is summed across shards (Pairs.Add, executeTopNShards :2845).
         So the counts are fetched as [shard][row] matrices (fbgpu_row_counts_per_shard: one launch for the rows' own counts, one
         more with the Src as filter; the Src counts of all shards come from one fbgpu_count).  Candidates: `ids`, else every row of the
-        field (what the internal second pass asks for when the first pass missed nothing; SURVEY Appendix D)."""
+        field (what the internal second pass asks for when the first pass missed nothing; SURVEY Appendix D).  A context with
+        topn_cutoffs does all of it in one device call, whose all-rows form is already in the answer's order."""
+        if hasattr(self.ctx, "topn_cutoffs"):
+            if ids is not None:
+                totals = self.ctx.topn_cutoffs(idx.id, f.id, VIEW_STANDARD, shards, row_ids=ids, src_ops=filt, min_threshold=thr, tanimoto=tan)
+                pairs = [(i, int(k)) for i, k in zip(ids, totals) if k > 0]
+                pairs.sort(key=lambda p: (-p[1], p[0]))
+                return pairs
+            rid, cnt = self.ctx.topn_cutoffs(idx.id, f.id, VIEW_STANDARD, shards, src_ops=filt, min_threshold=thr, tanimoto=tan)
+            return [(int(i), int(k)) for i, k in zip(rid, cnt)]
         if ids is None:
             rid, _ = self.ctx.row_counts(idx.id, f.id, VIEW_STANDARD, shards)
             ids = sorted(int(r) for r in rid)

@@ -52,7 +52,7 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_node_count_pairs", "fbgpu_node_row_counts", "fbgpu_node_groupby", "fbgpu_node_bsi_sum", "fbgpu_node_bsi_minmax",
            "fbgpu_groupby_values", "fbgpu_node_groupby_values", "fbgpu_row_counts_views", "fbgpu_node_row_counts_views", "fbgpu_groupby_views",
            "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum",
-           "fbgpu_groupby_distinct"]
+           "fbgpu_groupby_distinct", "fbgpu_topn_cutoffs", "fbgpu_node_topn_cutoffs"]
 
 
 def lib_path():
@@ -97,6 +97,8 @@ def load():
     L.fbgpu_bsi_select.restype = C.c_int
     L.fbgpu_row_counts.argtypes, L.fbgpu_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp, vp, i32, C.POINTER(i32)], C.c_int
     L.fbgpu_row_counts_per_shard.argtypes, L.fbgpu_row_counts_per_shard.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
+    L.fbgpu_topn_cutoffs.argtypes = [vp, u32, u32, u32, vp, i32, vp, i32, u64, u32, vp, i64, vp, vp, i32, C.POINTER(i32)]
+    L.fbgpu_topn_cutoffs.restype = C.c_int
     L.fbgpu_groupby.argtypes, L.fbgpu_groupby.restype = [vp, u32, vp, vp, i32, vp, vp, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_groupby_values.argtypes = [vp, u32, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i32, vp, i64, vp]
     L.fbgpu_groupby_values.restype = C.c_int
@@ -128,7 +130,7 @@ def load():
     L.fbgpu_node_devices.argtypes, L.fbgpu_node_devices.restype = [vp], i32
     L.fbgpu_node_owner.argtypes, L.fbgpu_node_owner.restype = [vp, u64], i32
     L.fbgpu_node_ctx.argtypes, L.fbgpu_node_ctx.restype = [vp, i32], vp
-    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "groupby_sum", "bsi_sum", "bsi_minmax"):
+    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "groupby_sum", "bsi_sum", "bsi_minmax", "topn_cutoffs"):
         src, dst = getattr(L, "fbgpu_" + name), getattr(L, "fbgpu_node_" + name)
         dst.argtypes, dst.restype = src.argtypes, src.restype
     L.fbgpu_node_row_counts.argtypes, L.fbgpu_node_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
@@ -450,6 +452,30 @@ class Context:
         self._check(self.L.fbgpu_row_counts_per_shard(self.h, index, field, view, ids.ctypes.data, len(ids), f, len(filter_ops) if filter_ops else 0,
                                                       sh.ctypes.data, len(sh), out.ctypes.data))
         return out
+
+    def topn_cutoffs(self, index, field, view, shards, row_ids=None, src_ops=None, min_threshold=0, tanimoto=0, cap=1 << 20):
+        """TopN's per-shard cut-offs summed over the shards (fbgpu_topn_cutoffs): with row_ids, the totals of those rows; without,
+        (row ids, totals) of every row with a total > 0, total descending, ties id ascending"""
+        sh = _u64arr(shards)
+        f = ops_array(src_ops) if src_ops else None
+        nf = len(src_ops) if src_ops else 0
+        n = C.c_int32(0)
+        if row_ids is not None:
+            ids = _u64arr(row_ids)
+            out = np.zeros(len(ids), dtype=np.uint64)
+            self._check(self.L.fbgpu_topn_cutoffs(self.h, index, field, view, ids.ctypes.data, len(ids), f, nf, int(min_threshold), int(tanimoto),
+                                                  sh.ctypes.data, len(sh), None, out.ctypes.data, len(ids), C.byref(n)))
+            return out
+        cap = min(cap, 1 << 16)
+        while True:                                  # the library reports how many rows there are when the buffers are too small
+            rid, out = np.zeros(cap, dtype=np.uint64), np.zeros(cap, dtype=np.uint64)
+            rc = self.L.fbgpu_topn_cutoffs(self.h, index, field, view, None, 0, f, nf, int(min_threshold), int(tanimoto), sh.ctypes.data, len(sh),
+                                           rid.ctypes.data, out.ctypes.data, cap, C.byref(n))
+            if rc == E_NOSPACE and n.value > cap:
+                cap = n.value
+                continue
+            self._check(rc)
+            return rid[: n.value], out[: n.value]
 
     def count_pairs(self, index, field_a, view_a, rows_a, field_b, view_b, rows_b, shards):
         sh, ra, rb = _u64arr(shards), _u64arr(rows_a), _u64arr(rows_b)

@@ -234,6 +234,27 @@ int fbgpu_row_counts(fbgpu_ctx *ctx, uint32_t index, uint32_t field, uint32_t vi
 int fbgpu_row_counts_per_shard(fbgpu_ctx *ctx, uint32_t index, uint32_t field, uint32_t view,
                                const uint64_t *row_ids, int32_t n_rows, const fbgpu_op *filter, int32_t n_filter_ops,
                                const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+/* TopN(f, Src, threshold=) and TopN(f, Src, tanimotoThreshold=): fragment.top's per-shard cut-offs for a cache that holds every
+ * row, without N-truncation (fragment.go:1317-1437), and the sum over the shards of what passes (Pairs.Add in
+ * executeTopNShards, executor.go:2831-2866), in one call.  For every listed shard s and candidate row r: cnt = |Row(field = r)|
+ * in s; with a Src program (n_src_ops > 0) S = Src in s, srcCount = |S| and count = |Row(r) ∩ S|, else count = cnt.  The pair
+ * is dropped
+ *   - Tanimoto mode (tanimoto_threshold t > 0 and a Src): if cnt == 0, (double)cnt <= (double)(srcCount * t) / 100,
+ *     (double)cnt >= (double)(srcCount * 100) / (double)t, count == 0, or
+ *     ceil((double)(count * 100) / (double)(cnt + srcCount - count)) <= (double)t (products in uint64, as in Go);
+ *   - otherwise, with m = max(min_threshold, 1): if cnt < m or count < m (t without a Src is ignored, as in the reference).
+ * total[r] = the sum of count over the shards where (s, r) is kept.  The output forms are fbgpu_row_counts': row_ids != NULL
+ * (any order, repeats allowed): out_counts[i] = total[row_ids[i]], all-reduced over the communicator.  row_ids == NULL: the
+ * candidates are the rows with a container in the field in at least one listed shard; the rows with total > 0 are written
+ * sorted by (total desc, row id asc) under the FBGPU_E_NOSPACE / *out_n contract, not all-reduced.
+ * tanimoto_threshold > 100 is FBGPU_E_INVALID, like NULL pointers, n_rows < 0 and n_src_ops < 0, all reported before the
+ * device check.  The node form takes the same arguments. */
+int fbgpu_topn_cutoffs(fbgpu_ctx *ctx, uint32_t index, uint32_t field, uint32_t view,
+                       const uint64_t *row_ids, int32_t n_rows,
+                       const fbgpu_op *src, int32_t n_src_ops,
+                       uint64_t min_threshold, uint32_t tanimoto_threshold,
+                       const uint64_t *shards, int64_t n_shards,
+                       uint64_t *out_row_ids, uint64_t *out_counts, int32_t cap, int32_t *out_n);
 /* fbgpu_row_counts with each row taken as its union over n_views (>= 1, any number) views of the field: the counts of TopK(f,
  * from=, to=) and the row ids of Rows(f, from=, to=) on a time field, whose covering views are listed in `views`
  * (executeTopKShardTime executor.go:2506-2533 over the mergerator :2570; executeRowsShard :4107-4127).
@@ -416,6 +437,11 @@ int fbgpu_node_row_counts(fbgpu_node *node, uint32_t index, uint32_t field, uint
 int fbgpu_node_row_counts_views(fbgpu_node *node, uint32_t index, uint32_t field, const uint32_t *views, int32_t n_views,
                                 const uint64_t *row_ids, int32_t n_rows, const fbgpu_op *filter, int32_t n_filter_ops,
                                 const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);
+/* both forms; all rows: each device's list merged by row id with the totals summed, then sorted (a shard lives on one device) */
+int fbgpu_node_topn_cutoffs(fbgpu_node *node, uint32_t index, uint32_t field, uint32_t view,
+                            const uint64_t *row_ids, int32_t n_rows, const fbgpu_op *src, int32_t n_src_ops,
+                            uint64_t min_threshold, uint32_t tanimoto_threshold, const uint64_t *shards, int64_t n_shards,
+                            uint64_t *out_row_ids, uint64_t *out_counts, int32_t cap, int32_t *out_n);
 int fbgpu_node_groupby_views(fbgpu_node *node, uint32_t index, const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views,
                              int32_t n_fields, const uint64_t *row_ids_flat, const int32_t *n_rows,
                              const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards, uint64_t *out_counts);

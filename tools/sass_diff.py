@@ -3,8 +3,9 @@
     python tools/sass_diff.py <commit>         # e.g. the last commit whose library was parity-tested and timed on an H100
 Builds that commit's csrc/ in a scratch directory with the same nvcc line, dumps both libraries with cuobjdump -sass and
 compares the instruction streams per kernel (addresses and encodings stripped; template arguments that did not exist yet
-or no longer exist are matched by kernel name: an untemplated kernel and its <false> instantiation, and groupby_values_kernel's
-<GvAgg(0)> / <GvAgg(1)> (count only / Sum) and the <false> / <true> of the bool template they replaced).  Kernels of the old
+or no longer exist are matched by kernel name: an untemplated kernel and its <false> instantiation, groupby_values_kernel's
+<GvAgg(0)> / <GvAgg(1)> (count only / Sum) and row_count_kernel's <RcOut(0)> / <RcOut(1)> (summed / per shard) and the
+<false> / <true> of the bool templates they replaced).  Kernels of the old
 build that the new one lacks are reported DELETED.  No GPU needed.  A kernel reported IDENTICAL is, bit for bit in its
 instructions, the one that was parity-tested and timed on the device."""
 import os
@@ -33,7 +34,8 @@ def kernels(path):
     return res
 
 
-ENUM_AS_BOOL = {"LNS_5GvAggE0": "Lb0", "LNS_5GvAggE1": "Lb1"}      # GvAgg::kCount / kSum took the place of <false> / <true>
+ENUM_AS_BOOL = {"LNS_5GvAggE0": "Lb0", "LNS_5GvAggE1": "Lb1",     # GvAgg::kCount / kSum took the place of <false> / <true>
+                "LNS_5RcOutE0": "Lb0", "LNS_5RcOutE1": "Lb1"}     # and row_count_kernel's RcOut::kSummed / kPerShard
 
 
 def short(name):
