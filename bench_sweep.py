@@ -20,6 +20,8 @@
             fbgpu_groupby_distinct against the Distinct-per-group composition (only when named in --configs).
   config N: TopN(f, Row(src=0), tanimotoThreshold=50) and TopN(f, Row(src=0), threshold=100) over --topn-rows rows of varied
             cardinality, fbgpu_topn_cutoffs against the per-shard count-matrix composition (only when named in --configs).
+  config O: Sort over config X's 32-bit field with and without a limit, fbgpu_bsi_sort against extracting every value and
+            sorting on the host (only when named in --configs).
 Every point is spot-checked against the CPU oracle on a few shards (the checker, not the thing measured)."""
 import argparse
 import json
@@ -942,13 +944,84 @@ def config4(args, out):
     h.ctx.close()
 
 
+class _NoBsiSort(_KernelMs):
+    """the same proxy without bsi_sort: the executor extracts every (column, value) pair and sorts them on the host"""
+
+    def __getattr__(self, name):
+        if name == "bsi_sort":
+            raise AttributeError(name)
+        return super().__getattr__(name)
+
+
+SORT_QUERIES = ["Sort(Row(v >= 0), field=v, sort-desc=true, limit=10)",       # every record, ten kept
+                "Sort(Row(f=0), field=v, limit=10, offset=1000)",              # the 1 % row, a window past its start
+                "Sort(Row(f=0), field=v)"]                                     # the 1 % row, no limit: about 100 K pairs returned
+
+
+def config_sort(args, out):
+    """Sort over config X's data (10 M records of a 32-bit field, a 1 % row f=0) through the executor: the device arm (one
+    fbgpu_bsi_sort) and the composition arm (fbgpu_extract of every pair of the row, a Python sort, then the window), alternated
+    step by step; the composition runs --composition-steps steps.  Both arms must return the same pairs."""
+    from featurebase_b200 import datagen as D, executor as X
+    n_rec = min(10_000_000, args.shards * SW)
+    n_sh = (n_rec + SW - 1) // SW
+    shards = np.arange(n_sh, dtype=np.uint64)
+    h = X.Holder()
+    idx = h.create_index("i", track_existence=False)
+    f = idx.create_field("f")
+    v = idx.create_field("v", "int", min=0, max=(1 << 32) - 1)
+    bulk = D.fragments(11, shards, [0], 0.01)
+    h.ctx.load_fragments(idx.id, f.id, X.VIEW_STANDARD, shards, bulk.buf, bulk.offsets)
+    for s in range(n_sh):
+        h.ctx.load_fragment(idx.id, v.id, X.VIEW_BSI, s, D.bsi_fragment(12, s, min(SW, n_rec - s * SW), 32, 0, (1 << 32) - 1))
+    h.ctx.commit()
+    idx.shards.update(range(n_sh))
+    real = h.ctx
+    card = _card()
+    arms = {"device": _KernelMs(real), "composition": _NoBsiSort(real)}
+    for q in SORT_QUERIES:
+        rec = {name: {"wall": [], "kernel_ms": [], "queries": []} for name in arms}
+        res = {}
+        for i in range(1 + args.steps):                      # one warm-up round of the device arm, then alternate the arms
+            for name in (sorted(arms) if i % 2 == 0 else sorted(arms, reverse=True)):
+                if name == "composition" and len(rec[name]["wall"]) >= args.composition_steps:
+                    continue
+                h.ctx = arms[name]
+                q0, arms[name].ms = real.counters()["queries"], 0.0
+                t0 = time.perf_counter()
+                r = X.Executor(h).execute("i", q)[0]
+                wall = (time.perf_counter() - t0) * 1e3
+                res.setdefault(name, r)
+                assert r == res[name], (q, name)
+                print(f"config O: {q}, {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                if i >= 1 or name == "composition":
+                    rec[name]["wall"].append(wall)
+                    rec[name]["kernel_ms"].append(arms[name].ms)
+                    rec[name]["queries"].append(real.counters()["queries"] - q0)
+        h.ctx = real
+        equal = res.get("composition") == res["device"] if "composition" in res else None
+        assert equal is not False, q
+        for name, d in rec.items():
+            if not d["wall"]:
+                continue
+            out({"config": "O", "query": q, "arm": name, "gpu": card, "records": n_rec, "shards": n_sh, "pairs": len(res[name]),
+                 "equal_to_composition": equal, "wall_ms": float(np.median(d["wall"])), "wall_ms_min": float(np.min(d["wall"])),
+                 "wall_ms_max": float(np.max(d["wall"])), "kernel_ms": float(np.median(d["kernel_ms"])), "queries": int(np.median(d["queries"])),
+                 "steps": len(d["wall"]),
+                 "kernel": ("eval_kernel + columns_emit_kernel + extract_values_kernel + sort_keys_kernel + sort_{hist,scan,scatter}_kernel"
+                            if name == "device" else "eval_kernel + columns_emit_kernel + extract_values_kernel, host sort"),
+                 "note": "median over the timed steps of the executor call (wall clock), of the summed last_query_gpu_ms and of the "
+                         "number of its library queries"})
+    real.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", default="5,3,4")
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--shards", type=int, default=1024)
     ap.add_argument("--groupby-shards", type=int, default=512)
-    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D, N: steps of the composition arm")
+    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D, N, O: steps of the composition arm")
     ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S, D, N: shards of the composition arm and of the device arm timed beside it")
     ap.add_argument("--topn-rows", type=int, default=1 << 14, help="config N: rows of the TopN field")
     ap.add_argument("--topn-shards", type=int, default=16, help="config N: shards (the fragments are encoded in Python: ~5 s per shard)")
@@ -980,6 +1053,8 @@ def main():
             config_groupby_distinct(args, out)
         elif c == "N":
             config_topn_cutoffs(args, out)
+        elif c == "O":
+            config_sort(args, out)
         elif c == "3L":     # the same BSI query at 256 shards (268 M records, 1.1 GB of planes): shows the kernel away from the launch-bound regime
             config3(args, out, n_rec=256 * SW, nf=1)
         else:

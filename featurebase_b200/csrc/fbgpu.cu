@@ -147,6 +147,7 @@ struct Workspace {
     DevBuf d_in, d_counts, d_bitmaps, d_info, d_emit_units, d_emit, d_rows, d_aux;
     DevBuf d_select;                     // fbgpu_bsi_select: per-rank candidate bitmaps of every unit of the call
     DevBuf d_present;                    // fbgpu_groupby_distinct: one leaf's presence bitset, (cell, listed value of x) -> present
+    DevBuf d_sort;                       // fbgpu_bsi_sort: (key, column) pairs, two halves (SortPairs)
     PinBuf h_in, h_out;
     bool busy = false;
 };
@@ -253,7 +254,7 @@ extern "C" void fbgpu_shutdown(fbgpu_ctx* c) {
     cudaDeviceSynchronize();
     if (c->comm && nccl_load()) g_nccl.CommDestroy(c->comm);
     for (auto& w : c->wss) {
-        for (DevBuf* b : { &w->d_in, &w->d_counts, &w->d_bitmaps, &w->d_info, &w->d_emit_units, &w->d_emit, &w->d_rows, &w->d_aux, &w->d_select, &w->d_present }) b->release();
+        for (DevBuf* b : { &w->d_in, &w->d_counts, &w->d_bitmaps, &w->d_info, &w->d_emit_units, &w->d_emit, &w->d_rows, &w->d_aux, &w->d_select, &w->d_present, &w->d_sort }) b->release();
         w->h_in.release(); w->h_out.release();
         if (w->ev0) cudaEventDestroy(w->ev0);
         if (w->ev1) cudaEventDestroy(w->ev1);
@@ -1073,16 +1074,22 @@ struct Query {
         info = (const uint2*)w->h_out.p;
         return 0;
     }
-    // Row / Columns: copies the unit list to d_emit_units, runs launch(d_units, units.size(), grid) (emit kernels that write d_emit) and
-    // reads `out_bytes` of d_emit back into h_in; ev1 closes the batch's timed bracket
+    // copies the unit list to d_emit_units and runs launch(d_units, units.size(), grid): emit kernels whose output stays on the device
     template <class Unit, class Launch>
-    int emit(const std::vector<Unit>& units, size_t out_bytes, Launch launch) {
+    int emit_on_device(const std::vector<Unit>& units, size_t out_bytes, Launch launch) {
         const size_t ub = units.size() * sizeof(Unit);
-        if (w->d_emit_units.ensure(ub) || w->d_emit.ensure(out_bytes) || w->h_in.ensure(std::max(ub, out_bytes))) return FBGPU_E_NOMEM;
+        if (w->d_emit_units.ensure(ub) || w->d_emit.ensure(out_bytes) || w->h_in.ensure(ub)) return FBGPU_E_NOMEM;
+        CUDA_TRY(cudaStreamSynchronize(w->stream));   // an earlier H2D copy out of h_in may still be pending
         memcpy(w->h_in.p, units.data(), ub);
         CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, w->h_in.p, ub, cudaMemcpyHostToDevice, w->stream));
         const int grid = (int)std::min<size_t>(units.size(), (size_t)c->sm_count * 8);
-        int rc = launch((const Unit*)w->d_emit_units.p, (int)units.size(), grid); if (rc) return rc;
+        return launch((const Unit*)w->d_emit_units.p, (int)units.size(), grid);
+    }
+    // Row / Columns: emit_on_device, then `out_bytes` of d_emit read back into h_in; ev1 closes the batch's timed bracket
+    template <class Unit, class Launch>
+    int emit(const std::vector<Unit>& units, size_t out_bytes, Launch launch) {
+        if (w->h_in.ensure(std::max(units.size() * sizeof(Unit), out_bytes))) return FBGPU_E_NOMEM;
+        int rc = emit_on_device(units, out_bytes, launch); if (rc) return rc;
         CUDA_TRY(cudaStreamSynchronize(w->stream));   // h_in is reused as the D2H landing buffer below
         CUDA_TRY(cudaMemcpyAsync(w->h_in.p, w->d_emit.p, out_bytes, cudaMemcpyDeviceToHost, w->stream));
         CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
@@ -1258,6 +1265,34 @@ extern "C" int fbgpu_row(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int3
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ Columns (Row.Columns(): ascending ids, with executeLimitCall's window) / Extract
+// [offset, offset + limit) as a half-open range of ranks; no limit (limit < 0) and an overflowing end are "to the end"
+static uint64_t window_end(uint64_t offset, int64_t limit) {
+    return limit < 0 ? ~0ull : (offset + (uint64_t)limit < offset ? ~0ull : offset + (uint64_t)limit);
+}
+
+// the emit units of one evaluated batch (units [u0, u0 + nu) of the sorted shard list, `info` their {N, runs}): its non-empty
+// units clipped to the ranks [offset, win_end) of the row, packed from out_off 0.  `seen` is the row's rank of the batch's first
+// column on entry and of the next batch's on return; the result is the number of columns the units emit.
+static uint64_t col_units(const uint2* info, long long u0, long long nu, const std::vector<uint64_t>& sorted, uint64_t offset, uint64_t win_end,
+                          uint64_t& seen, std::vector<ColUnit>& units) {
+    units.clear();
+    uint64_t out = 0;
+    for (long long u = 0; u < nu; u++) {
+        const uint64_t N = info[u].x;
+        if (!N) continue;
+        const uint64_t lo = std::max(seen, offset), hi = std::min(seen + N, win_end);    // the unit's ranks are [seen, seen + N)
+        if (hi > lo) {
+            ColUnit cu{};
+            cu.out_off = out; cu.unit = (uint32_t)u; cu.first = (uint32_t)(lo - seen); cu.last = (uint32_t)(hi - seen);
+            cu.col_base = (sorted[(u0 + u) / kSlotsPerRow] << 20) + (uint64_t)((u0 + u) % kSlotsPerRow) * 65536ull;
+            units.push_back(cu);
+            out += hi - lo;
+        }
+        seen += N;
+    }
+    return out;
+}
+
 // shared body: evaluate the row into per-unit bitmaps, cut the [offset, offset+limit) window into per-unit rank ranges, expand
 // the column ids on the device and — for Extract — gather the BSI planes of `fv_vals` for exactly those columns
 static int columns_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, const uint64_t* shards, int64_t n_shards,
@@ -1267,26 +1302,14 @@ static int columns_impl(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32
     const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);
     int rc = q.open(index, ops, n_ops, sorted.data(), (int64_t)sorted.size()); if (rc) return rc;
     const long long n_units = q.n_units;
-    const uint64_t win_end = limit < 0 ? ~0ull : (offset + (uint64_t)limit < offset ? ~0ull : offset + (uint64_t)limit);
+    const uint64_t win_end = window_end(offset, limit);
     uint64_t seen = 0, written = 0;
+    std::vector<ColUnit> units;
     for (long long u0 = 0; u0 < n_units; u0 += c->unit_batch) {
         const long long nu = std::min(c->unit_batch, n_units - u0);
         const uint2* info;
         rc = q.eval_info(u0, nu, info); if (rc) return rc;
-        std::vector<ColUnit> units; uint64_t batch_out = 0;
-        for (long long u = 0; u < nu; u++) {
-            const uint64_t N = info[u].x;
-            if (!N) continue;
-            const uint64_t lo = std::max(seen, offset), hi = std::min(seen + N, win_end);    // the unit's ranks are [seen, seen + N)
-            if (hi > lo) {
-                ColUnit cu{};
-                cu.out_off = batch_out; cu.unit = (uint32_t)u; cu.first = (uint32_t)(lo - seen); cu.last = (uint32_t)(hi - seen);
-                cu.col_base = (sorted[(u0 + u) / kSlotsPerRow] << 20) + (uint64_t)((u0 + u) % kSlotsPerRow) * 65536ull;
-                units.push_back(cu);
-                batch_out += hi - lo;
-            }
-            seen += N;
-        }
+        const uint64_t batch_out = col_units(info, u0, nu, sorted, offset, win_end, seen, units);
         if (batch_out && written + batch_out <= cap) {
             // d_emit: columns [batch_out] u64, then for Extract magnitudes [batch_out] u64 and sign bits [ceil(batch_out / 32)] u32
             const size_t vb = want_vals ? batch_out * 8 + ((batch_out + 31) / 32) * 4 : 0;
@@ -1337,6 +1360,171 @@ extern "C" int fbgpu_extract(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, 
     const std::vector<fbgpu_op> full = and_row(ops, n_ops, field, view, 0);    // <filter> ∩ exists (bsiExistsBit, row 0 of the bsig_ view; fragment.go:44)
     const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
     return columns_impl(c, index, full.data(), (int32_t)full.size(), shards, n_shards, offset, limit, true, fv, bit_depth, out_cols, out_vals, cap, out_n, out_total);
+} FBGPU_CATCH
+
+// ------------------------------------------------------------------ Sort over an int field (sort_keys_kernel and the radix sort, kernels.cuh)
+// The row is evaluated batch by batch as for fbgpu_extract.  Each batch's non-empty units are emitted in chunks of at most
+// kSortChunk pairs straight into the call's pair buffer, behind the pairs kept so far: the columns by columns_emit_kernel, the
+// keys by sort_keys_kernel from extract_values_kernel's output.  With a limit, the buffer is sorted and cut to the K = offset +
+// limit first pairs before a chunk that would take it past 2K pairs.  At the end it is sorted once more and only the window is
+// read back.
+constexpr uint64_t kSortChunk = 1ull << 24;
+
+static uint64_t sat_add(uint64_t a, uint64_t b) { return a + b < a ? ~0ull : a + b; }
+
+// w->d_sort as two halves of `cap` (key, column) pairs, [keys | columns] each, for the radix sort's ping-pong; half `cur` holds
+// the n pairs kept so far.  The buffer outlives the call, like the workspace's other buffers.
+struct SortPairs {
+    Workspace* w; uint64_t bound; uint64_t cap, n = 0; int cur = 0;
+    SortPairs(Workspace* ws, uint64_t max_pairs) : w(ws), bound(max_pairs), cap(ws->d_sort.cap / 32) {}
+    unsigned long long* keys(int h) const { return (unsigned long long*)w->d_sort.p + (size_t)h * 2 * cap; }
+    unsigned long long* cols(int h) const { return keys(h) + cap; }
+    // room for `need` pairs (need <= bound); a buffer that has to grow takes the kept pairs along into its half 0
+    int reserve(uint64_t need) {
+        if (need <= cap) return 0;
+        if (need > 0xffffffffull) return fail(FBGPU_E_NOMEM, "the sort would hold %llu pairs on the device: more than 2^32", (unsigned long long)need);
+        const uint64_t nc = std::min(std::max(need, cap + cap / 2), bound);
+        DevBuf nb;
+        if (nb.ensure((size_t)nc * 32)) return FBGPU_E_NOMEM;
+        if (n) {
+            CUDA_TRY(cudaMemcpyAsync(nb.p, keys(cur), n * 8, cudaMemcpyDeviceToDevice, w->stream));
+            CUDA_TRY(cudaMemcpyAsync((unsigned long long*)nb.p + nc, cols(cur), n * 8, cudaMemcpyDeviceToDevice, w->stream));
+            CUDA_TRY(cudaStreamSynchronize(w->stream));
+        }
+        w->d_sort.release(); w->d_sort = nb; cap = nc; cur = 0;
+        return 0;
+    }
+};
+
+// stable sort of the kept pairs by the low `bits` bits of their keys (8-bit digits, least significant first), then the first
+// `keep` of them kept
+static int sort_pairs(Query& q, SortPairs& sp, int bits, uint64_t keep) {
+    Workspace* w = q.w;
+    if (sp.n == 0) return 0;
+    const uint64_t n_tiles = (sp.n + kSortTile - 1) / kSortTile, m = n_tiles * 256;
+    if (w->d_counts.ensure((size_t)m * 4)) return FBGPU_E_NOMEM;
+    unsigned int* counts = (unsigned int*)w->d_counts.p;
+    for (int shift = 0; shift < bits; shift += 8) {
+        sort_hist_kernel<<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(sp.keys(sp.cur), sp.n, shift, counts);
+        CUDA_TRY(cudaGetLastError());
+        sort_scan_kernel<<<1, kSortScanThreads, 0, w->stream>>>(counts, m);
+        CUDA_TRY(cudaGetLastError());
+        sort_scatter_kernel<<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(sp.keys(sp.cur), sp.cols(sp.cur), sp.n, shift, counts,
+                                                                              sp.keys(1 - sp.cur), sp.cols(1 - sp.cur));
+        CUDA_TRY(cudaGetLastError());
+        q.launches += 3;
+        sp.cur = 1 - sp.cur;
+    }
+    sp.n = std::min(sp.n, keep);
+    return 0;
+}
+
+// the pairs [offset, min(win_end, |row|)) of the row <ops> ∩ exists(field) in sort order (store lock held): columns and stored
+// values into cols / vals, |row| into *total
+static int bsi_sort_run(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int depth,
+                        const uint64_t* shards, int64_t n_shards, bool desc, uint64_t offset, uint64_t win_end,
+                        std::vector<uint64_t>& cols, std::vector<int64_t>& vals, uint64_t* total) {
+    const std::vector<fbgpu_op> full = and_row(ops, n_ops, field, view, 0);    // as for fbgpu_extract
+    const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
+    Query q(c); Workspace* w = q.w;
+    const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);      // units in ascending column order
+    int rc = q.open(index, full.data(), (int32_t)full.size(), sorted.data(), (int64_t)sorted.size()); if (rc) return rc;
+    const bool limited = win_end != ~0ull;
+    const uint64_t K = win_end, twice_k = sat_add(K, K);
+    const int bits = sort_key_bits(depth);
+    SortPairs sp(w, limited ? std::max(twice_k, sat_add(K, kSortChunk)) : ~0ull);
+    uint64_t seen = 0;
+    std::vector<ColUnit> units, chunk;
+    for (long long u0 = 0; u0 < q.n_units; u0 += c->unit_batch) {
+        const long long nu = std::min(c->unit_batch, q.n_units - u0);
+        const uint2* info;
+        rc = q.eval_info(u0, nu, info); if (rc) return rc;
+        const uint64_t batch_out = col_units(info, u0, nu, sorted, 0, ~0ull, seen, units);
+        for (size_t a = 0; a < units.size();) {
+            const uint64_t base = units[a].out_off;
+            size_t b = a + 1;                               // the chunk: units [a, b), at least one
+            while (b < units.size() && units[b].out_off + (units[b].last - units[b].first) - base <= kSortChunk) b++;
+            const uint64_t cn = (b < units.size() ? units[b].out_off : batch_out) - base;
+            chunk.assign(units.begin() + (long)a, units.begin() + (long)b);
+            for (ColUnit& cu : chunk) cu.out_off -= base;
+            if (limited && sp.n > K && sp.n + cn > twice_k) { rc = sort_pairs(q, sp, bits, K); if (rc) return rc; }
+            rc = sp.reserve(sp.n + cn); if (rc) return rc;
+            // d_emit: magnitudes [cn] u64, then sign bits [ceil(cn / 32)] u32
+            const size_t vb = cn * 8 + ((cn + 31) / 32) * 4;
+            rc = q.emit_on_device(chunk, vb, [&](const ColUnit* d_units, int n, int grid) {
+                unsigned long long* d_mag = (unsigned long long*)w->d_emit.p;
+                unsigned int* d_sign = (unsigned int*)(d_mag + cn);
+                columns_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>((const uint4*)w->d_bitmaps.p, d_units, n, sp.cols(sp.cur) + sp.n);
+                CUDA_TRY(cudaGetLastError());
+                CUDA_TRY(cudaMemsetAsync(d_mag, 0, vb, w->stream));
+                extract_values_kernel<<<grid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv, depth, (const uint4*)w->d_bitmaps.p, d_units, n, d_mag, d_sign);
+                CUDA_TRY(cudaGetLastError());
+                const unsigned kgrid = (unsigned)std::min<uint64_t>((cn + kSortThreads - 1) / kSortThreads, (uint64_t)c->sm_count * 8);
+                sort_keys_kernel<<<kgrid, kSortThreads, 0, w->stream>>>(d_mag, d_sign, cn, depth, desc ? 1 : 0, sp.keys(sp.cur) + sp.n);
+                CUDA_TRY(cudaGetLastError());
+                q.launches += 3;
+                return 0;
+            });
+            if (rc) return rc;
+            sp.n += cn;
+            a = b;
+        }
+        CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        q.add_elapsed();
+    }
+    *total = seen;
+    // sp.n = min(K, |row|) after the last sort; the window is its part from offset on (offset <= K)
+    CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
+    rc = sort_pairs(q, sp, bits, K); if (rc) return rc;
+    const uint64_t lo = std::min(offset, sp.n), cnt = sp.n - lo;
+    if (w->h_out.ensure(std::max<size_t>(cnt * 16, 16))) return FBGPU_E_NOMEM;
+    const uint64_t* h_keys = (const uint64_t*)w->h_out.p; const uint64_t* h_cols = h_keys + cnt;
+    if (cnt) {
+        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, sp.keys(sp.cur) + lo, cnt * 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaMemcpyAsync((uint64_t*)w->h_out.p + cnt, sp.cols(sp.cur) + lo, cnt * 8, cudaMemcpyDeviceToHost, w->stream));
+    }
+    CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+    CUDA_TRY(cudaStreamSynchronize(w->stream));
+    q.add_elapsed();
+    const uint64_t mask = sort_key_mask(depth);
+    cols.assign(h_cols, h_cols + cnt);
+    vals.resize(cnt);
+    for (uint64_t i = 0; i < cnt; i++) {                 // sort_keys_kernel backwards
+        const uint64_t k = desc ? ~h_keys[i] & mask : h_keys[i];
+        vals[i] = (int64_t)(depth < 64 ? k - (1ull << depth) : k ^ (1ull << 63));
+    }
+    q.finish();
+    return FBGPU_OK;
+}
+
+// the FBGPU_E_INVALID checks of fbgpu_bsi_sort and its node form, with fbgpu_extract's messages
+static int bsi_sort_args(const void* handle, const fbgpu_op* ops, int32_t n_ops, int32_t bit_depth, const uint64_t* shards, int64_t n_shards,
+                         const uint64_t* out_cols, const int64_t* out_vals, uint64_t cap, const uint64_t* out_n) {
+    if (!handle || !out_n || n_shards < 0 || (n_shards && !shards) || (cap && (!out_cols || !out_vals)) || n_ops < 0 || (n_ops && !ops)) return fail(FBGPU_E_INVALID, "null argument");
+    if (bit_depth < 0 || bit_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", bit_depth);
+    return 0;
+}
+
+// a window into the caller's arrays under the NOSPACE contract: *out_n = its size, nothing written when it exceeds cap
+static int write_window(const std::vector<uint64_t>& cols, const std::vector<int64_t>& vals, uint64_t* out_cols, int64_t* out_vals, uint64_t cap, uint64_t* out_n) {
+    *out_n = cols.size();
+    if (cols.size() > cap) return fail(FBGPU_E_NOSPACE, "output needs room for %llu columns", (unsigned long long)cols.size());
+    if (!cols.empty()) { memcpy(out_cols, cols.data(), cols.size() * 8); memcpy(out_vals, vals.data(), vals.size() * 8); }
+    return FBGPU_OK;
+}
+
+extern "C" int fbgpu_bsi_sort(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
+                              const uint64_t* shards, int64_t n_shards, int32_t desc, uint64_t offset, int64_t limit,
+                              uint64_t* out_cols, int64_t* out_vals, uint64_t cap, uint64_t* out_n, uint64_t* out_total) try {
+    int rc = bsi_sort_args(c, ops, n_ops, bit_depth, shards, n_shards, out_cols, out_vals, cap, out_n); if (rc) return rc;
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    std::vector<uint64_t> cols; std::vector<int64_t> vals; uint64_t total = 0;
+    rc = bsi_sort_run(c, index, ops, n_ops, field, view, bit_depth, shards, n_shards, desc != 0, offset, window_end(offset, limit), cols, vals, &total);
+    if (rc) return rc;
+    if (out_total) *out_total = total;
+    return write_window(cols, vals, out_cols, out_vals, cap, out_n);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ BSI Min / Max (one pass over the planes)

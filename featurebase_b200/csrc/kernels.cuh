@@ -1307,6 +1307,125 @@ extract_values_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restri
     }
 }
 
+// ------------------------------------------------------------------ Sort over an int field (fbgpu_bsi_sort)
+// extract_values_kernel's (magnitude, sign bit) pairs become order-preserving unsigned keys of sort_key_bits(depth) bits, and
+// the (key, column) pairs are put in key order by a stable LSD radix sort of 8-bit digits: per pass a per-tile digit histogram
+// (sort_hist_kernel), an exclusive scan over the digit-major [digit][tile] count matrix (sort_scan_kernel) and a scatter that
+// ranks each pair inside its tile (sort_scatter_kernel).  Stability keeps equal keys in input order, which is ascending column
+// order: the kept pairs are already sorted and every appended column is larger than every kept one.
+constexpr int kSortThreads = 256;
+constexpr int kSortRounds = 16;                              // rounds of kSortThreads pairs per tile
+constexpr int kSortTile = kSortThreads * kSortRounds;
+constexpr int kSortScanThreads = 1024;
+constexpr int kSortScanItems = 16;                           // consecutive counts per thread and scan round
+
+// the key width: value + 2^depth takes depth + 1 bits below depth 64; at depth 64 the value is the int64 fbgpu_extract reports
+__host__ __device__ inline int sort_key_bits(int depth) { return depth < 64 ? depth + 1 : 64; }
+__host__ __device__ inline uint64_t sort_key_mask(int depth) { return depth < 64 ? (2ull << depth) - 1ull : ~0ull; }
+
+// keys[i] for the i-th of n values: value = sign ? 0 - mag : mag (a sign with magnitude 0 is the value 0), then value + 2^depth
+// (value ^ 2^63 at depth 64), complemented within the key's width for a descending sort
+__global__ void __launch_bounds__(kSortThreads)
+sort_keys_kernel(const unsigned long long* __restrict__ mag, const unsigned int* __restrict__ sign, unsigned long long n, int depth, int desc,
+                 unsigned long long* __restrict__ keys) {
+    const uint64_t mask = sort_key_mask(depth);
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const uint64_t m = mag[i];
+        const uint64_t v = ((sign[i >> 5] >> (i & 31)) & 1u) ? 0ull - m : m;
+        uint64_t k = depth < 64 ? v + (1ull << depth) : v ^ (1ull << 63);
+        if (desc) k = ~k & mask;
+        keys[i] = k;
+    }
+}
+
+// counts[d * n_tiles + t] = the pairs of tile t whose digit at `shift` is d
+__global__ void __launch_bounds__(kSortThreads)
+sort_hist_kernel(const unsigned long long* __restrict__ keys, unsigned long long n, int shift, unsigned int* __restrict__ counts) {
+    __shared__ unsigned int hist[256];
+    const unsigned n_tiles = gridDim.x, tile = blockIdx.x;
+    hist[threadIdx.x] = 0;
+    __syncthreads();
+    const unsigned long long t0 = (unsigned long long)tile * kSortTile;
+    for (int r = 0; r < kSortRounds; r++) {
+        const unsigned long long i = t0 + (unsigned long long)r * kSortThreads + threadIdx.x;
+        if (i < n) atomicAdd(&hist[(keys[i] >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    counts[(size_t)threadIdx.x * n_tiles + tile] = hist[threadIdx.x];
+}
+
+// in-place exclusive scan of the m counts, one CTA: rounds of kSortScanThreads x kSortScanItems consecutive counts with a carry
+__global__ void __launch_bounds__(kSortScanThreads)
+sort_scan_kernel(unsigned int* __restrict__ counts, unsigned long long m) {
+    __shared__ unsigned int wsum[kSortScanThreads / 32];
+    __shared__ unsigned int carry_s;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    unsigned int carry = 0;
+    for (unsigned long long r0 = 0; r0 < m; r0 += (unsigned long long)kSortScanThreads * kSortScanItems) {
+        const unsigned long long b = r0 + (unsigned long long)tid * kSortScanItems;
+        unsigned int v[kSortScanItems], s = 0;
+#pragma unroll
+        for (int k = 0; k < kSortScanItems; k++) { v[k] = b + k < m ? counts[b + k] : 0u; s += v[k]; }
+        unsigned int inc = s;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const unsigned int x = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += x; }
+        if (lane == 31) wsum[wid] = inc;
+        __syncthreads();
+        unsigned int run = carry + inc - s;
+        for (int k = 0; k < wid; k++) run += wsum[k];
+#pragma unroll
+        for (int k = 0; k < kSortScanItems; k++) { if (b + k < m) counts[b + k] = run; run += v[k]; }
+        if (tid == kSortScanThreads - 1) carry_s = run;
+        __syncthreads();
+        carry = carry_s;
+        __syncthreads();                                   // (wsum and carry_s are rewritten by the next round)
+    }
+}
+
+// the stable scatter of one pass: tile t's pairs with digit d go to [counts[d * n_tiles + t], ...) in their input order.  Per
+// round of kSortThreads pairs each warp splits its 32 pairs by digit with eight ballots (a warp multisplit: the lanes that agree
+// with this lane on every digit bit); the lowest lane of each group publishes the group's size, and one thread per digit turns
+// the eight warps' sizes into offsets after the tile's running offset for that digit.
+__global__ void __launch_bounds__(kSortThreads)
+sort_scatter_kernel(const unsigned long long* __restrict__ keys_in, const unsigned long long* __restrict__ cols_in, unsigned long long n, int shift,
+                    const unsigned int* __restrict__ counts, unsigned long long* __restrict__ keys_out, unsigned long long* __restrict__ cols_out) {
+    __shared__ unsigned int run[256];
+    __shared__ unsigned int wcnt[kSortThreads / 32][256];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const unsigned n_tiles = gridDim.x, tile = blockIdx.x;
+    const unsigned int lt = (1u << lane) - 1u;
+    run[tid] = counts[(size_t)tid * n_tiles + tile];
+    const unsigned long long t0 = (unsigned long long)tile * kSortTile;
+    for (int r = 0; r < kSortRounds; r++) {
+        const unsigned long long i = t0 + (unsigned long long)r * kSortThreads + tid;
+        const bool valid = i < n;
+        unsigned long long key = 0, col = 0;
+        if (valid) { key = keys_in[i]; col = cols_in[i]; }
+        const unsigned int d = (unsigned int)(key >> shift) & 255u;
+        unsigned int peers = __ballot_sync(0xffffffffu, valid);
+#pragma unroll
+        for (int b = 0; b < 8; b++) {
+            const unsigned int bal = __ballot_sync(0xffffffffu, (d >> b) & 1u);
+            peers &= ((d >> b) & 1u) ? bal : ~bal;
+        }
+#pragma unroll
+        for (int w = 0; w < kSortThreads / 32; w++) wcnt[w][tid] = 0;
+        __syncthreads();
+        if (valid && (peers & lt) == 0) wcnt[wid][d] = (unsigned int)__popc(peers);
+        __syncthreads();
+        unsigned int o = run[tid];
+#pragma unroll
+        for (int w = 0; w < kSortThreads / 32; w++) { const unsigned int c = wcnt[w][tid]; wcnt[w][tid] = o; o += c; }
+        run[tid] = o;
+        __syncthreads();
+        if (valid) {
+            const unsigned int pos = wcnt[wid][d] + (unsigned int)__popc(peers & lt);
+            keys_out[pos] = key; cols_out[pos] = col;
+        }
+        __syncthreads();                                   // (wcnt is cleared by the next round)
+    }
+}
+
 // Min / Max of an int field over a row (fragment.min / max fragment.go:752-838 with minUnsigned :788 / maxUnsigned :841),
 // one CTA per (shard, slot) unit, every plane container read once.  The unit's `consider` bitmap (filter ∩ exists, produced
 // by eval_kernel) is split by the sign row; the side that decides the answer is narrowed plane by plane from the top bit:

@@ -369,6 +369,43 @@ extern "C" int fbgpu_node_bsi_minmax(fbgpu_node* n, uint32_t index, const fbgpu_
     return FBGPU_OK;
 } FBGPU_CATCH
 
+// Sort over an int field: every device sorts its own shards and keeps its first offset + limit pairs; the devices' lists (their
+// columns are disjoint) are merged in the same order, as SortedRow.Merge does (executor.go:9574), and the window is cut after the
+// merge
+extern "C" int fbgpu_node_bsi_sort(fbgpu_node* n, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
+                                   const uint64_t* shards, int64_t n_shards, int32_t desc, uint64_t offset, int64_t limit,
+                                   uint64_t* out_cols, int64_t* out_vals, uint64_t cap, uint64_t* out_n, uint64_t* out_total) try {
+    int rc = bsi_sort_args(n, ops, n_ops, bit_depth, shards, n_shards, out_cols, out_vals, cap, out_n); if (rc) return rc;
+    const uint64_t win_end = window_end(offset, limit);
+    const NodeSplit sp = node_split(n, shards, n_shards);
+    std::vector<int> devs = node_owners(sp);
+    if (devs.empty()) devs.push_back(0);                 // no shard listed: still validate the program
+    std::vector<std::vector<uint64_t>> cols(n->ctx.size()); std::vector<std::vector<int64_t>> vals(n->ctx.size()); std::vector<uint64_t> tot(n->ctx.size(), 0);
+    rc = node_fan_out(n, devs, [&](int d) {
+        fbgpu_ctx* c = n->ctx[(size_t)d];
+        const auto& s = sp.shards[(size_t)d];
+        std::shared_lock<std::shared_mutex> lk;
+        int r = begin_query(c, lk); if (r) return r;
+        return bsi_sort_run(c, index, ops, n_ops, field, view, bit_depth, s.data(), (int64_t)s.size(), desc != 0, 0, win_end,
+                            cols[(size_t)d], vals[(size_t)d], &tot[(size_t)d]);
+    });
+    if (rc) return rc;
+    struct Pair { int64_t v; uint64_t col; };
+    const auto before = [desc](const Pair& a, const Pair& b) { return a.v != b.v ? (desc ? a.v > b.v : a.v < b.v) : a.col < b.col; };
+    std::vector<Pair> all; uint64_t total = 0;
+    for (int d : devs) {
+        const size_t mid = all.size();
+        for (size_t i = 0; i < cols[(size_t)d].size(); i++) all.push_back(Pair{ vals[(size_t)d][i], cols[(size_t)d][i] });
+        std::inplace_merge(all.begin(), all.begin() + (long)mid, all.end(), before);
+        total += tot[(size_t)d];
+    }
+    if (out_total) *out_total = total;
+    const size_t lo = (size_t)std::min<uint64_t>(offset, all.size()), hi = (size_t)std::min<uint64_t>(win_end, all.size());
+    std::vector<uint64_t> wc(hi - lo); std::vector<int64_t> wv(hi - lo);
+    for (size_t i = lo; i < hi; i++) { wc[i - lo] = all[i].col; wv[i - lo] = all[i].v; }
+    return write_window(wc, wv, out_cols, out_vals, cap, out_n);
+} FBGPU_CATCH
+
 // <bitmap call> returning a Row: every device emits the canonical Pilosa-roaring bytes of its own shards (absolute keys);
 // Row.Merge (row.go:202) of disjoint shard sets is a merge of the container tables by key.  Two passes over the per-device
 // images: sizes, then headers + payloads straight into the caller's buffer.

@@ -855,7 +855,9 @@ class Executor:
         """executeSort :9321 / executeSortShard :9387: the columns of the child row ordered by a field's value — int (values from
         fbgpu_extract), bool (falses then trues), mutex (by row id) — ascending or `sort-desc`, then offset / limit.  The
         reference merges per-shard lists in arrival order, so its order among equal values is unspecified; here ties keep
-        ascending column order.  Returns [(column, value)]."""
+        ascending column order.  A context with bsi_sort orders an int field on the device and returns only the window; other
+        contexts (and a negative offset or limit, which slice the list from its end) extract every value and sort here.
+        Returns [(column, value)]."""
         name = c.args.get("field", c.args.get("_field"))
         if name is None:
             raise QueryError("getting field: Sort(): field required")
@@ -864,6 +866,11 @@ class Executor:
         f = self._field(idx, name)
         desc = bool(c.args.get("sort-desc", False))
         filt = self._bitmap_call(idx, c.children[0])
+        off, lim = int(c.args.get("offset", 0)), c.args.get("limit")
+        if f.type == "int" and hasattr(self.ctx, "bsi_sort") and off >= 0 and (lim is None or int(lim) >= 0):
+            cols, vals, _ = self.ctx.bsi_sort(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, desc=desc, filter_ops=filt, offset=off,
+                                              limit=None if lim is None else int(lim))
+            return [(int(col), int(v) + f.base) for col, v in zip(cols.tolist(), vals.tolist())]
         if f.type == "int":
             cols, vals, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, filter_ops=filt)
             kvs = [(int(col), int(v) + f.base) for col, v in zip(cols.tolist(), vals.tolist())]
@@ -876,9 +883,7 @@ class Executor:
         else:
             raise QueryError(f"Sort of field type {f.type} not implemented yet")
         kvs.sort(key=lambda kv: (-kv[1] if desc else kv[1], kv[0]))
-        off = int(c.args.get("offset", 0))
         kvs = kvs[off:]
-        lim = c.args.get("limit")
         return kvs[:int(lim)] if lim is not None else kvs
 
     percentile_select = True            # False: Percentile always runs the query-driven bisection (the reference's own flow)

@@ -52,7 +52,7 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_node_count_pairs", "fbgpu_node_row_counts", "fbgpu_node_groupby", "fbgpu_node_bsi_sum", "fbgpu_node_bsi_minmax",
            "fbgpu_groupby_values", "fbgpu_node_groupby_values", "fbgpu_row_counts_views", "fbgpu_node_row_counts_views", "fbgpu_groupby_views",
            "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum",
-           "fbgpu_groupby_distinct", "fbgpu_topn_cutoffs", "fbgpu_node_topn_cutoffs"]
+           "fbgpu_groupby_distinct", "fbgpu_topn_cutoffs", "fbgpu_node_topn_cutoffs", "fbgpu_bsi_sort", "fbgpu_node_bsi_sort"]
 
 
 def lib_path():
@@ -90,6 +90,8 @@ def load():
     L.fbgpu_columns.argtypes, L.fbgpu_columns.restype = [vp, u32, vp, i32, vp, i64, u64, i64, vp, u64, C.POINTER(u64), C.POINTER(u64)], C.c_int
     L.fbgpu_extract.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, u64, i64, vp, vp, u64, C.POINTER(u64), C.POINTER(u64)]
     L.fbgpu_extract.restype = C.c_int
+    L.fbgpu_bsi_sort.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, i32, u64, i64, vp, vp, u64, C.POINTER(u64), C.POINTER(u64)]
+    L.fbgpu_bsi_sort.restype = C.c_int
     L.fbgpu_bsi_minmax.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, i32, C.POINTER(C.c_int64), C.POINTER(u64)]
     L.fbgpu_bsi_minmax.restype = C.c_int
     L.fbgpu_bsi_sum.argtypes, L.fbgpu_bsi_sum.restype = [vp, u32, vp, i32, u32, u32, i32, vp, i64, C.POINTER(C.c_int64), C.POINTER(u64)], C.c_int
@@ -130,7 +132,7 @@ def load():
     L.fbgpu_node_devices.argtypes, L.fbgpu_node_devices.restype = [vp], i32
     L.fbgpu_node_owner.argtypes, L.fbgpu_node_owner.restype = [vp, u64], i32
     L.fbgpu_node_ctx.argtypes, L.fbgpu_node_ctx.restype = [vp, i32], vp
-    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "groupby_sum", "bsi_sum", "bsi_minmax", "topn_cutoffs"):
+    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "groupby_sum", "bsi_sum", "bsi_minmax", "topn_cutoffs", "bsi_sort"):
         src, dst = getattr(L, "fbgpu_" + name), getattr(L, "fbgpu_node_" + name)
         dst.argtypes, dst.restype = src.argtypes, src.restype
     L.fbgpu_node_row_counts.argtypes, L.fbgpu_node_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
@@ -365,6 +367,27 @@ class Context:
                 cap = int(n.value)
                 continue
             self._check(rc)
+            return cols[: n.value].copy(), vals[: n.value].copy(), total.value
+
+    def bsi_sort(self, index, field, view, bit_depth, shards, desc=False, filter_ops=None, offset=0, limit=None):
+        """Sort over an int field on the device: (column ids, int64 values relative to the field's Base, number of columns with a
+        value under the filter) for the [offset, offset + limit) window of <filter> ∩ not-null ordered by value, ascending or
+        descending (`desc`), ties by ascending column.  bit_depth 0..64"""
+        sh = _u64arr(shards)
+        arr = ops_array(filter_ops) if filter_ops else None
+        nf = len(filter_ops) if filter_ops else 0
+        n, total = C.c_uint64(0), C.c_uint64(0)
+        cap = max(getattr(self, "_col_cap", 0), 1 << 16) if limit is None else max(min(int(limit), 1 << 16), 1)     # (a limit may exceed the row)
+        while True:
+            cols, vals = np.empty(cap, dtype=np.uint64), np.empty(cap, dtype=np.int64)
+            rc = self.L.fbgpu_bsi_sort(self.h, index, arr, nf, field, view, int(bit_depth), sh.ctypes.data, len(sh), 1 if desc else 0, int(offset),
+                                       -1 if limit is None else int(limit), cols.ctypes.data, vals.ctypes.data, cap, C.byref(n), C.byref(total))
+            if rc == E_NOSPACE:
+                cap = int(n.value)
+                continue
+            self._check(rc)
+            if limit is None:
+                self._col_cap = cap
             return cols[: n.value].copy(), vals[: n.value].copy(), total.value
 
     def bsi_minmax(self, index, field, view, bit_depth, shards, want_max, filter_ops=None):

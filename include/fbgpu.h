@@ -180,6 +180,29 @@ int fbgpu_extract(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n
                   const uint64_t *shards, int64_t n_shards, uint64_t offset, int64_t limit,
                   uint64_t *out_cols, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
 
+/* Sort(<filter>, field=, sort-desc=, offset=, limit=) over an int field (executeSort / executeSortShard executor.go:9321-9560):
+ * the row of fbgpu_extract, put in order on the device, and only a window of it returned.
+ *   - The row is <filter program> ∩ not-null(field), exactly as for fbgpu_extract (n_ops == 0: every column that has a value);
+ *     *out_total = |row| (when out_total is not NULL).
+ *   - The order is ascending by stored value (value - Base, read from the planes as fbgpu_extract reads them, INT64_MIN included
+ *     at depth 64), ties in ascending column order.  desc != 0: descending by value, ties still in ascending column order.  A
+ *     sign with magnitude 0 is the value 0 and sorts among the other zeros by column.
+ *   - The window is [offset, offset + limit) of that order; limit < 0 means no limit.  out_cols[i] / out_vals[i] receive its
+ *     i-th (column, stored value) pair, *out_n its size.  Same capacity contract as fbgpu_columns: a cap smaller than the
+ *     window is FBGPU_E_NOSPACE with nothing written and *out_n = the size needed.
+ *   - bit_depth 0..64.
+ *   - Local to the context: never reduced over a communicator.  Ranks merge their lists as SortedRow.Merge does, so a caller
+ *     asks each rank for offset 0 and limit offset + limit and cuts the window after the merge.
+ *   - Device memory: the call holds at most max(2K, K + 2^24) (key, column) pairs of 32 bytes (both halves of the radix sort),
+ *     K = offset + limit, or the whole row without a limit; FBGPU_E_NOMEM when that cannot be allocated.
+ *   - NULL pointers, a non-zero cap with NULL outputs, n_shards < 0 or n_ops < 0 ("null argument") and a bit_depth outside
+ *     0..64 are FBGPU_E_INVALID, reported before the device check.
+ * The node form runs each device with offset 0 and limit offset + limit (saturating), merges the devices' lists in the same
+ * order (their columns are disjoint) and cuts the window, under the same contracts. */
+int fbgpu_bsi_sort(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
+                   const uint64_t *shards, int64_t n_shards, int32_t desc, uint64_t offset, int64_t limit,
+                   uint64_t *out_cols, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
+
 /* Min / Max of an int field over a row (executeMin :1225 / executeMax :1261, fragment.min / max fragment.go:752-838): the row
  * is <filter program> ∩ not-null(field) (n_ops == 0: every column with a value).  *out_val receives the extreme stored
  * value, i.e. value - bsiGroup.Base (the caller adds Base), *out_count how many columns hold it — the reference's ValCount;
@@ -469,6 +492,9 @@ int fbgpu_node_bsi_sum(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, in
                        const uint64_t *shards, int64_t n_shards, int64_t *out_sum, uint64_t *out_count);
 int fbgpu_node_bsi_minmax(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                           const uint64_t *shards, int64_t n_shards, int32_t want_max, int64_t *out_val, uint64_t *out_count);
+int fbgpu_node_bsi_sort(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
+                        const uint64_t *shards, int64_t n_shards, int32_t desc, uint64_t offset, int64_t limit,
+                        uint64_t *out_cols, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
 
 /* Inspection (any context): the stack-machine program the library would run for `ops` -- records of 16 bytes {u8 op, u8 pad[3],
  * u32 view slot, u64 row} (csrc/fbgpu_types.h DevOp); *out_depth = operand stack depth.  With index == 0xffffffff,
