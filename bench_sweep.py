@@ -1015,13 +1015,91 @@ def config_sort(args, out):
     real.close()
 
 
+class _NoBsiDistinct(_KernelMs):
+    """the same proxy without bsi_distinct: the executor extracts every value of the row and takes the distinct set on the host"""
+
+    def __getattr__(self, name):
+        if name == "bsi_distinct":
+            raise AttributeError(name)
+        return super().__getattr__(name)
+
+
+DISTINCT_QUERIES = ["Distinct(field=v)",                                  # every record, nearly every value distinct
+                    "Distinct(Row(f=0), field=v)",                        # the 1 % row
+                    "Count(Distinct(field=w))",                           # every record, 64 values
+                    "GroupBy(Rows(w))"]                                   # w's values, then one groupby_mixed call
+
+
+def config_distinct(args, out):
+    """Distinct over config X's data (10 M records of a 32-bit field v, a 1 % row f=0) plus a field w of 64 values on the same
+    columns, through the executor: the device arm (one fbgpu_bsi_distinct per value list) and the composition arm (fbgpu_extract
+    of every value of the row, then np.unique), alternated step by step; the composition runs --composition-steps steps.  Both
+    arms must return the same result."""
+    from featurebase_b200 import datagen as D, executor as X
+    n_rec = min(10_000_000, args.shards * SW)
+    n_sh = (n_rec + SW - 1) // SW
+    shards = np.arange(n_sh, dtype=np.uint64)
+    h = X.Holder()
+    idx = h.create_index("i", track_existence=False)
+    f = idx.create_field("f")
+    v = idx.create_field("v", "int", min=0, max=(1 << 32) - 1)
+    w = idx.create_field("w", "int", min=0, max=63)
+    bulk = D.fragments(11, shards, [0], 0.01)
+    h.ctx.load_fragments(idx.id, f.id, X.VIEW_STANDARD, shards, bulk.buf, bulk.offsets)
+    for s in range(n_sh):
+        n_cols = min(SW, n_rec - s * SW)
+        h.ctx.load_fragment(idx.id, v.id, X.VIEW_BSI, s, D.bsi_fragment(12, s, n_cols, v.bit_depth, 0, (1 << 32) - 1))
+        h.ctx.load_fragment(idx.id, w.id, X.VIEW_BSI, s, D.bsi_fragment(13, s, n_cols, w.bit_depth, 0, 63))
+    h.ctx.commit()
+    idx.shards.update(range(n_sh))
+    real = h.ctx
+    card = _card()
+    arms = {"device": _KernelMs(real), "composition": _NoBsiDistinct(real)}
+    for q in DISTINCT_QUERIES:
+        rec = {name: {"wall": [], "kernel_ms": [], "queries": []} for name in arms}
+        res = {}
+        for i in range(1 + args.steps):                      # one warm-up round of the device arm, then alternate the arms
+            for name in (sorted(arms) if i % 2 == 0 else sorted(arms, reverse=True)):
+                if name == "composition" and len(rec[name]["wall"]) >= args.composition_steps:
+                    continue
+                h.ctx = arms[name]
+                q0, arms[name].ms = real.counters()["queries"], 0.0
+                t0 = time.perf_counter()
+                r = X.Executor(h).execute("i", q)[0]
+                wall = (time.perf_counter() - t0) * 1e3
+                res.setdefault(name, r)
+                assert r == res[name], (q, name)
+                print(f"config U: {q}, {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                if i >= 1 or name == "composition":
+                    rec[name]["wall"].append(wall)
+                    rec[name]["kernel_ms"].append(arms[name].ms)
+                    rec[name]["queries"].append(real.counters()["queries"] - q0)
+        h.ctx = real
+        equal = res.get("composition") == res["device"] if "composition" in res else None
+        assert equal is not False, q
+        r = res["device"]
+        size = r.count() if isinstance(r, X.SignedRow) else len(r) if isinstance(r, list) else int(r)
+        for name, d in rec.items():
+            if not d["wall"]:
+                continue
+            out({"config": "U", "query": q, "arm": name, "gpu": card, "records": n_rec, "shards": n_sh, "result_size": size,
+                 "equal_to_composition": equal, "wall_ms": float(np.median(d["wall"])), "wall_ms_min": float(np.min(d["wall"])),
+                 "wall_ms_max": float(np.max(d["wall"])), "kernel_ms": float(np.median(d["kernel_ms"])), "queries": int(np.median(d["queries"])),
+                 "steps": len(d["wall"]),
+                 "kernel": ("eval_kernel + extract_values_kernel + sort_keys_kernel + sort_{hist,scan,scatter}_kernel + distinct_{heads,compact}_kernel"
+                            if name == "device" else "eval_kernel + columns_emit_kernel + extract_values_kernel, host np.unique"),
+                 "note": "median over the timed steps of the executor call (wall clock), of the summed last_query_gpu_ms and of the "
+                         "number of its library queries; result_size: values listed, the count, or groups"})
+    real.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", default="5,3,4")
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--shards", type=int, default=1024)
     ap.add_argument("--groupby-shards", type=int, default=512)
-    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D, N, O: steps of the composition arm")
+    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D, N, O, U: steps of the composition arm")
     ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S, D, N: shards of the composition arm and of the device arm timed beside it")
     ap.add_argument("--topn-rows", type=int, default=1 << 14, help="config N: rows of the TopN field")
     ap.add_argument("--topn-shards", type=int, default=16, help="config N: shards (the fragments are encoded in Python: ~5 s per shard)")
@@ -1055,6 +1133,8 @@ def main():
             config_topn_cutoffs(args, out)
         elif c == "O":
             config_sort(args, out)
+        elif c == "U":
+            config_distinct(args, out)
         elif c == "3L":     # the same BSI query at 256 shards (268 M records, 1.1 GB of planes): shows the kernel away from the launch-bound regime
             config3(args, out, n_rec=256 * SW, nf=1)
         else:

@@ -1372,23 +1372,26 @@ constexpr uint64_t kSortChunk = 1ull << 24;
 
 static uint64_t sat_add(uint64_t a, uint64_t b) { return a + b < a ? ~0ull : a + b; }
 
-// w->d_sort as two halves of `cap` (key, column) pairs, [keys | columns] each, for the radix sort's ping-pong; half `cur` holds
-// the n pairs kept so far.  The buffer outlives the call, like the workspace's other buffers.
+// w->d_sort as two halves of `cap` elements for the radix sort's ping-pong; half `cur` holds the n kept so far.  An element is a
+// (key, column) pair, [keys | columns] in each half, 32 bytes over both halves, or with keys_only (fbgpu_bsi_distinct) a key
+// alone, 16 bytes.  The buffer outlives the call, like the workspace's other buffers.
 struct SortPairs {
-    Workspace* w; uint64_t bound; uint64_t cap, n = 0; int cur = 0;
-    SortPairs(Workspace* ws, uint64_t max_pairs) : w(ws), bound(max_pairs), cap(ws->d_sort.cap / 32) {}
-    unsigned long long* keys(int h) const { return (unsigned long long*)w->d_sort.p + (size_t)h * 2 * cap; }
-    unsigned long long* cols(int h) const { return keys(h) + cap; }
-    // room for `need` pairs (need <= bound); a buffer that has to grow takes the kept pairs along into its half 0
+    Workspace* w; uint64_t bound; uint64_t words; uint64_t cap, n = 0; int cur = 0;
+    SortPairs(Workspace* ws, uint64_t max_pairs, bool keys_only = false)
+        : w(ws), bound(max_pairs), words(keys_only ? 1 : 2), cap(ws->d_sort.cap / (16 * words)) {}
+    bool keys_only() const { return words == 1; }
+    unsigned long long* keys(int h) const { return (unsigned long long*)w->d_sort.p + (size_t)h * words * cap; }
+    unsigned long long* cols(int h) const { return keys_only() ? nullptr : keys(h) + cap; }
+    // room for `need` elements (need <= bound); a buffer that has to grow takes the kept ones along into its half 0
     int reserve(uint64_t need) {
         if (need <= cap) return 0;
         if (need > 0xffffffffull) return fail(FBGPU_E_NOMEM, "the sort would hold %llu pairs on the device: more than 2^32", (unsigned long long)need);
         const uint64_t nc = std::min(std::max(need, cap + cap / 2), bound);
         DevBuf nb;
-        if (nb.ensure((size_t)nc * 32)) return FBGPU_E_NOMEM;
+        if (nb.ensure((size_t)nc * 16 * words)) return FBGPU_E_NOMEM;
         if (n) {
             CUDA_TRY(cudaMemcpyAsync(nb.p, keys(cur), n * 8, cudaMemcpyDeviceToDevice, w->stream));
-            CUDA_TRY(cudaMemcpyAsync((unsigned long long*)nb.p + nc, cols(cur), n * 8, cudaMemcpyDeviceToDevice, w->stream));
+            if (!keys_only()) CUDA_TRY(cudaMemcpyAsync((unsigned long long*)nb.p + nc, cols(cur), n * 8, cudaMemcpyDeviceToDevice, w->stream));
             CUDA_TRY(cudaStreamSynchronize(w->stream));
         }
         w->d_sort.release(); w->d_sort = nb; cap = nc; cur = 0;
@@ -1396,7 +1399,7 @@ struct SortPairs {
     }
 };
 
-// stable sort of the kept pairs by the low `bits` bits of their keys (8-bit digits, least significant first), then the first
+// stable sort of the kept elements by the low `bits` bits of their keys (8-bit digits, least significant first), then the first
 // `keep` of them kept
 static int sort_pairs(Query& q, SortPairs& sp, int bits, uint64_t keep) {
     Workspace* w = q.w;
@@ -1409,14 +1412,55 @@ static int sort_pairs(Query& q, SortPairs& sp, int bits, uint64_t keep) {
         CUDA_TRY(cudaGetLastError());
         sort_scan_kernel<<<1, kSortScanThreads, 0, w->stream>>>(counts, m);
         CUDA_TRY(cudaGetLastError());
-        sort_scatter_kernel<<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(sp.keys(sp.cur), sp.cols(sp.cur), sp.n, shift, counts,
-                                                                              sp.keys(1 - sp.cur), sp.cols(1 - sp.cur));
+        if (sp.keys_only())
+            sort_scatter_kernel<true><<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(sp.keys(sp.cur), nullptr, sp.n, shift, counts, sp.keys(1 - sp.cur), nullptr);
+        else
+            sort_scatter_kernel<false><<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(sp.keys(sp.cur), sp.cols(sp.cur), sp.n, shift, counts,
+                                                                                         sp.keys(1 - sp.cur), sp.cols(1 - sp.cur));
         CUDA_TRY(cudaGetLastError());
         q.launches += 3;
         sp.cur = 1 - sp.cur;
     }
     sp.n = std::min(sp.n, keep);
     return 0;
+}
+
+// the chunk of one batch's emit units that starts at units[a]: units [a, b) holding at most kSortChunk columns (at least one
+// unit), re-based to out_off 0 in `chunk`.  Returns b; *cn = the chunk's columns.
+static size_t next_chunk(const std::vector<ColUnit>& units, size_t a, uint64_t batch_out, std::vector<ColUnit>& chunk, uint64_t* cn) {
+    const uint64_t base = units[a].out_off;
+    size_t b = a + 1;
+    while (b < units.size() && units[b].out_off + (units[b].last - units[b].first) - base <= kSortChunk) b++;
+    *cn = (b < units.size() ? units[b].out_off : batch_out) - base;
+    chunk.assign(units.begin() + (long)a, units.begin() + (long)b);
+    for (ColUnit& cu : chunk) cu.out_off -= base;
+    return b;
+}
+
+// one chunk's cn sort keys to keys_out (sort_keys_kernel from extract_values_kernel's magnitudes and signs) and, unless
+// cols_out is NULL, its columns to cols_out (columns_emit_kernel)
+static int emit_sort_keys(Query& q, const std::vector<ColUnit>& chunk, uint64_t cn, uint32_t fv, int depth, bool desc,
+                          unsigned long long* keys_out, unsigned long long* cols_out) {
+    Workspace* w = q.w;
+    // d_emit: magnitudes [cn] u64, then sign bits [ceil(cn / 32)] u32
+    const size_t vb = cn * 8 + ((cn + 31) / 32) * 4;
+    return q.emit_on_device(chunk, vb, [&](const ColUnit* d_units, int n, int grid) {
+        unsigned long long* d_mag = (unsigned long long*)w->d_emit.p;
+        unsigned int* d_sign = (unsigned int*)(d_mag + cn);
+        if (cols_out) {
+            columns_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>((const uint4*)w->d_bitmaps.p, d_units, n, cols_out);
+            CUDA_TRY(cudaGetLastError());
+            q.launches++;
+        }
+        CUDA_TRY(cudaMemsetAsync(d_mag, 0, vb, w->stream));
+        extract_values_kernel<<<grid, kExtractThreads, 0, w->stream>>>(store_ref(q.c), fv, depth, (const uint4*)w->d_bitmaps.p, d_units, n, d_mag, d_sign);
+        CUDA_TRY(cudaGetLastError());
+        const unsigned kgrid = (unsigned)std::min<uint64_t>((cn + kSortThreads - 1) / kSortThreads, (uint64_t)q.c->sm_count * 8);
+        sort_keys_kernel<<<kgrid, kSortThreads, 0, w->stream>>>(d_mag, d_sign, cn, depth, desc ? 1 : 0, keys_out);
+        CUDA_TRY(cudaGetLastError());
+        q.launches += 2;
+        return 0;
+    });
 }
 
 // the pairs [offset, min(win_end, |row|)) of the row <ops> ∩ exists(field) in sort order (store lock held): columns and stored
@@ -1441,31 +1485,11 @@ static int bsi_sort_run(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32
         rc = q.eval_info(u0, nu, info); if (rc) return rc;
         const uint64_t batch_out = col_units(info, u0, nu, sorted, 0, ~0ull, seen, units);
         for (size_t a = 0; a < units.size();) {
-            const uint64_t base = units[a].out_off;
-            size_t b = a + 1;                               // the chunk: units [a, b), at least one
-            while (b < units.size() && units[b].out_off + (units[b].last - units[b].first) - base <= kSortChunk) b++;
-            const uint64_t cn = (b < units.size() ? units[b].out_off : batch_out) - base;
-            chunk.assign(units.begin() + (long)a, units.begin() + (long)b);
-            for (ColUnit& cu : chunk) cu.out_off -= base;
+            uint64_t cn;
+            const size_t b = next_chunk(units, a, batch_out, chunk, &cn);
             if (limited && sp.n > K && sp.n + cn > twice_k) { rc = sort_pairs(q, sp, bits, K); if (rc) return rc; }
             rc = sp.reserve(sp.n + cn); if (rc) return rc;
-            // d_emit: magnitudes [cn] u64, then sign bits [ceil(cn / 32)] u32
-            const size_t vb = cn * 8 + ((cn + 31) / 32) * 4;
-            rc = q.emit_on_device(chunk, vb, [&](const ColUnit* d_units, int n, int grid) {
-                unsigned long long* d_mag = (unsigned long long*)w->d_emit.p;
-                unsigned int* d_sign = (unsigned int*)(d_mag + cn);
-                columns_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>((const uint4*)w->d_bitmaps.p, d_units, n, sp.cols(sp.cur) + sp.n);
-                CUDA_TRY(cudaGetLastError());
-                CUDA_TRY(cudaMemsetAsync(d_mag, 0, vb, w->stream));
-                extract_values_kernel<<<grid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv, depth, (const uint4*)w->d_bitmaps.p, d_units, n, d_mag, d_sign);
-                CUDA_TRY(cudaGetLastError());
-                const unsigned kgrid = (unsigned)std::min<uint64_t>((cn + kSortThreads - 1) / kSortThreads, (uint64_t)c->sm_count * 8);
-                sort_keys_kernel<<<kgrid, kSortThreads, 0, w->stream>>>(d_mag, d_sign, cn, depth, desc ? 1 : 0, sp.keys(sp.cur) + sp.n);
-                CUDA_TRY(cudaGetLastError());
-                q.launches += 3;
-                return 0;
-            });
-            if (rc) return rc;
+            rc = emit_sort_keys(q, chunk, cn, fv, depth, desc, sp.keys(sp.cur) + sp.n, sp.cols(sp.cur) + sp.n); if (rc) return rc;
             sp.n += cn;
             a = b;
         }
@@ -1525,6 +1549,104 @@ extern "C" int fbgpu_bsi_sort(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops,
     if (rc) return rc;
     if (out_total) *out_total = total;
     return write_window(cols, vals, out_cols, out_vals, cap, out_n);
+} FBGPU_CATCH
+
+// ------------------------------------------------------------------ Distinct values of an int field (the sort on keys alone, then one key per run)
+// The row is evaluated batch by batch and emitted in chunks as for fbgpu_bsi_sort, keys only (sort_keys_kernel, ascending).  Before
+// a chunk that would take the buffer past twice the U distinct keys left by the last dedupe, the buffer is sorted and deduped
+// (distinct_heads_kernel, sort_scan_kernel, distinct_compact_kernel); once more at the end, and only the U keys are read back.
+
+// sorts the kept keys and keeps the first of each run of equal keys: sk.n becomes the number of distinct keys
+static int distinct_keys(Query& q, SortPairs& sk, int bits) {
+    int rc = sort_pairs(q, sk, bits, ~0ull); if (rc) return rc;
+    if (sk.n == 0) return 0;
+    Workspace* w = q.w;
+    const uint64_t n_tiles = (sk.n + kSortTile - 1) / kSortTile;
+    if (w->d_counts.ensure((size_t)(n_tiles + 1) * 4) || w->h_out.ensure(8)) return FBGPU_E_NOMEM;
+    unsigned int* counts = (unsigned int*)w->d_counts.p;                    // [n_tiles] heads per tile, then their total
+    distinct_heads_kernel<<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(sk.keys(sk.cur), sk.n, counts);
+    CUDA_TRY(cudaGetLastError());
+    sort_scan_kernel<<<1, kSortScanThreads, 0, w->stream>>>(counts, n_tiles + 1);
+    CUDA_TRY(cudaGetLastError());
+    distinct_compact_kernel<<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(sk.keys(sk.cur), sk.n, counts, sk.keys(1 - sk.cur));
+    CUDA_TRY(cudaGetLastError());
+    q.launches += 3;
+    sk.cur = 1 - sk.cur;
+    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, counts + n_tiles, 4, cudaMemcpyDeviceToHost, w->stream));
+    CUDA_TRY(cudaStreamSynchronize(w->stream));
+    sk.n = *(const unsigned int*)w->h_out.p;
+    return 0;
+}
+
+// the distinct stored values of the row <ops> ∩ exists(field), ascending, into vals (store lock held); |row| into *total
+static int bsi_distinct_run(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int depth,
+                            const uint64_t* shards, int64_t n_shards, std::vector<int64_t>& vals, uint64_t* total) {
+    const std::vector<fbgpu_op> full = and_row(ops, n_ops, field, view, 0);    // as for fbgpu_extract
+    const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
+    Query q(c); Workspace* w = q.w;
+    const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);
+    int rc = q.open(index, full.data(), (int32_t)full.size(), sorted.data(), (int64_t)sorted.size()); if (rc) return rc;
+    const int bits = sort_key_bits(depth);
+    SortPairs sk(w, kSortChunk, true);              // bound: max(2U, U + kSortChunk) keys, U the distinct keys after the last dedupe
+    uint64_t u = 0, seen = 0;
+    std::vector<ColUnit> units, chunk;
+    for (long long u0 = 0; u0 < q.n_units; u0 += c->unit_batch) {
+        const long long nu = std::min(c->unit_batch, q.n_units - u0);
+        const uint2* info;
+        rc = q.eval_info(u0, nu, info); if (rc) return rc;
+        const uint64_t batch_out = col_units(info, u0, nu, sorted, 0, ~0ull, seen, units);
+        for (size_t a = 0; a < units.size();) {
+            uint64_t cn;
+            const size_t b = next_chunk(units, a, batch_out, chunk, &cn);
+            if (sk.n > u && sk.n + cn > sat_add(u, u)) {
+                rc = distinct_keys(q, sk, bits); if (rc) return rc;
+                u = sk.n;
+                sk.bound = std::max(sat_add(u, u), sat_add(u, kSortChunk));
+            }
+            rc = sk.reserve(sk.n + cn); if (rc) return rc;
+            rc = emit_sort_keys(q, chunk, cn, fv, depth, false, sk.keys(sk.cur) + sk.n, nullptr); if (rc) return rc;
+            sk.n += cn;
+            a = b;
+        }
+        CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        q.add_elapsed();
+    }
+    *total = seen;
+    CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
+    rc = distinct_keys(q, sk, bits); if (rc) return rc;
+    const uint64_t cnt = sk.n;
+    if (w->h_out.ensure(std::max<size_t>(cnt * 8, 8))) return FBGPU_E_NOMEM;
+    if (cnt) CUDA_TRY(cudaMemcpyAsync(w->h_out.p, sk.keys(sk.cur), cnt * 8, cudaMemcpyDeviceToHost, w->stream));
+    CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+    CUDA_TRY(cudaStreamSynchronize(w->stream));
+    q.add_elapsed();
+    const uint64_t* h_keys = (const uint64_t*)w->h_out.p;
+    vals.resize(cnt);
+    for (uint64_t i = 0; i < cnt; i++)                   // sort_keys_kernel backwards, as in bsi_sort_run
+        vals[i] = (int64_t)(depth < 64 ? h_keys[i] - (1ull << depth) : h_keys[i] ^ (1ull << 63));
+    q.finish();
+    return FBGPU_OK;
+}
+
+// a value list into the caller's array under the NOSPACE contract: *out_n = its size, nothing written when it exceeds cap
+static int write_values(const std::vector<int64_t>& vals, int64_t* out_vals, uint64_t cap, uint64_t* out_n) {
+    *out_n = vals.size();
+    if (vals.size() > cap) return fail(FBGPU_E_NOSPACE, "output needs room for %llu values", (unsigned long long)vals.size());
+    if (!vals.empty()) memcpy(out_vals, vals.data(), vals.size() * 8);
+    return FBGPU_OK;
+}
+
+extern "C" int fbgpu_bsi_distinct(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
+                                  const uint64_t* shards, int64_t n_shards, int64_t* out_vals, uint64_t cap, uint64_t* out_n, uint64_t* out_total) try {
+    // fbgpu_bsi_sort's checks, out_vals being the only output array
+    int rc = bsi_sort_args(c, ops, n_ops, bit_depth, shards, n_shards, (const uint64_t*)out_vals, out_vals, cap, out_n); if (rc) return rc;
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    std::vector<int64_t> vals; uint64_t total = 0;
+    rc = bsi_distinct_run(c, index, ops, n_ops, field, view, bit_depth, shards, n_shards, vals, &total); if (rc) return rc;
+    if (out_total) *out_total = total;
+    return write_values(vals, out_vals, cap, out_n);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ BSI Min / Max (one pass over the planes)

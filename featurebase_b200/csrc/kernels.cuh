@@ -1385,7 +1385,9 @@ sort_scan_kernel(unsigned int* __restrict__ counts, unsigned long long m) {
 // the stable scatter of one pass: tile t's pairs with digit d go to [counts[d * n_tiles + t], ...) in their input order.  Per
 // round of kSortThreads pairs each warp splits its 32 pairs by digit with eight ballots (a warp multisplit: the lanes that agree
 // with this lane on every digit bit); the lowest lane of each group publishes the group's size, and one thread per digit turns
-// the eight warps' sizes into offsets after the tile's running offset for that digit.
+// the eight warps' sizes into offsets after the tile's running offset for that digit.  kKeysOnly (fbgpu_bsi_distinct): keys
+// without columns; cols_in / cols_out are not touched.
+template <bool kKeysOnly>
 __global__ void __launch_bounds__(kSortThreads)
 sort_scatter_kernel(const unsigned long long* __restrict__ keys_in, const unsigned long long* __restrict__ cols_in, unsigned long long n, int shift,
                     const unsigned int* __restrict__ counts, unsigned long long* __restrict__ keys_out, unsigned long long* __restrict__ cols_out) {
@@ -1400,7 +1402,7 @@ sort_scatter_kernel(const unsigned long long* __restrict__ keys_in, const unsign
         const unsigned long long i = t0 + (unsigned long long)r * kSortThreads + tid;
         const bool valid = i < n;
         unsigned long long key = 0, col = 0;
-        if (valid) { key = keys_in[i]; col = cols_in[i]; }
+        if (valid) { key = keys_in[i]; if (!kKeysOnly) col = cols_in[i]; }
         const unsigned int d = (unsigned int)(key >> shift) & 255u;
         unsigned int peers = __ballot_sync(0xffffffffu, valid);
 #pragma unroll
@@ -1420,9 +1422,67 @@ sort_scatter_kernel(const unsigned long long* __restrict__ keys_in, const unsign
         __syncthreads();
         if (valid) {
             const unsigned int pos = wcnt[wid][d] + (unsigned int)__popc(peers & lt);
-            keys_out[pos] = key; cols_out[pos] = col;
+            keys_out[pos] = key;
+            if (!kKeysOnly) cols_out[pos] = col;
         }
         __syncthreads();                                   // (wcnt is cleared by the next round)
+    }
+}
+
+// ------------------------------------------------------------------ Distinct values of an int field (fbgpu_bsi_distinct)
+// The keys of sort_keys_kernel (ascending), sorted by the radix sort above without columns, keep one key per run of equal keys:
+// a per-tile count of run heads (i == 0 or keys[i] != keys[i - 1]), sort_scan_kernel over the tile counts, and a compaction
+// that writes each tile's heads in order from the tile's offset.  Tiles are the sort's kSortTile keys.
+
+// counts[t] = the run heads of tile t; block 0 also zeroes counts[n_tiles], which the exclusive scan turns into the total
+__global__ void __launch_bounds__(kSortThreads)
+distinct_heads_kernel(const unsigned long long* __restrict__ keys, unsigned long long n, unsigned int* __restrict__ counts) {
+    __shared__ unsigned int wsum[kSortThreads / 32];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const unsigned long long t0 = (unsigned long long)blockIdx.x * kSortTile;
+    unsigned int c = 0;
+    for (int r = 0; r < kSortRounds; r++) {
+        const unsigned long long i = t0 + (unsigned long long)r * kSortThreads + tid;
+        const bool head = i < n && (i == 0 || keys[i] != keys[i - 1]);
+        c += (unsigned int)__popc(__ballot_sync(0xffffffffu, head));
+    }
+    if (lane == 0) wsum[wid] = c;
+    __syncthreads();
+    if (tid == 0) {
+        unsigned int s = 0;
+        for (int k = 0; k < kSortThreads / 32; k++) s += wsum[k];
+        counts[blockIdx.x] = s;
+        if (blockIdx.x == 0) counts[gridDim.x] = 0;
+    }
+}
+
+// the heads of tile t in input order to keys_out[offs[t] ...]: per round each warp ranks its heads by ballot, and one thread
+// turns the eight warps' head counts into offsets after the tile's running offset
+__global__ void __launch_bounds__(kSortThreads)
+distinct_compact_kernel(const unsigned long long* __restrict__ keys_in, unsigned long long n, const unsigned int* __restrict__ offs,
+                        unsigned long long* __restrict__ keys_out) {
+    __shared__ unsigned int wbase[kSortThreads / 32];
+    __shared__ unsigned int run;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const unsigned int lt = (1u << lane) - 1u;
+    if (tid == 0) run = offs[blockIdx.x];
+    const unsigned long long t0 = (unsigned long long)blockIdx.x * kSortTile;
+    for (int r = 0; r < kSortRounds; r++) {
+        const unsigned long long i = t0 + (unsigned long long)r * kSortThreads + tid;
+        unsigned long long key = 0;
+        bool head = false;
+        if (i < n) { key = keys_in[i]; head = i == 0 || key != keys_in[i - 1]; }
+        const unsigned int bal = __ballot_sync(0xffffffffu, head);
+        if (lane == 0) wbase[wid] = (unsigned int)__popc(bal);
+        __syncthreads();
+        if (tid == 0) {
+            unsigned int o = run;
+            for (int k = 0; k < kSortThreads / 32; k++) { const unsigned int x = wbase[k]; wbase[k] = o; o += x; }
+            run = o;
+        }
+        __syncthreads();
+        if (head) keys_out[wbase[wid] + (unsigned int)__popc(bal & lt)] = key;
+        __syncthreads();                                   // (wbase is rewritten by the next round)
     }
 }
 

@@ -406,6 +406,35 @@ extern "C" int fbgpu_node_bsi_sort(fbgpu_node* n, uint32_t index, const fbgpu_op
     return write_window(wc, wv, out_cols, out_vals, cap, out_n);
 } FBGPU_CATCH
 
+// Distinct over an int field: every device lists the distinct values of its own shards; the lists merge by union, as
+// SignedRow.Union does (executeDistinct executor.go:1173), and the totals add up
+extern "C" int fbgpu_node_bsi_distinct(fbgpu_node* n, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
+                                       const uint64_t* shards, int64_t n_shards, int64_t* out_vals, uint64_t cap, uint64_t* out_n, uint64_t* out_total) try {
+    int rc = bsi_sort_args(n, ops, n_ops, bit_depth, shards, n_shards, (const uint64_t*)out_vals, out_vals, cap, out_n); if (rc) return rc;
+    const NodeSplit sp = node_split(n, shards, n_shards);
+    std::vector<int> devs = node_owners(sp);
+    if (devs.empty()) devs.push_back(0);                 // no shard listed: still validate the program
+    std::vector<std::vector<int64_t>> vals(n->ctx.size()); std::vector<uint64_t> tot(n->ctx.size(), 0);
+    rc = node_fan_out(n, devs, [&](int d) {
+        fbgpu_ctx* c = n->ctx[(size_t)d];
+        const auto& s = sp.shards[(size_t)d];
+        std::shared_lock<std::shared_mutex> lk;
+        int r = begin_query(c, lk); if (r) return r;
+        return bsi_distinct_run(c, index, ops, n_ops, field, view, bit_depth, s.data(), (int64_t)s.size(), vals[(size_t)d], &tot[(size_t)d]);
+    });
+    if (rc) return rc;
+    std::vector<int64_t> all; uint64_t total = 0;
+    for (int d : devs) {
+        const size_t mid = all.size();
+        all.insert(all.end(), vals[(size_t)d].begin(), vals[(size_t)d].end());
+        std::inplace_merge(all.begin(), all.begin() + (long)mid, all.end());
+        all.erase(std::unique(all.begin(), all.end()), all.end());
+        total += tot[(size_t)d];
+    }
+    if (out_total) *out_total = total;
+    return write_values(all, out_vals, cap, out_n);
+} FBGPU_CATCH
+
 // <bitmap call> returning a Row: every device emits the canonical Pilosa-roaring bytes of its own shards (absolute keys);
 // Row.Merge (row.go:202) of disjoint shard sets is a merge of the container tables by key.  Two passes over the per-device
 // images: sizes, then headers + payloads straight into the caller's buffer.

@@ -758,9 +758,9 @@ class Executor:
         """executeDistinct :1173 / executeDistinctShard :1820.  Set-like field: the ids of the rows that have a bit (under the
         optional filter), executeDistinctShardSet :1952 — one row-count launch.  Int field: the set of values present,
         executeDistinctShardBSI :2034, returned as a SignedRow.  The reference transposes the bit planes column by column;
-        the library does that on the device (fbgpu_extract: the values of the columns of filter ∩ not-null, gathered from the
-        planes in one pass) and the distinct set is taken from the value vector.  `index=` runs the call on another index
-        (foreign-index joins)."""
+        a context with bsi_distinct lists the distinct values of filter ∩ not-null on the device in one call; a context without
+        it gathers every value (fbgpu_extract) and takes the distinct set of the value vector.
+        `index=` runs the call on another index (foreign-index joins)."""
         name = c.args.get("field", c.args.get("_field"))
         if name is None:
             raise QueryError("missing field option in Distinct query")
@@ -781,12 +781,18 @@ class Executor:
         if f.type != "int":
             rid, cnt = self.ctx.row_counts(idx.id, f.id, VIEW_STANDARD, shards, filter_ops=filt)
             return sorted(int(r) for r, n in zip(rid, cnt) if n > 0)
-        _, vals, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, filter_ops=filt)
         pos, neg = set(), set()
-        for m in np.unique(vals).tolist():
+        for m in self._int_values(idx, f, shards, filt).tolist():
             v = int(m) + f.base                                        # value += offset (:2125)
             (neg if v < 0 else pos).add(abs(v))
         return SignedRow(pos, neg)
+
+    def _int_values(self, idx, f, shards, filt):
+        """the distinct stored values (value - Base) of int field f under filt ∩ not-null, ascending int64"""
+        if hasattr(self.ctx, "bsi_distinct"):
+            return self.ctx.bsi_distinct(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, filter_ops=filt)[0]
+        _, vals, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, filter_ops=filt)
+        return np.unique(np.asarray(vals, dtype=np.int64))
 
     def _extract(self, idx, c, shards):
         """executeExtract :4711 / executeExtractShard :4758: the table {column -> per-field cell} for the columns of the first
@@ -1141,11 +1147,10 @@ class Executor:
         parts = [x for x in (filt_call, *agg_distinct.children[:1]) if isinstance(x, pql.Call)]
         both = (parts[0] if len(parts) == 1 else pql.Call("Intersect", {}, parts)) if parts else None
         ops = self._bitmap_call(idx, both) if both is not None else None
-        _, vals, _ = self.ctx.extract(idx.id, xf.id, VIEW_BSI, xf.bit_depth, shards, filter_ops=ops)
-        xs = np.unique(np.asarray(vals, dtype=np.int64))
-        if len(xs) == 0:
-            return np.zeros(shape, dtype=np.uint64)
         try:
+            xs = self._int_values(idx, xf, shards, ops)
+            if len(xs) == 0:
+                return np.zeros(shape, dtype=np.uint64)
             return self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, ops, shards, distinct=(xf, xs))[0]
         except NotImplementedError:
             return None

@@ -52,7 +52,8 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_node_count_pairs", "fbgpu_node_row_counts", "fbgpu_node_groupby", "fbgpu_node_bsi_sum", "fbgpu_node_bsi_minmax",
            "fbgpu_groupby_values", "fbgpu_node_groupby_values", "fbgpu_row_counts_views", "fbgpu_node_row_counts_views", "fbgpu_groupby_views",
            "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum",
-           "fbgpu_groupby_distinct", "fbgpu_topn_cutoffs", "fbgpu_node_topn_cutoffs", "fbgpu_bsi_sort", "fbgpu_node_bsi_sort"]
+           "fbgpu_groupby_distinct", "fbgpu_topn_cutoffs", "fbgpu_node_topn_cutoffs", "fbgpu_bsi_sort", "fbgpu_node_bsi_sort",
+           "fbgpu_bsi_distinct", "fbgpu_node_bsi_distinct"]
 
 
 def lib_path():
@@ -92,6 +93,8 @@ def load():
     L.fbgpu_extract.restype = C.c_int
     L.fbgpu_bsi_sort.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, i32, u64, i64, vp, vp, u64, C.POINTER(u64), C.POINTER(u64)]
     L.fbgpu_bsi_sort.restype = C.c_int
+    L.fbgpu_bsi_distinct.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, vp, u64, C.POINTER(u64), C.POINTER(u64)]
+    L.fbgpu_bsi_distinct.restype = C.c_int
     L.fbgpu_bsi_minmax.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, i32, C.POINTER(C.c_int64), C.POINTER(u64)]
     L.fbgpu_bsi_minmax.restype = C.c_int
     L.fbgpu_bsi_sum.argtypes, L.fbgpu_bsi_sum.restype = [vp, u32, vp, i32, u32, u32, i32, vp, i64, C.POINTER(C.c_int64), C.POINTER(u64)], C.c_int
@@ -132,7 +135,7 @@ def load():
     L.fbgpu_node_devices.argtypes, L.fbgpu_node_devices.restype = [vp], i32
     L.fbgpu_node_owner.argtypes, L.fbgpu_node_owner.restype = [vp, u64], i32
     L.fbgpu_node_ctx.argtypes, L.fbgpu_node_ctx.restype = [vp, i32], vp
-    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "groupby_sum", "bsi_sum", "bsi_minmax", "topn_cutoffs", "bsi_sort"):
+    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "groupby_sum", "bsi_sum", "bsi_minmax", "topn_cutoffs", "bsi_sort", "bsi_distinct"):
         src, dst = getattr(L, "fbgpu_" + name), getattr(L, "fbgpu_node_" + name)
         dst.argtypes, dst.restype = src.argtypes, src.restype
     L.fbgpu_node_row_counts.argtypes, L.fbgpu_node_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
@@ -389,6 +392,25 @@ class Context:
             if limit is None:
                 self._col_cap = cap
             return cols[: n.value].copy(), vals[: n.value].copy(), total.value
+
+    def bsi_distinct(self, index, field, view, bit_depth, shards, filter_ops=None):
+        """Distinct over an int field on the device: (the distinct int64 values relative to the field's Base, ascending, number of
+        columns with a value under the filter) of <filter> ∩ not-null.  bit_depth 0..64"""
+        sh = _u64arr(shards)
+        arr = ops_array(filter_ops) if filter_ops else None
+        nf = len(filter_ops) if filter_ops else 0
+        n, total = C.c_uint64(0), C.c_uint64(0)
+        cap = max(getattr(self, "_distinct_cap", 0), 1 << 16)
+        while True:
+            vals = np.empty(cap, dtype=np.int64)
+            rc = self.L.fbgpu_bsi_distinct(self.h, index, arr, nf, field, view, int(bit_depth), sh.ctypes.data, len(sh), vals.ctypes.data, cap,
+                                           C.byref(n), C.byref(total))
+            if rc == E_NOSPACE:
+                cap = int(n.value)
+                continue
+            self._check(rc)
+            self._distinct_cap = cap
+            return vals[: n.value].copy(), total.value
 
     def bsi_minmax(self, index, field, view, bit_depth, shards, want_max, filter_ops=None):
         """(extreme stored value = value - Base, number of columns holding it) over <filter> ∩ not-null; count 0: empty row.

@@ -203,6 +203,25 @@ int fbgpu_bsi_sort(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t 
                    const uint64_t *shards, int64_t n_shards, int32_t desc, uint64_t offset, int64_t limit,
                    uint64_t *out_cols, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
 
+/* Distinct(<filter>, field=) over an int field (executeDistinct :1173 / executeDistinctShardBSI executor.go:2034): the distinct
+ * stored values of fbgpu_extract's row, found on the device.
+ *   - The row is <filter program> ∩ not-null(field), exactly as for fbgpu_extract (n_ops == 0: every column that has a value);
+ *     *out_total = |row| (when out_total is not NULL).
+ *   - out_vals receives the row's distinct stored values (value - Base, read from the planes as fbgpu_extract reads them),
+ *     strictly ascending as int64, and *out_n their number U.  A sign with magnitude 0 is the value 0; at depth 64 INT64_MIN
+ *     (sign + magnitude 2^63) is included.  The list equals np.unique of fbgpu_extract's values, bit for bit.  Same capacity
+ *     contract as fbgpu_columns: cap < U is FBGPU_E_NOSPACE with nothing written and *out_n = U.
+ *   - bit_depth 0..64.
+ *   - Local to the context: never reduced over a communicator.  Ranks merge their lists by union, as SignedRow.Union does.
+ *   - Device memory: the call holds at most max(2U, U + 2^24) keys of 16 bytes (both halves of the radix sort);
+ *     FBGPU_E_NOMEM when that cannot be allocated.
+ *   - NULL handle or out_n, a non-zero cap with NULL out_vals, n_shards < 0 or n_ops < 0 ("null argument") and a bit_depth
+ *     outside 0..64 are FBGPU_E_INVALID, reported before the device check.
+ * The node form lists each device's values, merges the lists into one ascending list without duplicates and adds up the
+ * totals, under the same contracts. */
+int fbgpu_bsi_distinct(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
+                       const uint64_t *shards, int64_t n_shards, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
+
 /* Min / Max of an int field over a row (executeMin :1225 / executeMax :1261, fragment.min / max fragment.go:752-838): the row
  * is <filter program> ∩ not-null(field) (n_ops == 0: every column with a value).  *out_val receives the extreme stored
  * value, i.e. value - bsiGroup.Base (the caller adds Base), *out_count how many columns hold it — the reference's ValCount;
@@ -495,6 +514,8 @@ int fbgpu_node_bsi_minmax(fbgpu_node *node, uint32_t index, const fbgpu_op *ops,
 int fbgpu_node_bsi_sort(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                         const uint64_t *shards, int64_t n_shards, int32_t desc, uint64_t offset, int64_t limit,
                         uint64_t *out_cols, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
+int fbgpu_node_bsi_distinct(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
+                            const uint64_t *shards, int64_t n_shards, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
 
 /* Inspection (any context): the stack-machine program the library would run for `ops` -- records of 16 bytes {u8 op, u8 pad[3],
  * u32 view slot, u64 row} (csrc/fbgpu_types.h DevOp); *out_depth = operand stack depth.  With index == 0xffffffff,
