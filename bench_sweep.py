@@ -22,6 +22,8 @@
             cardinality, fbgpu_topn_cutoffs against the per-shard count-matrix composition (only when named in --configs).
   config O: Sort over config X's 32-bit field with and without a limit, fbgpu_bsi_sort against extracting every value and
             sorting on the host (only when named in --configs).
+  config E: Extract over a 256-row set field, a 64-row mutex field and a bool field, and Sort over the mutex field, on 512
+            shards, fbgpu_extract_rows against the per-row column-expansion composition (only when named in --configs).
 Every point is spot-checked against the CPU oracle on a few shards (the checker, not the thing measured)."""
 import argparse
 import json
@@ -1093,14 +1095,98 @@ def config_distinct(args, out):
     real.close()
 
 
+class _NoExtractRows(_KernelMs):
+    """the same proxy without extract_rows: the executor lists the field's rows under the filter, then expands the columns of
+    filter ∩ Row(field=r) for every row r"""
+
+    def __getattr__(self, name):
+        if name == "extract_rows":
+            raise AttributeError(name)
+        return super().__getattr__(name)
+
+
+EXTRACT_QUERIES = ["Extract(Row(f=0), Rows(a), Rows(m), Rows(b))",        # the 1 % row, three set-like children
+                   "Extract(Limit(All(), limit=1000, offset=100000), Rows(a))",   # a window of the existence row
+                   "Sort(Row(f=0), field=m, limit=10)"]
+
+
+def config_extract_rows(args, out):
+    """Extract and Sort over set-like fields through the executor, on 512 shards whose first 65,536 columns each hold about 4 of
+    the 256 rows of a set field a, one of the 64 rows of a mutex field m and one row of a bool field b; f=0 holds 1 % of those
+    columns.  Every shard holds the same fragments, encoded once.  The device arm (one fbgpu_extract_rows per set-like child,
+    beside fbgpu_columns for Extract) runs over all shards; the composition arm (fbgpu_row_counts, then fbgpu_columns of
+    filter ∩ Row(field=r) for every row r) over the first --composition-shards shards, for --composition-steps steps alternated
+    with the device arm over the same shards.  Both arms must return the same result.  Progress goes to stderr."""
+    from featurebase_b200 import executor as X, roaring_io
+    S, n_cols = 512, 1 << 16
+    h = X.Holder()
+    idx = h.create_index("i")
+    for name, typ in (("f", "set"), ("a", "set"), ("m", "mutex"), ("b", "bool")):
+        idx.create_field(name, typ)
+    rng = np.random.default_rng(2027)
+    cols = np.arange(n_cols, dtype=np.uint64)
+    a_rows = rng.integers(0, 256, size=(n_cols, 4)).astype(np.uint64)            # duplicates fold: about 3.98 rows per column
+    data = {"a": roaring_io.encode((a_rows * np.uint64(SW) + cols[:, None]).ravel()),
+            "m": roaring_io.encode(rng.integers(0, 64, n_cols).astype(np.uint64) * np.uint64(SW) + cols),
+            "b": roaring_io.encode(rng.integers(0, 2, n_cols).astype(np.uint64) * np.uint64(SW) + cols),
+            "f": roaring_io.encode(np.sort(rng.choice(n_cols, n_cols // 100, replace=False)).astype(np.uint64)),
+            X.EXISTENCE_FIELD: roaring_io.encode(cols)}
+    t0 = time.perf_counter()
+    for s in range(S):
+        for name, d in data.items():
+            h.import_roaring("i", name, X.VIEW_STANDARD, s, d)
+    h.ctx.commit()
+    load_s = time.perf_counter() - t0
+    real = h.ctx
+    card = _card()
+    dev, comp = _KernelMs(real), _NoExtractRows(real)
+    CS = min(S, args.composition_shards)
+    for q in EXTRACT_QUERIES:
+        runs = [(S, {"device": dev})] + ([(CS, {"device": dev, "composition": comp})] if args.composition_steps > 0 else [])
+        for n_sh, arms in runs:
+            sh = list(range(n_sh))
+            rec = {name: {"wall": [], "kernel_ms": [], "queries": []} for name in arms}
+            res = {}
+            for i in range(1 + args.steps):                  # one warm-up round of the device arm, then alternate the arms
+                for name in (sorted(arms) if i % 2 == 0 else sorted(arms, reverse=True)):
+                    if name == "composition" and len(rec[name]["wall"]) >= args.composition_steps:
+                        continue
+                    h.ctx = arms[name]
+                    q0, arms[name].ms = real.counters()["queries"], 0.0
+                    t1 = time.perf_counter()
+                    r = X.Executor(h).execute("i", q, sh)[0]
+                    wall = (time.perf_counter() - t1) * 1e3
+                    res.setdefault(name, r)
+                    assert r == res[name], (q, name)
+                    print(f"config E: {q} over {n_sh} shards, {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                    if i >= 1 or name == "composition":
+                        rec[name]["wall"].append(wall)
+                        rec[name]["kernel_ms"].append(arms[name].ms)
+                        rec[name]["queries"].append(real.counters()["queries"] - q0)
+            h.ctx = real
+            equal = res.get("composition") == res["device"] if "composition" in res else None
+            assert equal is not False, q
+            r = res["device"]
+            size = len(r["columns"]) if isinstance(r, dict) else len(r)
+            for name, d in rec.items():
+                out({"config": "E", "query": q, "arm": name, "gpu": card, "shards": n_sh, "result_size": size, "equal_to_composition": equal,
+                     "wall_ms": float(np.median(d["wall"])), "wall_ms_min": float(np.min(d["wall"])), "wall_ms_max": float(np.max(d["wall"])),
+                     "kernel_ms": float(np.median(d["kernel_ms"])), "queries": int(np.median(d["queries"])), "steps": len(d["wall"]), "load_s": round(load_s, 1),
+                     "kernel": ("eval_kernel + extract_rows_kernel<kCount, kEmit> + columns_emit_kernel + sort_{hist,scan,scatter}_kernel"
+                                if name == "device" else "eval_kernel + row_count_kernel + columns_emit_kernel per row, host transposition"),
+                     "note": "median over the timed steps of the executor call (wall clock), of the summed last_query_gpu_ms and of the "
+                             "number of its library queries; result_size: Extract's columns or Sort's pairs"})
+    real.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", default="5,3,4")
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--shards", type=int, default=1024)
     ap.add_argument("--groupby-shards", type=int, default=512)
-    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D, N, O, U: steps of the composition arm")
-    ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S, D, N: shards of the composition arm and of the device arm timed beside it")
+    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D, N, O, U, E: steps of the composition arm")
+    ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S, D, N, E: shards of the composition arm and of the device arm timed beside it")
     ap.add_argument("--topn-rows", type=int, default=1 << 14, help="config N: rows of the TopN field")
     ap.add_argument("--topn-shards", type=int, default=16, help="config N: shards (the fragments are encoded in Python: ~5 s per shard)")
     ap.add_argument("--generators", default="uniform,clustered")
@@ -1135,6 +1221,8 @@ def main():
             config_sort(args, out)
         elif c == "U":
             config_distinct(args, out)
+        elif c == "E":
+            config_extract_rows(args, out)
         elif c == "3L":     # the same BSI query at 256 shards (268 M records, 1.1 GB of planes): shows the kernel away from the launch-bound regime
             config3(args, out, n_rec=256 * SW, nf=1)
         else:

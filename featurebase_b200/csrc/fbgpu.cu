@@ -148,6 +148,7 @@ struct Workspace {
     DevBuf d_select;                     // fbgpu_bsi_select: per-rank candidate bitmaps of every unit of the call
     DevBuf d_present;                    // fbgpu_groupby_distinct: one leaf's presence bitset, (cell, listed value of x) -> present
     DevBuf d_sort;                       // fbgpu_bsi_sort: (key, column) pairs, two halves (SortPairs)
+    DevBuf d_cells;                      // fbgpu_extract_rows: per window column of a batch, its number of rows, then its place in the chunk's pairs
     PinBuf h_in, h_out;
     bool busy = false;
 };
@@ -254,7 +255,7 @@ extern "C" void fbgpu_shutdown(fbgpu_ctx* c) {
     cudaDeviceSynchronize();
     if (c->comm && nccl_load()) g_nccl.CommDestroy(c->comm);
     for (auto& w : c->wss) {
-        for (DevBuf* b : { &w->d_in, &w->d_counts, &w->d_bitmaps, &w->d_info, &w->d_emit_units, &w->d_emit, &w->d_rows, &w->d_aux, &w->d_select, &w->d_present, &w->d_sort }) b->release();
+        for (DevBuf* b : { &w->d_in, &w->d_counts, &w->d_bitmaps, &w->d_info, &w->d_emit_units, &w->d_emit, &w->d_rows, &w->d_aux, &w->d_select, &w->d_present, &w->d_sort, &w->d_cells }) b->release();
         w->h_in.release(); w->h_out.release();
         if (w->ev0) cudaEventDestroy(w->ev0);
         if (w->ev1) cudaEventDestroy(w->ev1);
@@ -1647,6 +1648,129 @@ extern "C" int fbgpu_bsi_distinct(fbgpu_ctx* c, uint32_t index, const fbgpu_op* 
     rc = bsi_distinct_run(c, index, ops, n_ops, field, view, bit_depth, shards, n_shards, vals, &total); if (rc) return rc;
     if (out_total) *out_total = total;
     return write_values(vals, out_vals, cap, out_n);
+} FBGPU_CATCH
+
+// ------------------------------------------------------------------ The rows of a set-like field per column (extract_rows_kernel, kernels.cuh)
+// R is evaluated batch by batch and its window cut into per-unit rank ranges as for fbgpu_columns.  Per batch, the count pass
+// gives every window column its number of rows; the host turns them into the columns' offsets and cuts the batch into chunks
+// at column boundaries, of at most kSortChunk columns and kSortChunk (column, row) pairs each, a column holding more rows than
+// that being a chunk of its own.  Per chunk, columns_emit_kernel writes the columns, the emit pass the pairs keyed
+// (i << kbits) | k (i the column in the chunk, k the row's rank in its fragment), and the radix sort orders them by column,
+// then by row id.  Only the columns and the row ids are read back.
+
+// the parts of a batch's units that fall in its window columns [a, b), re-based to out_off 0
+static void chunk_units(const std::vector<ColUnit>& units, uint64_t a, uint64_t b, std::vector<ColUnit>& chunk) {
+    chunk.clear();
+    for (const ColUnit& u : units) {
+        const uint64_t lo = std::max<uint64_t>(u.out_off, a), hi = std::min<uint64_t>(u.out_off + (u.last - u.first), b);
+        if (lo >= hi) continue;
+        ColUnit cu = u;
+        cu.first = u.first + (uint32_t)(lo - u.out_off); cu.last = cu.first + (uint32_t)(hi - lo); cu.out_off = lo - a;
+        chunk.push_back(cu);
+    }
+}
+
+static int bit_width(uint64_t x) { return x ? 64 - __builtin_clzll(x) : 0; }
+
+// the window's columns, the offsets of their lists and the row ids of the lists (store lock held); |R| into *total
+static int extract_rows_run(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view,
+                            const uint64_t* shards, int64_t n_shards, uint64_t offset, int64_t limit,
+                            std::vector<uint64_t>& cols, std::vector<uint64_t>& offs, std::vector<uint64_t>& rows, uint64_t* total) {
+    const uint32_t fv = view_id_locked(c, ViewKey{ index, field, view }, false);
+    Query q(c); Workspace* w = q.w;
+    const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);
+    int rc = q.open(index, ops, n_ops, sorted.data(), (int64_t)sorted.size()); if (rc) return rc;
+    uint32_t max_rows = 0;                               // the most rows of one listed fragment: a row rank takes kbits bits
+    if (fv != kNoView)
+        for (uint64_t s : sorted) if (s < c->shardmaps[fv].size() && c->shardmaps[fv][s] >= 0) max_rows = std::max(max_rows, c->frags[(size_t)c->shardmaps[fv][s]].n_rows);
+    const int kbits = bit_width(max_rows ? max_rows - 1 : 0);
+    const uint64_t win_end = window_end(offset, limit);
+    SortPairs sp(w, kSortChunk);
+    uint64_t seen = 0;
+    std::vector<ColUnit> units, chunk;
+    std::vector<uint32_t> cnt;
+    cols.clear(); rows.clear(); offs.assign(1, 0);
+    for (long long u0 = 0; u0 < q.n_units; u0 += c->unit_batch) {
+        const long long nu = std::min(c->unit_batch, q.n_units - u0);
+        const uint2* info;
+        rc = q.eval_info(u0, nu, info); if (rc) return rc;
+        const uint64_t batch_out = col_units(info, u0, nu, sorted, offset, win_end, seen, units);
+        if (batch_out) {
+            if (w->d_cells.ensure(batch_out * 4) || w->h_out.ensure(batch_out * 4)) return FBGPU_E_NOMEM;
+            unsigned int* d_cells = (unsigned int*)w->d_cells.p;
+            uint32_t* h_cells = (uint32_t*)w->h_out.p;
+            CUDA_TRY(cudaMemsetAsync(d_cells, 0, batch_out * 4, w->stream));
+            rc = q.emit_on_device(units, 0, [&](const ColUnit* d_units, int n, int grid) {
+                extract_rows_kernel<ErOut::kCount><<<grid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv, (const uint4*)w->d_bitmaps.p, d_units, n,
+                                                                                            d_cells, 0, nullptr, nullptr);
+                CUDA_TRY(cudaGetLastError()); q.launches++;
+                return 0;
+            });
+            if (rc) return rc;
+            CUDA_TRY(cudaMemcpyAsync(h_cells, d_cells, batch_out * 4, cudaMemcpyDeviceToHost, w->stream));
+            CUDA_TRY(cudaStreamSynchronize(w->stream));
+            cnt.assign(h_cells, h_cells + batch_out);
+            const size_t c0 = cols.size();               // the window rank of the batch's first column
+            cols.resize(c0 + batch_out);
+            for (uint64_t i = 0; i < batch_out; i++) offs.push_back(offs.back() + cnt[i]);
+            rows.resize(offs.back());
+            for (uint64_t a = 0; a < batch_out;) {
+                uint64_t b = a, pairs = 0;
+                while (b < batch_out && b - a < kSortChunk && (b == a || pairs + cnt[b] <= kSortChunk)) pairs += cnt[b++];
+                chunk_units(units, a, b, chunk);
+                const uint64_t p0 = offs[c0 + a];
+                for (uint64_t i = a; i < b; i++) h_cells[i] = (uint32_t)(offs[c0 + i] - p0);     // column i's first place in the chunk's pairs
+                CUDA_TRY(cudaMemcpyAsync(d_cells + a, h_cells + a, (b - a) * 4, cudaMemcpyHostToDevice, w->stream));
+                sp.n = 0; sp.bound = std::max(kSortChunk, pairs);
+                rc = sp.reserve(std::max(pairs, b - a)); if (rc) return rc;
+                rc = q.emit_on_device(chunk, 0, [&](const ColUnit* d_units, int n, int grid) {
+                    unsigned long long* d_cols = sp.keys(1 - sp.cur);         // the sort's other half: read back before its first pass
+                    columns_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>((const uint4*)w->d_bitmaps.p, d_units, n, d_cols);
+                    CUDA_TRY(cudaGetLastError());
+                    CUDA_TRY(cudaMemcpyAsync(cols.data() + c0 + a, d_cols, (b - a) * 8, cudaMemcpyDeviceToHost, w->stream));
+                    q.launches++;
+                    if (pairs) {
+                        extract_rows_kernel<ErOut::kEmit><<<grid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv, (const uint4*)w->d_bitmaps.p, d_units, n,
+                                                                                                   d_cells + a, kbits, sp.keys(sp.cur), sp.cols(sp.cur));
+                        CUDA_TRY(cudaGetLastError()); q.launches++;
+                    }
+                    return 0;
+                });
+                if (rc) return rc;
+                sp.n = pairs;
+                rc = sort_pairs(q, sp, bit_width(b - a - 1) + kbits, ~0ull); if (rc) return rc;
+                if (pairs) CUDA_TRY(cudaMemcpyAsync(rows.data() + p0, sp.cols(sp.cur), pairs * 8, cudaMemcpyDeviceToHost, w->stream));
+                CUDA_TRY(cudaStreamSynchronize(w->stream));
+                a = b;
+            }
+        }
+        CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        q.add_elapsed();
+    }
+    *total = seen;
+    q.finish();
+    return FBGPU_OK;
+}
+
+extern "C" int fbgpu_extract_rows(fbgpu_ctx* c, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view,
+                                  const uint64_t* shards, int64_t n_shards, uint64_t offset, int64_t limit,
+                                  uint64_t* out_cols, uint64_t* out_offsets, uint64_t cap_cols, uint64_t* out_rows, uint64_t cap_rows,
+                                  uint64_t* out_n_cols, uint64_t* out_n_rows, uint64_t* out_total) try {
+    if (!c || !out_n_cols || !out_n_rows || (cap_cols && (!out_cols || !out_offsets)) || (cap_rows && !out_rows) || n_ops < 0 || (n_ops && !ops) ||
+        n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "null argument");
+    std::shared_lock<std::shared_mutex> lk;
+    int rc = begin_query(c, lk); if (rc) return rc;
+    std::vector<uint64_t> cols, offs, rows; uint64_t total = 0;
+    rc = extract_rows_run(c, index, ops, n_ops, field, view, shards, n_shards, offset, limit, cols, offs, rows, &total); if (rc) return rc;
+    if (out_total) *out_total = total;
+    *out_n_cols = cols.size(); *out_n_rows = rows.size();
+    if (cols.size() > cap_cols || rows.size() > cap_rows)
+        return fail(FBGPU_E_NOSPACE, "output needs room for %llu columns and %llu row ids", (unsigned long long)cols.size(), (unsigned long long)rows.size());
+    if (!cols.empty()) memcpy(out_cols, cols.data(), cols.size() * 8);
+    if (out_offsets) memcpy(out_offsets, offs.data(), offs.size() * 8);
+    if (!rows.empty()) memcpy(out_rows, rows.data(), rows.size() * 8);
+    return FBGPU_OK;
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ BSI Min / Max (one pass over the planes)

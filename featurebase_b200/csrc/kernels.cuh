@@ -1238,6 +1238,25 @@ columns_emit_kernel(const uint4* __restrict__ bitmaps, const ColUnit* __restrict
 // a column found in the sign row gets bit i of the `sign` bit array.  The sign is kept apart because a depth-64 magnitude
 // fills all 64 bits (INT64_MIN is stored as sign + 2^63).  Ranks match columns_emit_kernel, so the outputs line up.
 constexpr int kExtractThreads = 256;
+
+// stages a unit's base bitmap `src` in base[] and the number of its bits before word i in rank0[i] (kExtractThreads threads; the
+// previous unit's readers are done on entry, and the tables are complete on return)
+__device__ __forceinline__ void stage_base_ranks(const uint64_t* src, uint64_t* base, uint32_t* rank0, uint32_t* wsum, int tid, int lane, int wid) {
+    uint64_t w[4]; uint32_t c = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) { w[k] = src[4 * tid + k]; base[4 * tid + k] = w[k]; c += __popcll(w[k]); }
+    uint32_t inc = c;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { uint32_t x = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += x; }
+    if (lane == 31) wsum[wid] = inc;
+    __syncthreads();
+    uint32_t r = inc - c;
+    for (int k = 0; k < wid; k++) r += wsum[k];
+#pragma unroll
+    for (int k = 0; k < 4; k++) { rank0[4 * tid + k] = r; r += __popcll(w[k]); }
+    __syncthreads();
+}
+
 __global__ void __launch_bounds__(kExtractThreads)
 extract_values_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restrict__ bitmaps, const ColUnit* __restrict__ units, int n_units,
                       unsigned long long* __restrict__ out, unsigned int* __restrict__ sign) {
@@ -1249,19 +1268,7 @@ extract_values_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restri
         const ColUnit u = units[e];
         const uint64_t* src = reinterpret_cast<const uint64_t*>(bitmaps + (size_t)u.unit * 512);
         __syncthreads();                                   // the previous unit's readers are done
-        uint64_t w[4]; uint32_t c = 0;
-#pragma unroll
-        for (int k = 0; k < 4; k++) { w[k] = src[4 * tid + k]; base[4 * tid + k] = w[k]; c += __popcll(w[k]); }
-        uint32_t inc = c;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { uint32_t x = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += x; }
-        if (lane == 31) wsum[wid] = inc;
-        __syncthreads();
-        uint32_t r = inc - c;
-        for (int k = 0; k < wid; k++) r += wsum[k];
-#pragma unroll
-        for (int k = 0; k < 4; k++) { rank0[4 * tid + k] = r; r += __popcll(w[k]); }
-        __syncthreads();
+        stage_base_ranks(src, base, rank0, wsum, tid, lane, wid);
         const uint64_t shard = u.col_base >> 20; const int slot = (int)((u.col_base >> 16) & 15);
         // plane pl of base column v into its slot (a column outside the base or outside the window is skipped)
         auto hit = [&](uint32_t v, int pl) {
@@ -1300,6 +1307,82 @@ extract_values_kernel(StoreRef st, uint32_t fv, int depth, const uint4* __restri
                         if (i == (l0 >> 6)) m &= ~0ull >> (63 - (l0 & 63));
                         uint64_t v = base[i] & m;
                         while (v) { const int bit = __ffsll((long long)v) - 1; hit(i * 64 + (uint32_t)bit, pl); v &= v - 1; }
+                    }
+                }
+            }
+        }
+    }
+}
+
+// ------------------------------------------------------------------ The rows of a set-like field per column (fbgpu_extract_rows)
+// The bulk form of executeExtractShard (executor.go:4758-4960), which intersects every row of the fragment with the filter and
+// turns the hits into a column -> rows matrix: one CTA per ColUnit.  The unit's base bitmap and rank table are staged as in
+// extract_values_kernel; warp w then walks the fragment's rows[] entries w, w + 8, ... for (fv, shard) — shardmap -> frags ->
+// rows, which every view has, with or without the dense directory — and reads the unit's slot container of each row that has
+// one, once, in its own encoding.  A base column inside the window that the container holds is a hit (window rank i, row rank
+// k in the fragment; rows[] is sorted by row id, so k orders the rows).
+//   kCount: cells[i] += 1 — the number of rows of each window column of the batch.
+//   kEmit:  the pair ((i << kbits) | k, row id) at keys / row_ids[cells[i]++] — cells[i] enters as column i's first place in
+//           the chunk's pair buffer.  The keys are unique, so sorting them gives one order whatever order the atomics take.
+enum class ErOut { kCount, kEmit };
+
+template <ErOut kOut>
+__global__ void __launch_bounds__(kExtractThreads)
+extract_rows_kernel(StoreRef st, uint32_t fv, const uint4* __restrict__ bitmaps, const ColUnit* __restrict__ units, int n_units,
+                    unsigned int* __restrict__ cells, int kbits, unsigned long long* __restrict__ keys, unsigned long long* __restrict__ row_ids) {
+    __shared__ __align__(16) uint64_t base[1024];
+    __shared__ uint32_t rank0[1024];
+    __shared__ uint32_t wsum[kExtractThreads / 32];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nwarps = kExtractThreads / 32;
+    for (int e = blockIdx.x; e < n_units; e += gridDim.x) {
+        const ColUnit u = units[e];
+        const uint64_t* src = reinterpret_cast<const uint64_t*>(bitmaps + (size_t)u.unit * 512);
+        __syncthreads();                                   // the previous unit's readers are done
+        stage_base_ranks(src, base, rank0, wsum, tid, lane, wid);
+        const uint64_t shard = u.col_base >> 20; const int slot = (int)((u.col_base >> 16) & 15);
+        if (fv >= st.n_views) continue;                    // (block-uniform, as are the two below)
+        const ViewTab v = st.views[fv];
+        if (shard >= v.n_shards) continue;
+        const int f = st.shardmap[v.shard_off + shard];
+        if (f < 0) continue;
+        const FragHdr h = st.frags[f];
+        for (uint32_t k = (uint32_t)wid; k < h.n_rows; k += nwarps) {
+            const RowEnt re = st.rows[h.row_off + k];
+            if (!((re.mask >> slot) & 1)) continue;
+            const ContDesc d = st.descs[re.first_desc + __popc(re.mask & ((1u << slot) - 1u))];
+            const void* ptr = st.payload + (size_t)d.off16 * 16;
+            auto hit = [&](uint32_t c) {
+                const uint64_t bw = base[c >> 6];
+                if (!((bw >> (c & 63)) & 1ull)) return;
+                const uint32_t rk = rank0[c >> 6] + __popcll(bw & ((1ull << (c & 63)) - 1ull));
+                if (rk < u.first || rk >= u.last) return;
+                const uint64_t i = u.out_off + (rk - u.first);
+                if (kOut == ErOut::kCount) atomicAdd(&cells[i], 1u);
+                else {
+                    const unsigned int p = atomicAdd(&cells[i], 1u);
+                    keys[p] = (i << kbits) | k;
+                    row_ids[p] = re.row;
+                }
+            };
+            if (d.typ == kArray) {
+                const uint16_t* a = reinterpret_cast<const uint16_t*>(ptr);
+                for (uint32_t i = lane; i < d.card; i += 32) hit((uint32_t)__ldg(a + i));
+            } else if (d.typ == kBitmap) {
+                const uint64_t* g = reinterpret_cast<const uint64_t*>(ptr);
+                for (int i = lane; i < 1024; i += 32) {
+                    uint64_t x = __ldg(g + i) & base[i];
+                    while (x) { const int bit = __ffsll((long long)x) - 1; hit((uint32_t)(i * 64 + bit)); x &= x - 1; }
+                }
+            } else {
+                const uint32_t* r32 = reinterpret_cast<const uint32_t*>(ptr);
+                for (uint32_t j = 0; j < d.cnt; j++) {                    // the warp walks each interval's words together
+                    const uint32_t iv = __ldg(r32 + j), s0 = iv & 0xffffu, l0 = iv >> 16;
+                    for (uint32_t i = (s0 >> 6) + lane; i <= (l0 >> 6); i += 32) {
+                        uint64_t m = ~0ull;
+                        if (i == (s0 >> 6)) m &= ~0ull << (s0 & 63);
+                        if (i == (l0 >> 6)) m &= ~0ull >> (63 - (l0 & 63));
+                        uint64_t x = base[i] & m;
+                        while (x) { const int bit = __ffsll((long long)x) - 1; hit(i * 64 + (uint32_t)bit); x &= x - 1; }
                     }
                 }
             }

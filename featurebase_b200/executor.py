@@ -798,9 +798,10 @@ class Executor:
         """executeExtract :4711 / executeExtractShard :4758: the table {column -> per-field cell} for the columns of the first
         child.  The column list and the int cells come from the device (fbgpu_columns, fbgpu_extract: value + Base, None
         when the column has no value); a set / time cell is the ascending list of the field's rows that hold the column, a
-        mutex cell the single such row (None if none), a bool cell True / False / None — one column expansion of
-        filter ∩ Row(field=r) per row of the field.  Keys, decimals and timestamps are translation layers above the path.
-        Returns {"fields": [(name, type)], "columns": [(column id, [cell, ...])]}."""
+        mutex cell the lowest such row (None if none), a bool cell whether that row is 1 (None if none).  A context with
+        extract_rows takes each set-like field's lists from one call with the Extract's filter and window; other contexts
+        expand filter ∩ Row(field=r) for every row of the field.  Keys, decimals and timestamps are translation layers above
+        the path.  Returns {"fields": [(name, type)], "columns": [(column id, [cell, ...])]}."""
         if not c.children:
             raise QueryError("missing column filter in Extract")
         filt_call = c.children[0]
@@ -827,9 +828,13 @@ class Executor:
         else:
             cols, filt, win = sorted_cols, [], (1, None)         # (cells for exactly these columns: the narrowed filter below)
         pos = {col: i for i, col in enumerate(cols)}
-        if win != (0, None) and cols:                            # cells are only needed for the window: narrow the filter to it
-            ef, erow = self.holder.embed_row(idx.name, cols)
+        by_rows = hasattr(self.ctx, "extract_rows")
+        rows_filt, rows_win = filt, win                          # extract_rows cuts the window itself
+        if win != (0, None) and cols and (sorted_cols is not None or not by_rows or any(f.type == "int" for f in fields)):
+            ef, erow = self.holder.embed_row(idx.name, cols)     # cells are only needed for the window: narrow the filter to it
             filt = [L.Op(L.OP_ROW, ef.id, VIEW_STANDARD, 0, erow, 0, 0, 0)]
+            if sorted_cols is not None:
+                rows_filt, rows_win = filt, (0, None)
         table = [[None] * len(fields) for _ in cols]
         types = []
         for k, f in enumerate(fields):
@@ -845,6 +850,11 @@ class Executor:
             if multi:
                 for row in table:
                     row[k] = []
+            if by_rows:
+                for col, rs in self._cell_rows(idx, f, shards, rows_filt, rows_win) if cols else ():
+                    if rs and col in pos:
+                        table[pos[col]][k] = rs if multi else (rs[0] == 1) if f.type == "bool" else rs[0]
+                continue
             rid, _ = self.ctx.row_counts(idx.id, f.id, VIEW_STANDARD, shards, filter_ops=filt)
             for r in sorted(int(x) for x in rid):
                 ops = filt + [L.Op(L.OP_ROW, f.id, VIEW_STANDARD, 0, r, 0, 0, 0), L.Op(L.OP_INTERSECT, 0, 0, 2, 0, 0, 0, 0)]
@@ -857,12 +867,20 @@ class Executor:
                         table[pos[col]][k] = (r == 1) if f.type == "bool" else r
         return {"fields": [(f.name, t) for f, t in zip(fields, types)], "columns": list(zip(cols, table))}
 
+    def _cell_rows(self, idx, f, shards, filt, win=(0, None)):
+        """[(column, [row, ...])]: every column of the window of filt with the ascending rows of set-like field f that hold it
+        (one fbgpu_extract_rows call)"""
+        cols, offs, rows, _ = self.ctx.extract_rows(idx.id, f.id, VIEW_STANDARD, shards, filt, offset=win[0], limit=win[1])
+        offs, rows = offs.tolist(), rows.tolist()
+        return [(col, rows[offs[i]:offs[i + 1]]) for i, col in enumerate(cols.tolist())]
+
     def _sort(self, idx, c, shards):
         """executeSort :9321 / executeSortShard :9387: the columns of the child row ordered by a field's value — int (values from
         fbgpu_extract), bool (falses then trues), mutex (by row id) — ascending or `sort-desc`, then offset / limit.  The
         reference merges per-shard lists in arrival order, so its order among equal values is unspecified; here ties keep
         ascending column order.  A context with bsi_sort orders an int field on the device and returns only the window; other
-        contexts (and a negative offset or limit, which slice the list from its end) extract every value and sort here.
+        contexts (and a negative offset or limit, which slice the list from its end) extract every value and sort here.  A
+        context with extract_rows takes a bool or mutex field's (column, row) pairs from one call.
         Returns [(column, value)]."""
         name = c.args.get("field", c.args.get("_field"))
         if name is None:
@@ -880,6 +898,8 @@ class Executor:
         if f.type == "int":
             cols, vals, _ = self.ctx.extract(idx.id, f.id, VIEW_BSI, f.bit_depth, shards, filter_ops=filt)
             kvs = [(int(col), int(v) + f.base) for col, v in zip(cols.tolist(), vals.tolist())]
+        elif f.type in ("bool", "mutex") and hasattr(self.ctx, "extract_rows"):
+            kvs = [(col, (r == 1) if f.type == "bool" else r) for col, rs in self._cell_rows(idx, f, shards, filt) for r in rs]
         elif f.type in ("bool", "mutex"):
             kvs = []
             rid, _ = self.ctx.row_counts(idx.id, f.id, VIEW_STANDARD, shards, filter_ops=filt)

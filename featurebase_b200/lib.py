@@ -53,7 +53,7 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_groupby_values", "fbgpu_node_groupby_values", "fbgpu_row_counts_views", "fbgpu_node_row_counts_views", "fbgpu_groupby_views",
            "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum",
            "fbgpu_groupby_distinct", "fbgpu_topn_cutoffs", "fbgpu_node_topn_cutoffs", "fbgpu_bsi_sort", "fbgpu_node_bsi_sort",
-           "fbgpu_bsi_distinct", "fbgpu_node_bsi_distinct"]
+           "fbgpu_bsi_distinct", "fbgpu_node_bsi_distinct", "fbgpu_extract_rows"]
 
 
 def lib_path():
@@ -95,6 +95,8 @@ def load():
     L.fbgpu_bsi_sort.restype = C.c_int
     L.fbgpu_bsi_distinct.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, vp, u64, C.POINTER(u64), C.POINTER(u64)]
     L.fbgpu_bsi_distinct.restype = C.c_int
+    L.fbgpu_extract_rows.argtypes = [vp, u32, vp, i32, u32, u32, vp, i64, u64, i64, vp, vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
+    L.fbgpu_extract_rows.restype = C.c_int
     L.fbgpu_bsi_minmax.argtypes = [vp, u32, vp, i32, u32, u32, i32, vp, i64, i32, C.POINTER(C.c_int64), C.POINTER(u64)]
     L.fbgpu_bsi_minmax.restype = C.c_int
     L.fbgpu_bsi_sum.argtypes, L.fbgpu_bsi_sum.restype = [vp, u32, vp, i32, u32, u32, i32, vp, i64, C.POINTER(C.c_int64), C.POINTER(u64)], C.c_int
@@ -411,6 +413,27 @@ class Context:
             self._check(rc)
             self._distinct_cap = cap
             return vals[: n.value].copy(), total.value
+
+    def extract_rows(self, index, field, view, shards, filter_ops, offset=0, limit=None):
+        """The rows of a set, mutex, bool or time field for the columns of the row <filter_ops>, on the device: (the window's
+        ascending column ids, as columns() returns them; offsets, one more than the columns; row ids; cardinality of the whole
+        row).  Column i's rows, ascending, are rows[offsets[i]:offsets[i + 1]]; a column with no row has an empty list."""
+        sh = _u64arr(shards)
+        arr = ops_array(filter_ops)
+        nc, nr, total = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        cap_c = max(getattr(self, "_col_cap", 0), 1 << 16) if limit is None else max(min(int(limit), 1 << 16), 1)     # (a limit may exceed the row)
+        cap_r = max(getattr(self, "_cell_rows_cap", 0), 1 << 16)
+        while True:
+            cols, offs, rows = np.empty(cap_c, dtype=np.uint64), np.empty(cap_c + 1, dtype=np.uint64), np.empty(cap_r, dtype=np.uint64)
+            rc = self.L.fbgpu_extract_rows(self.h, index, arr, len(filter_ops), field, view, sh.ctypes.data, len(sh), int(offset),
+                                           -1 if limit is None else int(limit), cols.ctypes.data, offs.ctypes.data, cap_c, rows.ctypes.data, cap_r,
+                                           C.byref(nc), C.byref(nr), C.byref(total))
+            if rc == E_NOSPACE:
+                cap_c, cap_r = max(cap_c, int(nc.value)), max(cap_r, int(nr.value))
+                continue
+            self._check(rc)
+            self._cell_rows_cap = cap_r
+            return cols[: nc.value].copy(), offs[: nc.value + 1].copy(), rows[: nr.value].copy(), total.value
 
     def bsi_minmax(self, index, field, view, bit_depth, shards, want_max, filter_ops=None):
         """(extreme stored value = value - Base, number of columns holding it) over <filter> ∩ not-null; count 0: empty row.

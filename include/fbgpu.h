@@ -180,6 +180,33 @@ int fbgpu_extract(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n
                   const uint64_t *shards, int64_t n_shards, uint64_t offset, int64_t limit,
                   uint64_t *out_cols, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
 
+/* The rows of a set, mutex, bool or time field for every column of a row: the transposition Extract makes of each Rows(f)
+ * child (executeExtractShard executor.go:4758-4960 intersects every row of the fragment with the filter and turns the hits
+ * into a column -> rows matrix), and what Sort over a bool or mutex field orders by.
+ *   - The row R is <ops>, compiled and evaluated as for fbgpu_columns.  *out_total = |R| (when out_total is not NULL).
+ *   - The window is [offset, offset + limit) of R's columns in ascending order (limit < 0: no limit), as for fbgpu_columns:
+ *     out_cols[0 .. n_cols) is what fbgpu_columns returns for the same arguments, and *out_n_cols = n_cols.  A column with no
+ *     row in the field is listed too, with an empty list.
+ *   - For window column i, out_rows[out_offsets[i] .. out_offsets[i + 1]) holds the row ids r, strictly ascending, such that
+ *     the column is in Row(field = r) of `view`.  out_offsets receives n_cols + 1 entries (it has room for cap_cols + 1),
+ *     out_offsets[0] = 0, and *out_n_rows = out_offsets[n_cols].  A shard without the field's fragment, and a view that was
+ *     never loaded, give empty lists.
+ *   - cap_cols < n_cols or cap_rows < n_rows is FBGPU_E_NOSPACE with nothing written; *out_n_cols and *out_n_rows then both
+ *     hold the sizes needed, so one retry succeeds.
+ *   - Local to the context: never reduced over a communicator.
+ *   - Device memory: the call holds at most one radix-sort buffer of max(2^24, the most rows of one window column)
+ *     (key, row id) pairs of 32 bytes and 4 bytes per window column of one evaluation batch, whatever the window's size;
+ *     FBGPU_E_NOMEM when that cannot be allocated.
+ *   - A NULL handle, out_n_cols or out_n_rows, a non-zero cap_cols with NULL out_cols or out_offsets, a non-zero cap_rows with
+ *     NULL out_rows, n_ops < 0 or n_ops > 0 with NULL ops, n_shards < 0 or n_shards > 0 with NULL shards ("null argument") are
+ *     FBGPU_E_INVALID, reported before the device check.
+ * There is no node form. */
+int fbgpu_extract_rows(fbgpu_ctx *ctx, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view,
+                       const uint64_t *shards, int64_t n_shards, uint64_t offset, int64_t limit,
+                       uint64_t *out_cols, uint64_t *out_offsets, uint64_t cap_cols,
+                       uint64_t *out_rows, uint64_t cap_rows,
+                       uint64_t *out_n_cols, uint64_t *out_n_rows, uint64_t *out_total);
+
 /* Sort(<filter>, field=, sort-desc=, offset=, limit=) over an int field (executeSort / executeSortShard executor.go:9321-9560):
  * the row of fbgpu_extract, put in order on the device, and only a window of it returned.
  *   - The row is <filter program> ∩ not-null(field), exactly as for fbgpu_extract (n_ops == 0: every column that has a value);
