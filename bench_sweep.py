@@ -18,6 +18,9 @@
             Sum-per-group composition (only when named in --configs).
   config D: GroupBy(Rows(a), aggregate=Count(Distinct(field=v))), the same with Rows(w) or Rows(b) beside a, on config S's data,
             fbgpu_groupby_distinct against the Distinct-per-group composition (only when named in --configs).
+  config K: GroupBy(Rows(a), aggregate=Count(Distinct(field=x))) and the same with Rows(b) beside a, for x a mutex field of
+            100,000 rows and a set field of 64 rows, on config D's data, fbgpu_groupby_distinct_rows against the
+            Distinct-per-group composition (only when named in --configs).
   config N: TopN(f, Row(src=0), tanimotoThreshold=50) and TopN(f, Row(src=0), threshold=100) over --topn-rows rows of varied
             cardinality, fbgpu_topn_cutoffs against the per-shard count-matrix composition (only when named in --configs).
   config O: Sort over config X's 32-bit field with and without a limit, fbgpu_bsi_sort against extracting every value and
@@ -620,6 +623,15 @@ class _NoGroupByDistinct(_KernelMs):
         return super().__getattr__(name)
 
 
+class _NoGroupByDistinctRows(_KernelMs):
+    """the same proxy without groupby_distinct_rows: the executor runs one Distinct per group for a set-like x"""
+
+    def __getattr__(self, name):
+        if name == "groupby_distinct_rows":
+            raise AttributeError(name)
+        return super().__getattr__(name)
+
+
 def _config_s_world(args, tag):
     """config S's data over --groupby-shards shards: a and b are 256-row set fields at 1/256 density per row, c a 1 % filter row;
     w (64 distinct values) and v (values in ±2^20, 21 bits) are int fields holding a value for each of the first 16,384 columns
@@ -764,6 +776,80 @@ def config_groupby_distinct(args, out):
                          "kernel_ms": float(np.median(dd["kernel_ms"])), "queries": int(np.median(dd["queries"])), "steps": len(dd["wall"]), "load_s": round(load_s, 1),
                          "kernel": ("eval_kernel + groupby kernels, extract_values_kernel once, groupby_values_kernel<GvAgg::kDistinct> + gv_popcount_kernel"
                                     if name == "device" else "eval_kernel + groupby kernels, then eval_kernel + extract_values_kernel per group"),
+                         "note": "median over the timed steps of the executor call (wall clock, Rows / Distinct pre-passes included), of the summed "
+                                 "last_query_gpu_ms and of the number of its library queries"}
+                    if name == "composition":
+                        o["wall_ms_per_step"] = [round(x, 2) for x in dd["wall"]]
+                    out(o)
+    real.close()
+
+
+def config_groupby_distinct_rows(args, out):
+    """GroupBy(Rows(a), aggregate=Count(Distinct(field=x))) and the same with Rows(b) beside a, for x = m, a mutex field of
+    100,000 rows (one row per record), and x = s, a set field of 64 rows (0-4 rows per record), without and with a 1 % filter
+    row, through the executor.  The data is config D's (_config_s_world); m and s cover the first 16,384 columns of every shard,
+    the records that hold config D's int values, and every shard holds the same m and s fragments, encoded once.  The device arm
+    (one fbgpu_row_counts for x's rows, then fbgpu_groupby_distinct_rows, sliced by GROUPBY_DISTINCT_BITS) runs over all shards.
+    The composition arm (the group counts on the device, then one Distinct(Intersect(rows, filter), field=x) library query per
+    group) runs over the first --composition-shards shards, for --composition-steps steps alternated with the device arm over the
+    same shards, and only for queries of at most --composition-max-groups groups (a's 256; a x b's 65,536 are not timed).  Both
+    arms must return the same groups and every distinct count lies in 0 .. the group's count.  Progress goes to stderr."""
+    from featurebase_b200 import executor as X, roaring_io
+    S, n_cols = args.groupby_shards, 16384
+    h, idx, fa, fb, ff, fw, fv, load_s = _config_s_world(args, "K")
+    fm, fs = idx.create_field("m", "mutex"), idx.create_field("s")
+    rng = np.random.default_rng(2028)
+    cols = np.arange(n_cols, dtype=np.uint64)
+    s_bits = np.concatenate([rng.choice(64, int(k), replace=False).astype(np.uint64) * np.uint64(SW) + c for c, k in zip(cols, rng.integers(0, 5, n_cols))])
+    data = {fm: roaring_io.encode(np.sort(rng.integers(0, 100000, n_cols).astype(np.uint64) * np.uint64(SW) + cols)),
+            fs: roaring_io.encode(np.unique(s_bits))}
+    t0 = time.time()
+    for s in range(S):
+        for f, d in data.items():
+            h.ctx.load_fragment(idx.id, f.id, X.VIEW_STANDARD, s, d)
+    h.ctx.commit()
+    load_s += time.time() - t0
+    real = h.ctx
+    card = _card()
+    dev, comp = _KernelMs(real), _NoGroupByDistinctRows(real)
+    CS = min(S, args.composition_shards)
+    for second, x in (("", "m"), ("Rows(b), ", "m"), ("", "s"), ("Rows(b), ", "s")):
+        for q_filter in (False, True):
+            q = f"GroupBy(Rows(a), {second}aggregate=Count(Distinct(field={x}))" + (", filter=Row(c=0))" if q_filter else ")")
+            groups = 256 * (256 if second else 1)
+            runs = [(S, {"device": dev})]
+            if args.composition_steps > 0 and groups <= args.composition_max_groups:
+                runs.append((CS, {"device": dev, "composition": comp}))
+            for n_sh, arms in runs:
+                sh = list(range(n_sh))
+                rec = {name: {"wall": [], "kernel_ms": [], "queries": []} for name in arms}
+                res = {}
+                for i in range(1 + args.steps):              # one warm-up round of the device arm, then alternate the arms
+                    for name in (sorted(arms) if i % 2 == 0 else sorted(arms, reverse=True)):
+                        if name == "composition" and len(rec[name]["wall"]) >= args.composition_steps:
+                            continue
+                        h.ctx = arms[name]
+                        q0, arms[name].ms = real.counters()["queries"], 0.0
+                        t1 = time.perf_counter()
+                        r = X.Executor(h).execute("i", q, sh)[0]
+                        wall = (time.perf_counter() - t1) * 1e3
+                        res.setdefault(name, r)
+                        assert r == res[name], (q, name)
+                        print(f"config K: {q} over {n_sh} shards, {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                        if i >= 1 or name == "composition":
+                            rec[name]["wall"].append(wall)
+                            rec[name]["kernel_ms"].append(arms[name].ms)
+                            rec[name]["queries"].append(real.counters()["queries"] - q0)
+                h.ctx = real
+                assert all(r == res["device"] for r in res.values()), q
+                assert all(0 <= g[2] <= g[1] for g in res["device"]) and any(g[2] for g in res["device"]), q
+                for name, dd in rec.items():
+                    o = {"config": "K", "query": q, "arm": name, "gpu": card, "shards": n_sh, "groups": len(res[name]),
+                         "equal_to_composition": ("composition" in res) or None,
+                         "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])), "wall_ms_max": float(np.max(dd["wall"])),
+                         "kernel_ms": float(np.median(dd["kernel_ms"])), "queries": int(np.median(dd["queries"])), "steps": len(dd["wall"]), "load_s": round(load_s, 1),
+                         "kernel": ("eval_kernel + groupby kernels, row_count_kernel once, groupby_values_kernel<GvAgg::kDistinctRows> + gv_popcount_kernel"
+                                    if name == "device" else "eval_kernel + groupby kernels, then eval_kernel + row_count_kernel per group"),
                          "note": "median over the timed steps of the executor call (wall clock, Rows / Distinct pre-passes included), of the summed "
                                  "last_query_gpu_ms and of the number of its library queries"}
                     if name == "composition":
@@ -1185,8 +1271,9 @@ def main():
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--shards", type=int, default=1024)
     ap.add_argument("--groupby-shards", type=int, default=512)
-    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D, N, O, U, E: steps of the composition arm")
-    ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S, D, N, E: shards of the composition arm and of the device arm timed beside it")
+    ap.add_argument("--composition-steps", type=int, default=1, help="configs V, T, M, S, D, K, N, O, U, E: steps of the composition arm")
+    ap.add_argument("--composition-shards", type=int, default=1, help="configs T, M, S, D, K, N, E: shards of the composition arm and of the device arm timed beside it")
+    ap.add_argument("--composition-max-groups", type=int, default=4096, help="config K: the composition arm runs only for queries of at most this many groups")
     ap.add_argument("--topn-rows", type=int, default=1 << 14, help="config N: rows of the TopN field")
     ap.add_argument("--topn-shards", type=int, default=16, help="config N: shards (the fragments are encoded in Python: ~5 s per shard)")
     ap.add_argument("--generators", default="uniform,clustered")
@@ -1215,6 +1302,8 @@ def main():
             config_groupby_sum(args, out)
         elif c == "D":
             config_groupby_distinct(args, out)
+        elif c == "K":
+            config_groupby_distinct_rows(args, out)
         elif c == "N":
             config_topn_cutoffs(args, out)
         elif c == "O":

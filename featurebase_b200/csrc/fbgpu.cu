@@ -2306,8 +2306,9 @@ static int groupby_views_args(const void* handle, const uint32_t* fields, const 
 
 // ------------------------------------------------------------------ GroupBy over the values of int fields
 // one int dimension of fbgpu_groupby_values / fbgpu_groupby_mixed: field, BSI view, depth and the ascending stored values that are its groups.
-// As the aggregate field x: values is null for Sum, and for Count(Distinct) the ascending stored values whose presence is counted
-struct GvInt { uint32_t field, view; int32_t depth; const int64_t* values; int32_t n_values; };
+// As the aggregate field x: values is null for Sum, and for Count(Distinct) the ascending stored values whose presence is counted;
+// for Count(Distinct) over a set-like field, rows holds the n_values ascending row ids whose presence is counted (values null)
+struct GvInt { uint32_t field, view; int32_t depth; const int64_t* values; int32_t n_values; const uint64_t* rows = nullptr; };
 
 // the argument checks fbgpu_groupby_values and its node form make before any device is touched
 static int groupby_values_args(const void* handle, const uint32_t* fields, const uint32_t* views, int32_t n_fields, const uint64_t* row_ids_flat,
@@ -2351,9 +2352,9 @@ static int groupby_mixed_args(const void* handle, const uint32_t* fields, const 
     return 0;
 }
 
-// the argument checks fbgpu_groupby_sum and fbgpu_groupby_distinct (and the node form of Sum) make before any device is touched
-// (n_rows is checked after it): agg_array is out_sums of Sum, x_values of Count(Distinct), the aggregate field's depth is named
-// depth_name in the message.  Count(Distinct) checks its x_values next
+// the argument checks fbgpu_groupby_sum, fbgpu_groupby_distinct and fbgpu_groupby_distinct_rows (and the node form of Sum) make
+// before any device is touched (n_rows is checked after it): agg_array is out_sums of Sum, x_values / x_rows of Count(Distinct),
+// the aggregate field's depth is named depth_name in the message.  Count(Distinct) checks its x list next
 static int groupby_agg_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
                             const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews,
                             const int32_t* bit_depths, int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, const void* agg_array,
@@ -2370,14 +2371,21 @@ static int groupby_agg_args(const void* handle, const uint32_t* fields, const ui
 
 // one groupby_values_kernel pass over the shards: counts[nB or 1][groups] of consider = filter ∩ exists(v_1) ∩ ... (∩ Row(b = row));
 // with an aggregate x, consider also ∩ exists(x) and sums[nB or 1][groups] the columns' stored values of x (Sum), or out[nB or 1]
-// [groups] the number of x's listed values present in the cell (Count(Distinct): x->values set, out_sums null).  The presence
-// bitset stays on the device; only the per-cell counts come back
+// [groups] the number of x's listed values present in the cell (Count(Distinct): x->values set, out_sums null), or with x->rows
+// set the number of x's listed rows that hold a column of the cell (consider without exists(x)).  The presence bitset stays on
+// the device; only the per-cell counts come back
 static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* null: no set dimension */, const std::vector<GvInt>& v,
                                const GvInt* x /* null: counts only */, const std::vector<fbgpu_op>& filter, const uint64_t* shards, int64_t n_shards,
                                uint64_t* out, uint64_t* out_sums) {
     std::vector<fbgpu_op> full = filter;
     for (const GvInt& f : v) full = and_row(full.data(), (int32_t)full.size(), f.field, f.view, 0);
-    if (x) full = and_row(full.data(), (int32_t)full.size(), x->field, x->view, 0);
+    const bool rows_x = x && x->rows;                                 // Count(Distinct) over a set-like x: no exists row
+    if (x && !rows_x) full = and_row(full.data(), (int32_t)full.size(), x->field, x->view, 0);
+    if (full.empty()) {                                              // (rows_x, b alone, no filter) consider: b's listed rows, which b's walk keeps anyway
+        for (int r = 0; r < b->n_rows; r++)
+            for (int32_t i = 0; i < b->n_views; i++) { fbgpu_op o{}; o.opcode = FBGPU_OP_ROW; o.field = b->field; o.view = b->views[i]; o.a = b->rows[r]; full.push_back(o); }
+        if (full.size() > 1) { fbgpu_op u{}; u.opcode = FBGPU_OP_UNION; u.argc = (uint32_t)full.size(); full.push_back(u); }
+    }
     Query q(c); Workspace* w = q.w;
     int rc = q.open(index, full.data(), (int32_t)full.size(), shards, n_shards); if (rc) return rc;
     GvInts k{};
@@ -2389,9 +2397,10 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
         k.n_groups *= v[(size_t)i].n_values;
         in.insert(in.end(), v[(size_t)i].values, v[(size_t)i].values + v[(size_t)i].n_values);
     }
-    const bool distinct = x && x->values;
+    const bool distinct = x && (x->values || rows_x);
     const size_t x_off = in.size();
-    if (distinct) in.insert(in.end(), x->values, x->values + x->n_values);
+    if (rows_x) in.insert(in.end(), x->rows, x->rows + x->n_values);
+    else if (distinct) in.insert(in.end(), x->values, x->values + x->n_values);
     const size_t n_vals = in.size();
     const uint32_t fvX = x ? view_id_locked(c, ViewKey{ index, x->field, x->view }, false) : kNoView;
     const int nB = b ? b->n_rows : 0;
@@ -2419,7 +2428,11 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
         rc = q.eval(u0, nu); if (rc) return rc;
         const long long grid = std::min<long long>(nu, (long long)c->sm_count * kGvCtasPerSm);
         unsigned long long* d_counts = (unsigned long long*)w->d_counts.p;
-        if (distinct)
+        if (rows_x)
+            groupby_values_kernel<GvAgg::kDistinctRows><<<(unsigned)grid, kGvThreads, 0, w->stream>>>(
+                store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB, (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, d_counts,
+                fvX, 0, nullptr, d_values + x_off, x->n_values, (unsigned long long*)w->d_present.p);
+        else if (distinct)
             groupby_values_kernel<GvAgg::kDistinct><<<(unsigned)grid, kGvThreads, 0, w->stream>>>(
                 store_ref(c), k, d_values, d_rowsB, nB, fvsB[0], d_fvsB, (int)nvB, (const uint4*)w->d_bitmaps.p, q.d_shards + u0 / kSlotsPerRow, nu, d_counts,
                 fvX, x->depth, nullptr, d_values + x_off, x->n_values, (unsigned long long*)w->d_present.p);
@@ -2452,7 +2465,7 @@ static int groupby_values_leaf(fbgpu_ctx* c, uint32_t index, const GbDim* b /* n
 // ------------------------------------------------------------------ one GroupBy request: every GroupBy entry point
 // The tensor's axes are the set dimensions, then the int dimensions.  Per cell: the number of columns of filter ∩ the cell's rows
 // (∩ exists(x) with an aggregate), and with agg kSum the sum of x's stored values behind it, or with kDistinct, in place of the
-// count, how many of x.values the cell holds
+// count, how many of x.values the cell holds, or with kDistinctRows how many of the rows x.rows hold a column of the cell
 struct GbRequest {
     std::vector<GbDim> dims;
     std::vector<GvInt> ints;
@@ -2613,6 +2626,27 @@ extern "C" int fbgpu_groupby_distinct(fbgpu_ctx* c, uint32_t index, const uint32
     return groupby_run(c, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows),
                                             gb_int_dims(vfields, vviews, bit_depths, n_ints, values_flat, n_values), GvAgg::kDistinct,
                                             GvInt{ xfield, xview, x_depth, x_values, n_x }, filter, n_filter_ops, shards, n_shards }, out_distinct);
+} FBGPU_CATCH
+
+// GroupBy(..., aggregate=Count(Distinct(field=x))) over a set-like x: fbgpu_groupby_distinct's dimensions with, per cell, how
+// many of x's listed rows hold at least one column of filter ∩ the cell's rows.  Local to one context, as fbgpu_groupby_distinct
+extern "C" int fbgpu_groupby_distinct_rows(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                           const uint64_t* row_ids_flat, const int32_t* n_rows, const uint32_t* vfields, const uint32_t* vviews,
+                                           const int32_t* bit_depths, int32_t n_ints, const int64_t* values_flat, const int32_t* n_values, uint32_t xfield,
+                                           uint32_t xview, const uint64_t* x_rows, int32_t n_x, const fbgpu_op* filter, int32_t n_filter_ops,
+                                           const uint64_t* shards, int64_t n_shards, uint64_t* out_distinct) try {
+    int rc = groupby_agg_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, vfields, vviews, bit_depths, n_ints, values_flat, n_values,
+                              x_rows, "x_depth", 0 /* x has no depth */, filter, n_filter_ops, shards, n_shards, out_distinct);
+    if (rc) return rc;
+    if (n_x < 1) return fail(FBGPU_E_INVALID, "n_x=%d < 1", n_x);
+    for (int32_t i = 1; i < n_x; i++)
+        if (x_rows[i] <= x_rows[i - 1]) return fail(FBGPU_E_INVALID, "x_rows are not strictly ascending at position %d", i);
+    if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_groupby_distinct_rows is local to one context: distinct sets of the ranks merge by union, not by sum");
+    GvInt x{ xfield, xview, 0, nullptr, n_x };
+    x.rows = x_rows;
+    return groupby_run(c, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows),
+                                            gb_int_dims(vfields, vviews, bit_depths, n_ints, values_flat, n_values), GvAgg::kDistinctRows,
+                                            x, filter, n_filter_ops, shards, n_shards }, out_distinct);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ comm

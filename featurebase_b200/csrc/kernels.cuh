@@ -2304,6 +2304,21 @@ groupby_direct_kernel(StoreRef st, uint32_t fvA, const uint64_t* __restrict__ ro
 // (or kGvNoPos) left in mag.  Every counted (b-row, column) with a group and a position sets bit j of its cell's row of
 // `present` (cells of ceil(nX / 64) words, 64-bit indexed) with atomicOr, a lane skipping the bit it set last;
 // gv_popcount_kernel then counts each cell's bits.
+// kDistinctRows (fbgpu_groupby_distinct_rows, Count(Distinct(field=x)) over a set-like x): consider is filter ∩ exists of the
+// int fields only (x has no exists row and no planes), and xvals holds x's nX strictly ascending row ids, bit for bit.  The
+// same presence bitset, bit j standing for the row xrows[j].  x is walked through its fragment's row directory, as
+// extract_rows_kernel walks rows[]: only the entries whose ids lie in [xrows[0], xrows[nX - 1]] (contiguous, found once per
+// unit), the lanes of a warp taking 32 entries at a time, mapping each id to j by binary search and skipping unlisted ids,
+// so the cost follows x's directory span and containers in the unit, not nX; the span is scanned once per range (and round),
+// 16 times per unit.  Per range, once the group indices are made (gv_rows_range, which only this mode instantiates):
+//   without b, each column c of a listed row's container ∩ cons with a group marks (vidx[c], j); a column of several listed
+//   rows marks several bits;
+//   with b, a join of two row sets over the range's columns, in rounds.  In each round every column takes its smallest listed
+//   position above the one it took last round (mag[c]: the last position + 1 in the high half, atomicMin of the new one on the
+//   low half), then b's walk (kDistinct's, single- or multi-view) marks (b-row, vidx[c], mag[c]).  sign marks the columns
+//   that met a second eligible row in this round's x walk; the rounds end after a round where none did, or before one where
+//   no column took a position.  Data where no column holds two listed rows (mutex and bool fields) costs one x walk and one
+//   b walk per range, and each further listed row a column holds one more of each.
 // ------------------------------------------------------------------------------------------------
 constexpr int kGvThreads = 256;
 constexpr int kGvCtasPerSm = 4;
@@ -2315,7 +2330,7 @@ constexpr int kGvMaxInts = 8;
 constexpr int kGvPlanes = 184;                     // plane table entries: what 48 KiB of static shared memory leaves
 constexpr unsigned long long kGvNoPos = ~0ull;     // kDistinct: the column's value of x is not listed
 
-enum class GvAgg { kCount, kSum, kDistinct };      // what groupby_values_kernel adds up per cell
+enum class GvAgg { kCount, kSum, kDistinct, kDistinctRows };      // what groupby_values_kernel adds up per cell
 
 // the int dimensions of one launch, passed by value
 struct GvInts {
@@ -2394,6 +2409,155 @@ struct GvMark {
     }
 };
 
+// kDistinctRows: the entries rows[x0 .. x1) of x's row directory for the shard whose ids lie in [xrows[0], xrows[nX - 1]]
+// (none when the shard lacks x's fragment)
+__device__ __forceinline__ void gv_x_entries(const StoreRef& st, uint32_t fv, uint64_t shard, const uint64_t* xrows, int nX, uint32_t& x0, uint32_t& x1) {
+    x0 = x1 = 0;
+    if (fv >= st.n_views) return;
+    const ViewTab vt = st.views[fv];
+    if (shard >= vt.n_shards) return;
+    const int f = st.shardmap[vt.shard_off + shard];
+    if (f < 0) return;
+    const FragHdr h = st.frags[f];
+    const uint64_t first = __ldg(xrows), last = __ldg(xrows + nX - 1);
+    uint32_t a = 0, b = h.n_rows;
+    while (a < b) { const uint32_t m = (a + b) >> 1; if (st.rows[h.row_off + m].row < first) a = m + 1; else b = m; }
+    uint32_t e = h.n_rows;
+    for (b = a; b < e;) { const uint32_t m = (b + e) >> 1; if (st.rows[h.row_off + m].row <= last) b = m + 1; else e = m; }
+    x0 = h.row_off + a; x1 = h.row_off + b;
+}
+
+// kDistinctRows: calls f(local column, j) for every column of [lo, lo + kGvRange) in cons that the listed row xrows[j] holds,
+// walking the directory entries rows[x0 .. x1) that have a container in the slot; warp-wide, the lanes resolving 32 entries
+// at a time and the warps taking every nwarps-th group of 32
+template <class F>
+__device__ __forceinline__ void gv_for_each_x(const StoreRef& st, uint32_t x0, uint32_t x1, const uint64_t* xrows, int nX, int slot, uint32_t lo,
+                                              const unsigned long long* cons, int lane, int wid, int nwarps, F f) {
+    for (uint32_t k0 = x0 + (uint32_t)wid * 32; k0 < x1; k0 += (uint32_t)nwarps * 32) {
+        Resolved mine; mine.ptr = nullptr; mine.card = 0; mine.typ = 0; mine.cnt = 0;
+        uint32_t jm = 0;
+        if (k0 + lane < x1) {
+            const RowEnt re = st.rows[k0 + lane];
+            if ((re.mask >> slot) & 1) {
+                int a = 0, b = nX;
+                while (a < b) { const int h = (int)(((unsigned)a + (unsigned)b) >> 1); if (__ldg(xrows + h) < re.row) a = h + 1; else b = h; }
+                if (a < nX && __ldg(xrows + a) == re.row) {
+                    const ContDesc d = st.descs[re.first_desc + __popc(re.mask & ((1u << slot) - 1u))];
+                    mine.ptr = st.payload + (size_t)d.off16 * 16; mine.card = d.card; mine.typ = d.typ; mine.cnt = d.cnt;
+                    jm = (uint32_t)a;
+                }
+            }
+        }
+        unsigned have = __ballot_sync(0xffffffffu, mine.ptr != nullptr);
+        while (have) {
+            const int l = __ffs(have) - 1; have &= have - 1;
+            const uint32_t j = __shfl_sync(0xffffffffu, jm, l);
+            gv_for_each(shfl_resolved(mine, l), lo, cons, lane, [&](uint32_t c) { f(c, j); });
+        }
+    }
+}
+
+// kDistinctRows: x's directory span of the CTA's current unit, rows[gv_x_span[0] .. gv_x_span[1]) (gv_x_entries).  Only the
+// kDistinctRows instantiation references it, so no other kernel holds it in its shared memory.
+__shared__ uint32_t gv_x_span[2];
+
+// kDistinctRows: one range of groupby_values_kernel once the int fields' group indices are in vidx (v.n == 0: made here);
+// called by every thread of the CTA, which leaves it with its shared arrays free for the next range
+__device__ __forceinline__ void gv_rows_range(const StoreRef& st, const GvInts& v, const uint64_t* rowsB, int nB, uint32_t fvB, const uint32_t* fvsB, int nvB,
+                                              uint64_t shard, int slot, uint32_t lo, const unsigned long long* cons, uint16_t* vidx,
+                                              unsigned long long* mag, uint32_t* sign, uint32_t* hist, const uint64_t* xrows, int nX,
+                                              unsigned long long* present) {
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nwarps = kGvThreads / 32;
+    const uint32_t x0 = gv_x_span[0], x1 = gv_x_span[1];
+    const unsigned long long xbits = gv_cell_bits(nX);
+    if (v.n == 0)
+        for (int i = tid; i < (int)kGvRange; i += kGvThreads) vidx[i] = ((cons[i >> 6] >> (i & 63)) & 1ull) ? 0 : kGvNone;
+    if (!rowsB) {                                          // every (group, listed row) met is present
+        __syncthreads();
+        GvMark mk;
+        gv_for_each_x(st, x0, x1, xrows, nX, slot, lo, cons, lane, wid, nwarps, [&](uint32_t c, uint32_t j) {
+            const uint32_t k = vidx[c];
+            if (k != kGvNone) mk.mark(present, (unsigned long long)k * xbits + j);
+        });
+        return;
+    }
+    for (int i = tid; i < (int)kGvRange; i += kGvThreads) mag[i] = 0xffffffffull;        // no position taken, none found
+    for (bool again = true; again;) {                     // one round: each column takes its next listed row of x into mag
+        for (int i = tid; i < (int)kGvRange / 32; i += kGvThreads) sign[i] = 0;
+        __syncthreads();
+        bool hit = false, twice = false;
+        gv_for_each_x(st, x0, x1, xrows, nX, slot, lo, cons, lane, wid, nwarps, [&](uint32_t c, uint32_t j) {
+            if (vidx[c] == kGvNone) return;
+            const unsigned long long m = mag[c];          // (its high half does not change within the round)
+            if (j < (uint32_t)(m >> 32)) return;          // taken in an earlier round
+            hit = true;
+            if ((atomicOr(&sign[c >> 5], 1u << (c & 31)) >> (c & 31)) & 1u) twice = true;
+            atomicMin(&mag[c], (m & ~0xffffffffull) | j);
+        });
+        if (!__syncthreads_or(hit)) return;
+        again = __syncthreads_or(twice);
+        for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
+            const uint32_t j = (uint32_t)mag[i];
+            mag[i] = j == 0xffffffffu ? kGvNoPos : (unsigned long long)j;
+        }
+        __syncthreads();
+        // b's walk marks (b-row, group, position): kDistinct's walks, with the position of this round
+        if (nvB > 1) {
+            uint32_t* bm = hist + wid * 2 * kGvRangeWords;          // this warp's row bitmap, word i as halves 2i, 2i + 1
+            for (int i = lane; i < 2 * kGvRangeWords; i += 32) bm[i] = 0;
+            __syncwarp();
+            for (int br = wid; br < nB; br += nwarps) {
+                const uint64_t row = rowsB[br];
+                for (int v0 = 0; v0 < nvB; v0 += 32) {
+                    Resolved r; r.ptr = nullptr; r.card = 0; r.typ = 0; r.cnt = 0;
+                    if (v0 + lane < nvB) r = resolve(st, fvsB[v0 + lane], shard, row, slot);
+                    unsigned have = __ballot_sync(0xffffffffu, r.ptr != nullptr);
+                    while (have) {
+                        const int l = __ffs(have) - 1; have &= have - 1;
+                        gv_for_each_word(shfl_resolved(r, l), lo, lane, [&](uint32_t i, uint64_t m) {
+                            if ((uint32_t)m) atomicOr(&bm[2 * i], (uint32_t)m);
+                            if (m >> 32) atomicOr(&bm[2 * i + 1], (uint32_t)(m >> 32));
+                        });
+                    }
+                }
+                __syncwarp();
+                const unsigned long long rbit = (unsigned long long)br * (unsigned long long)v.n_groups * xbits;
+                GvMark mk;
+                for (int i = lane; i < kGvRangeWords; i += 32) {
+                    uint64_t m = ((uint64_t)bm[2 * i] | ((uint64_t)bm[2 * i + 1] << 32)) & cons[i];
+                    bm[2 * i] = 0; bm[2 * i + 1] = 0;
+                    while (m) {
+                        const int b = __ffsll((long long)m) - 1; const uint32_t g = vidx[i * 64 + b]; const unsigned long long j = mag[i * 64 + b];
+                        if (g != kGvNone && j != kGvNoPos) mk.mark(present, rbit + (unsigned long long)g * xbits + j);
+                        m &= m - 1;
+                    }
+                }
+                __syncwarp();
+            }
+        } else {
+            for (int b0 = wid * 32; b0 < nB; b0 += nwarps * 32) {
+                Resolved mine; mine.ptr = nullptr; mine.card = 0; mine.typ = 0; mine.cnt = 0;
+                if (b0 + lane < nB) mine = resolve(st, fvB, shard, rowsB[b0 + lane], slot);
+                const int n = min(32, nB - b0);
+                for (int j = 0; j < n; j++) {
+                    const unsigned long long rbit = (unsigned long long)(b0 + j) * (unsigned long long)v.n_groups * xbits;
+                    GvMark mk;
+                    gv_for_each(shfl_resolved(mine, j), lo, cons, lane, [&](uint32_t c) {
+                        const uint32_t k = vidx[c]; const unsigned long long jx = mag[c];
+                        if (k != kGvNone && jx != kGvNoPos) mk.mark(present, rbit + (unsigned long long)k * xbits + jx);
+                    });
+                }
+            }
+        }
+        __syncthreads();                                   // b's walk is done
+        if (again)
+            for (int i = tid; i < (int)kGvRange; i += kGvThreads) {
+                const unsigned long long m = mag[i];
+                if (m != kGvNoPos) mag[i] = ((m + 1) << 32) | 0xffffffffull;           // kGvNoPos: the column is done
+            }
+    }
+}
+
 template <GvAgg kAgg>
 __global__ void __launch_bounds__(kGvThreads, kGvCtasPerSm)
 groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__ values,
@@ -2403,8 +2567,8 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                       unsigned long long* __restrict__ counts /* [nB or 1][v.n_groups], zeroed by the host */,
                       uint32_t fvX = 0, int depthX = 0 /* kSum: the aggregate field's BSI view slot and depth */,
                       unsigned long long* __restrict__ sums = nullptr /* kSum: shaped as counts, zeroed by the host */,
-                      const long long* __restrict__ xvals = nullptr, int nX = 0 /* kDistinct: x's ascending stored values */,
-                      unsigned long long* __restrict__ present = nullptr /* kDistinct: [nB or 1][v.n_groups][ceil(nX / 64)] words, zeroed */) {
+                      const long long* __restrict__ xvals = nullptr, int nX = 0 /* kDistinct: x's ascending stored values; kDistinctRows: its row ids */,
+                      unsigned long long* __restrict__ present = nullptr /* kDistinct*: [nB or 1][v.n_groups][ceil(nX / 64)] words, zeroed */) {
     constexpr bool kSum = kAgg == GvAgg::kSum, kDistinct = kAgg == GvAgg::kDistinct, kX = kSum || kDistinct;
     __shared__ unsigned long long mag[kGvRange];      // (with a multi-view b, the warps' row bitmaps once the groups are made)
     __shared__ uint16_t vidx[kGvRange];               // group index per column
@@ -2424,6 +2588,11 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
         uint64_t any = 0;
         for (int i = tid; i < 1024; i += kGvThreads) any |= cu[i];
         if (!__syncthreads_or(any != 0)) continue;
+        if constexpr (kAgg == GvAgg::kDistinctRows) {
+            if (tid == 0) gv_x_entries(st, fvX, shard, reinterpret_cast<const uint64_t*>(xvals), nX, gv_x_span[0], gv_x_span[1]);
+            __syncthreads();
+            if (gv_x_span[0] == gv_x_span[1]) continue;   // no listed row of x in this shard
+        }
         if (unit_planes)
             for (int k = 0, base = 0; k < v.n; base += v.depth[k] + 1, k++)
                 for (int p = tid; p <= v.depth[k]; p += kGvThreads) planes[base + p] = resolve(st, v.fv[k], shard, (uint64_t)(p + 1), slot);
@@ -2500,6 +2669,10 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
                     }
                 }
                 __syncthreads();
+            }
+            if constexpr (kAgg == GvAgg::kDistinctRows) {
+                gv_rows_range(st, v, rowsB, nB, fvB, fvsB, nvB, shard, slot, lo, cons, vidx, mag, sign, hist, reinterpret_cast<const uint64_t*>(xvals), nX, present);
+                continue;
             }
             if (!rowsB) {
                 if constexpr (kSum) {
@@ -2632,8 +2805,8 @@ groupby_values_kernel(StoreRef st, const GvInts v, const long long* __restrict__
     }
 }
 
-// gv_popcount_kernel (fbgpu_groupby_distinct): out[cell] = the number of bits set in the cell's `words` words of groupby_values_kernel
-// <kDistinct>'s presence bitset; one warp per cell, the lanes striding its words
+// gv_popcount_kernel (fbgpu_groupby_distinct, fbgpu_groupby_distinct_rows): out[cell] = the number of bits set in the cell's
+// `words` words of groupby_values_kernel<kDistinct / kDistinctRows>'s presence bitset; one warp per cell, the lanes striding its words
 __global__ void __launch_bounds__(256)
 gv_popcount_kernel(const unsigned long long* __restrict__ present, long long words, long long n_cells, unsigned long long* __restrict__ out) {
     const int lane = threadIdx.x & 31;

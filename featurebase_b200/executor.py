@@ -1025,8 +1025,8 @@ class Executor:
     # ------------------------------------------------------------------ GroupBy (executeGroupBy :3176)
     def _groupby(self, idx, c, shards):
         """The device returns the dense count tensor over the children's row lists (with aggregate=Sum over an int field, the
-        counts of columns holding a value and their sums, from the same call; with aggregate=Count(Distinct) over an int field,
-        the distinct counts from one more call after one Distinct for the field's values); everything after it is the host-side
+        counts of columns holding a value and their sums, from the same call; with aggregate=Count(Distinct), the distinct
+        counts from one more call after one Distinct for the field's values or rows); everything after it is the host-side
         post-processing executeGroupBy does in Go: previous (iterator start, newGroupByIterator :8779-8826), aggregate=Sum
         (groupByIterator.Next :8893-8911: Count becomes the number of columns holding a value), having (:3388-3406),
         sort (:3130-3162, 3408-3414), offset / limit (:3441-3459).  Results: (group, count) or (group, count, agg)."""
@@ -1090,10 +1090,11 @@ class Executor:
         start = self._groupby_start(c, row_ids)
         if start is None:
             return []
-        dist = None                                               # Count(Distinct) over an int field of this index: per-cell counts
-        if distinct_agg and hasattr(self.ctx, "groupby_distinct") and "index" not in agg_distinct.args and counts.any():
+        dist = None                                               # Count(Distinct) over a field of this index: per-cell counts
+        if distinct_agg and "index" not in agg_distinct.args and counts.any():
             f = idx.fields.get(agg_distinct.args.get("field", agg_distinct.args.get("_field")))
-            if f is not None and f.type == "int":                 # otherwise the per-group Distinct below raises or counts rows
+            call = None if f is None else "groupby_distinct" if f.type == "int" else "groupby_distinct_rows"
+            if call is not None and hasattr(self.ctx, call):      # otherwise the per-group Distinct below raises or runs
                 dist = self._groupby_distinct(idx, fields, row_ids, time_args, int_dims, filt_call, agg_distinct, f, counts.shape, shards)
         has_sort, has_having = "sort" in c.args, isinstance(c.args.get("having"), pql.Call)
         limit = c.args.get("limit") if not (has_sort or has_having) else None       # :3196-3212: no early limit when sorting / filtering
@@ -1155,20 +1156,25 @@ class Executor:
         return self._window(c, out)
 
     GROUPBY_MIXED_MAX = 65535                                     # groups (product of the int children's value counts) per fbgpu_groupby_mixed / _sum / _distinct call
-    # presence bits ((rows of the last set child, or 1) x groups x listed values of x) per fbgpu_groupby_distinct call: 256 MiB
+    # presence bits ((rows of the last set child, or 1) x groups x listed values or rows of x) per fbgpu_groupby_distinct(_rows) call: 256 MiB
     # of device workspace.  A choice that bounds the workspace, not a measured optimum.
     GROUPBY_DISTINCT_BITS = 1 << 31
 
     def _groupby_distinct(self, idx, fields, row_ids, time_args, int_dims, filt_call, agg_distinct, xf, shape, shards):
         """the Count(Distinct(field=xf)) tensor of a GroupBy (shape: the count tensor's), or None when the context answers
-        FBGPU_E_COMM or has no such call (a node): the composition runs instead.  x's listed values are its stored values under
-        filter ∩ Distinct's child (one Distinct, as the int children's lists are made); the device then counts, per cell, those
-        present under filter ∩ Distinct's child ∩ the cell's rows."""
+        FBGPU_E_COMM or has no such call (a node): the composition runs instead.  x's list is, for an int field, its stored values
+        under filter ∩ Distinct's child (one Distinct, as the int children's lists are made), for a set, mutex, bool or time
+        field the rows that hold a column there (one row-count call, as Distinct's set branch); the device then counts, per
+        cell, those present under filter ∩ Distinct's child ∩ the cell's rows."""
         parts = [x for x in (filt_call, *agg_distinct.children[:1]) if isinstance(x, pql.Call)]
         both = (parts[0] if len(parts) == 1 else pql.Call("Intersect", {}, parts)) if parts else None
         ops = self._bitmap_call(idx, both) if both is not None else None
         try:
-            xs = self._int_values(idx, xf, shards, ops)
+            if xf.type == "int":
+                xs = self._int_values(idx, xf, shards, ops)
+            else:
+                rid, cnt = self.ctx.row_counts(idx.id, xf.id, VIEW_STANDARD, shards, filter_ops=ops)
+                xs = np.asarray(sorted(int(r) for r, n in zip(rid, cnt) if n > 0), dtype=np.uint64)
             if len(xs) == 0:
                 return np.zeros(shape, dtype=np.uint64)
             return self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, ops, shards, distinct=(xf, xs))[0]
@@ -1182,12 +1188,13 @@ class Executor:
     def _groupby_tensors(self, idx, fields, row_ids, time_args, int_dims, filt, shards, agg=None, distinct=None):
         """[counts] of a GroupBy with int children (positions int_dims), from fbgpu_groupby_mixed, or with agg (the int field of
         aggregate=Sum) [counts, sums] from fbgpu_groupby_sum, or with distinct = (x, its listed stored values) [distinct counts]
-        from fbgpu_groupby_distinct, where int_dims may be empty: the other children are the set dimensions (a time-range child
+        from fbgpu_groupby_distinct (fbgpu_groupby_distinct_rows, with its listed row ids, when x is not an int field), where
+        int_dims may be empty: the other children are the set dimensions (a time-range child
         with its covering views), the int children's values the trailing dimensions, moved back to the children's order.  No
         Row(v == value) per value and no scratch rows.  When the value lists' product exceeds GROUPBY_MIXED_MAX, each int child's
         list is cut into slices whose product fits and every combination of slices is one call: a column's value lies in exactly
         one slice per field, so the pieces tile the tensors.  x's list is cut so that each call's presence bits stay within
-        GROUPBY_DISTINCT_BITS; the slices are disjoint, so their distinct counts add up per cell."""
+        GROUPBY_DISTINCT_BITS; the slices are disjoint, so their distinct counts add up per cell (a set-like x's list alike)."""
         set_k = [j for j in range(len(fields)) if j not in int_dims]
         set_dims = [(fields[j].id, self._time_view_ids(fields[j], time_args[j]) if time_args[j] else [VIEW_STANDARD], row_ids[j]) for j in set_k]
         stored = [[v - fields[k].base for v in row_ids[k]] for k in int_dims]      # values as the planes hold them (value - Base)
@@ -1207,7 +1214,9 @@ class Executor:
             cut = [slice(s, s + n) for s, n in zip(starts, step)]
             int_part = [(fields[k].id, VIEW_BSI, fields[k].bit_depth, v[c]) for k, v, c in zip(int_dims, stored, cut)]
             for xc in x_cuts:
-                if distinct is not None:
+                if distinct is not None and xf.type != "int":
+                    got = [self.ctx.groupby_distinct_rows(idx.id, set_dims, int_part, (xf.id, VIEW_STANDARD, xc), shards, filter_ops=filt)]
+                elif distinct is not None:
                     got = [self.ctx.groupby_distinct(idx.id, set_dims, int_part, (xf.id, VIEW_BSI, xf.bit_depth, xc), shards, filter_ops=filt)]
                 elif agg is None:
                     got = [self.ctx.groupby_mixed(idx.id, set_dims, int_part, shards, filter_ops=filt)]

@@ -53,7 +53,7 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_groupby_values", "fbgpu_node_groupby_values", "fbgpu_row_counts_views", "fbgpu_node_row_counts_views", "fbgpu_groupby_views",
            "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum",
            "fbgpu_groupby_distinct", "fbgpu_topn_cutoffs", "fbgpu_node_topn_cutoffs", "fbgpu_bsi_sort", "fbgpu_node_bsi_sort",
-           "fbgpu_bsi_distinct", "fbgpu_node_bsi_distinct", "fbgpu_extract_rows"]
+           "fbgpu_bsi_distinct", "fbgpu_node_bsi_distinct", "fbgpu_extract_rows", "fbgpu_groupby_distinct_rows"]
 
 
 def lib_path():
@@ -118,6 +118,8 @@ def load():
     L.fbgpu_groupby_sum.restype = C.c_int
     L.fbgpu_groupby_distinct.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i32, vp, i64, vp]
     L.fbgpu_groupby_distinct.restype = C.c_int
+    L.fbgpu_groupby_distinct_rows.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, vp, vp, u32, u32, vp, i32, vp, i32, vp, i64, vp]
+    L.fbgpu_groupby_distinct_rows.restype = C.c_int
     L.fbgpu_count_pairs.argtypes, L.fbgpu_count_pairs.restype = [vp, u32, u32, u32, vp, u32, u32, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_comm_unique_id.argtypes, L.fbgpu_comm_unique_id.restype = [vp], C.c_int
     L.fbgpu_comm_init.argtypes, L.fbgpu_comm_init.restype = [vp, i32, i32, vp], C.c_int
@@ -613,6 +615,19 @@ class Context:
                                                   g.shards, g.n_shards, out.ctypes.data))
         return out
 
+    def groupby_distinct_rows(self, index, set_dims, int_dims, x, shards, filter_ops=None):
+        """GroupBy(..., aggregate=Count(Distinct(field=x))) over a set, mutex, bool or time field x in one call
+        (fbgpu_groupby_distinct_rows).  set_dims and int_dims as for groupby_sum; x: (field, view, strictly ascending row ids).
+        Returns a uint64 tensor of groupby_mixed's shape: per cell the number of x's listed rows that hold at least one column
+        of filter ∩ the cell's rows."""
+        g = _groupby_args(set_dims, int_dims, shards, filter_ops)
+        xr = _u64arr(x[2])
+        out = np.zeros(g.shape, dtype=np.uint64)
+        self._check(self.L.fbgpu_groupby_distinct_rows(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, g.vfields, g.vviews,
+                                                       g.depths, g.n_ints, g.values, g.n_values, int(x[0]), int(x[1]), xr.ctypes.data, len(xr), g.filter,
+                                                       g.n_filter, g.shards, g.n_shards, out.ctypes.data))
+        return out
+
     def rows_payload_bytes(self, index, field, view, shards, row_ids=None):
         sh = _u64arr(shards)
         pay, nc = C.c_uint64(0), C.c_uint64(0)
@@ -703,6 +718,9 @@ class Node(Context):
 
     def groupby_distinct(self, index, set_dims, int_dims, x, shards, filter_ops=None):
         raise NotImplementedError("fbgpu_groupby_distinct has no node form: the devices' distinct sets merge by union, not by sum")
+
+    def groupby_distinct_rows(self, index, set_dims, int_dims, x, shards, filter_ops=None):
+        raise NotImplementedError("fbgpu_groupby_distinct_rows has no node form: the devices' distinct sets merge by union, not by sum")
 
     def row_counts(self, index, field, view, shards, row_ids=None, filter_ops=None, cap=1 << 20):
         if row_ids is None:

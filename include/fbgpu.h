@@ -440,6 +440,28 @@ int fbgpu_groupby_distinct(fbgpu_ctx *ctx, uint32_t index,
                            uint32_t xfield, uint32_t xview, int32_t x_depth, const int64_t *x_values, int32_t n_x,
                            const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards,
                            uint64_t *out_distinct);
+/* GroupBy(..., aggregate=Count(Distinct(field=x))) over a set, mutex, bool or time field x in one device call (SQL
+ * SELECT a, COUNT(DISTINCT s) ... GROUP BY a over a string, id, stringset or idset column).  The dimensions, limits and
+ * out_distinct's shape and layout are fbgpu_groupby_distinct's.  xfield / xview: a set-like view of x (executeDistinctShardSet
+ * reads the standard view); x_rows: n_x >= 1 strictly ascending row ids, any u64.  Per cell, the number of listed rows x_rows[j]
+ * for which filter ∩ the cell's rows ∩ Row(x = x_rows[j]) holds at least one column: the listed rows among those
+ * fbgpu_row_counts(x, all rows) counts as non-zero under `filter ∩ the cell's rows`.  A column held by several listed rows
+ * counts toward each of them; the data need not be mutex-shaped.  A shard lacking x's fragment contributes nothing; missing set
+ * or int fragments as for fbgpu_groupby_mixed.  Argument errors other than n_rows (those of fbgpu_groupby_distinct, n_x < 1,
+ * x_rows not strictly ascending) are reported before the device check; a presence workspace (rows of the last set dimension,
+ * or 1) x groups x ceil(n_x / 64) x 8 bytes that cannot be allocated gives FBGPU_E_NOMEM.  A context with a communicator
+ * attached returns FBGPU_E_COMM, as fbgpu_groupby_distinct does.  Device cost per 4,096-column range (16 per container
+ * slot): one scan of x's row-directory entries whose ids lie between x_rows[0] and x_rows[n_x - 1], reading the containers of
+ * the listed ones in the range, and one walk of the dimensions' last set field, plus one more of each for every further
+ * listed row a column of the range holds. */
+int fbgpu_groupby_distinct_rows(fbgpu_ctx *ctx, uint32_t index,
+                                const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                                const uint64_t *row_ids_flat, const int32_t *n_rows,
+                                const uint32_t *vfields, const uint32_t *vviews, const int32_t *bit_depths, int32_t n_ints,
+                                const int64_t *values_flat, const int32_t *n_values,
+                                uint32_t xfield, uint32_t xview, const uint64_t *x_rows, int32_t n_x,
+                                const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards,
+                                uint64_t *out_distinct);
 
 /* ---- multi-GPU reduce (replaces the HTTP fan-in of mapReduce/remoteExec, executor.go:6392-6533) ----
  * One context (process) per GPU; rank 0 creates the id, every rank joins.  When a communicator is attached,
