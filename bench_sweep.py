@@ -21,6 +21,9 @@
   config K: GroupBy(Rows(a), aggregate=Count(Distinct(field=x))) and the same with Rows(b) beside a, for x a mutex field of
             100,000 rows and a set field of 64 rows, on config D's data, fbgpu_groupby_distinct_rows against the
             Distinct-per-group composition (only when named in --configs).
+  config G: fbgpu_groupby_sparse against fbgpu_groupby on config S's 256 x 256 GroupBy(Rows(a), Rows(b)), against the host
+            composition (one fbgpu_extract_rows per dimension and a numpy join) for a 1,000,000-row mutex field x a, and paged
+            with limit=1000 (only when named in --configs).
   config N: TopN(f, Row(src=0), tanimotoThreshold=50) and TopN(f, Row(src=0), threshold=100) over --topn-rows rows of varied
             cardinality, fbgpu_topn_cutoffs against the per-shard count-matrix composition (only when named in --configs).
   config O: Sort over config X's 32-bit field with and without a limit, fbgpu_bsi_sort against extracting every value and
@@ -858,6 +861,90 @@ def config_groupby_distinct_rows(args, out):
     real.close()
 
 
+def config_groupby_sparse(args, out):
+    """fbgpu_groupby_sparse over --groupby-shards shards of config S's data (_config_s_world) plus m, a mutex field of 1,000,000
+    rows holding one row for each of the first 16,384 columns of every shard (every shard the same fragment, encoded once), as
+    library calls (no executor):
+      (a) a x b, 256 x 256: the sparse call against fbgpu_groupby (the dense tensor), alternated; the same groups and counts;
+      (b) m x a: the sparse call against the host composition, one fbgpu_extract_rows per dimension over Row(e=0) (a row
+          holding the columns m covers) and a numpy join of the per-column row lists, alternated; the same groups and counts;
+      (c) m x a paged: limit=1000 pages, each starting one past the last cell of the page before, for 8 pages.
+    Wall clock per call (each ends in a device synchronise and a copy to the host), with the call's last_query_gpu_ms."""
+    from featurebase_b200 import executor as X, lib as L, roaring_io
+    S, n_cols = args.groupby_shards, 16384
+    h, idx, fa, fb, ff, fw, fv, load_s = _config_s_world(args, "G")
+    fm, fe = idx.create_field("m", "mutex"), idx.create_field("e")
+    rng = np.random.default_rng(2029)
+    data = roaring_io.encode(np.sort(rng.integers(0, 1_000_000, n_cols).astype(np.uint64) * np.uint64(SW) + np.arange(n_cols, dtype=np.uint64)))
+    every = roaring_io.encode(np.arange(n_cols, dtype=np.uint64))          # e=0: the columns m covers
+    for s_ in range(S):
+        h.ctx.load_fragment(idx.id, fm.id, X.VIEW_STANDARD, s_, data)
+        h.ctx.load_fragment(idx.id, fe.id, X.VIEW_STANDARD, s_, every)
+    h.ctx.commit()
+    ctx, card, sh = h.ctx, _card(), list(range(S))
+    ra, rm = np.arange(256, dtype=np.uint64), np.arange(1_000_000, dtype=np.uint64)
+    dims_ab = [(fa.id, [X.VIEW_STANDARD], ra), (fb.id, [X.VIEW_STANDARD], ra)]
+    dims_ma = [(fm.id, [X.VIEW_STANDARD], rm), (fa.id, [X.VIEW_STANDARD], ra)]
+    m_cols = [L.Op(L.OP_ROW, fe.id, X.VIEW_STANDARD, 0, 0, 0, 0, 0)]
+
+    def composition():
+        cm, om, rows_m, _ = ctx.extract_rows(idx.id, fm.id, X.VIEW_STANDARD, sh, m_cols)
+        ca, oa, rows_a, _ = ctx.extract_rows(idx.id, fa.id, X.VIEW_STANDARD, sh, m_cols)
+        nm, na = np.diff(om.astype(np.int64)), np.diff(oa.astype(np.int64))
+        rep = nm * na                                          # the cells of each column: its m rows x its a rows
+        col = np.repeat(np.arange(len(cm)), rep)
+        k = np.arange(len(col)) - np.repeat(np.cumsum(rep) - rep, rep)
+        im = om[:-1].astype(np.int64)[col] + k // na[col]
+        ia = oa[:-1].astype(np.int64)[col] + k % na[col]
+        cells, counts = np.unique(np.searchsorted(rm, rows_m[im]).astype(np.uint64) * np.uint64(256) + np.searchsorted(ra, rows_a[ia]).astype(np.uint64),
+                                  return_counts=True)
+        return cells, counts.astype(np.uint64)
+
+    def paged():
+        start, got = 0, 0
+        for _ in range(8):
+            c, n = ctx.groupby_sparse(idx.id, dims_ma, sh, start=start, limit=1000)
+            if len(c) == 0:
+                break
+            got += len(c)
+            start = int(c[-1]) + 1
+        return got
+
+    arms = {"a": {"sparse": lambda: ctx.groupby_sparse(idx.id, dims_ab, sh), "dense": lambda: ctx.groupby(idx.id, [fa.id, fb.id], [0, 0], [ra, ra], sh)},
+            "b": {"sparse": lambda: ctx.groupby_sparse(idx.id, dims_ma, sh), "composition": composition},
+            "c": {"sparse_paged": paged}}
+    for part, fns in arms.items():
+        rec = {name: {"wall": [], "gpu_ms": [], "queries": []} for name in fns}
+        res = {}
+        for i in range(1 + args.steps):                          # one warm-up round, then alternate the arms
+            for name in (sorted(fns) if i % 2 == 0 else sorted(fns, reverse=True)):
+                q0 = ctx.counters()["queries"]
+                t1 = time.perf_counter()
+                r = fns[name]()
+                wall = (time.perf_counter() - t1) * 1e3
+                if name == "dense":                              # the dense tensor's non-zero cells, for the comparison
+                    flat = r.reshape(-1)
+                    nz = np.flatnonzero(flat)
+                    r = (nz.astype(np.uint64), flat[nz])
+                res.setdefault(name, r)
+                print(f"config G ({part}): {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                if i >= 1:
+                    rec[name]["wall"].append(wall)
+                    rec[name]["gpu_ms"].append(ctx.counters()["last_query_gpu_ms"])
+                    rec[name]["queries"].append(ctx.counters()["queries"] - q0)
+        vals = list(res.values())
+        if part != "c":
+            assert all(np.array_equal(v[0], vals[0][0]) and np.array_equal(v[1], vals[0][1]) for v in vals), part
+        for name, dd in rec.items():
+            r = res[name]
+            out({"config": "G", "part": part, "arm": name, "gpu": card, "shards": S, "groups": int(r if part == "c" else len(r[0])),
+                 "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])), "wall_ms_max": float(np.max(dd["wall"])),
+                 "last_query_gpu_ms": float(np.median(dd["gpu_ms"])), "queries": int(np.median(dd["queries"])), "steps": len(dd["wall"]),
+                 "load_s": round(load_s, 1),
+                 "note": "median over the timed steps of the call's wall clock, of the last library query's GPU ms and of the library queries"})
+    ctx.close()
+
+
 class _NoTopnCutoffs(_KernelMs):
     """the same proxy without topn_cutoffs: the executor fetches per-shard count matrices and applies the cut-offs on the host"""
 
@@ -1304,6 +1391,8 @@ def main():
             config_groupby_distinct(args, out)
         elif c == "K":
             config_groupby_distinct_rows(args, out)
+        elif c == "G":
+            config_groupby_sparse(args, out)
         elif c == "N":
             config_topn_cutoffs(args, out)
         elif c == "O":

@@ -1375,13 +1375,14 @@ static uint64_t sat_add(uint64_t a, uint64_t b) { return a + b < a ? ~0ull : a +
 
 // w->d_sort as two halves of `cap` elements for the radix sort's ping-pong; half `cur` holds the n kept so far.  An element is a
 // (key, column) pair, [keys | columns] in each half, 32 bytes over both halves, or with keys_only (fbgpu_bsi_distinct) a key
-// alone, 16 bytes.  The buffer outlives the call, like the workspace's other buffers.
+// alone, 16 bytes.  The buffer outlives the call, like the workspace's other buffers; fbgpu_groupby_sparse also sorts in
+// buffers of its own (`buf`).
 struct SortPairs {
-    Workspace* w; uint64_t bound; uint64_t words; uint64_t cap, n = 0; int cur = 0;
-    SortPairs(Workspace* ws, uint64_t max_pairs, bool keys_only = false)
-        : w(ws), bound(max_pairs), words(keys_only ? 1 : 2), cap(ws->d_sort.cap / (16 * words)) {}
+    Workspace* w; DevBuf* buf; uint64_t bound; uint64_t words; uint64_t cap, n = 0; int cur = 0;
+    SortPairs(Workspace* ws, uint64_t max_pairs, bool keys_only = false, DevBuf* b = nullptr)
+        : w(ws), buf(b ? b : &ws->d_sort), bound(max_pairs), words(keys_only ? 1 : 2), cap(buf->cap / (16 * words)) {}
     bool keys_only() const { return words == 1; }
-    unsigned long long* keys(int h) const { return (unsigned long long*)w->d_sort.p + (size_t)h * words * cap; }
+    unsigned long long* keys(int h) const { return (unsigned long long*)buf->p + (size_t)h * words * cap; }
     unsigned long long* cols(int h) const { return keys_only() ? nullptr : keys(h) + cap; }
     // room for `need` elements (need <= bound); a buffer that has to grow takes the kept ones along into its half 0
     int reserve(uint64_t need) {
@@ -1395,7 +1396,7 @@ struct SortPairs {
             if (!keys_only()) CUDA_TRY(cudaMemcpyAsync((unsigned long long*)nb.p + nc, cols(cur), n * 8, cudaMemcpyDeviceToDevice, w->stream));
             CUDA_TRY(cudaStreamSynchronize(w->stream));
         }
-        w->d_sort.release(); w->d_sort = nb; cap = nc; cur = 0;
+        buf->release(); *buf = nb; cap = nc; cur = 0;
         return 0;
     }
 };
@@ -2647,6 +2648,269 @@ extern "C" int fbgpu_groupby_distinct_rows(fbgpu_ctx* c, uint32_t index, const u
     return groupby_run(c, index, GbRequest{ gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows),
                                             gb_int_dims(vfields, vviews, bit_depths, n_ints, values_flat, n_values), GvAgg::kDistinctRows,
                                             x, filter, n_filter_ops, shards, n_shards }, out_distinct);
+} FBGPU_CATCH
+
+// ------------------------------------------------------------------ GroupBy as a sorted list of its non-empty groups
+// (sparse_rows_kernel, sparse_join_kernel, kernels.cuh).  A cell is the row-major flat index of fbgpu_groupby_views' tensor.
+// Per evaluation batch of units: the filter is evaluated (none: every column counts), and the count pass of sparse_rows_kernel
+// gives each unit its hits per dimension; units that miss a dimension are dropped, and the rest are cut into chunks of at most
+// kSortChunk hits per dimension.  Per chunk, each dimension's (column, list index) keys are emitted, sorted and, over several
+// views, deduped.  sparse_join_kernel turns dimension 0's entries, in ranges of at most kSortChunk cells, into the cells
+// >= start; the cells are sorted and run-length coded into (cell, count), and merged into the call's running list by a sort of
+// (cell, count) pairs and a sum of equal cells.  With a limit, the list is cut to its first `limit` cells after each merge, and
+// once it holds that many, cells past its last one are not emitted.
+
+// the argument checks fbgpu_groupby_sparse and its node form make before any device is touched
+static int groupby_sparse_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                               const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
+                               const uint64_t* shards, int64_t n_shards, const uint64_t* out_cells, const uint64_t* out_counts, uint64_t cap,
+                               const uint64_t* out_n) {
+    if (!handle || !fields || !views_flat || !n_views || !row_ids_flat || !n_rows || !out_n || (cap && (!out_cells || !out_counts)) ||
+        n_filter_ops < 0 || (n_filter_ops && !filter) || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
+    if (n_fields < 1 || n_fields > kSpMaxDims) return fail(FBGPU_E_INVALID, "n_fields=%d outside 1..%d", n_fields, kSpMaxDims);
+    const uint64_t* rows = row_ids_flat;
+    uint64_t cells = 1;
+    for (int32_t i = 0; i < n_fields; i++) {
+        if (n_views[i] < 1) return fail(FBGPU_E_INVALID, "n_views[%d]=%d < 1", i, n_views[i]);
+        if (n_rows[i] < 1) return fail(FBGPU_E_INVALID, "n_rows[%d]=%d < 1", i, n_rows[i]);
+        for (int32_t k = 1; k < n_rows[i]; k++)
+            if (rows[k] <= rows[k - 1]) return fail(FBGPU_E_INVALID, "row_ids[%d] are not strictly ascending at position %d", i, k);
+        if (cells > ~0ull / (uint64_t)n_rows[i]) return fail(FBGPU_E_INVALID, "product of n_rows exceeds 2^64 - 1");
+        cells *= (uint64_t)n_rows[i];
+        rows += n_rows[i];
+    }
+    return 0;
+}
+
+// device buffers of one fbgpu_groupby_sparse call, freed when it returns: they can be large, and are not reused by other calls
+struct SparseBufs {
+    DevBuf b[kSpMaxDims + 2];
+    ~SparseBufs() { for (DevBuf& x : b) x.release(); }
+};
+
+// the sorted cells of cs into (cell, count) pairs merged into acc, whose cells are distinct and sorted; then acc cut to its first
+// `limit` cells (limit < 0: no cut), and *hi lowered to one past its last cell once it holds that many
+static int sparse_merge(Query& q, SortPairs& cs, SortPairs& acc, int bits, int64_t limit, unsigned long long* hi) {
+    Workspace* w = q.w;
+    const uint64_t n = cs.n, n_tiles = (n + kSortTile - 1) / kSortTile;
+    if (w->d_counts.ensure((size_t)(n_tiles + 1) * 4) || w->h_out.ensure(8)) return FBGPU_E_NOMEM;
+    unsigned int* counts = (unsigned int*)w->d_counts.p;
+    distinct_heads_kernel<<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(cs.keys(cs.cur), n, counts);
+    CUDA_TRY(cudaGetLastError());
+    sort_scan_kernel<<<1, kSortScanThreads, 0, w->stream>>>(counts, n_tiles + 1);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, counts + n_tiles, 4, cudaMemcpyDeviceToHost, w->stream));
+    CUDA_TRY(cudaStreamSynchronize(w->stream));
+    const uint64_t u = *(const unsigned int*)w->h_out.p;
+    int rc = acc.reserve(acc.n + u); if (rc) return rc;
+    unsigned long long* pos = cs.keys(1 - cs.cur);          // the sort's free half: the runs' first positions
+    sparse_compact_kernel<false><<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(cs.keys(cs.cur), nullptr, n, counts, acc.keys(acc.cur) + acc.n, pos);
+    CUDA_TRY(cudaGetLastError());
+    const unsigned grid = (unsigned)std::min<uint64_t>((u + 255) / 256, (uint64_t)q.c->sm_count * 8);
+    sparse_run_lengths_kernel<<<grid, 256, 0, w->stream>>>(pos, u, n, acc.cols(acc.cur) + acc.n);
+    CUDA_TRY(cudaGetLastError());
+    q.launches += 4;
+    const bool merge = acc.n > 0;
+    acc.n += u;
+    if (merge) {
+        rc = sort_pairs(q, acc, bits, ~0ull); if (rc) return rc;
+        const uint64_t m = acc.n, m_tiles = (m + kSortTile - 1) / kSortTile;
+        if (w->d_counts.ensure((size_t)(m_tiles + 1) * 4)) return FBGPU_E_NOMEM;
+        counts = (unsigned int*)w->d_counts.p;
+        distinct_heads_kernel<<<(unsigned)m_tiles, kSortThreads, 0, w->stream>>>(acc.keys(acc.cur), m, counts);
+        CUDA_TRY(cudaGetLastError());
+        sort_scan_kernel<<<1, kSortScanThreads, 0, w->stream>>>(counts, m_tiles + 1);
+        CUDA_TRY(cudaGetLastError());
+        sparse_compact_kernel<true><<<(unsigned)m_tiles, kSortThreads, 0, w->stream>>>(acc.keys(acc.cur), acc.cols(acc.cur), m, counts,
+                                                                                      acc.keys(1 - acc.cur), acc.cols(1 - acc.cur));
+        CUDA_TRY(cudaGetLastError());
+        q.launches += 3;
+        acc.cur = 1 - acc.cur;
+        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, counts + m_tiles, 4, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        acc.n = *(const unsigned int*)w->h_out.p;
+    }
+    if (limit >= 0 && acc.n >= (uint64_t)limit) {
+        acc.n = (uint64_t)limit;
+        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, acc.keys(acc.cur) + acc.n - 1, 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        *hi = *(const uint64_t*)w->h_out.p + 1;
+    }
+    return 0;
+}
+
+// the non-empty cells >= start of the dimensions `dims` under the filter, ascending, at most `limit` of them (limit < 0: all), and
+// their counts (store lock held)
+static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<GbDim>& dims, const fbgpu_op* filter, int32_t n_filter_ops,
+                              const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
+                              std::vector<uint64_t>& cells, std::vector<uint64_t>& counts) {
+    cells.clear(); counts.clear();
+    const int nd = (int)dims.size();
+    Query q(c); Workspace* w = q.w;
+    const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);
+    const bool have_filter = n_filter_ops > 0;
+    int rc = have_filter ? q.open(index, filter, n_filter_ops, sorted.data(), (int64_t)sorted.size()) : q.open(sorted.data(), (int64_t)sorted.size());
+    if (rc) return rc;
+    if (limit == 0) { q.finish(); return FBGPU_OK; }
+    SparseBufs sb;                    // b[d]: dimension d's keys; b[nd]: the cells; b[kSpMaxDims + 1]: two cursors, the row lists, the view slots
+    SpJoin jn{}; jn.nd = nd; jn.lo = start; jn.hi = ~0ull;
+    // b[kSpMaxDims + 1]: [cursor | rows of every dimension (u64) | view slots of every dimension (u32)]
+    std::vector<uint64_t> rows_h(1, 0);
+    std::vector<uint32_t> fvs_h;
+    std::vector<size_t> row_at(nd), fv_at(nd); std::vector<int> n_fv(nd);
+    for (int d = 0; d < nd; d++) {
+        row_at[d] = rows_h.size(); rows_h.insert(rows_h.end(), dims[d].rows, dims[d].rows + dims[d].n_rows);
+        const std::vector<uint32_t> fvs = view_slots(c, index, dims[d].field, dims[d].views, dims[d].n_views);
+        fv_at[d] = fvs_h.size(); n_fv[d] = (int)fvs.size(); fvs_h.insert(fvs_h.end(), fvs.begin(), fvs.end());
+    }
+    DevBuf& meta = sb.b[kSpMaxDims + 1];
+    if (meta.ensure(rows_h.size() * 8 + fvs_h.size() * 4)) return FBGPU_E_NOMEM;
+    unsigned long long* cursor = (unsigned long long*)meta.p;
+    const uint64_t* d_rows = (const uint64_t*)meta.p;
+    const uint32_t* d_fv0 = (const uint32_t*)(d_rows + rows_h.size());
+    CUDA_TRY(cudaMemcpyAsync(meta.p, rows_h.data(), rows_h.size() * 8, cudaMemcpyHostToDevice, w->stream));
+    CUDA_TRY(cudaMemcpyAsync((void*)d_fv0, fvs_h.data(), fvs_h.size() * 4, cudaMemcpyHostToDevice, w->stream));
+    CUDA_TRY(cudaStreamSynchronize(w->stream));
+    uint64_t total = 1;
+    for (int d = nd - 1; d >= 0; d--) { jn.stride[d] = total; total *= (uint64_t)dims[d].n_rows; jn.jbits[d] = bit_width((uint64_t)dims[d].n_rows - 1); }
+    const int cell_bits = bit_width(total - 1);
+    std::vector<SortPairs> dk;
+    for (int d = 0; d < nd; d++) dk.emplace_back(w, ~0ull, true, &sb.b[d]);
+    SortPairs cs(w, ~0ull, true, &sb.b[nd]), acc(w, ~0ull);
+    const long long batch = std::min<long long>(c->unit_batch, 1ll << 16);     // a unit's place in a chunk takes 16 bits of a key
+    std::vector<uint32_t> units, keep, chunk;
+    std::vector<uint64_t> ucnt;
+    for (long long u0 = 0; u0 < q.n_units; u0 += batch) {
+        const long long nu = std::min(batch, q.n_units - u0);
+        CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
+        units.clear();
+        if (have_filter) {
+            const uint2* info;
+            rc = q.eval_info(u0, nu, info); if (rc) return rc;
+            for (long long u = 0; u < nu; u++) if (info[u].x) units.push_back((uint32_t)u);
+        } else {
+            for (long long u = 0; u < nu; u++) units.push_back((uint32_t)u);
+        }
+        if (units.empty()) continue;
+        const uint4* bitmaps = have_filter ? (const uint4*)w->d_bitmaps.p : nullptr;
+        const uint64_t* bshards = q.d_shards + u0 / kSlotsPerRow;
+        const size_t nun = units.size();
+        // count pass: the hits of every unit in every dimension
+        if (w->d_emit_units.ensure(nun * 4) || w->d_cells.ensure(nun * nd * 8) || w->h_out.ensure(nun * nd * 8)) return FBGPU_E_NOMEM;
+        CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, units.data(), nun * 4, cudaMemcpyHostToDevice, w->stream));
+        CUDA_TRY(cudaMemsetAsync(w->d_cells.p, 0, nun * nd * 8, w->stream));
+        const unsigned grid = (unsigned)std::min<size_t>(nun, (size_t)c->sm_count * 8);
+        for (int d = 0; d < nd; d++) {
+            sparse_rows_kernel<SrOut::kCount><<<grid, kSrThreads, 0, w->stream>>>(store_ref(c), d_fv0 + fv_at[d], n_fv[d], d_rows + row_at[d], dims[d].n_rows, jn.jbits[d],
+                bitmaps, (const uint32_t*)w->d_emit_units.p, (int)nun, bshards, (unsigned long long*)w->d_cells.p + (size_t)d * nun, nullptr, nullptr);
+            CUDA_TRY(cudaGetLastError()); q.launches++;
+        }
+        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_cells.p, nun * nd * 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        ucnt.assign((const uint64_t*)w->h_out.p, (const uint64_t*)w->h_out.p + nun * nd);
+        keep.clear();                                        // the units every dimension meets, as their places in `units`
+        for (size_t e = 0; e < nun; e++) {
+            bool all = true;
+            for (int d = 0; d < nd && all; d++) all = ucnt[(size_t)d * nun + e] > 0;
+            if (all) keep.push_back((uint32_t)e);
+        }
+        for (size_t a = 0; a < keep.size();) {
+            // the chunk keep[a, b): at most kSortChunk hits per dimension (at least one unit)
+            std::vector<uint64_t> hits(nd, 0);
+            size_t b = a;
+            for (; b < keep.size(); b++) {
+                bool fits = true;
+                for (int d = 0; d < nd; d++) fits = fits && hits[d] + ucnt[(size_t)d * nun + keep[b]] <= kSortChunk;
+                if (!fits && b > a) break;
+                for (int d = 0; d < nd; d++) hits[d] += ucnt[(size_t)d * nun + keep[b]];
+            }
+            chunk.clear();
+            for (size_t k = a; k < b; k++) chunk.push_back(units[keep[k]]);
+            const int ebits = bit_width(chunk.size() - 1);
+            if (w->d_emit_units.ensure(chunk.size() * 4)) return FBGPU_E_NOMEM;
+            CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, chunk.data(), chunk.size() * 4, cudaMemcpyHostToDevice, w->stream));
+            const unsigned cgrid = (unsigned)std::min<size_t>(chunk.size(), (size_t)c->sm_count * 8);
+            for (int d = 0; d < nd; d++) {
+                SortPairs& k = dk[(size_t)d];
+                k.n = 0;
+                rc = k.reserve(hits[d]); if (rc) return rc;
+                CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
+                sparse_rows_kernel<SrOut::kEmit><<<cgrid, kSrThreads, 0, w->stream>>>(store_ref(c), d_fv0 + fv_at[d], n_fv[d], d_rows + row_at[d], dims[d].n_rows, jn.jbits[d],
+                    bitmaps, (const uint32_t*)w->d_emit_units.p, (int)chunk.size(), bshards, nullptr, cursor, k.keys(k.cur));
+                CUDA_TRY(cudaGetLastError()); q.launches++;
+                k.n = hits[d];
+                const int kbits = ebits + 16 + jn.jbits[d];
+                rc = n_fv[d] > 1 ? distinct_keys(q, k, kbits) : sort_pairs(q, k, kbits, ~0ull); if (rc) return rc;
+                jn.keys[d] = k.keys(k.cur); jn.n[d] = k.n;
+            }
+            // the join, over ranges of dimension 0's entries that give at most kSortChunk cells (at least one entry)
+            const uint64_t n0 = jn.n[0];
+            const unsigned jgrid = (unsigned)std::min<uint64_t>((n0 + 255) / 256, (uint64_t)c->sm_count * 8);
+            for (uint64_t e0 = 0; e0 < n0;) {
+                uint64_t e1 = n0, got = 0;
+                for (;;) {
+                    CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
+                    sparse_join_kernel<SrOut::kCount><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, nullptr);
+                    CUDA_TRY(cudaGetLastError()); q.launches++;
+                    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, cursor, 8, cudaMemcpyDeviceToHost, w->stream));
+                    CUDA_TRY(cudaStreamSynchronize(w->stream));
+                    got = *(const uint64_t*)w->h_out.p;
+                    if (got <= kSortChunk || e1 - e0 == 1) break;
+                    e1 = e0 + (e1 - e0) / 2;
+                }
+                if (got) {
+                    cs.n = 0;
+                    rc = cs.reserve(got); if (rc) return rc;
+                    CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
+                    sparse_join_kernel<SrOut::kEmit><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, cs.keys(cs.cur));
+                    CUDA_TRY(cudaGetLastError()); q.launches++;
+                    cs.n = got;
+                    rc = sort_pairs(q, cs, cell_bits, ~0ull); if (rc) return rc;
+                    rc = sparse_merge(q, cs, acc, cell_bits, limit, &jn.hi); if (rc) return rc;
+                }
+                e0 = e1;
+            }
+            a = b;
+        }
+        CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        q.add_elapsed();
+    }
+    cells.resize(acc.n); counts.resize(acc.n);
+    if (acc.n) {
+        CUDA_TRY(cudaMemcpyAsync(cells.data(), acc.keys(acc.cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaMemcpyAsync(counts.data(), acc.cols(acc.cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+    }
+    q.finish();
+    return FBGPU_OK;
+}
+
+// a (cell, count) list into the caller's arrays under the NOSPACE contract: *out_n = its size, nothing written when it exceeds cap
+static int write_cells(const std::vector<uint64_t>& cells, const std::vector<uint64_t>& counts, uint64_t* out_cells, uint64_t* out_counts, uint64_t cap, uint64_t* out_n) {
+    *out_n = cells.size();
+    if (cells.size() > cap) return fail(FBGPU_E_NOSPACE, "output needs room for %llu cells", (unsigned long long)cells.size());
+    if (!cells.empty()) { memcpy(out_cells, cells.data(), cells.size() * 8); memcpy(out_counts, counts.data(), counts.size() * 8); }
+    return FBGPU_OK;
+}
+
+// GroupBy over set-like dimensions of any number of rows: fbgpu_groupby_views' cells, as the sorted list of the non-empty ones
+// from `start` on, at most `limit` of them (executeGroupBy's walk of groupByIterator, executor.go:3176, with previous= / limit=)
+extern "C" int fbgpu_groupby_sparse(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                    const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
+                                    const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
+                                    uint64_t* out_cells, uint64_t* out_counts, uint64_t cap, uint64_t* out_n) try {
+    int rc = groupby_sparse_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards,
+                                 out_cells, out_counts, cap, out_n);
+    if (rc) return rc;
+    if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_groupby_sparse is local to one context: group lists merge by cell, not by an all-reduce");
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    std::vector<uint64_t> cells, counts;
+    rc = groupby_sparse_run(c, index, gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows), filter, n_filter_ops, shards, n_shards,
+                            start, limit, cells, counts);
+    if (rc) return rc;
+    return write_cells(cells, counts, out_cells, out_counts, cap, out_n);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ comm

@@ -2820,6 +2820,224 @@ gv_popcount_kernel(const unsigned long long* __restrict__ present, long long wor
     }
 }
 
+// ------------------------------------------------------------------ GroupBy as a sorted list of its non-empty groups (fbgpu_groupby_sparse)
+// Per evaluation batch and dimension, sparse_rows_kernel runs one CTA per listed (shard, slot) unit.  It stages the unit's filter
+// bitmap (all ones without a filter) and walks, in each view of the dimension, the fragment's directory entries whose ids lie
+// between the first and the last listed row (gv_x_entries).  The lanes take 32 entries at a time and binary-search each id in
+// the list, so the cost follows the fragment's directory and containers, not the list's length.  Every filter column that the
+// container of listed row j holds is a hit (e the unit's place in the launch's unit list, c the column in the slot):
+//   kCount: counts[e] += the unit's hits.
+//   kEmit:  the key ((e << 16 | c) << jbits) | j at keys[(*cursor)++].  Warps reserve their hits with one atomic, so the order
+//           is arbitrary: the host sorts the keys, and dedupes them when a row is present in several views.
+enum class SrOut { kCount, kEmit };
+constexpr int kSrThreads = 256;
+
+// one warp-wide step of sparse_rows_kernel: each lane holds the hit mask x of word wi of the unit (0: none)
+template <SrOut kOut>
+__device__ __forceinline__ void sr_hits(uint64_t x, uint32_t wi, uint32_t e, uint32_t j, int jbits, int lane, unsigned long long& hits,
+                                        unsigned long long* cursor, unsigned long long* keys) {
+    const uint32_t n = (uint32_t)__popcll(x);
+    uint32_t inc = n;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += y; }
+    const uint32_t total = __shfl_sync(0xffffffffu, inc, 31);
+    if (total == 0) return;
+    if (kOut == SrOut::kCount) { hits += total; return; }
+    unsigned long long at = 0;
+    if (lane == 0) at = atomicAdd(cursor, (unsigned long long)total);
+    at = __shfl_sync(0xffffffffu, at, 0) + (inc - n);
+    while (x) {
+        const int bit = __ffsll((long long)x) - 1; x &= x - 1;
+        keys[at++] = ((((unsigned long long)e << 16) | (wi * 64 + (uint32_t)bit)) << jbits) | j;
+    }
+}
+
+template <SrOut kOut>
+__global__ void __launch_bounds__(kSrThreads)
+sparse_rows_kernel(StoreRef st, const uint32_t* __restrict__ fvs, int nv, const uint64_t* __restrict__ rows, int n_rows, int jbits,
+                   const uint4* __restrict__ bitmaps /* null: no filter */, const uint32_t* __restrict__ units, int n_units,
+                   const uint64_t* __restrict__ shards, unsigned long long* __restrict__ counts, unsigned long long* __restrict__ cursor,
+                   unsigned long long* __restrict__ keys) {
+    __shared__ __align__(16) uint64_t base[1024];
+    __shared__ uint32_t span[2];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nwarps = kSrThreads / 32;
+    for (int e = blockIdx.x; e < n_units; e += gridDim.x) {
+        const uint32_t u = units[e];                       // the unit in the batch: shards[u / 16], slot u % 16
+        const uint64_t shard = shards[u / kSlotsPerRow]; const int slot = (int)(u % kSlotsPerRow);
+        __syncthreads();                                   // the previous unit's readers are done
+        const uint64_t* src = bitmaps ? reinterpret_cast<const uint64_t*>(bitmaps + (size_t)u * 512) : nullptr;
+        for (int i = tid; i < 1024; i += kSrThreads) base[i] = src ? src[i] : ~0ull;
+        unsigned long long hits = 0;
+        for (int v = 0; v < nv; v++) {
+            __syncthreads();                               // base is staged; the previous view's span has been read
+            if (tid == 0) gv_x_entries(st, fvs[v], shard, rows, n_rows, span[0], span[1]);
+            __syncthreads();
+            const uint32_t x0 = span[0], x1 = span[1];
+            for (uint32_t k0 = x0 + (uint32_t)wid * 32; k0 < x1; k0 += (uint32_t)nwarps * 32) {
+                const void* mine = nullptr; uint32_t card = 0, meta = 0, jm = 0;
+                if (k0 + lane < x1) {
+                    const RowEnt re = st.rows[k0 + lane];
+                    if ((re.mask >> slot) & 1) {
+                        int a = 0, b = n_rows;
+                        while (a < b) { const int h = (int)(((unsigned)a + (unsigned)b) >> 1); if (__ldg(rows + h) < re.row) a = h + 1; else b = h; }
+                        if (a < n_rows && __ldg(rows + a) == re.row) {
+                            const ContDesc d = st.descs[re.first_desc + __popc(re.mask & ((1u << slot) - 1u))];
+                            mine = st.payload + (size_t)d.off16 * 16; card = d.card; meta = ((uint32_t)d.typ << 16) | d.cnt; jm = (uint32_t)a;
+                        }
+                    }
+                }
+                unsigned have = __ballot_sync(0xffffffffu, mine != nullptr);
+                while (have) {
+                    const int l = __ffs(have) - 1; have &= have - 1;
+                    const void* ptr = (const void*)__shfl_sync(0xffffffffu, (unsigned long long)mine, l);
+                    const uint32_t n = __shfl_sync(0xffffffffu, card, l), m = __shfl_sync(0xffffffffu, meta, l), j = __shfl_sync(0xffffffffu, jm, l);
+                    const uint32_t typ = m >> 16, cnt = m & 0xffffu;
+                    if (typ == kArray) {
+                        const uint16_t* a = reinterpret_cast<const uint16_t*>(ptr);
+                        for (uint32_t i0 = 0; i0 < n; i0 += 32) {
+                            uint64_t x = 0; uint32_t wi = 0;
+                            if (i0 + lane < n) { const uint32_t cc = __ldg(a + i0 + lane); wi = cc >> 6; x = base[wi] & (1ull << (cc & 63)); }
+                            sr_hits<kOut>(x, wi, (uint32_t)e, j, jbits, lane, hits, cursor, keys);
+                        }
+                    } else if (typ == kBitmap) {
+                        const uint64_t* g = reinterpret_cast<const uint64_t*>(ptr);
+                        for (int i = lane; i < 1024; i += 32) sr_hits<kOut>(__ldg(g + i) & base[i], (uint32_t)i, (uint32_t)e, j, jbits, lane, hits, cursor, keys);
+                    } else {
+                        const uint32_t* r32 = reinterpret_cast<const uint32_t*>(ptr);
+                        for (uint32_t r = 0; r < cnt; r++) {              // the warp walks each interval's words together
+                            const uint32_t iv = __ldg(r32 + r), s0 = iv & 0xffffu, l0 = iv >> 16;
+                            for (uint32_t i0 = s0 >> 6; i0 <= (l0 >> 6); i0 += 32) {
+                                const uint32_t i = i0 + (uint32_t)lane;
+                                uint64_t x = 0;
+                                if (i <= (l0 >> 6)) {
+                                    uint64_t mk = ~0ull;
+                                    if (i == (s0 >> 6)) mk &= ~0ull << (s0 & 63);
+                                    if (i == (l0 >> 6)) mk &= ~0ull >> (63 - (l0 & 63));
+                                    x = base[i] & mk;
+                                }
+                                sr_hits<kOut>(x, i, (uint32_t)e, j, jbits, lane, hits, cursor, keys);
+                            }
+                        }
+                    }
+                }
+            }
+        }
+        if (kOut == SrOut::kCount && lane == 0 && hits) atomicAdd(&counts[e], hits);
+    }
+}
+
+// sparse_join_kernel: the dimensions' sorted keys of one chunk, keys[d][0 .. n[d]), each (column << jbits[d]) | list index.  Per
+// entry e of dimension 0 in [e0, e1), the column's entries in every other dimension are found by binary search, and their cross
+// product gives the flat cells Σ_d j_d · stride[d] that lie in [lo, hi).  A column missing from any dimension gives none.
+//   kCount: *cursor += the cells.
+//   kEmit:  the cells at cells[(*cursor)++], reserved per warp; the host sorts them.
+constexpr int kSpMaxDims = 8;
+struct SpJoin {
+    const unsigned long long* keys[kSpMaxDims]; unsigned long long n[kSpMaxDims], stride[kSpMaxDims]; int jbits[kSpMaxDims]; int nd;
+    unsigned long long lo, hi;
+};
+
+__device__ __forceinline__ unsigned long long sp_lower_bound(const unsigned long long* k, unsigned long long n, unsigned long long key) {
+    unsigned long long a = 0, b = n;
+    while (a < b) { const unsigned long long m = (a + b) >> 1; if (__ldg(k + m) < key) a = m + 1; else b = m; }
+    return a;
+}
+
+template <SrOut kOut>
+__global__ void __launch_bounds__(256)
+sparse_join_kernel(SpJoin jn, unsigned long long e0, unsigned long long e1, unsigned long long* __restrict__ cursor, unsigned long long* __restrict__ cells) {
+    const int lane = threadIdx.x & 31;
+    const unsigned long long step = (unsigned long long)gridDim.x * blockDim.x;
+    for (unsigned long long e = e0 + (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; e - threadIdx.x % 32 < e1; e += step) {   // whole warps
+        unsigned long long lo[kSpMaxDims], hi[kSpMaxDims], idx[kSpMaxDims];
+        unsigned long long c0 = 0, n = 0;
+        bool any = e < e1;
+        if (any) {
+            const unsigned long long k0 = jn.keys[0][e];
+            const unsigned long long col = k0 >> jn.jbits[0];
+            c0 = (k0 & ((1ull << jn.jbits[0]) - 1ull)) * jn.stride[0];
+            any = c0 + jn.stride[0] > jn.lo && c0 < jn.hi;            // the cells of this j0 are [c0, c0 + stride[0])
+            for (int d = 1; d < jn.nd && any; d++) {
+                lo[d] = sp_lower_bound(jn.keys[d], jn.n[d], col << jn.jbits[d]);
+                hi[d] = sp_lower_bound(jn.keys[d], jn.n[d], (col + 1) << jn.jbits[d]);
+                idx[d] = lo[d];
+                any = lo[d] < hi[d];
+            }
+        }
+        // the cross product in odometer order, the last dimension fastest; pass 0 counts the cells in [lo, hi), pass 1 writes them
+        unsigned long long at = 0;
+        for (int pass = 0; pass < (kOut == SrOut::kEmit ? 2 : 1); pass++) {
+            if (pass == 1) {
+                unsigned long long inc = n;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += y; }
+                const unsigned long long total = __shfl_sync(0xffffffffu, inc, 31);
+                if (lane == 31 && total) at = atomicAdd(cursor, total);
+                at = __shfl_sync(0xffffffffu, at, 31) + inc - n;
+            }
+            if (!any) continue;
+            for (int d = 1; d < jn.nd; d++) idx[d] = lo[d];
+            for (;;) {
+                unsigned long long cell = c0;
+                for (int d = 1; d < jn.nd; d++) cell += (__ldg(jn.keys[d] + idx[d]) & ((1ull << jn.jbits[d]) - 1ull)) * jn.stride[d];
+                if (cell >= jn.lo && cell < jn.hi) { if (pass == 0) n++; else cells[at++] = cell; }
+                int d = jn.nd - 1;
+                while (d >= 1 && ++idx[d] == hi[d]) { idx[d] = lo[d]; d--; }
+                if (d < 1) break;
+            }
+        }
+        if (kOut == SrOut::kCount) {
+#pragma unroll
+            for (int o = 16; o; o >>= 1) n += __shfl_down_sync(0xffffffffu, n, o);
+            if (lane == 0 && n) atomicAdd(cursor, n);
+        }
+    }
+}
+
+// the runs of n sorted keys, one per head (distinct_heads_kernel's heads, offsets from sort_scan_kernel), written in order as
+// distinct_compact_kernel writes them, each with a value: kSum == false, the head's position (sparse_run_lengths_kernel turns
+// the positions into run lengths); kSum == true, vals_in of the head plus that of the next key when it is equal (the caller's
+// runs are at most two long: two lists of distinct keys merged)
+template <bool kSum>
+__global__ void __launch_bounds__(kSortThreads)
+sparse_compact_kernel(const unsigned long long* __restrict__ keys_in, const unsigned long long* __restrict__ vals_in, unsigned long long n,
+                      const unsigned int* __restrict__ offs, unsigned long long* __restrict__ keys_out, unsigned long long* __restrict__ vals_out) {
+    __shared__ unsigned int wbase[kSortThreads / 32];
+    __shared__ unsigned int run;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const unsigned int lt = (1u << lane) - 1u;
+    if (tid == 0) run = offs[blockIdx.x];
+    const unsigned long long t0 = (unsigned long long)blockIdx.x * kSortTile;
+    for (int r = 0; r < kSortRounds; r++) {
+        const unsigned long long i = t0 + (unsigned long long)r * kSortThreads + tid;
+        unsigned long long key = 0;
+        bool head = false;
+        if (i < n) { key = keys_in[i]; head = i == 0 || key != keys_in[i - 1]; }
+        const unsigned int bal = __ballot_sync(0xffffffffu, head);
+        if (lane == 0) wbase[wid] = (unsigned int)__popc(bal);
+        __syncthreads();
+        if (tid == 0) {
+            unsigned int o = run;
+            for (int k = 0; k < kSortThreads / 32; k++) { const unsigned int x = wbase[k]; wbase[k] = o; o += x; }
+            run = o;
+        }
+        __syncthreads();
+        if (head) {
+            const unsigned int p = wbase[wid] + (unsigned int)__popc(bal & lt);
+            keys_out[p] = key;
+            vals_out[p] = kSum ? vals_in[i] + (i + 1 < n && keys_in[i + 1] == key ? vals_in[i + 1] : 0ull) : i;
+        }
+        __syncthreads();                                   // (wbase is rewritten by the next round)
+    }
+}
+
+// lens[k] = the length of run k of n keys whose u runs start at pos[0 .. u)
+__global__ void __launch_bounds__(256)
+sparse_run_lengths_kernel(const unsigned long long* __restrict__ pos, unsigned long long u, unsigned long long n, unsigned long long* __restrict__ lens) {
+    for (unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; k < u; k += (unsigned long long)gridDim.x * blockDim.x)
+        lens[k] = (k + 1 < u ? pos[k + 1] : n) - pos[k];
+}
+
 // ------------------------------------------------------------------------------------------------
 // arena_gather_kernel (fbgpu_compact): copies containers one by one from the old payload arena into the new one — one warp per
 // container, 16 bytes per lane and step.  Used for fragments that fbgpu_apply_containers left with holes.

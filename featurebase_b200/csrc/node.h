@@ -334,6 +334,41 @@ extern "C" int fbgpu_node_groupby_sum(fbgpu_node* n, uint32_t index, const uint3
                                              filter, n_filter_ops, shards, n_shards }, out_counts, out_sums);
 } FBGPU_CATCH
 
+// GroupBy as a list of non-empty cells: every device lists its own shards' cells from `start` on, at most `limit`; the lists merge
+// by cell with the counts summed, and the window is cut after the merge.  Exact: a cell among the first K non-empty cells of the
+// node is among the first K of every device where it is non-empty, as for the all-rows branch of fbgpu_node_topn_cutoffs.
+extern "C" int fbgpu_node_groupby_sparse(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                         const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
+                                         const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
+                                         uint64_t* out_cells, uint64_t* out_counts, uint64_t cap, uint64_t* out_n) try {
+    int rc = groupby_sparse_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards,
+                                 out_cells, out_counts, cap, out_n);
+    if (rc) return rc;
+    const std::vector<GbDim> dims = gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows);
+    const NodeSplit sp = node_split(n, shards, n_shards);
+    std::vector<int> devs = node_owners(sp);
+    if (devs.empty()) devs.push_back(0);                 // no shard listed: still validate the filter
+    std::vector<std::vector<uint64_t>> cells(n->ctx.size()), counts(n->ctx.size());
+    rc = node_fan_out(n, devs, [&](int d) {
+        fbgpu_ctx* c = n->ctx[(size_t)d];
+        const auto& s = sp.shards[(size_t)d];
+        std::shared_lock<std::shared_mutex> lk;
+        int r = begin_query(c, lk); if (r) return r;
+        return groupby_sparse_run(c, index, dims, filter, n_filter_ops, s.data(), (int64_t)s.size(), start, limit, cells[(size_t)d], counts[(size_t)d]);
+    });
+    if (rc) return rc;
+    std::vector<std::pair<uint64_t, uint64_t>> all;
+    for (int d : devs) for (size_t i = 0; i < cells[(size_t)d].size(); i++) all.emplace_back(cells[(size_t)d][i], counts[(size_t)d][i]);
+    std::sort(all.begin(), all.end());
+    std::vector<uint64_t> mc, mn;
+    for (const auto& p : all) {
+        if (!mc.empty() && mc.back() == p.first) mn.back() += p.second;
+        else { mc.push_back(p.first); mn.push_back(p.second); }
+    }
+    if (limit >= 0 && mc.size() > (uint64_t)limit) { mc.resize((size_t)limit); mn.resize((size_t)limit); }
+    return write_cells(mc, mn, out_cells, out_counts, cap, out_n);
+} FBGPU_CATCH
+
 // Sum / Min / Max of an int field: per-device partials merged as ValCount.Add / Smaller / Larger do (executor.go:8446-8560)
 extern "C" int fbgpu_node_bsi_sum(fbgpu_node* n, uint32_t index, const fbgpu_op* ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                                   const uint64_t* shards, int64_t n_shards, int64_t* out_sum, uint64_t* out_count) try {

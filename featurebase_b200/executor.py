@@ -1026,7 +1026,8 @@ class Executor:
     def _groupby(self, idx, c, shards):
         """The device returns the dense count tensor over the children's row lists (with aggregate=Sum over an int field, the
         counts of columns holding a value and their sums, from the same call; with aggregate=Count(Distinct), the distinct
-        counts from one more call after one Distinct for the field's values or rows); everything after it is the host-side
+        counts from one more call after one Distinct for the field's values or rows; over set-like children too large for the
+        dense tensor, the list of non-empty groups from fbgpu_groupby_sparse, _groupby_sparse); everything after it is the host-side
         post-processing executeGroupBy does in Go: previous (iterator start, newGroupByIterator :8779-8826), aggregate=Sum
         (groupByIterator.Next :8893-8911: Count becomes the number of columns holding a value), having (:3388-3406),
         sort (:3130-3162, 3408-3414), offset / limit (:3441-3459).  Results: (group, count) or (group, count, agg)."""
@@ -1066,7 +1067,18 @@ class Executor:
             f = idx.fields.get(agg.args.get("field", agg.args.get("_field")))
             if f is not None and f.type == "int":                 # otherwise the per-group Sum below raises or finds no values
                 sum_f = f
-        if sum_f is not None:
+        has_sort, has_having = "sort" in c.args, isinstance(c.args.get("having"), pql.Call)
+        sparse = None                                             # (cells, counts) of the non-empty groups from `start` on
+        if not int_dims and hasattr(self.ctx, "groupby_sparse") and (
+                max(len(r) for r in row_ids) > 65535 or math.prod(len(r) for r in row_ids) > self.GROUPBY_DENSE_MAX_CELLS):
+            start = self._groupby_start(c, row_ids)
+            if start is None:
+                return []
+            sparse = self._groupby_sparse(idx, c, fields, row_ids, time_args, filt, start, shards,
+                                          device_limit=agg is None and not (has_sort or has_having))
+        if sparse is not None:
+            sum_f = None                                          # Sum and Count(Distinct) per group, below
+        elif sum_f is not None:
             counts, sums = self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, filt, shards, agg=sum_f)
         elif int_dims and hasattr(self.ctx, "groupby_mixed"):
             counts, = self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, filt, shards)
@@ -1087,26 +1099,27 @@ class Executor:
                 dev_fields.append(sf.id)
                 dev_rows.append(operands)
             counts = self.ctx.groupby(idx.id, dev_fields, [VIEW_STANDARD] * len(fields), dev_rows, shards, filter_ops=filt)
-        start = self._groupby_start(c, row_ids)
-        if start is None:
-            return []
+        if sparse is None:
+            start = self._groupby_start(c, row_ids)
+            if start is None:
+                return []
         dist = None                                               # Count(Distinct) over a field of this index: per-cell counts
-        if distinct_agg and "index" not in agg_distinct.args and counts.any():
+        if sparse is None and distinct_agg and "index" not in agg_distinct.args and counts.any():
             f = idx.fields.get(agg_distinct.args.get("field", agg_distinct.args.get("_field")))
             call = None if f is None else "groupby_distinct" if f.type == "int" else "groupby_distinct_rows"
             if call is not None and hasattr(self.ctx, call):      # otherwise the per-group Distinct below raises or runs
                 dist = self._groupby_distinct(idx, fields, row_ids, time_args, int_dims, filt_call, agg_distinct, f, counts.shape, shards)
-        has_sort, has_having = "sort" in c.args, isinstance(c.args.get("having"), pql.Call)
         limit = c.args.get("limit") if not (has_sort or has_having) else None       # :3196-3212: no early limit when sorting / filtering
         out = []
-        flat0 = int(np.ravel_multi_index(start, counts.shape))
-        for flat in np.flatnonzero(counts.reshape(-1)):          # only Count > 0, lexicographic (:3960)
-            if flat < flat0:
-                continue
-            ix = np.unravel_index(int(flat), counts.shape)
+        if sparse is not None:
+            groups = ((_unravel(int(flat), [len(r) for r in row_ids]), int(n)) for flat, n in zip(*sparse))
+        else:
+            flat0 = int(np.ravel_multi_index(start, counts.shape))
+            flat_counts = counts.reshape(-1)
+            groups = ((np.unravel_index(int(flat), counts.shape), int(flat_counts[flat])) for flat in np.flatnonzero(flat_counts) if flat >= flat0)
+        for ix, n in groups:                                      # only Count > 0, lexicographic (:3960)
             group = [(f.name, row_ids[k][int(i)]) for k, (f, i) in enumerate(zip(fields, ix))]
             if sum_f is not None:                                 # counts here: columns of the group holding a value of the field
-                n = int(counts[ix])
                 out.append((group, n, _i64(int(sums[ix]) + n * sum_f.base)))      # executeSumCountShard :2203-2206
             elif isinstance(agg, pql.Call):
                 rows = [pql.Call("Row", {name: rid, **(targs or {})}) for (name, rid), targs in zip(group, time_args)]
@@ -1118,9 +1131,9 @@ class Executor:
                     continue                                      # ret.Count == 0 => skipped (:8913-8919)
                 out.append((group, vc.count, vc.val))
             elif dist is not None:
-                out.append((group, int(counts[ix]), int(dist[ix])))   # a distinct count of 0 is kept (:3343-3385)
+                out.append((group, n, int(dist[ix])))             # a distinct count of 0 is kept (:3343-3385)
             else:
-                out.append((group, int(counts[ix])))
+                out.append((group, n))
             if limit and len(out) >= limit and "offset" not in c.args:
                 break
         if distinct_agg and dist is None:
@@ -1154,6 +1167,32 @@ class Executor:
             for col, asc in reversed(keys):                       # stable sorts, last key first == sort.Stable on the tuple
                 out.sort(key=lambda g: (g[col] if len(g) > col else 0), reverse=not asc)
         return self._window(c, out)
+
+    # cells of the dense count tensor above which a GroupBy over set-like children takes fbgpu_groupby_sparse (128 MiB of
+    # counts): a bound on memory, not a measured optimum.  A child of more than 65,535 rows takes it whatever the product.
+    GROUPBY_DENSE_MAX_CELLS = 1 << 24
+
+    def _groupby_sparse(self, idx, c, fields, row_ids, time_args, filt, start, shards, device_limit):
+        """(cells, counts) of a GroupBy over set-like children from fbgpu_groupby_sparse: the non-empty groups from the iterator's
+        start position on, as row-major flat indices over the children's row lists, ascending; with device_limit (no sort, having or
+        Sum, which skips groups after the fact) at most offset + limit of them.  None when the context answers FBGPU_E_COMM or has
+        no such call: the dense tensor is asked for instead.  aggregate=Sum and Count(Distinct) then take the per-group
+        composition, one query per group."""
+        sizes = [len(r) for r in row_ids]
+        flat0 = 0
+        for p, n in zip(start, sizes):
+            flat0 = flat0 * n + p
+        lim = c.args.get("limit")
+        limit = int(lim) + int(c.args.get("offset") or 0) if device_limit and lim else None
+        set_dims = [(f.id, self._time_view_ids(f, targs) if targs else [VIEW_STANDARD], rows) for f, rows, targs in zip(fields, row_ids, time_args)]
+        try:
+            return self.ctx.groupby_sparse(idx.id, set_dims, shards, filter_ops=filt, start=flat0, limit=limit)
+        except NotImplementedError:
+            return None
+        except L.FbgpuError as e:
+            if e.code != L.E_COMM:
+                raise
+            return None
 
     GROUPBY_MIXED_MAX = 65535                                     # groups (product of the int children's value counts) per fbgpu_groupby_mixed / _sum / _distinct call
     # presence bits ((rows of the last set child, or 1) x groups x listed values or rows of x) per fbgpu_groupby_distinct(_rows) call: 256 MiB
@@ -1262,6 +1301,15 @@ class Executor:
                         return None
                     pos[j] = 0
         return pos
+
+
+def _unravel(flat, shape):
+    """np.unravel_index for a Python int over a shape whose size may exceed int64"""
+    ix = []
+    for n in reversed(shape):
+        flat, i = divmod(flat, n)
+        ix.append(i)
+    return tuple(reversed(ix))
 
 
 def _cond_holds(v, cond):

@@ -462,6 +462,26 @@ int fbgpu_groupby_distinct_rows(fbgpu_ctx *ctx, uint32_t index,
                                 uint32_t xfield, uint32_t xview, const uint64_t *x_rows, int32_t n_x,
                                 const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards,
                                 uint64_t *out_distinct);
+/* GroupBy over set, mutex, bool or time dimensions of any size, as the sorted list of its non-empty groups (executeGroupBy's
+ * walk of groupByIterator, with previous= and limit=).  The dimensions are fbgpu_groupby_views': 1..8, dimension i the rows
+ * row_ids_flat[..n_rows[i]] of fields[i], each taken as its union over n_views[i] >= 1 views; the filter is optional.  n_rows[i]
+ * may be 1..2^31-1, and each list must be strictly ascending; the product of the n_rows must fit in u64.  A cell is the
+ * row-major flat index Σ idx_i · Π_{j>i} n_rows[j] of the dense tensor fbgpu_groupby_views would fill (the last dimension
+ * fastest, the reference's iteration order), and its count is what that call would put there: |filter ∩ ⋂_i row_i|.
+ * Output: the cells with a non-zero count and cell >= start, ascending, at most `limit` of them (limit < 0: no limit), into
+ * out_cells / out_counts under fbgpu_columns' NOSPACE contract (cap too small: nothing written, FBGPU_E_NOSPACE, *out_n = the
+ * size needed).  Argument errors (null pointers, n_fields outside 1..8, n_views < 1, n_rows < 1, a list not strictly ascending,
+ * an overflowing product) are reported before the device check.  A context with a communicator attached returns FBGPU_E_COMM:
+ * lists of cells do not all-reduce.  Device memory: 16 bytes per (column, listed row) hit of each dimension in a chunk of at
+ * most 2^24 hits per dimension, 16 bytes per cell of a join range of at most 2^24 cells (one column's cross product may exceed
+ * that), and 32 bytes per cell of the running list, which the limit bounds. */
+int fbgpu_groupby_sparse(fbgpu_ctx *ctx, uint32_t index,
+                         const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                         const uint64_t *row_ids_flat, const int32_t *n_rows,
+                         const fbgpu_op *filter, int32_t n_filter_ops,
+                         const uint64_t *shards, int64_t n_shards,
+                         uint64_t start, int64_t limit,
+                         uint64_t *out_cells, uint64_t *out_counts, uint64_t cap, uint64_t *out_n);
 
 /* ---- multi-GPU reduce (replaces the HTTP fan-in of mapReduce/remoteExec, executor.go:6392-6533) ----
  * One context (process) per GPU; rank 0 creates the id, every rank joins.  When a communicator is attached,
@@ -565,6 +585,14 @@ int fbgpu_node_bsi_sort(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, i
                         uint64_t *out_cols, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
 int fbgpu_node_bsi_distinct(fbgpu_node *node, uint32_t index, const fbgpu_op *ops, int32_t n_ops, uint32_t field, uint32_t view, int32_t bit_depth,
                             const uint64_t *shards, int64_t n_shards, int64_t *out_vals, uint64_t cap, uint64_t *out_n, uint64_t *out_total);
+/* Every device lists its own shards' cells with the same start and limit; the lists merge by cell, counts summed, and the
+ * window is cut after the merge (exact: a cell among the node's first K non-empty cells is among the first K of every device
+ * where it is non-empty). */
+int fbgpu_node_groupby_sparse(fbgpu_node *node, uint32_t index,
+                              const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                              const uint64_t *row_ids_flat, const int32_t *n_rows, const fbgpu_op *filter, int32_t n_filter_ops,
+                              const uint64_t *shards, int64_t n_shards, uint64_t start, int64_t limit,
+                              uint64_t *out_cells, uint64_t *out_counts, uint64_t cap, uint64_t *out_n);
 
 /* Inspection (any context): the stack-machine program the library would run for `ops` -- records of 16 bytes {u8 op, u8 pad[3],
  * u32 view slot, u64 row} (csrc/fbgpu_types.h DevOp); *out_depth = operand stack depth.  With index == 0xffffffff,
