@@ -24,6 +24,9 @@
   config G: fbgpu_groupby_sparse against fbgpu_groupby on config S's 256 x 256 GroupBy(Rows(a), Rows(b)), against the host
             composition (one fbgpu_extract_rows per dimension and a numpy join) for a 1,000,000-row mutex field x a, and paged
             with limit=1000 (only when named in --configs).
+  config H: config G's data with aggregate=Sum(field=v): GroupBy(Rows(m), aggregate=Sum(field=v), limit=1000) through the
+            executor, fbgpu_groupby_sparse_sum against the sparse list plus one Sum per group; m x a with Sum against the
+            counts-only sparse call; a x b with Sum against fbgpu_groupby_sum (only when named in --configs).
   config N: TopN(f, Row(src=0), tanimotoThreshold=50) and TopN(f, Row(src=0), threshold=100) over --topn-rows rows of varied
             cardinality, fbgpu_topn_cutoffs against the per-shard count-matrix composition (only when named in --configs).
   config O: Sort over config X's 32-bit field with and without a limit, fbgpu_bsi_sort against extracting every value and
@@ -861,6 +864,27 @@ def config_groupby_distinct_rows(args, out):
     real.close()
 
 
+def _config_g_world(args, tag, m_fragments=1):
+    """config G's data: _config_s_world plus m, a mutex field of 1,000,000 rows holding one row for each of the first 16,384
+    columns of every shard (shard s takes the (s % m_fragments)-th of m_fragments fragments, each encoded once; config G's one
+    fragment gives about 16,000 distinct rows, eight give more than 65,535), and e, whose row 0 holds those columns.  Returns
+    (holder, index, fields a, b, c, w, v, m, e, load seconds)."""
+    from featurebase_b200 import executor as X, roaring_io
+    n_cols = 16384
+    h, idx, fa, fb, ff, fw, fv, load_s = _config_s_world(args, tag)
+    fm, fe = idx.create_field("m", "mutex"), idx.create_field("e")
+    rng = np.random.default_rng(2029)
+    data = [roaring_io.encode(np.sort(rng.integers(0, 1_000_000, n_cols).astype(np.uint64) * np.uint64(SW) + np.arange(n_cols, dtype=np.uint64)))
+            for _ in range(m_fragments)]
+    every = roaring_io.encode(np.arange(n_cols, dtype=np.uint64))          # e=0: the columns m covers
+    t0 = time.time()
+    for s_ in range(args.groupby_shards):
+        h.ctx.load_fragment(idx.id, fm.id, X.VIEW_STANDARD, s_, data[s_ % m_fragments])
+        h.ctx.load_fragment(idx.id, fe.id, X.VIEW_STANDARD, s_, every)
+    h.ctx.commit()
+    return h, idx, fa, fb, ff, fw, fv, fm, fe, load_s + time.time() - t0
+
+
 def config_groupby_sparse(args, out):
     """fbgpu_groupby_sparse over --groupby-shards shards of config S's data (_config_s_world) plus m, a mutex field of 1,000,000
     rows holding one row for each of the first 16,384 columns of every shard (every shard the same fragment, encoded once), as
@@ -870,17 +894,9 @@ def config_groupby_sparse(args, out):
           holding the columns m covers) and a numpy join of the per-column row lists, alternated; the same groups and counts;
       (c) m x a paged: limit=1000 pages, each starting one past the last cell of the page before, for 8 pages.
     Wall clock per call (each ends in a device synchronise and a copy to the host), with the call's last_query_gpu_ms."""
-    from featurebase_b200 import executor as X, lib as L, roaring_io
-    S, n_cols = args.groupby_shards, 16384
-    h, idx, fa, fb, ff, fw, fv, load_s = _config_s_world(args, "G")
-    fm, fe = idx.create_field("m", "mutex"), idx.create_field("e")
-    rng = np.random.default_rng(2029)
-    data = roaring_io.encode(np.sort(rng.integers(0, 1_000_000, n_cols).astype(np.uint64) * np.uint64(SW) + np.arange(n_cols, dtype=np.uint64)))
-    every = roaring_io.encode(np.arange(n_cols, dtype=np.uint64))          # e=0: the columns m covers
-    for s_ in range(S):
-        h.ctx.load_fragment(idx.id, fm.id, X.VIEW_STANDARD, s_, data)
-        h.ctx.load_fragment(idx.id, fe.id, X.VIEW_STANDARD, s_, every)
-    h.ctx.commit()
+    from featurebase_b200 import executor as X, lib as L
+    S = args.groupby_shards
+    h, idx, fa, fb, ff, fw, fv, fm, fe, load_s = _config_g_world(args, "G")
     ctx, card, sh = h.ctx, _card(), list(range(S))
     ra, rm = np.arange(256, dtype=np.uint64), np.arange(1_000_000, dtype=np.uint64)
     dims_ab = [(fa.id, [X.VIEW_STANDARD], ra), (fb.id, [X.VIEW_STANDARD], ra)]
@@ -943,6 +959,80 @@ def config_groupby_sparse(args, out):
                  "load_s": round(load_s, 1),
                  "note": "median over the timed steps of the call's wall clock, of the last library query's GPU ms and of the library queries"})
     ctx.close()
+
+
+def config_groupby_sparse_sum(args, out):
+    """aggregate=Sum(field=v) over config G's data (_config_g_world with eight m fragments, so that Rows(m) lists more than
+    65,535 rows and the executor takes the sparse path; v holds a value on every column m covers), over --groupby-shards shards:
+      (a) GroupBy(Rows(m), aggregate=Sum(field=v), limit=1000) through the executor: fbgpu_groupby_sparse_sum against today's
+          composition without it (the sparse list of groups, then one Sum query per group until 1,000 are listed), alternated;
+          the same groups, counts and sums;
+      (b) GroupBy(Rows(m), Rows(a), aggregate=Sum(field=v)), every group, as library calls: fbgpu_groupby_sparse_sum against the
+          counts-only fbgpu_groupby_sparse on the same dimensions, alternated; the same cells and counts (every column of m holds
+          a value of v), so the difference is the cost of carrying the aggregate;
+      (c) a x b, 256 x 256, with Sum, as library calls: fbgpu_groupby_sparse_sum against the dense fbgpu_groupby_sum, alternated;
+          the same cells, counts and sums.
+    Per arm: the median wall clock, the summed last_query_gpu_ms of the arm's library queries and their number."""
+    from featurebase_b200 import executor as X
+    S = args.groupby_shards
+    h, idx, fa, fb, ff, fw, fv, fm, fe, load_s = _config_g_world(args, "H", m_fragments=8)
+    real, card, sh = h.ctx, _card(), list(range(S))
+    dev, comp = _KernelMs(real), _NoGroupBySum(real)
+    ra, rm = np.arange(256, dtype=np.uint64), np.arange(1_000_000, dtype=np.uint64)
+    agg = (fv.id, X.VIEW_BSI, fv.bit_depth)
+    dims_ab = [(fa.id, [X.VIEW_STANDARD], ra), (fb.id, [X.VIEW_STANDARD], ra)]
+    dims_ma = [(fm.id, [X.VIEW_STANDARD], rm), (fa.id, [X.VIEW_STANDARD], ra)]
+    q = "GroupBy(Rows(m), aggregate=Sum(field=v), limit=1000)"
+
+    def executor(ctx):
+        def run():
+            h.ctx = ctx
+            try:
+                return X.Executor(h).execute("i", q, sh)[0]
+            finally:
+                h.ctx = real
+        return run
+
+    def dense_sum():
+        counts, sums = dev.groupby_sum(idx.id, dims_ab, [], agg, sh)
+        counts, sums = counts.reshape(-1), sums.reshape(-1)
+        nz = np.flatnonzero(counts)
+        return nz.astype(np.uint64), counts[nz], sums[nz]
+
+    arms = {"a": {"device": (dev, executor(dev)), "composition": (comp, executor(comp))},
+            "b": {"sparse_sum": (dev, lambda: dev.groupby_sparse(idx.id, dims_ma, sh, agg=agg)),
+                  "sparse_counts": (dev, lambda: dev.groupby_sparse(idx.id, dims_ma, sh))},
+            "c": {"sparse_sum": (dev, lambda: dev.groupby_sparse(idx.id, dims_ab, sh, agg=agg)), "dense_sum": (dev, dense_sum)}}
+    for part, fns in arms.items():
+        rec = {name: {"wall": [], "gpu_ms": [], "queries": []} for name in fns}
+        res = {}
+        for i in range(1 + args.steps):                          # one warm-up round, then alternate the arms
+            for name in (sorted(fns) if i % 2 == 0 else sorted(fns, reverse=True)):
+                proxy, fn = fns[name]
+                q0, proxy.ms = real.counters()["queries"], 0.0
+                t1 = time.perf_counter()
+                r = fn()
+                wall = (time.perf_counter() - t1) * 1e3
+                res.setdefault(name, r)
+                print(f"config H ({part}): {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                if i >= 1:
+                    rec[name]["wall"].append(wall)
+                    rec[name]["gpu_ms"].append(proxy.ms)
+                    rec[name]["queries"].append(real.counters()["queries"] - q0)
+        v = list(res.values())
+        if part == "a":
+            assert v[0] == v[1] and len(v[0]) == 1000, part
+        else:
+            n_cmp = 2 if part == "b" else 3                      # (b): the counts-only call has no sums
+            assert all(np.array_equal(x[k], v[0][k]) for x in v for k in range(n_cmp)), part
+        for name, dd in rec.items():
+            out({"config": "H", "part": part, "arm": name, "gpu": card, "shards": S, "groups": len(res[name] if part == "a" else res[name][0]),
+                 "equal_to_other_arm": True, "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])),
+                 "wall_ms_max": float(np.max(dd["wall"])), "gpu_ms": float(np.median(dd["gpu_ms"])), "queries": int(np.median(dd["queries"])),
+                 "steps": len(dd["wall"]), "load_s": round(load_s, 1),
+                 "note": "median over the timed steps of the wall clock (executor: Rows pre-pass included), of the summed last_query_gpu_ms "
+                         "of the arm's library queries and of their number"})
+    real.close()
 
 
 class _NoTopnCutoffs(_KernelMs):
@@ -1393,6 +1483,8 @@ def main():
             config_groupby_distinct_rows(args, out)
         elif c == "G":
             config_groupby_sparse(args, out)
+        elif c == "H":
+            config_groupby_sparse_sum(args, out)
         elif c == "N":
             config_topn_cutoffs(args, out)
         elif c == "O":

@@ -2659,6 +2659,11 @@ extern "C" int fbgpu_groupby_distinct_rows(fbgpu_ctx* c, uint32_t index, const u
 // >= start; the cells are sorted and run-length coded into (cell, count), and merged into the call's running list by a sort of
 // (cell, count) pairs and a sum of equal cells.  With a limit, the list is cut to its first `limit` cells after each merge, and
 // once it holds that many, cells past its last one are not emitted.
+// With an aggregate x (fbgpu_groupby_sparse_sum) the evaluated filter is <filter> ∩ exists(x), so every hit is a column holding
+// a value.  Chunks also hold at most kSortChunk filter columns, and each chunk's filter columns get their stored values of x
+// (columns_emit_kernel and extract_values_kernel over the chunk's units, in (unit, column) order).  The join emits (cell, value)
+// pairs, sorted by cell; each run becomes (cell, count) as before and its wrapping sum (sparse_run_sums_kernel).  The sums form a
+// second running list with the same cells, merged by the same deterministic sort and compaction, so the two stay aligned.
 
 // the argument checks fbgpu_groupby_sparse and its node form make before any device is touched
 static int groupby_sparse_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
@@ -2682,15 +2687,22 @@ static int groupby_sparse_args(const void* handle, const uint32_t* fields, const
     return 0;
 }
 
-// device buffers of one fbgpu_groupby_sparse call, freed when it returns: they can be large, and are not reused by other calls
+// the aggregate of fbgpu_groupby_sparse_sum: an int field's BSI view and bit depth
+struct SpAgg { uint32_t field, view; int depth; };
+
+// device buffers of one fbgpu_groupby_sparse call, freed when it returns: they can be large, and are not reused by other calls.
+// b[d]: dimension d's keys; b[nd]: the cells (with an aggregate, (cell, value) pairs); b[kSpMaxDims + 1]: the cursor, row lists
+// and view slots; with an aggregate, b[kSpMaxDims + 2]: a chunk's value list, b[kSpMaxDims + 3]: its two ColUnit lists,
+// b[kSpMaxDims + 4]: the running list of sums.
 struct SparseBufs {
-    DevBuf b[kSpMaxDims + 2];
+    DevBuf b[kSpMaxDims + 5];
     ~SparseBufs() { for (DevBuf& x : b) x.release(); }
 };
 
 // the sorted cells of cs into (cell, count) pairs merged into acc, whose cells are distinct and sorted; then acc cut to its first
-// `limit` cells (limit < 0: no cut), and *hi lowered to one past its last cell once it holds that many
-static int sparse_merge(Query& q, SortPairs& cs, SortPairs& acc, int bits, int64_t limit, unsigned long long* hi) {
+// `limit` cells (limit < 0: no cut), and *hi lowered to one past its last cell once it holds that many.  With `sums`, cs holds
+// (cell, value) pairs, and each run's wrapping sum of values goes into *sums, a list with acc's cells, merged and cut alike.
+static int sparse_merge(Query& q, SortPairs& cs, SortPairs& acc, SortPairs* sums, int bits, int64_t limit, unsigned long long* hi) {
     Workspace* w = q.w;
     const uint64_t n = cs.n, n_tiles = (n + kSortTile - 1) / kSortTile;
     if (w->d_counts.ensure((size_t)(n_tiles + 1) * 4) || w->h_out.ensure(8)) return FBGPU_E_NOMEM;
@@ -2703,6 +2715,7 @@ static int sparse_merge(Query& q, SortPairs& cs, SortPairs& acc, int bits, int64
     CUDA_TRY(cudaStreamSynchronize(w->stream));
     const uint64_t u = *(const unsigned int*)w->h_out.p;
     int rc = acc.reserve(acc.n + u); if (rc) return rc;
+    if (sums) { rc = sums->reserve(sums->n + u); if (rc) return rc; }
     unsigned long long* pos = cs.keys(1 - cs.cur);          // the sort's free half: the runs' first positions
     sparse_compact_kernel<false><<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(cs.keys(cs.cur), nullptr, n, counts, acc.keys(acc.cur) + acc.n, pos);
     CUDA_TRY(cudaGetLastError());
@@ -2710,10 +2723,19 @@ static int sparse_merge(Query& q, SortPairs& cs, SortPairs& acc, int bits, int64
     sparse_run_lengths_kernel<<<grid, 256, 0, w->stream>>>(pos, u, n, acc.cols(acc.cur) + acc.n);
     CUDA_TRY(cudaGetLastError());
     q.launches += 4;
+    if (sums) {
+        CUDA_TRY(cudaMemcpyAsync(sums->keys(sums->cur) + sums->n, acc.keys(acc.cur) + acc.n, u * 8, cudaMemcpyDeviceToDevice, w->stream));
+        CUDA_TRY(cudaMemsetAsync(sums->cols(sums->cur) + sums->n, 0, u * 8, w->stream));
+        sparse_run_sums_kernel<<<(unsigned)n_tiles, kSortThreads, 0, w->stream>>>(cs.keys(cs.cur), cs.cols(cs.cur), n, counts, sums->cols(sums->cur) + sums->n);
+        CUDA_TRY(cudaGetLastError());
+        q.launches++;
+        sums->n += u;
+    }
     const bool merge = acc.n > 0;
     acc.n += u;
     if (merge) {
         rc = sort_pairs(q, acc, bits, ~0ull); if (rc) return rc;
+        if (sums) { rc = sort_pairs(q, *sums, bits, ~0ull); if (rc) return rc; }    // the same keys: the same order
         const uint64_t m = acc.n, m_tiles = (m + kSortTile - 1) / kSortTile;
         if (w->d_counts.ensure((size_t)(m_tiles + 1) * 4)) return FBGPU_E_NOMEM;
         counts = (unsigned int*)w->d_counts.p;
@@ -2726,12 +2748,21 @@ static int sparse_merge(Query& q, SortPairs& cs, SortPairs& acc, int bits, int64
         CUDA_TRY(cudaGetLastError());
         q.launches += 3;
         acc.cur = 1 - acc.cur;
+        if (sums) {
+            sparse_compact_kernel<true><<<(unsigned)m_tiles, kSortThreads, 0, w->stream>>>(sums->keys(sums->cur), sums->cols(sums->cur), m, counts,
+                                                                                          sums->keys(1 - sums->cur), sums->cols(1 - sums->cur));
+            CUDA_TRY(cudaGetLastError());
+            q.launches++;
+            sums->cur = 1 - sums->cur;
+        }
         CUDA_TRY(cudaMemcpyAsync(w->h_out.p, counts + m_tiles, 4, cudaMemcpyDeviceToHost, w->stream));
         CUDA_TRY(cudaStreamSynchronize(w->stream));
         acc.n = *(const unsigned int*)w->h_out.p;
+        if (sums) sums->n = acc.n;
     }
     if (limit >= 0 && acc.n >= (uint64_t)limit) {
         acc.n = (uint64_t)limit;
+        if (sums) sums->n = (uint64_t)limit;
         CUDA_TRY(cudaMemcpyAsync(w->h_out.p, acc.keys(acc.cur) + acc.n - 1, 8, cudaMemcpyDeviceToHost, w->stream));
         CUDA_TRY(cudaStreamSynchronize(w->stream));
         *hi = *(const uint64_t*)w->h_out.p + 1;
@@ -2740,19 +2771,28 @@ static int sparse_merge(Query& q, SortPairs& cs, SortPairs& acc, int bits, int64
 }
 
 // the non-empty cells >= start of the dimensions `dims` under the filter, ascending, at most `limit` of them (limit < 0: all), and
-// their counts (store lock held)
+// their counts (store lock held).  With `agg`, the filter is <filter> ∩ exists(x), a cell is non-empty when its count there is,
+// and `sums` gets each listed cell's wrapping sum of x's stored values.
 static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<GbDim>& dims, const fbgpu_op* filter, int32_t n_filter_ops,
                               const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
-                              std::vector<uint64_t>& cells, std::vector<uint64_t>& counts) {
+                              std::vector<uint64_t>& cells, std::vector<uint64_t>& counts, const SpAgg* agg = nullptr, std::vector<int64_t>* sums = nullptr) {
     cells.clear(); counts.clear();
+    if (sums) sums->clear();
     const int nd = (int)dims.size();
     Query q(c); Workspace* w = q.w;
     const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);
+    std::vector<fbgpu_op> full;
+    uint32_t fv_x = 0;
+    if (agg) {
+        full = and_row(filter, n_filter_ops, agg->field, agg->view, 0);    // <filter> ∩ exists, as for fbgpu_bsi_sum
+        fv_x = view_id_locked(c, ViewKey{ index, agg->field, agg->view }, false);
+        filter = full.data(); n_filter_ops = (int32_t)full.size();
+    }
     const bool have_filter = n_filter_ops > 0;
     int rc = have_filter ? q.open(index, filter, n_filter_ops, sorted.data(), (int64_t)sorted.size()) : q.open(sorted.data(), (int64_t)sorted.size());
     if (rc) return rc;
     if (limit == 0) { q.finish(); return FBGPU_OK; }
-    SparseBufs sb;                    // b[d]: dimension d's keys; b[nd]: the cells; b[kSpMaxDims + 1]: two cursors, the row lists, the view slots
+    SparseBufs sb;
     SpJoin jn{}; jn.nd = nd; jn.lo = start; jn.hi = ~0ull;
     // b[kSpMaxDims + 1]: [cursor | rows of every dimension (u64) | view slots of every dimension (u32)]
     std::vector<uint64_t> rows_h(1, 0);
@@ -2776,18 +2816,19 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
     const int cell_bits = bit_width(total - 1);
     std::vector<SortPairs> dk;
     for (int d = 0; d < nd; d++) dk.emplace_back(w, ~0ull, true, &sb.b[d]);
-    SortPairs cs(w, ~0ull, true, &sb.b[nd]), acc(w, ~0ull);
+    SortPairs cs(w, ~0ull, !agg, &sb.b[nd]), acc(w, ~0ull), acc_sums(w, ~0ull, false, &sb.b[kSpMaxDims + 4]);
     const long long batch = std::min<long long>(c->unit_batch, 1ll << 16);     // a unit's place in a chunk takes 16 bits of a key
-    std::vector<uint32_t> units, keep, chunk;
+    std::vector<uint32_t> units, keep, chunk, ncol;                            // ncol: with agg, the filter columns of units[k]
     std::vector<uint64_t> ucnt;
+    std::vector<ColUnit> vunits;
     for (long long u0 = 0; u0 < q.n_units; u0 += batch) {
         const long long nu = std::min(batch, q.n_units - u0);
         CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
-        units.clear();
+        units.clear(); ncol.clear();
         if (have_filter) {
             const uint2* info;
             rc = q.eval_info(u0, nu, info); if (rc) return rc;
-            for (long long u = 0; u < nu; u++) if (info[u].x) units.push_back((uint32_t)u);
+            for (long long u = 0; u < nu; u++) if (info[u].x) { units.push_back((uint32_t)u); ncol.push_back(info[u].x); }
         } else {
             for (long long u = 0; u < nu; u++) units.push_back((uint32_t)u);
         }
@@ -2815,14 +2856,16 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
             if (all) keep.push_back((uint32_t)e);
         }
         for (size_t a = 0; a < keep.size();) {
-            // the chunk keep[a, b): at most kSortChunk hits per dimension (at least one unit)
+            // the chunk keep[a, b): at most kSortChunk hits per dimension and, with agg, filter columns (at least one unit)
             std::vector<uint64_t> hits(nd, 0);
+            uint64_t vn = 0;
             size_t b = a;
             for (; b < keep.size(); b++) {
-                bool fits = true;
+                bool fits = !agg || vn + ncol[keep[b]] <= kSortChunk;
                 for (int d = 0; d < nd; d++) fits = fits && hits[d] + ucnt[(size_t)d * nun + keep[b]] <= kSortChunk;
                 if (!fits && b > a) break;
                 for (int d = 0; d < nd; d++) hits[d] += ucnt[(size_t)d * nun + keep[b]];
+                if (agg) vn += ncol[keep[b]];
             }
             chunk.clear();
             for (size_t k = a; k < b; k++) chunk.push_back(units[keep[k]]);
@@ -2843,6 +2886,38 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
                 rc = n_fv[d] > 1 ? distinct_keys(q, k, kbits) : sort_pairs(q, k, kbits, ~0ull); if (rc) return rc;
                 jn.keys[d] = k.keys(k.cur); jn.n[d] = k.n;
             }
+            // with agg, the chunk's value list: the filter columns of its units in (unit, column) order, as (e << 16 | c) keys
+            // (columns_emit_kernel over units based at e << 16) and their values' magnitudes and sign bits (extract_values_kernel)
+            SpVals vl{};
+            if (agg) {
+                vunits.clear();
+                for (int pass = 0; pass < 2; pass++) {
+                    uint64_t off = 0;
+                    for (size_t k = a; k < b; k++) {
+                        ColUnit cu{};
+                        const uint32_t u = units[keep[k]];
+                        cu.out_off = off; cu.unit = u; cu.first = 0; cu.last = ncol[keep[k]];
+                        cu.col_base = pass == 0 ? (sorted[(u0 + u) / kSlotsPerRow] << 20) + (uint64_t)((u0 + u) % kSlotsPerRow) * 65536ull
+                                                : (uint64_t)(k - a) << 16;
+                        vunits.push_back(cu);
+                        off += cu.last;
+                    }
+                }
+                DevBuf& vb = sb.b[kSpMaxDims + 2]; DevBuf& ub = sb.b[kSpMaxDims + 3];
+                const size_t sign_bytes = ((vn + 31) / 32) * 4;
+                if (vb.ensure(vn * 16 + sign_bytes) || ub.ensure(vunits.size() * sizeof(ColUnit))) return FBGPU_E_NOMEM;
+                unsigned long long* vcols = (unsigned long long*)vb.p; unsigned long long* mag = vcols + vn;
+                unsigned int* sign = (unsigned int*)(mag + vn);
+                const ColUnit* d_vu = (const ColUnit*)ub.p;
+                CUDA_TRY(cudaMemcpyAsync(ub.p, vunits.data(), vunits.size() * sizeof(ColUnit), cudaMemcpyHostToDevice, w->stream));
+                CUDA_TRY(cudaMemsetAsync(mag, 0, vn * 8 + sign_bytes, w->stream));
+                columns_emit_kernel<<<cgrid, kEmitThreads, 0, w->stream>>>(bitmaps, d_vu + chunk.size(), (int)chunk.size(), vcols);
+                CUDA_TRY(cudaGetLastError());
+                extract_values_kernel<<<cgrid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv_x, agg->depth, bitmaps, d_vu, (int)chunk.size(), mag, sign);
+                CUDA_TRY(cudaGetLastError());
+                q.launches += 2;
+                vl.cols = vcols; vl.mag = mag; vl.sign = sign; vl.n = vn;
+            }
             // the join, over ranges of dimension 0's entries that give at most kSortChunk cells (at least one entry)
             const uint64_t n0 = jn.n[0];
             const unsigned jgrid = (unsigned)std::min<uint64_t>((n0 + 255) / 256, (uint64_t)c->sm_count * 8);
@@ -2850,7 +2925,7 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
                 uint64_t e1 = n0, got = 0;
                 for (;;) {
                     CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
-                    sparse_join_kernel<SrOut::kCount><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, nullptr);
+                    sparse_join_kernel<SrOut::kCount><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, nullptr, SpVals{});
                     CUDA_TRY(cudaGetLastError()); q.launches++;
                     CUDA_TRY(cudaMemcpyAsync(w->h_out.p, cursor, 8, cudaMemcpyDeviceToHost, w->stream));
                     CUDA_TRY(cudaStreamSynchronize(w->stream));
@@ -2862,11 +2937,16 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
                     cs.n = 0;
                     rc = cs.reserve(got); if (rc) return rc;
                     CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
-                    sparse_join_kernel<SrOut::kEmit><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, cs.keys(cs.cur));
+                    if (agg) {
+                        vl.out = cs.cols(cs.cur);
+                        sparse_join_kernel<SrOut::kSum><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, cs.keys(cs.cur), vl);
+                    } else {
+                        sparse_join_kernel<SrOut::kEmit><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, cs.keys(cs.cur), SpVals{});
+                    }
                     CUDA_TRY(cudaGetLastError()); q.launches++;
                     cs.n = got;
                     rc = sort_pairs(q, cs, cell_bits, ~0ull); if (rc) return rc;
-                    rc = sparse_merge(q, cs, acc, cell_bits, limit, &jn.hi); if (rc) return rc;
+                    rc = sparse_merge(q, cs, acc, agg ? &acc_sums : nullptr, cell_bits, limit, &jn.hi); if (rc) return rc;
                 }
                 e0 = e1;
             }
@@ -2880,6 +2960,10 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
     if (acc.n) {
         CUDA_TRY(cudaMemcpyAsync(cells.data(), acc.keys(acc.cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
         CUDA_TRY(cudaMemcpyAsync(counts.data(), acc.cols(acc.cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
+        if (agg) {
+            sums->resize(acc.n);
+            CUDA_TRY(cudaMemcpyAsync(sums->data(), acc_sums.cols(acc_sums.cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
+        }
         CUDA_TRY(cudaStreamSynchronize(w->stream));
     }
     q.finish();
@@ -2911,6 +2995,48 @@ extern "C" int fbgpu_groupby_sparse(fbgpu_ctx* c, uint32_t index, const uint32_t
                             start, limit, cells, counts);
     if (rc) return rc;
     return write_cells(cells, counts, out_cells, out_counts, cap, out_n);
+} FBGPU_CATCH
+
+// the argument checks of fbgpu_groupby_sparse_sum and its node form: fbgpu_groupby_sparse's, then the aggregate's
+static int groupby_sparse_sum_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                   const uint64_t* row_ids_flat, const int32_t* n_rows, int32_t a_depth, const fbgpu_op* filter, int32_t n_filter_ops,
+                                   const uint64_t* shards, int64_t n_shards, const uint64_t* out_cells, const uint64_t* out_counts, const int64_t* out_sums,
+                                   uint64_t cap, const uint64_t* out_n) {
+    int rc = groupby_sparse_args(handle, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards,
+                                 out_cells, out_counts, cap, out_n);
+    if (rc) return rc;
+    if (a_depth < 0 || a_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", a_depth);
+    if (cap && !out_sums) return fail(FBGPU_E_INVALID, "bad argument");
+    return 0;
+}
+
+// write_cells with each cell's sum beside its count
+static int write_cells(const std::vector<uint64_t>& cells, const std::vector<uint64_t>& counts, const std::vector<int64_t>& sums,
+                       uint64_t* out_cells, uint64_t* out_counts, int64_t* out_sums, uint64_t cap, uint64_t* out_n) {
+    int rc = write_cells(cells, counts, out_cells, out_counts, cap, out_n);
+    if (rc == FBGPU_OK && !sums.empty()) memcpy(out_sums, sums.data(), sums.size() * 8);
+    return rc;
+}
+
+// GroupBy(..., aggregate=Sum(field=x)) over set-like dimensions of any number of rows: fbgpu_groupby_sparse's list, where a cell is
+// listed when filter ∩ its rows ∩ exists(x) is non-empty, with that count and the wrapping sum of the columns' stored values
+// (groupByIterator.Next's Sum, executor.go:8893-8919, which skips a group whose count is 0)
+extern "C" int fbgpu_groupby_sparse_sum(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                        const uint64_t* row_ids_flat, const int32_t* n_rows, uint32_t afield, uint32_t aview, int32_t a_depth,
+                                        const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
+                                        uint64_t* out_cells, uint64_t* out_counts, int64_t* out_sums, uint64_t cap, uint64_t* out_n) try {
+    int rc = groupby_sparse_sum_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, a_depth, filter, n_filter_ops, shards, n_shards,
+                                     out_cells, out_counts, out_sums, cap, out_n);
+    if (rc) return rc;
+    if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_groupby_sparse_sum is local to one context: group lists merge by cell, not by an all-reduce");
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    std::vector<uint64_t> cells, counts; std::vector<int64_t> sums;
+    const SpAgg agg{ afield, aview, a_depth };
+    rc = groupby_sparse_run(c, index, gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows), filter, n_filter_ops, shards, n_shards,
+                            start, limit, cells, counts, &agg, &sums);
+    if (rc) return rc;
+    return write_cells(cells, counts, sums, out_cells, out_counts, out_sums, cap, out_n);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ comm

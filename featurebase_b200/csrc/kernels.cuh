@@ -2829,7 +2829,8 @@ gv_popcount_kernel(const unsigned long long* __restrict__ present, long long wor
 //   kCount: counts[e] += the unit's hits.
 //   kEmit:  the key ((e << 16 | c) << jbits) | j at keys[(*cursor)++].  Warps reserve their hits with one atomic, so the order
 //           is arbitrary: the host sorts the keys, and dedupes them when a row is present in several views.
-enum class SrOut { kCount, kEmit };
+// (kSum is a mode of sparse_join_kernel alone.)
+enum class SrOut { kCount, kEmit, kSum };
 constexpr int kSrThreads = 256;
 
 // one warp-wide step of sparse_rows_kernel: each lane holds the hit mask x of word wi of the unit (0: none)
@@ -2931,10 +2932,18 @@ sparse_rows_kernel(StoreRef st, const uint32_t* __restrict__ fvs, int nv, const 
 // product gives the flat cells Σ_d j_d · stride[d] that lie in [lo, hi).  A column missing from any dimension gives none.
 //   kCount: *cursor += the cells.
 //   kEmit:  the cells at cells[(*cursor)++], reserved per warp; the host sorts them.
+//   kSum:   as kEmit, and beside each cell, at vl.out[(*cursor)++], the stored value of the entry's column: its place i in the
+//           chunk's ascending value list vl.cols (keys of the same (e << 16 | c) form) by binary search, the value
+//           vl.mag[i] negated when bit i of vl.sign is set (extract_values_kernel's output), wrapping like fbgpu_extract.
+//           Every column of dimension 0 lies in the filter, which holds exists(x), so the search always finds it.
 constexpr int kSpMaxDims = 8;
 struct SpJoin {
     const unsigned long long* keys[kSpMaxDims]; unsigned long long n[kSpMaxDims], stride[kSpMaxDims]; int jbits[kSpMaxDims]; int nd;
     unsigned long long lo, hi;
+};
+struct SpVals {
+    const unsigned long long* cols; const unsigned long long* mag; const unsigned int* sign; unsigned long long n;
+    unsigned long long* out;
 };
 
 __device__ __forceinline__ unsigned long long sp_lower_bound(const unsigned long long* k, unsigned long long n, unsigned long long key) {
@@ -2945,12 +2954,13 @@ __device__ __forceinline__ unsigned long long sp_lower_bound(const unsigned long
 
 template <SrOut kOut>
 __global__ void __launch_bounds__(256)
-sparse_join_kernel(SpJoin jn, unsigned long long e0, unsigned long long e1, unsigned long long* __restrict__ cursor, unsigned long long* __restrict__ cells) {
+sparse_join_kernel(SpJoin jn, unsigned long long e0, unsigned long long e1, unsigned long long* __restrict__ cursor, unsigned long long* __restrict__ cells,
+                   SpVals vl) {
     const int lane = threadIdx.x & 31;
     const unsigned long long step = (unsigned long long)gridDim.x * blockDim.x;
     for (unsigned long long e = e0 + (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; e - threadIdx.x % 32 < e1; e += step) {   // whole warps
         unsigned long long lo[kSpMaxDims], hi[kSpMaxDims], idx[kSpMaxDims];
-        unsigned long long c0 = 0, n = 0;
+        unsigned long long c0 = 0, n = 0, v = 0;
         bool any = e < e1;
         if (any) {
             const unsigned long long k0 = jn.keys[0][e];
@@ -2963,10 +2973,14 @@ sparse_join_kernel(SpJoin jn, unsigned long long e0, unsigned long long e1, unsi
                 idx[d] = lo[d];
                 any = lo[d] < hi[d];
             }
+            if (kOut == SrOut::kSum && any) {
+                const unsigned long long i = sp_lower_bound(vl.cols, vl.n, col), m = __ldg(vl.mag + i);
+                v = ((__ldg(vl.sign + (i >> 5)) >> (i & 31)) & 1u) ? 0ull - m : m;
+            }
         }
         // the cross product in odometer order, the last dimension fastest; pass 0 counts the cells in [lo, hi), pass 1 writes them
         unsigned long long at = 0;
-        for (int pass = 0; pass < (kOut == SrOut::kEmit ? 2 : 1); pass++) {
+        for (int pass = 0; pass < (kOut == SrOut::kCount ? 1 : 2); pass++) {
             if (pass == 1) {
                 unsigned long long inc = n;
 #pragma unroll
@@ -2980,7 +2994,10 @@ sparse_join_kernel(SpJoin jn, unsigned long long e0, unsigned long long e1, unsi
             for (;;) {
                 unsigned long long cell = c0;
                 for (int d = 1; d < jn.nd; d++) cell += (__ldg(jn.keys[d] + idx[d]) & ((1ull << jn.jbits[d]) - 1ull)) * jn.stride[d];
-                if (cell >= jn.lo && cell < jn.hi) { if (pass == 0) n++; else cells[at++] = cell; }
+                if (cell >= jn.lo && cell < jn.hi) {
+                    if (pass == 0) n++;
+                    else { if (kOut == SrOut::kSum) vl.out[at] = v; cells[at++] = cell; }
+                }
                 int d = jn.nd - 1;
                 while (d >= 1 && ++idx[d] == hi[d]) { idx[d] = lo[d]; d--; }
                 if (d < 1) break;
@@ -3036,6 +3053,48 @@ __global__ void __launch_bounds__(256)
 sparse_run_lengths_kernel(const unsigned long long* __restrict__ pos, unsigned long long u, unsigned long long n, unsigned long long* __restrict__ lens) {
     for (unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; k < u; k += (unsigned long long)gridDim.x * blockDim.x)
         lens[k] = (k + 1 < u ? pos[k + 1] : n) - pos[k];
+}
+
+// sums[r] += the values of run r of n sorted keys (sums zeroed by the caller; offs as for sparse_compact_kernel), wrapping.  A
+// run can hold millions of keys (one cell of a skewed row), so no thread walks a run: each element finds its run's index from
+// the tile's offset and the heads before it, each warp sums its 32 elements per run with a segmented scan, and the last lane of
+// each of the warp's runs adds that partial sum with one atomic.  A run of L keys costs about L / 32 atomics on its sum.
+__global__ void __launch_bounds__(kSortThreads)
+sparse_run_sums_kernel(const unsigned long long* __restrict__ keys, const unsigned long long* __restrict__ vals, unsigned long long n,
+                       const unsigned int* __restrict__ offs, unsigned long long* __restrict__ sums) {
+    __shared__ unsigned int wbase[kSortThreads / 32];
+    __shared__ unsigned int run;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const unsigned int le = 0xffffffffu >> (31 - lane);            // lanes 0 .. lane
+    if (tid == 0) run = offs[blockIdx.x];
+    const unsigned long long t0 = (unsigned long long)blockIdx.x * kSortTile;
+    for (int r = 0; r < kSortRounds; r++) {
+        const unsigned long long i = t0 + (unsigned long long)r * kSortThreads + tid;
+        const bool in = i < n;
+        const bool head = in && (i == 0 || keys[i] != keys[i - 1]);
+        const unsigned int bal = __ballot_sync(0xffffffffu, head);
+        if (lane == 0) wbase[wid] = (unsigned int)__popc(bal);
+        __syncthreads();
+        if (tid == 0) {
+            unsigned int o = run;
+            for (int k = 0; k < kSortThreads / 32; k++) { const unsigned int x = wbase[k]; wbase[k] = o; o += x; }
+            run = o;
+        }
+        __syncthreads();
+        // the run of element i: the heads before the warp, plus the warp's heads up to i, minus one (i == 0 is a head)
+        const unsigned int k = wbase[wid] + (unsigned int)__popc(bal & le) - 1u;
+        unsigned long long s = in ? vals[i] : 0ull;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, s, d);
+            const unsigned int ky = __shfl_up_sync(0xffffffffu, k, d);
+            if (lane >= d && ky == k) s += y;
+        }
+        const unsigned int kn = __shfl_down_sync(0xffffffffu, k, 1);
+        const bool next_in = __shfl_down_sync(0xffffffffu, (unsigned int)in, 1) != 0u;
+        if (in && (lane == 31 || !next_in || kn != k)) atomicAdd(&sums[k], s);
+        __syncthreads();                                   // (wbase is rewritten by the next round)
+    }
 }
 
 // ------------------------------------------------------------------------------------------------

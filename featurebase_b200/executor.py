@@ -1068,16 +1068,16 @@ class Executor:
             if f is not None and f.type == "int":                 # otherwise the per-group Sum below raises or finds no values
                 sum_f = f
         has_sort, has_having = "sort" in c.args, isinstance(c.args.get("having"), pql.Call)
-        sparse = None                                             # (cells, counts) of the non-empty groups from `start` on
+        sparse = None                                             # (cells, counts[, sums]) of the non-empty groups from `start` on
         if not int_dims and hasattr(self.ctx, "groupby_sparse") and (
                 max(len(r) for r in row_ids) > 65535 or math.prod(len(r) for r in row_ids) > self.GROUPBY_DENSE_MAX_CELLS):
             start = self._groupby_start(c, row_ids)
             if start is None:
                 return []
             sparse = self._groupby_sparse(idx, c, fields, row_ids, time_args, filt, start, shards,
-                                          device_limit=agg is None and not (has_sort or has_having))
+                                          device_limit=agg is None and not (has_sort or has_having), sum_f=sum_f)
         if sparse is not None:
-            sum_f = None                                          # Sum and Count(Distinct) per group, below
+            pass                                                  # groups in hand; Count(Distinct), and Sum over a non-int field, per group below
         elif sum_f is not None:
             counts, sums = self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, filt, shards, agg=sum_f)
         elif int_dims and hasattr(self.ctx, "groupby_mixed"):
@@ -1112,15 +1112,16 @@ class Executor:
         limit = c.args.get("limit") if not (has_sort or has_having) else None       # :3196-3212: no early limit when sorting / filtering
         out = []
         if sparse is not None:
-            groups = ((_unravel(int(flat), [len(r) for r in row_ids]), int(n)) for flat, n in zip(*sparse))
+            groups = ((_unravel(int(flat), [len(r) for r in row_ids]), int(n)) for flat, n in zip(sparse[0], sparse[1]))
         else:
             flat0 = int(np.ravel_multi_index(start, counts.shape))
             flat_counts = counts.reshape(-1)
             groups = ((np.unravel_index(int(flat), counts.shape), int(flat_counts[flat])) for flat in np.flatnonzero(flat_counts) if flat >= flat0)
-        for ix, n in groups:                                      # only Count > 0, lexicographic (:3960)
+        for g, (ix, n) in enumerate(groups):                      # only Count > 0, lexicographic (:3960)
             group = [(f.name, row_ids[k][int(i)]) for k, (f, i) in enumerate(zip(fields, ix))]
             if sum_f is not None:                                 # counts here: columns of the group holding a value of the field
-                out.append((group, n, _i64(int(sums[ix]) + n * sum_f.base)))      # executeSumCountShard :2203-2206
+                stored = int(sparse[2][g]) if sparse is not None else int(sums[ix])
+                out.append((group, n, _i64(stored + n * sum_f.base)))      # executeSumCountShard :2203-2206
             elif isinstance(agg, pql.Call):
                 rows = [pql.Call("Row", {name: rid, **(targs or {})}) for (name, rid), targs in zip(group, time_args)]
                 if isinstance(filt_call, pql.Call):
@@ -1172,11 +1173,13 @@ class Executor:
     # counts): a bound on memory, not a measured optimum.  A child of more than 65,535 rows takes it whatever the product.
     GROUPBY_DENSE_MAX_CELLS = 1 << 24
 
-    def _groupby_sparse(self, idx, c, fields, row_ids, time_args, filt, start, shards, device_limit):
+    def _groupby_sparse(self, idx, c, fields, row_ids, time_args, filt, start, shards, device_limit, sum_f=None):
         """(cells, counts) of a GroupBy over set-like children from fbgpu_groupby_sparse: the non-empty groups from the iterator's
         start position on, as row-major flat indices over the children's row lists, ascending; with device_limit (no sort, having or
-        Sum, which skips groups after the fact) at most offset + limit of them.  None when the context answers FBGPU_E_COMM or has
-        no such call: the dense tensor is asked for instead.  aggregate=Sum and Count(Distinct) then take the per-group
+        Sum, which skips groups after the fact) at most offset + limit of them.  With sum_f (the int field of aggregate=Sum),
+        (cells, counts, sums) from fbgpu_groupby_sparse_sum in the same call: a count is the group's columns holding a value of
+        the field, and a group is listed when it is non-zero.  None when the context answers FBGPU_E_COMM or has no such call:
+        the dense tensor is asked for instead.  Count(Distinct), and Sum over a field that is not int, take the per-group
         composition, one query per group."""
         sizes = [len(r) for r in row_ids]
         flat0 = 0
@@ -1186,6 +1189,9 @@ class Executor:
         limit = int(lim) + int(c.args.get("offset") or 0) if device_limit and lim else None
         set_dims = [(f.id, self._time_view_ids(f, targs) if targs else [VIEW_STANDARD], rows) for f, rows, targs in zip(fields, row_ids, time_args)]
         try:
+            if sum_f is not None:
+                return self.ctx.groupby_sparse(idx.id, set_dims, shards, filter_ops=filt, start=flat0, limit=limit,
+                                               agg=(sum_f.id, VIEW_BSI, sum_f.bit_depth))
             return self.ctx.groupby_sparse(idx.id, set_dims, shards, filter_ops=filt, start=flat0, limit=limit)
         except NotImplementedError:
             return None

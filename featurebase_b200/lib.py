@@ -54,7 +54,7 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum",
            "fbgpu_groupby_distinct", "fbgpu_topn_cutoffs", "fbgpu_node_topn_cutoffs", "fbgpu_bsi_sort", "fbgpu_node_bsi_sort",
            "fbgpu_bsi_distinct", "fbgpu_node_bsi_distinct", "fbgpu_extract_rows", "fbgpu_groupby_distinct_rows",
-           "fbgpu_groupby_sparse", "fbgpu_node_groupby_sparse"]
+           "fbgpu_groupby_sparse", "fbgpu_node_groupby_sparse", "fbgpu_groupby_sparse_sum", "fbgpu_node_groupby_sparse_sum"]
 
 
 def lib_path():
@@ -123,6 +123,8 @@ def load():
     L.fbgpu_groupby_distinct_rows.restype = C.c_int
     L.fbgpu_groupby_sparse.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, vp, i32, vp, i64, u64, i64, vp, vp, u64, C.POINTER(u64)]
     L.fbgpu_groupby_sparse.restype = C.c_int
+    L.fbgpu_groupby_sparse_sum.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i64, u64, i64, vp, vp, vp, u64, C.POINTER(u64)]
+    L.fbgpu_groupby_sparse_sum.restype = C.c_int
     L.fbgpu_count_pairs.argtypes, L.fbgpu_count_pairs.restype = [vp, u32, u32, u32, vp, u32, u32, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_comm_unique_id.argtypes, L.fbgpu_comm_unique_id.restype = [vp], C.c_int
     L.fbgpu_comm_init.argtypes, L.fbgpu_comm_init.restype = [vp, i32, i32, vp], C.c_int
@@ -142,7 +144,7 @@ def load():
     L.fbgpu_node_devices.argtypes, L.fbgpu_node_devices.restype = [vp], i32
     L.fbgpu_node_owner.argtypes, L.fbgpu_node_owner.restype = [vp, u64], i32
     L.fbgpu_node_ctx.argtypes, L.fbgpu_node_ctx.restype = [vp, i32], vp
-    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "groupby_sum", "bsi_sum", "bsi_minmax", "topn_cutoffs", "bsi_sort", "bsi_distinct", "groupby_sparse"):
+    for name in ("load_fragment", "load_fragments", "load_rbf_dir", "drop_fragment", "commit", "get_stats", "count", "any", "row", "count_pairs", "groupby", "groupby_values", "groupby_views", "groupby_mixed", "groupby_sum", "bsi_sum", "bsi_minmax", "topn_cutoffs", "bsi_sort", "bsi_distinct", "groupby_sparse", "groupby_sparse_sum"):
         src, dst = getattr(L, "fbgpu_" + name), getattr(L, "fbgpu_node_" + name)
         dst.argtypes, dst.restype = src.argtypes, src.restype
     L.fbgpu_node_row_counts.argtypes, L.fbgpu_node_row_counts.restype = [vp, u32, u32, u32, vp, i32, vp, i32, vp, i64, vp], C.c_int
@@ -631,27 +633,37 @@ class Context:
                                                        g.n_filter, g.shards, g.n_shards, out.ctypes.data))
         return out
 
-    def groupby_sparse(self, index, set_dims, shards, filter_ops=None, start=0, limit=None):
+    def groupby_sparse(self, index, set_dims, shards, filter_ops=None, start=0, limit=None, agg=None):
         """GroupBy over set, mutex, bool or time dimensions of any size as a list of its non-empty groups (fbgpu_groupby_sparse).
         set_dims: [(field, views, strictly ascending row ids)], 1..8 of them, each row taken as its union over the views.
         Returns (cells, counts), uint64 arrays: the row-major flat indices into the tensor groupby_views would fill (the last
         dimension fastest) of the cells with a non-zero count and cell >= start, ascending, at most `limit` of them, and their
-        counts."""
+        counts.  With agg = (field, BSI view, bit depth) of an int field x (fbgpu_groupby_sparse_sum), returns (cells, counts,
+        sums): a count is the number of the cell's columns holding a value of x, a cell is listed when it is non-zero, and sums
+        (int64) are the wrapping sums of those columns' stored values (value - Base)."""
         g = _groupby_args(set_dims, [], shards, filter_ops)
         n = C.c_uint64(0)
         cap = max(getattr(self, "_sparse_cap", 0), 1 << 12) if limit is None else max(min(int(limit), 1 << 16), 1)
+        lim = -1 if limit is None else int(limit)
         while True:
             cells, counts = np.empty(cap, dtype=np.uint64), np.empty(cap, dtype=np.uint64)
-            rc = self.L.fbgpu_groupby_sparse(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, g.filter, g.n_filter,
-                                             g.shards, g.n_shards, int(start), -1 if limit is None else int(limit), cells.ctypes.data,
-                                             counts.ctypes.data, cap, C.byref(n))
+            if agg is None:
+                rc = self.L.fbgpu_groupby_sparse(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, g.filter, g.n_filter,
+                                                 g.shards, g.n_shards, int(start), lim, cells.ctypes.data, counts.ctypes.data, cap, C.byref(n))
+            else:
+                sums = np.empty(cap, dtype=np.int64)
+                rc = self.L.fbgpu_groupby_sparse_sum(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows,
+                                                     int(agg[0]), int(agg[1]), int(agg[2]), g.filter, g.n_filter, g.shards, g.n_shards,
+                                                     int(start), lim, cells.ctypes.data, counts.ctypes.data, sums.ctypes.data, cap, C.byref(n))
             if rc == E_NOSPACE:
                 cap = int(n.value)
                 continue
             self._check(rc)
             if limit is None:
                 self._sparse_cap = cap
-            return cells[: n.value].copy(), counts[: n.value].copy()
+            if agg is None:
+                return cells[: n.value].copy(), counts[: n.value].copy()
+            return cells[: n.value].copy(), counts[: n.value].copy(), sums[: n.value].copy()
 
     def rows_payload_bytes(self, index, field, view, shards, row_ids=None):
         sh = _u64arr(shards)

@@ -482,6 +482,25 @@ int fbgpu_groupby_sparse(fbgpu_ctx *ctx, uint32_t index,
                          const uint64_t *shards, int64_t n_shards,
                          uint64_t start, int64_t limit,
                          uint64_t *out_cells, uint64_t *out_counts, uint64_t cap, uint64_t *out_n);
+/* GroupBy(..., aggregate=Sum(field=x)) over fbgpu_groupby_sparse's dimensions, in one call.  Dimensions, cells, start, limit
+ * and the NOSPACE contract are fbgpu_groupby_sparse's.  x: the int field afield, its BSI view aview and bit depth a_depth
+ * (0..64).  Per listed cell, out_counts = |filter ∩ the cell's rows ∩ exists(x)| and out_sums = the wrapping int64 sum of those
+ * columns' stored values of x (value - Base): the pair fbgpu_groupby_sum puts in that cell, and the pair fbgpu_bsi_sum returns
+ * under `filter ∩ the cell's rows`.  A sign with magnitude 0 counts, with value 0.  The caller adds count x Base.  A cell is
+ * listed when that count is non-zero, so a group whose columns hold no value of x is absent (the reference skips a group whose
+ * Sum count is 0), and `limit` counts listed cells.  A shard lacking x's fragments contributes nothing.  Argument errors
+ * (fbgpu_groupby_sparse's, a_depth outside 0..64, a null out_sums with cap > 0) are reported before the device check.  A context
+ * with a communicator attached returns FBGPU_E_COMM.  Device memory: fbgpu_groupby_sparse's bounds, with a chunk also holding
+ * at most 2^24 columns of filter ∩ exists(x), which take about 16 bytes each (column and magnitude, plus a sign bit); 32 bytes
+ * instead of 16 per (cell, value) pair of a join range of at most 2^24 pairs; and 64 bytes instead of 32 per cell of the
+ * running list, whose sums are a second list beside the counts. */
+int fbgpu_groupby_sparse_sum(fbgpu_ctx *ctx, uint32_t index,
+                             const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                             const uint64_t *row_ids_flat, const int32_t *n_rows,
+                             uint32_t afield, uint32_t aview, int32_t a_depth,
+                             const fbgpu_op *filter, int32_t n_filter_ops,
+                             const uint64_t *shards, int64_t n_shards, uint64_t start, int64_t limit,
+                             uint64_t *out_cells, uint64_t *out_counts, int64_t *out_sums, uint64_t cap, uint64_t *out_n);
 
 /* ---- multi-GPU reduce (replaces the HTTP fan-in of mapReduce/remoteExec, executor.go:6392-6533) ----
  * One context (process) per GPU; rank 0 creates the id, every rank joins.  When a communicator is attached,
@@ -593,6 +612,15 @@ int fbgpu_node_groupby_sparse(fbgpu_node *node, uint32_t index,
                               const uint64_t *row_ids_flat, const int32_t *n_rows, const fbgpu_op *filter, int32_t n_filter_ops,
                               const uint64_t *shards, int64_t n_shards, uint64_t start, int64_t limit,
                               uint64_t *out_cells, uint64_t *out_counts, uint64_t cap, uint64_t *out_n);
+/* The same for fbgpu_groupby_sparse_sum: the lists merge by cell with counts and sums added (the sums wrap), and the window is
+ * cut after the merge; exact for the same reason, since a cell is listed on a device exactly when its count there is non-zero. */
+int fbgpu_node_groupby_sparse_sum(fbgpu_node *node, uint32_t index,
+                                  const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                                  const uint64_t *row_ids_flat, const int32_t *n_rows,
+                                  uint32_t afield, uint32_t aview, int32_t a_depth,
+                                  const fbgpu_op *filter, int32_t n_filter_ops,
+                                  const uint64_t *shards, int64_t n_shards, uint64_t start, int64_t limit,
+                                  uint64_t *out_cells, uint64_t *out_counts, int64_t *out_sums, uint64_t cap, uint64_t *out_n);
 
 /* Inspection (any context): the stack-machine program the library would run for `ops` -- records of 16 bytes {u8 op, u8 pad[3],
  * u32 view slot, u64 row} (csrc/fbgpu_types.h DevOp); *out_depth = operand stack depth.  With index == 0xffffffff,
