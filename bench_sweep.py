@@ -27,6 +27,10 @@
   config H: config G's data with aggregate=Sum(field=v): GroupBy(Rows(m), aggregate=Sum(field=v), limit=1000) through the
             executor, fbgpu_groupby_sparse_sum against the sparse list plus one Sum per group; m x a with Sum against the
             counts-only sparse call; a x b with Sum against fbgpu_groupby_sum (only when named in --configs).
+  config J: config G's data with aggregate=Count(Distinct): GroupBy(Rows(m), aggregate=Count(Distinct(field=v)), limit=1000)
+            through the executor, fbgpu_groupby_sparse_distinct against the sparse list plus one Distinct per group; m x a with
+            Count(Distinct(field=b)) against the counts-only sparse call; a x b with Count(Distinct(field=w)) against
+            fbgpu_groupby_distinct (only when named in --configs).
   config N: TopN(f, Row(src=0), tanimotoThreshold=50) and TopN(f, Row(src=0), threshold=100) over --topn-rows rows of varied
             cardinality, fbgpu_topn_cutoffs against the per-shard count-matrix composition (only when named in --configs).
   config O: Sort over config X's 32-bit field with and without a limit, fbgpu_bsi_sort against extracting every value and
@@ -1442,6 +1446,91 @@ def config_extract_rows(args, out):
     real.close()
 
 
+class _NoSparseDistinct(_KernelMs):
+    """the same proxy without the sparse distinct calls: the executor lists the groups, then runs one Distinct per group"""
+
+    def __getattr__(self, name):
+        if name in ("groupby_sparse_distinct", "groupby_sparse_distinct_rows"):
+            raise AttributeError(name)
+        return super().__getattr__(name)
+
+
+def config_groupby_sparse_distinct(args, out):
+    """aggregate=Count(Distinct) over config G's data (_config_g_world with eight m fragments, so that Rows(m) lists more than
+    65,535 rows and the executor takes the sparse path), over --groupby-shards shards:
+      (a) GroupBy(Rows(m), aggregate=Count(Distinct(field=v)), limit=1000) through the executor: fbgpu_groupby_sparse_distinct
+          against today's composition without it (the sparse list of groups, then one Distinct per group until 1,000 are
+          listed), alternated; the same groups, counts and distinct counts;
+      (b) GroupBy(Rows(m), Rows(a), aggregate=Count(Distinct(field=b))), every group, as library calls:
+          fbgpu_groupby_sparse_distinct_rows over b's 256 rows against the counts-only fbgpu_groupby_sparse on the same
+          dimensions, alternated, to show the cost of carrying x; the distinct call's cells must be among the counts-only
+          call's, each with a distinct count of at least 1;
+      (c) a x b, 256 x 256, with Count(Distinct(field=w)), as library calls: fbgpu_groupby_sparse_distinct against the dense
+          fbgpu_groupby_distinct, alternated; the same cells (the dense tensor's non-zero ones) and distinct counts.
+    Per arm: the median wall clock, the summed last_query_gpu_ms of the arm's library queries and their number."""
+    from featurebase_b200 import executor as X
+    S = args.groupby_shards
+    h, idx, fa, fb, ff, fw, fv, fm, fe, load_s = _config_g_world(args, "J", m_fragments=8)
+    real, card, sh = h.ctx, _card(), list(range(S))
+    dev, comp = _KernelMs(real), _NoSparseDistinct(real)
+    ra, rm = np.arange(256, dtype=np.uint64), np.arange(1_000_000, dtype=np.uint64)
+    dims_ab = [(fa.id, [X.VIEW_STANDARD], ra), (fb.id, [X.VIEW_STANDARD], ra)]
+    dims_ma = [(fm.id, [X.VIEW_STANDARD], rm), (fa.id, [X.VIEW_STANDARD], ra)]
+    xw = (fw.id, X.VIEW_BSI, fw.bit_depth, np.arange(64, dtype=np.int64))      # w's stored values (Base 0)
+    q = "GroupBy(Rows(m), aggregate=Count(Distinct(field=v)), limit=1000)"
+
+    def executor(ctx):
+        def run():
+            h.ctx = ctx
+            try:
+                return X.Executor(h).execute("i", q, sh)[0]
+            finally:
+                h.ctx = real
+        return run
+
+    def dense_distinct():
+        t = dev.groupby_distinct(idx.id, dims_ab, [], xw, sh).reshape(-1)
+        nz = np.flatnonzero(t)
+        return nz.astype(np.uint64), t[nz]
+
+    arms = {"a": {"device": (dev, executor(dev)), "composition": (comp, executor(comp))},
+            "b": {"sparse_distinct_rows": (dev, lambda: dev.groupby_sparse_distinct_rows(idx.id, dims_ma, (fb.id, X.VIEW_STANDARD, ra), sh)),
+                  "sparse_counts": (dev, lambda: dev.groupby_sparse(idx.id, dims_ma, sh))},
+            "c": {"sparse_distinct": (dev, lambda: dev.groupby_sparse_distinct(idx.id, dims_ab, xw, sh)), "dense_distinct": (dev, dense_distinct)}}
+    for part, fns in arms.items():
+        rec = {name: {"wall": [], "gpu_ms": [], "queries": []} for name in fns}
+        res = {}
+        for i in range(1 + args.steps):                          # one warm-up round, then alternate the arms
+            for name in (sorted(fns) if i % 2 == 0 else sorted(fns, reverse=True)):
+                proxy, fn = fns[name]
+                q0, proxy.ms = real.counters()["queries"], 0.0
+                t1 = time.perf_counter()
+                r = fn()
+                wall = (time.perf_counter() - t1) * 1e3
+                res.setdefault(name, r)
+                print(f"config J ({part}): {name} step {i}: {wall:.1f} ms", file=sys.stderr, flush=True)
+                if i >= 1:
+                    rec[name]["wall"].append(wall)
+                    rec[name]["gpu_ms"].append(proxy.ms)
+                    rec[name]["queries"].append(real.counters()["queries"] - q0)
+        v = list(res.values())
+        if part == "a":
+            assert v[0] == v[1] and len(v[0]) == 1000, part
+        elif part == "b":                                      # a listed cell is a group, and holds at least one row of b
+            cells, dist = res["sparse_distinct_rows"]
+            assert len(cells) and np.isin(cells, res["sparse_counts"][0]).all() and dist.min() >= 1, part
+        else:
+            assert all(np.array_equal(x[k], v[0][k]) for x in v for k in range(2)), part
+        for name, dd in rec.items():
+            out({"config": "J", "part": part, "arm": name, "gpu": card, "shards": S, "groups": len(res[name] if part == "a" else res[name][0]),
+                 "checked": True, "wall_ms": float(np.median(dd["wall"])), "wall_ms_min": float(np.min(dd["wall"])),
+                 "wall_ms_max": float(np.max(dd["wall"])), "gpu_ms": float(np.median(dd["gpu_ms"])), "queries": int(np.median(dd["queries"])),
+                 "steps": len(dd["wall"]), "load_s": round(load_s, 1),
+                 "note": "median over the timed steps of the wall clock (executor: Rows pre-pass included), of the summed last_query_gpu_ms "
+                         "of the arm's library queries and of their number"})
+    real.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", default="5,3,4")
@@ -1485,6 +1574,8 @@ def main():
             config_groupby_sparse(args, out)
         elif c == "H":
             config_groupby_sparse_sum(args, out)
+        elif c == "J":
+            config_groupby_sparse_distinct(args, out)
         elif c == "N":
             config_topn_cutoffs(args, out)
         elif c == "O":

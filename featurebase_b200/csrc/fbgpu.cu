@@ -2664,6 +2664,13 @@ extern "C" int fbgpu_groupby_distinct_rows(fbgpu_ctx* c, uint32_t index, const u
 // (columns_emit_kernel and extract_values_kernel over the chunk's units, in (unit, column) order).  The join emits (cell, value)
 // pairs, sorted by cell; each run becomes (cell, count) as before and its wrapping sum (sparse_run_sums_kernel).  The sums form a
 // second running list with the same cells, merged by the same deterministic sort and compaction, so the two stay aligned.
+// With a distinct x (fbgpu_groupby_sparse_distinct(_rows)) x is one more, trailing, dimension of the join, whose index j is x's
+// place in its list, and the join's strides are packed so that it emits the key cell << xbits | j (xbits = bit_width(n_x - 1)),
+// within [start << xbits, end << xbits).  A set-like x is walked by sparse_rows_kernel like any dimension.  For an int x the
+// filter holds exists(x), and the chunk's value list (as for Sum) becomes x's keys (sparse_xkeys_kernel, then sorted).  Each
+// join range's keys are sorted and deduped, and merged into the running list of distinct (cell, j) keys by an append and
+// another dedupe.  At the end the keys are shifted down to their cells and run-length coded: a run's length is the cell's
+// distinct count.
 
 // the argument checks fbgpu_groupby_sparse and its node form make before any device is touched
 static int groupby_sparse_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
@@ -2690,10 +2697,15 @@ static int groupby_sparse_args(const void* handle, const uint32_t* fields, const
 // the aggregate of fbgpu_groupby_sparse_sum: an int field's BSI view and bit depth
 struct SpAgg { uint32_t field, view; int depth; };
 
+// the x of fbgpu_groupby_sparse_distinct(_rows): its field and view; for an int x (values != NULL) its bit depth and n strictly
+// ascending listed stored values, for a set-like x (rows != NULL) its n strictly ascending listed rows
+struct SpDistinct { uint32_t field, view; int depth; const int64_t* values; const uint64_t* rows; int32_t n; };
+
 // device buffers of one fbgpu_groupby_sparse call, freed when it returns: they can be large, and are not reused by other calls.
-// b[d]: dimension d's keys; b[nd]: the cells (with an aggregate, (cell, value) pairs); b[kSpMaxDims + 1]: the cursor, row lists
-// and view slots; with an aggregate, b[kSpMaxDims + 2]: a chunk's value list, b[kSpMaxDims + 3]: its two ColUnit lists,
-// b[kSpMaxDims + 4]: the running list of sums.
+// b[d]: dimension d's keys (with a distinct x, x is the last dimension); b[nd]: the cells (with an aggregate, (cell, value)
+// pairs; with a distinct x, (cell, x) keys); b[kSpMaxDims + 1]: the cursor, row lists, an int x's listed values and view slots;
+// with an aggregate or an int x, b[kSpMaxDims + 2]: a chunk's value list, b[kSpMaxDims + 3]: its two ColUnit lists;
+// b[kSpMaxDims + 4]: the running list of sums, or with a distinct x the final (cell, distinct count) list.
 struct SparseBufs {
     DevBuf b[kSpMaxDims + 5];
     ~SparseBufs() { for (DevBuf& x : b) x.release(); }
@@ -2770,55 +2782,82 @@ static int sparse_merge(Query& q, SortPairs& cs, SortPairs& acc, SortPairs* sums
     return 0;
 }
 
-// the non-empty cells >= start of the dimensions `dims` under the filter, ascending, at most `limit` of them (limit < 0: all), and
+// the distinct sorted keys of cs added to acc, a keys-only list of distinct sorted keys: appended, then sorted and deduped
+static int sparse_union(Query& q, const SortPairs& cs, SortPairs& acc, int bits) {
+    const bool merge = acc.n > 0;
+    int rc = acc.reserve(acc.n + cs.n); if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(acc.keys(acc.cur) + acc.n, cs.keys(cs.cur), cs.n * 8, cudaMemcpyDeviceToDevice, q.w->stream));
+    acc.n += cs.n;
+    return merge ? distinct_keys(q, acc, bits) : 0;
+}
+
+// the non-empty cells >= start of the dimensions `gdims` under the filter, ascending, at most `limit` of them (limit < 0: all), and
 // their counts (store lock held).  With `agg`, the filter is <filter> ∩ exists(x), a cell is non-empty when its count there is,
-// and `sums` gets each listed cell's wrapping sum of x's stored values.
-static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<GbDim>& dims, const fbgpu_op* filter, int32_t n_filter_ops,
+// and `sums` gets each listed cell's wrapping sum of x's stored values.  With `dx` (limit < 0), the cells in [start, end) where
+// at least one listed x value (row) is held by a column of the filter ∩ the cell's rows, and as counts the number of such x.
+static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<GbDim>& gdims, const fbgpu_op* filter, int32_t n_filter_ops,
                               const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
-                              std::vector<uint64_t>& cells, std::vector<uint64_t>& counts, const SpAgg* agg = nullptr, std::vector<int64_t>* sums = nullptr) {
+                              std::vector<uint64_t>& cells, std::vector<uint64_t>& counts, const SpAgg* agg = nullptr, std::vector<int64_t>* sums = nullptr,
+                              const SpDistinct* dx = nullptr, uint64_t end = ~0ull) {
     cells.clear(); counts.clear();
     if (sums) sums->clear();
-    const int nd = (int)dims.size();
+    const int ng = (int)gdims.size();
+    const bool x_int = dx && dx->values, x_rows = dx && dx->rows;
+    std::vector<GbDim> dims = gdims;                 // the dimensions sparse_rows_kernel walks: a set-like x is the last one
+    if (x_rows) dims.push_back(GbDim{ dx->field, &dx->view, 1, dx->rows, dx->n });
+    const int nr = (int)dims.size(), nd = nr + (x_int ? 1 : 0);        // nd: the join's dimensions
+    const bool vals = agg || x_int;                  // a value list per chunk, of Sum's x or of an int distinct x
+    const SpAgg vx = agg ? *agg : x_int ? SpAgg{ dx->field, dx->view, dx->depth } : SpAgg{};
+    const int xbits = dx ? bit_width((uint64_t)dx->n - 1) : 0;
     Query q(c); Workspace* w = q.w;
     const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);
     std::vector<fbgpu_op> full;
     uint32_t fv_x = 0;
-    if (agg) {
-        full = and_row(filter, n_filter_ops, agg->field, agg->view, 0);    // <filter> ∩ exists, as for fbgpu_bsi_sum
-        fv_x = view_id_locked(c, ViewKey{ index, agg->field, agg->view }, false);
+    if (vals) {
+        full = and_row(filter, n_filter_ops, vx.field, vx.view, 0);    // <filter> ∩ exists, as for fbgpu_bsi_sum
+        fv_x = view_id_locked(c, ViewKey{ index, vx.field, vx.view }, false);
         filter = full.data(); n_filter_ops = (int32_t)full.size();
     }
     const bool have_filter = n_filter_ops > 0;
     int rc = have_filter ? q.open(index, filter, n_filter_ops, sorted.data(), (int64_t)sorted.size()) : q.open(sorted.data(), (int64_t)sorted.size());
     if (rc) return rc;
-    if (limit == 0) { q.finish(); return FBGPU_OK; }
-    SparseBufs sb;
     SpJoin jn{}; jn.nd = nd; jn.lo = start; jn.hi = ~0ull;
-    // b[kSpMaxDims + 1]: [cursor | rows of every dimension (u64) | view slots of every dimension (u32)]
+    uint64_t total = 1;                              // the group dimensions' cells; x, when there is one, has stride 1
+    for (int d = ng - 1; d >= 0; d--) { jn.stride[d] = total << xbits; total *= (uint64_t)dims[d].n_rows; jn.jbits[d] = bit_width((uint64_t)dims[d].n_rows - 1); }
+    if (dx) {
+        jn.stride[ng] = 1; jn.jbits[ng] = xbits;
+        const uint64_t e = std::min(end, total);
+        jn.lo = std::min(start, e) << xbits; jn.hi = e << xbits;
+    }
+    const int cell_bits = bit_width((total << xbits) - 1);                 // a join key's bits
+    if (limit == 0 || jn.lo >= jn.hi) { q.finish(); return FBGPU_OK; }
+    SparseBufs sb;
+    // b[kSpMaxDims + 1]: [cursor | rows of every dimension (u64) | an int x's listed values | view slots of every dimension (u32)]
     std::vector<uint64_t> rows_h(1, 0);
     std::vector<uint32_t> fvs_h;
-    std::vector<size_t> row_at(nd), fv_at(nd); std::vector<int> n_fv(nd);
-    for (int d = 0; d < nd; d++) {
+    std::vector<size_t> row_at(nr), fv_at(nr); std::vector<int> n_fv(nr);
+    for (int d = 0; d < nr; d++) {
         row_at[d] = rows_h.size(); rows_h.insert(rows_h.end(), dims[d].rows, dims[d].rows + dims[d].n_rows);
         const std::vector<uint32_t> fvs = view_slots(c, index, dims[d].field, dims[d].views, dims[d].n_views);
         fv_at[d] = fvs_h.size(); n_fv[d] = (int)fvs.size(); fvs_h.insert(fvs_h.end(), fvs.begin(), fvs.end());
     }
+    const size_t xv_at = rows_h.size();
+    if (x_int) for (int32_t i = 0; i < dx->n; i++) rows_h.push_back((uint64_t)dx->values[i]);
     DevBuf& meta = sb.b[kSpMaxDims + 1];
     if (meta.ensure(rows_h.size() * 8 + fvs_h.size() * 4)) return FBGPU_E_NOMEM;
     unsigned long long* cursor = (unsigned long long*)meta.p;
     const uint64_t* d_rows = (const uint64_t*)meta.p;
+    const long long* d_xs = (const long long*)(d_rows + xv_at);
     const uint32_t* d_fv0 = (const uint32_t*)(d_rows + rows_h.size());
     CUDA_TRY(cudaMemcpyAsync(meta.p, rows_h.data(), rows_h.size() * 8, cudaMemcpyHostToDevice, w->stream));
     CUDA_TRY(cudaMemcpyAsync((void*)d_fv0, fvs_h.data(), fvs_h.size() * 4, cudaMemcpyHostToDevice, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
-    uint64_t total = 1;
-    for (int d = nd - 1; d >= 0; d--) { jn.stride[d] = total; total *= (uint64_t)dims[d].n_rows; jn.jbits[d] = bit_width((uint64_t)dims[d].n_rows - 1); }
-    const int cell_bits = bit_width(total - 1);
     std::vector<SortPairs> dk;
     for (int d = 0; d < nd; d++) dk.emplace_back(w, ~0ull, true, &sb.b[d]);
-    SortPairs cs(w, ~0ull, !agg, &sb.b[nd]), acc(w, ~0ull), acc_sums(w, ~0ull, false, &sb.b[kSpMaxDims + 4]);
+    // acc: the running list, (cell, count) pairs or, with dx, distinct (cell, x) keys
+    SortPairs cs(w, ~0ull, !agg, &sb.b[nd]), acc(w, ~0ull, dx != nullptr), acc_sums(w, ~0ull, false, &sb.b[kSpMaxDims + 4]);
     const long long batch = std::min<long long>(c->unit_batch, 1ll << 16);     // a unit's place in a chunk takes 16 bits of a key
-    std::vector<uint32_t> units, keep, chunk, ncol;                            // ncol: with agg, the filter columns of units[k]
+    std::vector<uint32_t> units, keep, chunk, ncol;                            // ncol: with a filter, the filter columns of units[k]
     std::vector<uint64_t> ucnt;
     std::vector<ColUnit> vunits;
     for (long long u0 = 0; u0 < q.n_units; u0 += batch) {
@@ -2837,35 +2876,35 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
         const uint64_t* bshards = q.d_shards + u0 / kSlotsPerRow;
         const size_t nun = units.size();
         // count pass: the hits of every unit in every dimension
-        if (w->d_emit_units.ensure(nun * 4) || w->d_cells.ensure(nun * nd * 8) || w->h_out.ensure(nun * nd * 8)) return FBGPU_E_NOMEM;
+        if (w->d_emit_units.ensure(nun * 4) || w->d_cells.ensure(nun * nr * 8) || w->h_out.ensure(nun * nr * 8)) return FBGPU_E_NOMEM;
         CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, units.data(), nun * 4, cudaMemcpyHostToDevice, w->stream));
-        CUDA_TRY(cudaMemsetAsync(w->d_cells.p, 0, nun * nd * 8, w->stream));
+        CUDA_TRY(cudaMemsetAsync(w->d_cells.p, 0, nun * nr * 8, w->stream));
         const unsigned grid = (unsigned)std::min<size_t>(nun, (size_t)c->sm_count * 8);
-        for (int d = 0; d < nd; d++) {
+        for (int d = 0; d < nr; d++) {
             sparse_rows_kernel<SrOut::kCount><<<grid, kSrThreads, 0, w->stream>>>(store_ref(c), d_fv0 + fv_at[d], n_fv[d], d_rows + row_at[d], dims[d].n_rows, jn.jbits[d],
                 bitmaps, (const uint32_t*)w->d_emit_units.p, (int)nun, bshards, (unsigned long long*)w->d_cells.p + (size_t)d * nun, nullptr, nullptr);
             CUDA_TRY(cudaGetLastError()); q.launches++;
         }
-        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_cells.p, nun * nd * 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_cells.p, nun * nr * 8, cudaMemcpyDeviceToHost, w->stream));
         CUDA_TRY(cudaStreamSynchronize(w->stream));
-        ucnt.assign((const uint64_t*)w->h_out.p, (const uint64_t*)w->h_out.p + nun * nd);
+        ucnt.assign((const uint64_t*)w->h_out.p, (const uint64_t*)w->h_out.p + nun * nr);
         keep.clear();                                        // the units every dimension meets, as their places in `units`
         for (size_t e = 0; e < nun; e++) {
             bool all = true;
-            for (int d = 0; d < nd && all; d++) all = ucnt[(size_t)d * nun + e] > 0;
+            for (int d = 0; d < nr && all; d++) all = ucnt[(size_t)d * nun + e] > 0;
             if (all) keep.push_back((uint32_t)e);
         }
         for (size_t a = 0; a < keep.size();) {
-            // the chunk keep[a, b): at most kSortChunk hits per dimension and, with agg, filter columns (at least one unit)
-            std::vector<uint64_t> hits(nd, 0);
+            // the chunk keep[a, b): at most kSortChunk hits per dimension and, with a value list, filter columns (at least one unit)
+            std::vector<uint64_t> hits(nr, 0);
             uint64_t vn = 0;
             size_t b = a;
             for (; b < keep.size(); b++) {
-                bool fits = !agg || vn + ncol[keep[b]] <= kSortChunk;
-                for (int d = 0; d < nd; d++) fits = fits && hits[d] + ucnt[(size_t)d * nun + keep[b]] <= kSortChunk;
+                bool fits = !vals || vn + ncol[keep[b]] <= kSortChunk;
+                for (int d = 0; d < nr; d++) fits = fits && hits[d] + ucnt[(size_t)d * nun + keep[b]] <= kSortChunk;
                 if (!fits && b > a) break;
-                for (int d = 0; d < nd; d++) hits[d] += ucnt[(size_t)d * nun + keep[b]];
-                if (agg) vn += ncol[keep[b]];
+                for (int d = 0; d < nr; d++) hits[d] += ucnt[(size_t)d * nun + keep[b]];
+                if (vals) vn += ncol[keep[b]];
             }
             chunk.clear();
             for (size_t k = a; k < b; k++) chunk.push_back(units[keep[k]]);
@@ -2873,7 +2912,7 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
             if (w->d_emit_units.ensure(chunk.size() * 4)) return FBGPU_E_NOMEM;
             CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, chunk.data(), chunk.size() * 4, cudaMemcpyHostToDevice, w->stream));
             const unsigned cgrid = (unsigned)std::min<size_t>(chunk.size(), (size_t)c->sm_count * 8);
-            for (int d = 0; d < nd; d++) {
+            for (int d = 0; d < nr; d++) {
                 SortPairs& k = dk[(size_t)d];
                 k.n = 0;
                 rc = k.reserve(hits[d]); if (rc) return rc;
@@ -2886,10 +2925,10 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
                 rc = n_fv[d] > 1 ? distinct_keys(q, k, kbits) : sort_pairs(q, k, kbits, ~0ull); if (rc) return rc;
                 jn.keys[d] = k.keys(k.cur); jn.n[d] = k.n;
             }
-            // with agg, the chunk's value list: the filter columns of its units in (unit, column) order, as (e << 16 | c) keys
-            // (columns_emit_kernel over units based at e << 16) and their values' magnitudes and sign bits (extract_values_kernel)
+            // with agg or an int x, the chunk's value list: the filter columns of its units in (unit, column) order, as (e << 16 | c)
+            // keys (columns_emit_kernel over units based at e << 16) and their values' magnitudes and sign bits (extract_values_kernel)
             SpVals vl{};
-            if (agg) {
+            if (vals) {
                 vunits.clear();
                 for (int pass = 0; pass < 2; pass++) {
                     uint64_t off = 0;
@@ -2913,10 +2952,24 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
                 CUDA_TRY(cudaMemsetAsync(mag, 0, vn * 8 + sign_bytes, w->stream));
                 columns_emit_kernel<<<cgrid, kEmitThreads, 0, w->stream>>>(bitmaps, d_vu + chunk.size(), (int)chunk.size(), vcols);
                 CUDA_TRY(cudaGetLastError());
-                extract_values_kernel<<<cgrid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv_x, agg->depth, bitmaps, d_vu, (int)chunk.size(), mag, sign);
+                extract_values_kernel<<<cgrid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv_x, vx.depth, bitmaps, d_vu, (int)chunk.size(), mag, sign);
                 CUDA_TRY(cudaGetLastError());
                 q.launches += 2;
                 vl.cols = vcols; vl.mag = mag; vl.sign = sign; vl.n = vn;
+            }
+            if (x_int) {                                     // x's keys: the chunk's columns holding a listed value, sorted
+                SortPairs& k = dk[(size_t)nr];
+                k.n = 0;
+                rc = k.reserve(vn); if (rc) return rc;
+                CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
+                const unsigned xgrid = (unsigned)std::min<uint64_t>((vn + 255) / 256, (uint64_t)c->sm_count * 8);
+                sparse_xkeys_kernel<<<xgrid, 256, 0, w->stream>>>(vl.cols, vl.mag, vl.sign, vn, d_xs, dx->n, xbits, cursor, k.keys(k.cur));
+                CUDA_TRY(cudaGetLastError()); q.launches++;
+                CUDA_TRY(cudaMemcpyAsync(w->h_out.p, cursor, 8, cudaMemcpyDeviceToHost, w->stream));
+                CUDA_TRY(cudaStreamSynchronize(w->stream));
+                k.n = *(const uint64_t*)w->h_out.p;
+                rc = sort_pairs(q, k, ebits + 16 + xbits, ~0ull); if (rc) return rc;
+                jn.keys[nr] = k.keys(k.cur); jn.n[nr] = k.n;
             }
             // the join, over ranges of dimension 0's entries that give at most kSortChunk cells (at least one entry)
             const uint64_t n0 = jn.n[0];
@@ -2945,8 +2998,13 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
                     }
                     CUDA_TRY(cudaGetLastError()); q.launches++;
                     cs.n = got;
-                    rc = sort_pairs(q, cs, cell_bits, ~0ull); if (rc) return rc;
-                    rc = sparse_merge(q, cs, acc, agg ? &acc_sums : nullptr, cell_bits, limit, &jn.hi); if (rc) return rc;
+                    if (dx) {
+                        rc = distinct_keys(q, cs, cell_bits); if (rc) return rc;
+                        rc = sparse_union(q, cs, acc, cell_bits); if (rc) return rc;
+                    } else {
+                        rc = sort_pairs(q, cs, cell_bits, ~0ull); if (rc) return rc;
+                        rc = sparse_merge(q, cs, acc, agg ? &acc_sums : nullptr, cell_bits, limit, &jn.hi); if (rc) return rc;
+                    }
                 }
                 e0 = e1;
             }
@@ -2956,10 +3014,23 @@ static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<Gb
         CUDA_TRY(cudaStreamSynchronize(w->stream));
         q.add_elapsed();
     }
-    cells.resize(acc.n); counts.resize(acc.n);
-    if (acc.n) {
-        CUDA_TRY(cudaMemcpyAsync(cells.data(), acc.keys(acc.cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
-        CUDA_TRY(cudaMemcpyAsync(counts.data(), acc.cols(acc.cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
+    // with dx, the distinct (cell, x) keys as their cells, run-length coded into (cell, distinct count) pairs
+    SortPairs& res = dx ? acc_sums : acc;
+    if (dx && acc.n) {
+        CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
+        const unsigned sgrid = (unsigned)std::min<uint64_t>((acc.n + 255) / 256, (uint64_t)c->sm_count * 8);
+        sparse_shift_kernel<<<sgrid, 256, 0, w->stream>>>(acc.keys(acc.cur), acc.n, xbits);
+        CUDA_TRY(cudaGetLastError()); q.launches++;
+        unsigned long long no_hi = ~0ull;
+        rc = sparse_merge(q, acc, acc_sums, nullptr, cell_bits, -1, &no_hi); if (rc) return rc;
+        CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        q.add_elapsed();
+    }
+    cells.resize(res.n); counts.resize(res.n);
+    if (res.n) {
+        CUDA_TRY(cudaMemcpyAsync(cells.data(), res.keys(res.cur), res.n * 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaMemcpyAsync(counts.data(), res.cols(res.cur), res.n * 8, cudaMemcpyDeviceToHost, w->stream));
         if (agg) {
             sums->resize(acc.n);
             CUDA_TRY(cudaMemcpyAsync(sums->data(), acc_sums.cols(acc_sums.cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
@@ -3037,6 +3108,75 @@ extern "C" int fbgpu_groupby_sparse_sum(fbgpu_ctx* c, uint32_t index, const uint
                             start, limit, cells, counts, &agg, &sums);
     if (rc) return rc;
     return write_cells(cells, counts, sums, out_cells, out_counts, out_sums, cap, out_n);
+} FBGPU_CATCH
+
+// the argument checks of fbgpu_groupby_sparse_distinct(_rows): fbgpu_groupby_sparse's, then at most kSpMaxDims - 1 dimensions
+// (x takes the join's last slot), x's list (values for an int x, rows for a set-like one) and depth, the range, and room in a
+// u64 for cell << bit_width(n_x - 1)
+static int groupby_sparse_distinct_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                                        const uint64_t* row_ids_flat, const int32_t* n_rows, const int64_t* x_values, const uint64_t* x_rows, int32_t n_x,
+                                        int32_t x_depth, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
+                                        uint64_t start, uint64_t end, const uint64_t* out_cells, const uint64_t* out_distinct, uint64_t cap, const uint64_t* out_n) {
+    int rc = groupby_sparse_args(handle, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards,
+                                 out_cells, out_distinct, cap, out_n);
+    if (rc) return rc;
+    if (n_fields > kSpMaxDims - 1) return fail(FBGPU_E_INVALID, "n_fields=%d outside 1..%d", n_fields, kSpMaxDims - 1);
+    if (!x_values && !x_rows) return fail(FBGPU_E_INVALID, "bad argument");
+    if (n_x < 1) return fail(FBGPU_E_INVALID, "n_x=%d < 1", n_x);
+    for (int32_t i = 1; i < n_x; i++) {
+        if (x_values && x_values[i] <= x_values[i - 1]) return fail(FBGPU_E_INVALID, "x_values are not strictly ascending at position %d", i);
+        if (x_rows && x_rows[i] <= x_rows[i - 1]) return fail(FBGPU_E_INVALID, "x_rows are not strictly ascending at position %d", i);
+    }
+    if (x_depth < 0 || x_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", x_depth);
+    if (start > end) return fail(FBGPU_E_INVALID, "start=%llu > end=%llu", (unsigned long long)start, (unsigned long long)end);
+    uint64_t cells = 1;
+    for (int32_t i = 0; i < n_fields; i++) cells *= (uint64_t)n_rows[i];                 // fits: checked above
+    const int xbits = bit_width((uint64_t)n_x - 1);
+    if (cells > (~0ull >> xbits)) return fail(FBGPU_E_INVALID, "product of n_rows times 2^%d exceeds 2^64 - 1", xbits);
+    return 0;
+}
+
+// fbgpu_groupby_sparse_distinct and fbgpu_groupby_sparse_distinct_rows, x described by dx
+static int groupby_sparse_distinct_call(fbgpu_ctx* c, const char* name, uint32_t index, const uint32_t* fields, const uint32_t* views_flat,
+                                        const int32_t* n_views, int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows, const SpDistinct& dx,
+                                        const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t start, uint64_t end,
+                                        uint64_t* out_cells, uint64_t* out_distinct, uint64_t cap, uint64_t* out_n) {
+    int rc = groupby_sparse_distinct_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, dx.values, dx.rows, dx.n, dx.depth,
+                                          filter, n_filter_ops, shards, n_shards, start, end, out_cells, out_distinct, cap, out_n);
+    if (rc) return rc;
+    if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "%s is local to one context: distinct sets of the ranks merge by union, not by sum", name);
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    std::vector<uint64_t> cells, distinct;
+    rc = groupby_sparse_run(c, index, gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows), filter, n_filter_ops, shards, n_shards,
+                            start, -1, cells, distinct, nullptr, nullptr, &dx, end);
+    if (rc) return rc;
+    return write_cells(cells, distinct, out_cells, out_distinct, cap, out_n);
+}
+
+// GroupBy(..., aggregate=Count(Distinct(field=x))) over set-like dimensions of any number of rows, x an int field: per cell of
+// fbgpu_groupby_sparse's in [start, end), the number of listed stored values of x that a column of filter ∩ the cell's rows
+// holds, listed where it is non-zero (executeGroupBy's Count(Distinct), executor.go:3343-3385, for every group at once)
+extern "C" int fbgpu_groupby_sparse_distinct(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views,
+                                             int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows, uint32_t xfield, uint32_t xview,
+                                             int32_t x_depth, const int64_t* x_values, int32_t n_x, const fbgpu_op* filter, int32_t n_filter_ops,
+                                             const uint64_t* shards, int64_t n_shards, uint64_t start, uint64_t end,
+                                             uint64_t* out_cells, uint64_t* out_distinct, uint64_t cap, uint64_t* out_n) try {
+    return groupby_sparse_distinct_call(c, "fbgpu_groupby_sparse_distinct", index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
+                                        SpDistinct{ xfield, xview, x_depth, x_values, nullptr, n_x }, filter, n_filter_ops, shards, n_shards,
+                                        start, end, out_cells, out_distinct, cap, out_n);
+} FBGPU_CATCH
+
+// the same with a set, mutex, bool or time field x: per cell, the number of listed rows of x holding a column of filter ∩ the
+// cell's rows
+extern "C" int fbgpu_groupby_sparse_distinct_rows(fbgpu_ctx* c, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views,
+                                                  int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows, uint32_t xfield, uint32_t xview,
+                                                  const uint64_t* x_rows, int32_t n_x, const fbgpu_op* filter, int32_t n_filter_ops,
+                                                  const uint64_t* shards, int64_t n_shards, uint64_t start, uint64_t end,
+                                                  uint64_t* out_cells, uint64_t* out_distinct, uint64_t cap, uint64_t* out_n) try {
+    return groupby_sparse_distinct_call(c, "fbgpu_groupby_sparse_distinct_rows", index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
+                                        SpDistinct{ xfield, xview, 0, nullptr, x_rows, n_x }, filter, n_filter_ops, shards, n_shards,
+                                        start, end, out_cells, out_distinct, cap, out_n);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ comm

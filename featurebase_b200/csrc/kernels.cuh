@@ -3097,6 +3097,43 @@ sparse_run_sums_kernel(const unsigned long long* __restrict__ keys, const unsign
     }
 }
 
+// the dimension keys of an int x in fbgpu_groupby_sparse_distinct, from one chunk's value list: column i (cols[i], of the
+// (e << 16 | c) form) holds the stored value mag[i], negated when bit i of sign is set (extract_values_kernel's output, wrapping
+// like fbgpu_extract, so a sign with magnitude 0 is 0 and depth 64 gives INT64_MIN).  When that value is xs[j] of the n_x
+// ascending listed values (binary search), the key (cols[i] << xbits) | j goes to keys[(*cursor)++]; an unlisted value gives
+// none.  Warps reserve their keys with one atomic, so the order is arbitrary: the host sorts the keys.
+__global__ void __launch_bounds__(256)
+sparse_xkeys_kernel(const unsigned long long* __restrict__ cols, const unsigned long long* __restrict__ mag, const unsigned int* __restrict__ sign,
+                    unsigned long long n, const long long* __restrict__ xs, int n_x, int xbits, unsigned long long* __restrict__ cursor,
+                    unsigned long long* __restrict__ keys) {
+    const int lane = threadIdx.x & 31;
+    const unsigned long long step = (unsigned long long)gridDim.x * blockDim.x;
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i - lane < n; i += step) {   // whole warps
+        bool hit = false;
+        unsigned long long key = 0;
+        if (i < n) {
+            const unsigned long long m = mag[i];
+            const long long v = (long long)(((sign[i >> 5] >> (i & 31)) & 1u) ? 0ull - m : m);
+            int a = 0, b = n_x;
+            while (a < b) { const int h = (int)(((unsigned)a + (unsigned)b) >> 1); if (__ldg(xs + h) < v) a = h + 1; else b = h; }
+            if (a < n_x && __ldg(xs + a) == v) { hit = true; key = (cols[i] << xbits) | (unsigned long long)a; }
+        }
+        const unsigned int bal = __ballot_sync(0xffffffffu, hit);
+        if (bal == 0u) continue;
+        unsigned long long at = 0;
+        if (lane == 0) at = atomicAdd(cursor, (unsigned long long)__popc(bal));
+        at = __shfl_sync(0xffffffffu, at, 0);
+        if (hit) keys[at + (unsigned int)__popc(bal & ((1u << lane) - 1u))] = key;
+    }
+}
+
+// keys[i] >>= bits: the sorted (cell << xbits | j) pairs of fbgpu_groupby_sparse_distinct as their cells, still sorted
+__global__ void __launch_bounds__(256)
+sparse_shift_kernel(unsigned long long* __restrict__ keys, unsigned long long n, int bits) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x)
+        keys[i] >>= bits;
+}
+
 // ------------------------------------------------------------------------------------------------
 // arena_gather_kernel (fbgpu_compact): copies containers one by one from the old payload arena into the new one — one warp per
 // container, 16 bytes per lane and step.  Used for fragments that fbgpu_apply_containers left with holes.

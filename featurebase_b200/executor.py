@@ -1077,7 +1077,7 @@ class Executor:
             sparse = self._groupby_sparse(idx, c, fields, row_ids, time_args, filt, start, shards,
                                           device_limit=agg is None and not (has_sort or has_having), sum_f=sum_f)
         if sparse is not None:
-            pass                                                  # groups in hand; Count(Distinct), and Sum over a non-int field, per group below
+            pass                                                  # groups in hand; Count(Distinct) below (_groupby_sparse_distinct), Sum over a non-int field per group
         elif sum_f is not None:
             counts, sums = self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, filt, shards, agg=sum_f)
         elif int_dims and hasattr(self.ctx, "groupby_mixed"):
@@ -1137,7 +1137,17 @@ class Executor:
                 out.append((group, n))
             if limit and len(out) >= limit and "offset" not in c.args:
                 break
-        if distinct_agg and dist is None:
+        sparse_dist = None                                        # Count(Distinct) of the sparse path's listed groups: {cell: count}
+        if distinct_agg and sparse is not None:
+            pairs = list(zip((int(x) for x in sparse[0][:len(out)]), out))            # (cell, (group, count)) of the listed groups
+            if not (has_sort or has_having):                      # limits first, as below
+                pairs = self._window(c, pairs)
+            sparse_dist = self._groupby_sparse_distinct(idx, fields, row_ids, time_args, filt_call, agg_distinct, pairs, sparse, shards)
+            if sparse_dist is not None:
+                out = [(group, n, sparse_dist.get(cell, 0)) for cell, (group, n) in pairs]    # a distinct count of 0 is kept (:3343-3385)
+                if not (has_sort or has_having):
+                    return out
+        if distinct_agg and dist is None and sparse_dist is None:
             if not (has_sort or has_having):                      # limits first: the aggregate is expensive per group (:3327-3335)
                 out = self._window(c, out)
             for k, (group, n) in enumerate(out):                  # Count(Distinct(Intersect(group rows, filter, Distinct's child), field=..)) :3343-3385
@@ -1179,8 +1189,8 @@ class Executor:
         Sum, which skips groups after the fact) at most offset + limit of them.  With sum_f (the int field of aggregate=Sum),
         (cells, counts, sums) from fbgpu_groupby_sparse_sum in the same call: a count is the group's columns holding a value of
         the field, and a group is listed when it is non-zero.  None when the context answers FBGPU_E_COMM or has no such call:
-        the dense tensor is asked for instead.  Count(Distinct), and Sum over a field that is not int, take the per-group
-        composition, one query per group."""
+        the dense tensor is asked for instead.  Count(Distinct) takes _groupby_sparse_distinct after the window is cut; Sum
+        over a field that is not int takes the per-group composition, one query per group."""
         sizes = [len(r) for r in row_ids]
         flat0 = 0
         for p, n in zip(start, sizes):
@@ -1200,6 +1210,71 @@ class Executor:
                 raise
             return None
 
+    # (cell, x) pairs a fbgpu_groupby_sparse_distinct(_rows) call may produce, bounded before the call by Σ min(count, listed
+    # x) over its cells: 2 GiB of keys over both halves of the device sort.  A bound on memory, not a measured optimum.
+    GROUPBY_SPARSE_DISTINCT_PAIRS = 1 << 27
+
+    def _groupby_sparse_distinct(self, idx, fields, row_ids, time_args, filt_call, agg_distinct, pairs, sparse, shards):
+        """{cell: Count(Distinct(field=x))} for the listed groups `pairs` ((cell, group) in ascending cells) of a GroupBy on the
+        sparse path, from fbgpu_groupby_sparse_distinct(_rows); cells absent from it have a distinct count of 0.  x's list is
+        made once, as _groupby_distinct makes it, and the calls run over filter ∩ Distinct's child.  The cells are cut into
+        consecutive ranges whose Σ min(count, listed x) stays within GROUPBY_SPARSE_DISTINCT_PAIRS, and x's list into disjoint
+        slices that fit beside the cell in a 64-bit key; the pieces add up per cell.  None (the per-group composition runs
+        instead) for Distinct(index=..), an x that is not a field of this index, more than 7 children, or a context that
+        answers FBGPU_E_COMM or has no such call (a node)."""
+        xf = idx.fields.get(agg_distinct.args.get("field", agg_distinct.args.get("_field")))
+        if xf is None or "index" in agg_distinct.args or len(fields) > 7:
+            return None
+        call = "groupby_sparse_distinct" if xf.type == "int" else "groupby_sparse_distinct_rows"
+        if not hasattr(self.ctx, call):
+            return None
+        if not pairs:
+            return {}
+        set_dims = [(f.id, self._time_view_ids(f, targs) if targs else [VIEW_STANDARD], rows) for f, rows, targs in zip(fields, row_ids, time_args)]
+        counts = dict(zip((int(x) for x in sparse[0]), (int(n) for n in sparse[1])))
+        total = math.prod(len(r) for r in row_ids)
+        try:
+            ops, xs = self._distinct_list(idx, filt_call, agg_distinct, xf, shards)
+            got = {}
+            if len(xs) == 0:
+                return got
+            room = self.GROUPBY_SPARSE_DISTINCT_PAIRS
+            xbits = 0                                             # the widest x index the key leaves room for
+            while xbits < 63 and total <= ((1 << 64) - 1) >> (xbits + 1):
+                xbits += 1
+            x_step = max(1, min(len(xs), room, 1 << xbits))
+            for s in range(0, len(xs), x_step):
+                xc = xs[s:s + x_step]
+                x = (xf.id, VIEW_STANDARD, xc) if xf.type != "int" else (xf.id, VIEW_BSI, xf.bit_depth, xc)
+                a = 0
+                while a < len(pairs):
+                    b, used = a, 0
+                    while b < len(pairs) and (b == a or used + min(counts[pairs[b][0]], len(xc)) <= room):
+                        used += min(counts[pairs[b][0]], len(xc))
+                        b += 1
+                    cells, dist = getattr(self.ctx, call)(idx.id, set_dims, x, shards, filter_ops=ops, start=pairs[a][0], end=pairs[b - 1][0] + 1)
+                    for cell, d in zip(cells.tolist(), dist.tolist()):
+                        got[cell] = got.get(cell, 0) + d
+                    a = b
+            return got
+        except NotImplementedError:
+            return None
+        except L.FbgpuError as e:
+            if e.code != L.E_COMM:
+                raise
+            return None
+
+    def _distinct_list(self, idx, filt_call, agg_distinct, xf, shards):
+        """(filter ∩ Distinct's child as ops, x's list there): an int field's distinct stored values (one Distinct), a set, mutex,
+        bool or time field's rows that hold a column (one row-count call, as Distinct's set branch)"""
+        parts = [x for x in (filt_call, *agg_distinct.children[:1]) if isinstance(x, pql.Call)]
+        both = (parts[0] if len(parts) == 1 else pql.Call("Intersect", {}, parts)) if parts else None
+        ops = self._bitmap_call(idx, both) if both is not None else None
+        if xf.type == "int":
+            return ops, self._int_values(idx, xf, shards, ops)
+        rid, cnt = self.ctx.row_counts(idx.id, xf.id, VIEW_STANDARD, shards, filter_ops=ops)
+        return ops, np.asarray(sorted(int(r) for r, n in zip(rid, cnt) if n > 0), dtype=np.uint64)
+
     GROUPBY_MIXED_MAX = 65535                                     # groups (product of the int children's value counts) per fbgpu_groupby_mixed / _sum / _distinct call
     # presence bits ((rows of the last set child, or 1) x groups x listed values or rows of x) per fbgpu_groupby_distinct(_rows) call: 256 MiB
     # of device workspace.  A choice that bounds the workspace, not a measured optimum.
@@ -1211,15 +1286,8 @@ class Executor:
         under filter ∩ Distinct's child (one Distinct, as the int children's lists are made), for a set, mutex, bool or time
         field the rows that hold a column there (one row-count call, as Distinct's set branch); the device then counts, per
         cell, those present under filter ∩ Distinct's child ∩ the cell's rows."""
-        parts = [x for x in (filt_call, *agg_distinct.children[:1]) if isinstance(x, pql.Call)]
-        both = (parts[0] if len(parts) == 1 else pql.Call("Intersect", {}, parts)) if parts else None
-        ops = self._bitmap_call(idx, both) if both is not None else None
         try:
-            if xf.type == "int":
-                xs = self._int_values(idx, xf, shards, ops)
-            else:
-                rid, cnt = self.ctx.row_counts(idx.id, xf.id, VIEW_STANDARD, shards, filter_ops=ops)
-                xs = np.asarray(sorted(int(r) for r, n in zip(rid, cnt) if n > 0), dtype=np.uint64)
+            ops, xs = self._distinct_list(idx, filt_call, agg_distinct, xf, shards)
             if len(xs) == 0:
                 return np.zeros(shape, dtype=np.uint64)
             return self._groupby_tensors(idx, fields, row_ids, time_args, int_dims, ops, shards, distinct=(xf, xs))[0]

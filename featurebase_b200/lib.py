@@ -54,7 +54,8 @@ EXPORTS = ["fbgpu_init", "fbgpu_shutdown", "fbgpu_last_error", "fbgpu_abi_versio
            "fbgpu_node_groupby_views", "fbgpu_groupby_mixed", "fbgpu_node_groupby_mixed", "fbgpu_groupby_sum", "fbgpu_node_groupby_sum",
            "fbgpu_groupby_distinct", "fbgpu_topn_cutoffs", "fbgpu_node_topn_cutoffs", "fbgpu_bsi_sort", "fbgpu_node_bsi_sort",
            "fbgpu_bsi_distinct", "fbgpu_node_bsi_distinct", "fbgpu_extract_rows", "fbgpu_groupby_distinct_rows",
-           "fbgpu_groupby_sparse", "fbgpu_node_groupby_sparse", "fbgpu_groupby_sparse_sum", "fbgpu_node_groupby_sparse_sum"]
+           "fbgpu_groupby_sparse", "fbgpu_node_groupby_sparse", "fbgpu_groupby_sparse_sum", "fbgpu_node_groupby_sparse_sum",
+           "fbgpu_groupby_sparse_distinct", "fbgpu_groupby_sparse_distinct_rows"]
 
 
 def lib_path():
@@ -125,6 +126,10 @@ def load():
     L.fbgpu_groupby_sparse.restype = C.c_int
     L.fbgpu_groupby_sparse_sum.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i64, u64, i64, vp, vp, vp, u64, C.POINTER(u64)]
     L.fbgpu_groupby_sparse_sum.restype = C.c_int
+    L.fbgpu_groupby_sparse_distinct.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, u32, u32, i32, vp, i32, vp, i32, vp, i64, u64, u64, vp, vp, u64, C.POINTER(u64)]
+    L.fbgpu_groupby_sparse_distinct.restype = C.c_int
+    L.fbgpu_groupby_sparse_distinct_rows.argtypes = [vp, u32, vp, vp, vp, i32, vp, vp, u32, u32, vp, i32, vp, i32, vp, i64, u64, u64, vp, vp, u64, C.POINTER(u64)]
+    L.fbgpu_groupby_sparse_distinct_rows.restype = C.c_int
     L.fbgpu_count_pairs.argtypes, L.fbgpu_count_pairs.restype = [vp, u32, u32, u32, vp, u32, u32, vp, i32, vp, i64, vp], C.c_int
     L.fbgpu_comm_unique_id.argtypes, L.fbgpu_comm_unique_id.restype = [vp], C.c_int
     L.fbgpu_comm_init.argtypes, L.fbgpu_comm_init.restype = [vp, i32, i32, vp], C.c_int
@@ -665,6 +670,41 @@ class Context:
                 return cells[: n.value].copy(), counts[: n.value].copy()
             return cells[: n.value].copy(), counts[: n.value].copy(), sums[: n.value].copy()
 
+    def groupby_sparse_distinct(self, index, set_dims, x, shards, filter_ops=None, start=0, end=None):
+        """GroupBy(..., aggregate=Count(Distinct(field=x))) over groupby_sparse's dimensions (1..7 of them), x an int field, in one
+        call (fbgpu_groupby_sparse_distinct).  x: (field, BSI view, bit depth, strictly ascending stored values).  Returns
+        (cells, distinct), uint64 arrays: the cells in [start, end) (end None: every cell) where at least one listed value is held
+        by a column of filter ∩ the cell's rows, ascending, and how many listed values are."""
+        return self._groupby_sparse_distinct(index, set_dims, x, shards, filter_ops, start, end, rows=False)
+
+    def groupby_sparse_distinct_rows(self, index, set_dims, x, shards, filter_ops=None, start=0, end=None):
+        """groupby_sparse_distinct over a set, mutex, bool or time field x (fbgpu_groupby_sparse_distinct_rows): x is (field, view,
+        strictly ascending row ids), and a cell's count is the number of listed rows holding a column of filter ∩ its rows."""
+        return self._groupby_sparse_distinct(index, set_dims, x, shards, filter_ops, start, end, rows=True)
+
+    def _groupby_sparse_distinct(self, index, set_dims, x, shards, filter_ops, start, end, rows):
+        g = _groupby_args(set_dims, [], shards, filter_ops)
+        xs = _u64arr(x[2]) if rows else np.ascontiguousarray(np.asarray(x[3], dtype=np.int64))
+        end = (1 << 64) - 1 if end is None else int(end)
+        n = C.c_uint64(0)
+        cap = max(getattr(self, "_sparse_cap", 0), 1 << 12)
+        while True:
+            cells, distinct = np.empty(cap, dtype=np.uint64), np.empty(cap, dtype=np.uint64)
+            if rows:
+                rc = self.L.fbgpu_groupby_sparse_distinct_rows(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, int(x[0]), int(x[1]),
+                                                               xs.ctypes.data, len(xs), g.filter, g.n_filter, g.shards, g.n_shards, int(start), end,
+                                                               cells.ctypes.data, distinct.ctypes.data, cap, C.byref(n))
+            else:
+                rc = self.L.fbgpu_groupby_sparse_distinct(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, int(x[0]), int(x[1]),
+                                                          int(x[2]), xs.ctypes.data, len(xs), g.filter, g.n_filter, g.shards, g.n_shards, int(start), end,
+                                                          cells.ctypes.data, distinct.ctypes.data, cap, C.byref(n))
+            if rc == E_NOSPACE:
+                cap = int(n.value)
+                continue
+            self._check(rc)
+            self._sparse_cap = cap
+            return cells[: n.value].copy(), distinct[: n.value].copy()
+
     def rows_payload_bytes(self, index, field, view, shards, row_ids=None):
         sh = _u64arr(shards)
         pay, nc = C.c_uint64(0), C.c_uint64(0)
@@ -758,6 +798,12 @@ class Node(Context):
 
     def groupby_distinct_rows(self, index, set_dims, int_dims, x, shards, filter_ops=None):
         raise NotImplementedError("fbgpu_groupby_distinct_rows has no node form: the devices' distinct sets merge by union, not by sum")
+
+    def groupby_sparse_distinct(self, index, set_dims, x, shards, filter_ops=None, start=0, end=None):
+        raise NotImplementedError("fbgpu_groupby_sparse_distinct has no node form: the devices' distinct sets merge by union, not by sum")
+
+    def groupby_sparse_distinct_rows(self, index, set_dims, x, shards, filter_ops=None, start=0, end=None):
+        raise NotImplementedError("fbgpu_groupby_sparse_distinct_rows has no node form: the devices' distinct sets merge by union, not by sum")
 
     def row_counts(self, index, field, view, shards, row_ids=None, filter_ops=None, cap=1 << 20):
         if row_ids is None:

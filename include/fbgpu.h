@@ -501,6 +501,41 @@ int fbgpu_groupby_sparse_sum(fbgpu_ctx *ctx, uint32_t index,
                              const fbgpu_op *filter, int32_t n_filter_ops,
                              const uint64_t *shards, int64_t n_shards, uint64_t start, int64_t limit,
                              uint64_t *out_cells, uint64_t *out_counts, int64_t *out_sums, uint64_t cap, uint64_t *out_n);
+/* GroupBy(..., aggregate=Count(Distinct(field=x))) over set-like dimensions of any size, in one call (SQL SELECT k,
+ * COUNT(DISTINCT x) ... GROUP BY k over a column of more than 65,535 values).  Dimensions and cells are fbgpu_groupby_sparse's,
+ * but at most 7 dimensions: x takes the eighth place of the join.  xfield / xview / x_depth (0..64): x's BSI view and depth;
+ * x_values: n_x >= 1 strictly ascending stored values (value - Base), as for fbgpu_groupby_distinct.  For every cell in
+ * [start, end), the number of listed x_values[j] held by at least one column of filter ∩ the cell's rows ∩ exists(x) (a sign
+ * with magnitude 0 is the value 0; a column whose value is not listed counts nowhere).  Only the cells where that number is
+ * non-zero are written, ascending, into out_cells / out_distinct under fbgpu_columns' NOSPACE contract.  Where the dense tensor
+ * fits, these are the non-zero cells of fbgpu_groupby_distinct.  Argument errors (fbgpu_groupby_sparse's with out_distinct in
+ * the place of out_counts, n_fields > 7, n_x < 1, x_values not strictly ascending, x_depth outside 0..64, start > end, a
+ * product of n_rows that does not fit in u64 once shifted left by bit_width(n_x - 1)) are reported before the device check.  A
+ * context with a communicator attached returns FBGPU_E_COMM: distinct sets merge by union.  There is no node form.  Device
+ * memory: fbgpu_groupby_sparse_sum's bounds per chunk (its value list, and 16 bytes per listed value a column holds); 16 bytes
+ * per (cell, x) pair of a join range of at most 2^24 pairs (one column's cross product may exceed that); 16 bytes per
+ * distinct (cell, x) pair of the running list, which has no limit: a caller bounds it by the range and x's list (the pairs
+ * are at most Σ over the range's cells of min(count, n_x)); and at the end 32 bytes per listed cell. */
+int fbgpu_groupby_sparse_distinct(fbgpu_ctx *ctx, uint32_t index,
+                                  const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                                  const uint64_t *row_ids_flat, const int32_t *n_rows,
+                                  uint32_t xfield, uint32_t xview, int32_t x_depth, const int64_t *x_values, int32_t n_x,
+                                  const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards,
+                                  uint64_t start, uint64_t end,
+                                  uint64_t *out_cells, uint64_t *out_distinct, uint64_t cap, uint64_t *out_n);
+/* The same over a set, mutex, bool or time field x: xfield / xview a set-like view of x, x_rows n_x >= 1 strictly ascending
+ * row ids (any u64).  Per cell in [start, end), the number of listed rows x_rows[j] that hold at least one column of
+ * filter ∩ the cell's rows; a column held by several listed rows counts toward each of them.  Where the dense tensor fits,
+ * these are the non-zero cells of fbgpu_groupby_distinct_rows.  Argument errors as for fbgpu_groupby_sparse_distinct (x_rows
+ * not strictly ascending in the place of x_values; no depth), and FBGPU_E_COMM alike.  Device memory: fbgpu_groupby_sparse's
+ * per chunk, x counted as one more dimension, then as for fbgpu_groupby_sparse_distinct from the join on. */
+int fbgpu_groupby_sparse_distinct_rows(fbgpu_ctx *ctx, uint32_t index,
+                                       const uint32_t *fields, const uint32_t *views_flat, const int32_t *n_views, int32_t n_fields,
+                                       const uint64_t *row_ids_flat, const int32_t *n_rows,
+                                       uint32_t xfield, uint32_t xview, const uint64_t *x_rows, int32_t n_x,
+                                       const fbgpu_op *filter, int32_t n_filter_ops, const uint64_t *shards, int64_t n_shards,
+                                       uint64_t start, uint64_t end,
+                                       uint64_t *out_cells, uint64_t *out_distinct, uint64_t cap, uint64_t *out_n);
 
 /* ---- multi-GPU reduce (replaces the HTTP fan-in of mapReduce/remoteExec, executor.go:6392-6533) ----
  * One context (process) per GPU; rank 0 creates the id, every rank joins.  When a communicator is attached,
