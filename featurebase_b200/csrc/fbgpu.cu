@@ -2672,13 +2672,32 @@ extern "C" int fbgpu_groupby_distinct_rows(fbgpu_ctx* c, uint32_t index, const u
 // another dedupe.  At the end the keys are shifted down to their cells and run-length coded: a run's length is the cell's
 // distinct count.
 
-// the argument checks fbgpu_groupby_sparse and its node form make before any device is touched
+namespace {                                                         // (internal linkage: not exported beside the C entry points)
+// one sparse GroupBy request: the set dimensions, the aggregate as GbRequest carries it (kCount, kSum, kDistinct or kDistinctRows
+// with its x), the filter, the shards and the window: the cells >= start, below end and at most `limit` of them (limit < 0: no
+// cut).  The distinct pair takes end and no limit, kCount and kSum a limit and no end (~0).
+struct SpRequest {
+    std::vector<GbDim> dims;
+    GvAgg agg; GvInt x;                                             // (x unused for kCount)
+    const fbgpu_op* filter; int32_t n_filter_ops;
+    const uint64_t* shards; int64_t n_shards;
+    uint64_t start, end; int64_t limit;
+    bool distinct() const { return agg == GvAgg::kDistinct || agg == GvAgg::kDistinctRows; }
+};
+
+// a sparse GroupBy's list: its cells, ascending, their counts (for the distinct pair the distinct counts) and, for kSum only, sums
+struct SpResult { std::vector<uint64_t> cells, counts; std::vector<int64_t> sums; };
+}  // namespace
+
+// the argument checks every sparse GroupBy entry point and node form makes before any device is touched: the dimensions of the
+// ABI's flat arrays and the outputs; for kSum x's depth and out_sums; for the distinct pair at most kSpMaxDims - 1 dimensions (x
+// takes the join's last slot), x's list (values for an int x, rows for a set-like one) and depth, the range, and room in a u64
+// for cell << bit_width(n_x - 1).  q's dimensions are not read: they are built from the arrays checked here.
 static int groupby_sparse_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
-                               const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
-                               const uint64_t* shards, int64_t n_shards, const uint64_t* out_cells, const uint64_t* out_counts, uint64_t cap,
-                               const uint64_t* out_n) {
+                               const uint64_t* row_ids_flat, const int32_t* n_rows, const SpRequest& q, const uint64_t* out_cells,
+                               const uint64_t* out_counts, const int64_t* out_sums, uint64_t cap, const uint64_t* out_n) {
     if (!handle || !fields || !views_flat || !n_views || !row_ids_flat || !n_rows || !out_n || (cap && (!out_cells || !out_counts)) ||
-        n_filter_ops < 0 || (n_filter_ops && !filter) || n_shards < 0 || (n_shards && !shards)) return fail(FBGPU_E_INVALID, "bad argument");
+        q.n_filter_ops < 0 || (q.n_filter_ops && !q.filter) || q.n_shards < 0 || (q.n_shards && !q.shards)) return fail(FBGPU_E_INVALID, "bad argument");
     if (n_fields < 1 || n_fields > kSpMaxDims) return fail(FBGPU_E_INVALID, "n_fields=%d outside 1..%d", n_fields, kSpMaxDims);
     const uint64_t* rows = row_ids_flat;
     uint64_t cells = 1;
@@ -2691,15 +2710,25 @@ static int groupby_sparse_args(const void* handle, const uint32_t* fields, const
         cells *= (uint64_t)n_rows[i];
         rows += n_rows[i];
     }
+    const GvInt& x = q.x;
+    if (q.agg == GvAgg::kSum) {
+        if (x.depth < 0 || x.depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", x.depth);
+        if (cap && !out_sums) return fail(FBGPU_E_INVALID, "bad argument");
+    }
+    if (!q.distinct()) return 0;
+    if (n_fields > kSpMaxDims - 1) return fail(FBGPU_E_INVALID, "n_fields=%d outside 1..%d", n_fields, kSpMaxDims - 1);
+    if (!x.values && !x.rows) return fail(FBGPU_E_INVALID, "bad argument");
+    if (x.n_values < 1) return fail(FBGPU_E_INVALID, "n_x=%d < 1", x.n_values);
+    for (int32_t i = 1; i < x.n_values; i++) {
+        if (x.values && x.values[i] <= x.values[i - 1]) return fail(FBGPU_E_INVALID, "x_values are not strictly ascending at position %d", i);
+        if (x.rows && x.rows[i] <= x.rows[i - 1]) return fail(FBGPU_E_INVALID, "x_rows are not strictly ascending at position %d", i);
+    }
+    if (x.depth < 0 || x.depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", x.depth);
+    if (q.start > q.end) return fail(FBGPU_E_INVALID, "start=%llu > end=%llu", (unsigned long long)q.start, (unsigned long long)q.end);
+    const int xbits = bit_width((uint64_t)x.n_values - 1);
+    if (cells > (~0ull >> xbits)) return fail(FBGPU_E_INVALID, "product of n_rows times 2^%d exceeds 2^64 - 1", xbits);
     return 0;
 }
-
-// the aggregate of fbgpu_groupby_sparse_sum: an int field's BSI view and bit depth
-struct SpAgg { uint32_t field, view; int depth; };
-
-// the x of fbgpu_groupby_sparse_distinct(_rows): its field and view; for an int x (values != NULL) its bit depth and n strictly
-// ascending listed stored values, for a set-like x (rows != NULL) its n strictly ascending listed rows
-struct SpDistinct { uint32_t field, view; int depth; const int64_t* values; const uint64_t* rows; int32_t n; };
 
 // device buffers of one fbgpu_groupby_sparse call, freed when it returns: they can be large, and are not reused by other calls.
 // b[d]: dimension d's keys (with a distinct x, x is the last dimension); b[nd]: the cells (with an aggregate, (cell, value)
@@ -2791,262 +2820,377 @@ static int sparse_union(Query& q, const SortPairs& cs, SortPairs& acc, int bits)
     return merge ? distinct_keys(q, acc, bits) : 0;
 }
 
-// the non-empty cells >= start of the dimensions `gdims` under the filter, ascending, at most `limit` of them (limit < 0: all), and
-// their counts (store lock held).  With `agg`, the filter is <filter> ∩ exists(x), a cell is non-empty when its count there is,
-// and `sums` gets each listed cell's wrapping sum of x's stored values.  With `dx` (limit < 0), the cells in [start, end) where
-// at least one listed x value (row) is held by a column of the filter ∩ the cell's rows, and as counts the number of such x.
-static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const std::vector<GbDim>& gdims, const fbgpu_op* filter, int32_t n_filter_ops,
-                              const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
-                              std::vector<uint64_t>& cells, std::vector<uint64_t>& counts, const SpAgg* agg = nullptr, std::vector<int64_t>* sums = nullptr,
-                              const SpDistinct* dx = nullptr, uint64_t end = ~0ull) {
-    cells.clear(); counts.clear();
-    if (sums) sums->clear();
-    const int ng = (int)gdims.size();
-    const bool x_int = dx && dx->values, x_rows = dx && dx->rows;
-    std::vector<GbDim> dims = gdims;                 // the dimensions sparse_rows_kernel walks: a set-like x is the last one
-    if (x_rows) dims.push_back(GbDim{ dx->field, &dx->view, 1, dx->rows, dx->n });
-    const int nr = (int)dims.size(), nd = nr + (x_int ? 1 : 0);        // nd: the join's dimensions
-    const bool vals = agg || x_int;                  // a value list per chunk, of Sum's x or of an int distinct x
-    const SpAgg vx = agg ? *agg : x_int ? SpAgg{ dx->field, dx->view, dx->depth } : SpAgg{};
-    const int xbits = dx ? bit_width((uint64_t)dx->n - 1) : 0;
-    Query q(c); Workspace* w = q.w;
-    const std::vector<uint64_t> sorted = sorted_unique(shards, n_shards);
-    std::vector<fbgpu_op> full;
+namespace {
+// one groupby_sparse_run: the request, its query and join, the call's device buffers and what was uploaded into them, and the
+// running lists.  The stages below work on it; the batch and the chunk a stage works on are passed to it.
+struct SpCall {
+    fbgpu_ctx* c;
+    uint32_t index;
+    const SpRequest& r;
+    const bool x_int = r.agg == GvAgg::kDistinct;
+    const bool vals = x_int || r.agg == GvAgg::kSum;                // a value list per chunk, of Sum's x or of an int distinct x
+    std::vector<GbDim> dims = r.dims;                               // the dimensions sparse_rows_kernel walks: a set-like x is the last one
+    const int ng = (int)r.dims.size();
+    const int nd = ng + (r.distinct() ? 1 : 0);                     // the join's dimensions
+    const int xbits = r.distinct() ? bit_width((uint64_t)r.x.n_values - 1) : 0;
+    int cell_bits = 0;                                              // a join key's bits
+    Query q{ c };
+    Workspace* w = q.w;
+    const std::vector<uint64_t> sorted = sorted_unique(r.shards, r.n_shards);
+    bool have_filter = false;
     uint32_t fv_x = 0;
-    if (vals) {
-        full = and_row(filter, n_filter_ops, vx.field, vx.view, 0);    // <filter> ∩ exists, as for fbgpu_bsi_sum
-        fv_x = view_id_locked(c, ViewKey{ index, vx.field, vx.view }, false);
+    SpJoin jn{};
+    SparseBufs sb;
+    // sb.b[kSpMaxDims + 1]: [cursor | dimension d's rows at row_at[d] | an int x's values at d_xs | its n_fv[d] view slots at fv_at[d] of d_fv0]
+    unsigned long long* cursor = nullptr;
+    const long long* d_xs = nullptr;
+    const uint32_t* d_fv0 = nullptr;
+    std::vector<size_t> row_at, fv_at;
+    std::vector<int> n_fv;
+    std::vector<SortPairs> dk;                                      // each join dimension's keys
+    SortPairs cs{ w, ~0ull, r.agg != GvAgg::kSum, &sb.b[nd] };      // a join range's cells ((cell, value) pairs for kSum)
+    SortPairs acc{ w, ~0ull, r.distinct() };                        // the running list: (cell, count) pairs or distinct (cell, x) keys
+    SortPairs acc_sums{ w, ~0ull, false, &sb.b[kSpMaxDims + 4] };   // kSum's running sums, or the distinct pair's final list
+    SortPairs* sums = nullptr;                                      // acc_sums for kSum
+    int (*fold)(SpCall&) = nullptr;                                 // folds cs into the running list
+};
+
+// an evaluation batch from unit u0: the units with filter columns (ncol[k] in units[k]), their hits per walked dimension
+// (ucnt[d * units.size() + k]) and, as places in `units`, the ones every dimension meets
+struct SpBatch {
+    long long u0;
+    const uint4* bitmaps;
+    const uint64_t* shards;
+    std::vector<uint32_t> units, ncol, keep;
+    std::vector<uint64_t> ucnt;
+};
+
+// a chunk: keep[a, b) of its batch, its units, their hits per dimension and filter columns, and their value list
+struct SpChunk {
+    size_t a, b;
+    std::vector<uint32_t> units;
+    std::vector<uint64_t> hits;
+    uint64_t vn;
+    SpVals vl;
+};
+}  // namespace
+
+// folding a join range into the running list: merge counts (and, for kSum, sums), or union distinct keys; set-up picks which
+static int sparse_fold_merge(SpCall& s) {
+    int rc = sort_pairs(s.q, s.cs, s.cell_bits, ~0ull); if (rc) return rc;
+    return sparse_merge(s.q, s.cs, s.acc, s.sums, s.cell_bits, s.r.limit, &s.jn.hi);
+}
+static int sparse_fold_union(SpCall& s) {
+    int rc = distinct_keys(s.q, s.cs, s.cell_bits); if (rc) return rc;
+    return sparse_union(s.q, s.cs, s.acc, s.cell_bits);
+}
+
+// set-up: filter ∩ exists(x) (with a value list, as for fbgpu_bsi_sum), the strides, the fold; *empty when the window holds no
+// cell, else the metadata uploaded
+static int sparse_setup(SpCall& s, bool* empty) {
+    const SpRequest& r = s.r;
+    const fbgpu_op* filter = r.filter;
+    int32_t n_filter_ops = r.n_filter_ops;
+    std::vector<fbgpu_op> full;
+    if (s.vals) {
+        full = and_row(filter, n_filter_ops, r.x.field, r.x.view, 0);
+        s.fv_x = view_id_locked(s.c, ViewKey{ s.index, r.x.field, r.x.view }, false);
         filter = full.data(); n_filter_ops = (int32_t)full.size();
     }
-    const bool have_filter = n_filter_ops > 0;
-    int rc = have_filter ? q.open(index, filter, n_filter_ops, sorted.data(), (int64_t)sorted.size()) : q.open(sorted.data(), (int64_t)sorted.size());
+    s.have_filter = n_filter_ops > 0;
+    int rc = s.have_filter ? s.q.open(s.index, filter, n_filter_ops, s.sorted.data(), (int64_t)s.sorted.size()) : s.q.open(s.sorted.data(), (int64_t)s.sorted.size());
     if (rc) return rc;
-    SpJoin jn{}; jn.nd = nd; jn.lo = start; jn.hi = ~0ull;
+    SpJoin& jn = s.jn;
+    jn.nd = s.nd; jn.lo = r.start; jn.hi = ~0ull;
     uint64_t total = 1;                              // the group dimensions' cells; x, when there is one, has stride 1
-    for (int d = ng - 1; d >= 0; d--) { jn.stride[d] = total << xbits; total *= (uint64_t)dims[d].n_rows; jn.jbits[d] = bit_width((uint64_t)dims[d].n_rows - 1); }
-    if (dx) {
-        jn.stride[ng] = 1; jn.jbits[ng] = xbits;
-        const uint64_t e = std::min(end, total);
-        jn.lo = std::min(start, e) << xbits; jn.hi = e << xbits;
+    for (int d = s.ng - 1; d >= 0; d--) { jn.stride[d] = total << s.xbits; total *= (uint64_t)r.dims[d].n_rows; jn.jbits[d] = bit_width((uint64_t)r.dims[d].n_rows - 1); }
+    s.sums = r.agg == GvAgg::kSum ? &s.acc_sums : nullptr;
+    s.fold = r.distinct() ? sparse_fold_union : sparse_fold_merge;
+    if (r.distinct()) {
+        jn.stride[s.ng] = 1; jn.jbits[s.ng] = s.xbits;
+        const uint64_t e = std::min(r.end, total);
+        jn.lo = std::min(r.start, e) << s.xbits; jn.hi = e << s.xbits;
     }
-    const int cell_bits = bit_width((total << xbits) - 1);                 // a join key's bits
-    if (limit == 0 || jn.lo >= jn.hi) { q.finish(); return FBGPU_OK; }
-    SparseBufs sb;
-    // b[kSpMaxDims + 1]: [cursor | rows of every dimension (u64) | an int x's listed values | view slots of every dimension (u32)]
-    std::vector<uint64_t> rows_h(1, 0);
+    s.cell_bits = bit_width((total << s.xbits) - 1);
+    *empty = r.limit == 0 || jn.lo >= jn.hi;
+    if (*empty) return 0;
+    if (r.agg == GvAgg::kDistinctRows) s.dims.push_back(GbDim{ r.x.field, &r.x.view, 1, r.x.rows, r.x.n_values });
+    std::vector<uint64_t> rows_h(1, 0);              // the cursor, then the rows
     std::vector<uint32_t> fvs_h;
-    std::vector<size_t> row_at(nr), fv_at(nr); std::vector<int> n_fv(nr);
-    for (int d = 0; d < nr; d++) {
-        row_at[d] = rows_h.size(); rows_h.insert(rows_h.end(), dims[d].rows, dims[d].rows + dims[d].n_rows);
-        const std::vector<uint32_t> fvs = view_slots(c, index, dims[d].field, dims[d].views, dims[d].n_views);
-        fv_at[d] = fvs_h.size(); n_fv[d] = (int)fvs.size(); fvs_h.insert(fvs_h.end(), fvs.begin(), fvs.end());
+    for (const GbDim& g : s.dims) {
+        s.row_at.push_back(rows_h.size()); rows_h.insert(rows_h.end(), g.rows, g.rows + g.n_rows);
+        const std::vector<uint32_t> fvs = view_slots(s.c, s.index, g.field, g.views, g.n_views);
+        s.fv_at.push_back(fvs_h.size()); s.n_fv.push_back((int)fvs.size()); fvs_h.insert(fvs_h.end(), fvs.begin(), fvs.end());
     }
     const size_t xv_at = rows_h.size();
-    if (x_int) for (int32_t i = 0; i < dx->n; i++) rows_h.push_back((uint64_t)dx->values[i]);
-    DevBuf& meta = sb.b[kSpMaxDims + 1];
+    if (s.x_int) rows_h.insert(rows_h.end(), r.x.values, r.x.values + r.x.n_values);
+    DevBuf& meta = s.sb.b[kSpMaxDims + 1];
     if (meta.ensure(rows_h.size() * 8 + fvs_h.size() * 4)) return FBGPU_E_NOMEM;
-    unsigned long long* cursor = (unsigned long long*)meta.p;
-    const uint64_t* d_rows = (const uint64_t*)meta.p;
-    const long long* d_xs = (const long long*)(d_rows + xv_at);
-    const uint32_t* d_fv0 = (const uint32_t*)(d_rows + rows_h.size());
-    CUDA_TRY(cudaMemcpyAsync(meta.p, rows_h.data(), rows_h.size() * 8, cudaMemcpyHostToDevice, w->stream));
-    CUDA_TRY(cudaMemcpyAsync((void*)d_fv0, fvs_h.data(), fvs_h.size() * 4, cudaMemcpyHostToDevice, w->stream));
+    s.cursor = (unsigned long long*)meta.p;
+    s.d_xs = (const long long*)s.cursor + xv_at;
+    s.d_fv0 = (const uint32_t*)(s.cursor + rows_h.size());
+    CUDA_TRY(cudaMemcpyAsync(meta.p, rows_h.data(), rows_h.size() * 8, cudaMemcpyHostToDevice, s.w->stream));
+    CUDA_TRY(cudaMemcpyAsync((void*)s.d_fv0, fvs_h.data(), fvs_h.size() * 4, cudaMemcpyHostToDevice, s.w->stream));
+    CUDA_TRY(cudaStreamSynchronize(s.w->stream));
+    for (int d = 0; d < s.nd; d++) s.dk.emplace_back(s.w, ~0ull, true, &s.sb.b[d]);
+    return 0;
+}
+
+// sparse_rows_kernel over walked dimension d for the n units at d_units: their hits into counts (kCount) or their keys at the
+// cursor into keys (kEmit)
+template <SrOut kMode>
+static int sparse_rows(SpCall& s, const SpBatch& bt, size_t d, int n, unsigned long long* counts, unsigned long long* keys) {
+    const unsigned grid = (unsigned)std::min<size_t>((size_t)n, (size_t)s.c->sm_count * 8);
+    sparse_rows_kernel<kMode><<<grid, kSrThreads, 0, s.w->stream>>>(store_ref(s.c), s.d_fv0 + s.fv_at[d], s.n_fv[d], (const uint64_t*)s.cursor + s.row_at[d],
+        s.dims[d].n_rows, s.jn.jbits[d], bt.bitmaps, (const uint32_t*)s.w->d_emit_units.p, n, bt.shards, counts, keys ? s.cursor : nullptr, keys);
+    CUDA_TRY(cudaGetLastError()); s.q.launches++;
+    return 0;
+}
+
+// a batch's units [u0, u0 + nu): evaluation, the kCount pass, the units every dimension meets
+static int sparse_batch(SpCall& s, long long u0, long long nu, SpBatch& bt) {
+    Workspace* w = s.w;
+    bt.u0 = u0;
+    bt.units.clear(); bt.ncol.clear();
+    if (s.have_filter) {
+        const uint2* info;
+        int rc = s.q.eval_info(u0, nu, info); if (rc) return rc;
+        for (long long u = 0; u < nu; u++) if (info[u].x) { bt.units.push_back((uint32_t)u); bt.ncol.push_back(info[u].x); }
+    } else {
+        for (long long u = 0; u < nu; u++) bt.units.push_back((uint32_t)u);
+    }
+    if (bt.units.empty()) return 0;
+    bt.bitmaps = s.have_filter ? (const uint4*)w->d_bitmaps.p : nullptr;
+    bt.shards = s.q.d_shards + u0 / kSlotsPerRow;
+    const size_t nun = bt.units.size(), nr = s.dims.size();
+    if (w->d_emit_units.ensure(nun * 4) || w->d_cells.ensure(nun * nr * 8) || w->h_out.ensure(nun * nr * 8)) return FBGPU_E_NOMEM;
+    CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, bt.units.data(), nun * 4, cudaMemcpyHostToDevice, w->stream));
+    CUDA_TRY(cudaMemsetAsync(w->d_cells.p, 0, nun * nr * 8, w->stream));
+    for (size_t d = 0; d < nr; d++) {
+        int rc = sparse_rows<SrOut::kCount>(s, bt, d, (int)nun, (unsigned long long*)w->d_cells.p + d * nun, nullptr); if (rc) return rc;
+    }
+    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_cells.p, nun * nr * 8, cudaMemcpyDeviceToHost, w->stream));
     CUDA_TRY(cudaStreamSynchronize(w->stream));
-    std::vector<SortPairs> dk;
-    for (int d = 0; d < nd; d++) dk.emplace_back(w, ~0ull, true, &sb.b[d]);
-    // acc: the running list, (cell, count) pairs or, with dx, distinct (cell, x) keys
-    SortPairs cs(w, ~0ull, !agg, &sb.b[nd]), acc(w, ~0ull, dx != nullptr), acc_sums(w, ~0ull, false, &sb.b[kSpMaxDims + 4]);
-    const long long batch = std::min<long long>(c->unit_batch, 1ll << 16);     // a unit's place in a chunk takes 16 bits of a key
-    std::vector<uint32_t> units, keep, chunk, ncol;                            // ncol: with a filter, the filter columns of units[k]
-    std::vector<uint64_t> ucnt;
+    bt.ucnt.assign((const uint64_t*)w->h_out.p, (const uint64_t*)w->h_out.p + nun * nr);
+    bt.keep.clear();
+    for (size_t e = 0; e < nun; e++) {
+        bool all = true;
+        for (size_t d = 0; d < nr && all; d++) all = bt.ucnt[d * nun + e] > 0;
+        if (all) bt.keep.push_back((uint32_t)e);
+    }
+    return 0;
+}
+
+// chunk planning: keep[a, b) of at most kSortChunk hits per dimension and, with a value list, filter columns (at least one unit)
+static int sparse_plan(SpCall& s, const SpBatch& bt, size_t a, SpChunk& ch) {
+    const size_t nun = bt.units.size(), nr = s.dims.size();
+    ch.a = a;
+    ch.hits.assign(nr, 0);
+    ch.vn = 0;
+    for (ch.b = a; ch.b < bt.keep.size(); ch.b++) {
+        const uint32_t e = bt.keep[ch.b];
+        bool fits = !s.vals || ch.vn + bt.ncol[e] <= kSortChunk;
+        for (size_t d = 0; d < nr; d++) fits = fits && ch.hits[d] + bt.ucnt[d * nun + e] <= kSortChunk;
+        if (!fits && ch.b > a) break;
+        for (size_t d = 0; d < nr; d++) ch.hits[d] += bt.ucnt[d * nun + e];
+        if (s.vals) ch.vn += bt.ncol[e];
+    }
+    ch.units.clear();
+    for (size_t k = a; k < ch.b; k++) ch.units.push_back(bt.units[bt.keep[k]]);
+    if (s.w->d_emit_units.ensure(ch.units.size() * 4)) return FBGPU_E_NOMEM;
+    CUDA_TRY(cudaMemcpyAsync(s.w->d_emit_units.p, ch.units.data(), ch.units.size() * 4, cudaMemcpyHostToDevice, s.w->stream));
+    return 0;
+}
+
+// a chunk's dimension keys
+static int sparse_keys(SpCall& s, const SpBatch& bt, const SpChunk& ch) {
+    for (size_t d = 0; d < s.dims.size(); d++) {
+        SortPairs& k = s.dk[d];
+        k.n = 0;
+        int rc = k.reserve(ch.hits[d]); if (rc) return rc;
+        CUDA_TRY(cudaMemsetAsync(s.cursor, 0, 8, s.w->stream));
+        rc = sparse_rows<SrOut::kEmit>(s, bt, d, (int)ch.units.size(), nullptr, k.keys(k.cur)); if (rc) return rc;
+        k.n = ch.hits[d];
+        const int kbits = bit_width(ch.units.size() - 1) + 16 + s.jn.jbits[d];
+        rc = s.n_fv[d] > 1 ? distinct_keys(s.q, k, kbits) : sort_pairs(s.q, k, kbits, ~0ull); if (rc) return rc;
+        s.jn.keys[d] = k.keys(k.cur); s.jn.n[d] = k.n;
+    }
+    return 0;
+}
+
+// a chunk's value list (kSum or an int x): its units' filter columns in (unit, column) order as (e << 16 | c) keys, and their
+// values' magnitudes and sign bits; for an int x, x's keys from it
+static int sparse_values(SpCall& s, const SpBatch& bt, SpChunk& ch) {
+    if (!s.vals) return 0;
+    Workspace* w = s.w;
+    const uint64_t vn = ch.vn;
+    const int nc = (int)ch.units.size();
+    const unsigned grid = (unsigned)std::min<size_t>((size_t)nc, (size_t)s.c->sm_count * 8);
     std::vector<ColUnit> vunits;
-    for (long long u0 = 0; u0 < q.n_units; u0 += batch) {
-        const long long nu = std::min(batch, q.n_units - u0);
-        CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
-        units.clear(); ncol.clear();
-        if (have_filter) {
-            const uint2* info;
-            rc = q.eval_info(u0, nu, info); if (rc) return rc;
-            for (long long u = 0; u < nu; u++) if (info[u].x) { units.push_back((uint32_t)u); ncol.push_back(info[u].x); }
-        } else {
-            for (long long u = 0; u < nu; u++) units.push_back((uint32_t)u);
+    for (int pass = 0; pass < 2; pass++) {
+        uint64_t off = 0;
+        for (size_t k = ch.a; k < ch.b; k++) {
+            ColUnit cu{};
+            const uint32_t u = bt.units[bt.keep[k]];
+            cu.out_off = off; cu.unit = u; cu.first = 0; cu.last = bt.ncol[bt.keep[k]];
+            cu.col_base = pass == 0 ? (s.sorted[(bt.u0 + u) / kSlotsPerRow] << 20) + (uint64_t)((bt.u0 + u) % kSlotsPerRow) * 65536ull
+                                    : (uint64_t)(k - ch.a) << 16;
+            vunits.push_back(cu);
+            off += cu.last;
         }
-        if (units.empty()) continue;
-        const uint4* bitmaps = have_filter ? (const uint4*)w->d_bitmaps.p : nullptr;
-        const uint64_t* bshards = q.d_shards + u0 / kSlotsPerRow;
-        const size_t nun = units.size();
-        // count pass: the hits of every unit in every dimension
-        if (w->d_emit_units.ensure(nun * 4) || w->d_cells.ensure(nun * nr * 8) || w->h_out.ensure(nun * nr * 8)) return FBGPU_E_NOMEM;
-        CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, units.data(), nun * 4, cudaMemcpyHostToDevice, w->stream));
-        CUDA_TRY(cudaMemsetAsync(w->d_cells.p, 0, nun * nr * 8, w->stream));
-        const unsigned grid = (unsigned)std::min<size_t>(nun, (size_t)c->sm_count * 8);
-        for (int d = 0; d < nr; d++) {
-            sparse_rows_kernel<SrOut::kCount><<<grid, kSrThreads, 0, w->stream>>>(store_ref(c), d_fv0 + fv_at[d], n_fv[d], d_rows + row_at[d], dims[d].n_rows, jn.jbits[d],
-                bitmaps, (const uint32_t*)w->d_emit_units.p, (int)nun, bshards, (unsigned long long*)w->d_cells.p + (size_t)d * nun, nullptr, nullptr);
-            CUDA_TRY(cudaGetLastError()); q.launches++;
-        }
-        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, w->d_cells.p, nun * nr * 8, cudaMemcpyDeviceToHost, w->stream));
-        CUDA_TRY(cudaStreamSynchronize(w->stream));
-        ucnt.assign((const uint64_t*)w->h_out.p, (const uint64_t*)w->h_out.p + nun * nr);
-        keep.clear();                                        // the units every dimension meets, as their places in `units`
-        for (size_t e = 0; e < nun; e++) {
-            bool all = true;
-            for (int d = 0; d < nr && all; d++) all = ucnt[(size_t)d * nun + e] > 0;
-            if (all) keep.push_back((uint32_t)e);
-        }
-        for (size_t a = 0; a < keep.size();) {
-            // the chunk keep[a, b): at most kSortChunk hits per dimension and, with a value list, filter columns (at least one unit)
-            std::vector<uint64_t> hits(nr, 0);
-            uint64_t vn = 0;
-            size_t b = a;
-            for (; b < keep.size(); b++) {
-                bool fits = !vals || vn + ncol[keep[b]] <= kSortChunk;
-                for (int d = 0; d < nr; d++) fits = fits && hits[d] + ucnt[(size_t)d * nun + keep[b]] <= kSortChunk;
-                if (!fits && b > a) break;
-                for (int d = 0; d < nr; d++) hits[d] += ucnt[(size_t)d * nun + keep[b]];
-                if (vals) vn += ncol[keep[b]];
-            }
-            chunk.clear();
-            for (size_t k = a; k < b; k++) chunk.push_back(units[keep[k]]);
-            const int ebits = bit_width(chunk.size() - 1);
-            if (w->d_emit_units.ensure(chunk.size() * 4)) return FBGPU_E_NOMEM;
-            CUDA_TRY(cudaMemcpyAsync(w->d_emit_units.p, chunk.data(), chunk.size() * 4, cudaMemcpyHostToDevice, w->stream));
-            const unsigned cgrid = (unsigned)std::min<size_t>(chunk.size(), (size_t)c->sm_count * 8);
-            for (int d = 0; d < nr; d++) {
-                SortPairs& k = dk[(size_t)d];
-                k.n = 0;
-                rc = k.reserve(hits[d]); if (rc) return rc;
-                CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
-                sparse_rows_kernel<SrOut::kEmit><<<cgrid, kSrThreads, 0, w->stream>>>(store_ref(c), d_fv0 + fv_at[d], n_fv[d], d_rows + row_at[d], dims[d].n_rows, jn.jbits[d],
-                    bitmaps, (const uint32_t*)w->d_emit_units.p, (int)chunk.size(), bshards, nullptr, cursor, k.keys(k.cur));
-                CUDA_TRY(cudaGetLastError()); q.launches++;
-                k.n = hits[d];
-                const int kbits = ebits + 16 + jn.jbits[d];
-                rc = n_fv[d] > 1 ? distinct_keys(q, k, kbits) : sort_pairs(q, k, kbits, ~0ull); if (rc) return rc;
-                jn.keys[d] = k.keys(k.cur); jn.n[d] = k.n;
-            }
-            // with agg or an int x, the chunk's value list: the filter columns of its units in (unit, column) order, as (e << 16 | c)
-            // keys (columns_emit_kernel over units based at e << 16) and their values' magnitudes and sign bits (extract_values_kernel)
-            SpVals vl{};
-            if (vals) {
-                vunits.clear();
-                for (int pass = 0; pass < 2; pass++) {
-                    uint64_t off = 0;
-                    for (size_t k = a; k < b; k++) {
-                        ColUnit cu{};
-                        const uint32_t u = units[keep[k]];
-                        cu.out_off = off; cu.unit = u; cu.first = 0; cu.last = ncol[keep[k]];
-                        cu.col_base = pass == 0 ? (sorted[(u0 + u) / kSlotsPerRow] << 20) + (uint64_t)((u0 + u) % kSlotsPerRow) * 65536ull
-                                                : (uint64_t)(k - a) << 16;
-                        vunits.push_back(cu);
-                        off += cu.last;
-                    }
-                }
-                DevBuf& vb = sb.b[kSpMaxDims + 2]; DevBuf& ub = sb.b[kSpMaxDims + 3];
-                const size_t sign_bytes = ((vn + 31) / 32) * 4;
-                if (vb.ensure(vn * 16 + sign_bytes) || ub.ensure(vunits.size() * sizeof(ColUnit))) return FBGPU_E_NOMEM;
-                unsigned long long* vcols = (unsigned long long*)vb.p; unsigned long long* mag = vcols + vn;
-                unsigned int* sign = (unsigned int*)(mag + vn);
-                const ColUnit* d_vu = (const ColUnit*)ub.p;
-                CUDA_TRY(cudaMemcpyAsync(ub.p, vunits.data(), vunits.size() * sizeof(ColUnit), cudaMemcpyHostToDevice, w->stream));
-                CUDA_TRY(cudaMemsetAsync(mag, 0, vn * 8 + sign_bytes, w->stream));
-                columns_emit_kernel<<<cgrid, kEmitThreads, 0, w->stream>>>(bitmaps, d_vu + chunk.size(), (int)chunk.size(), vcols);
-                CUDA_TRY(cudaGetLastError());
-                extract_values_kernel<<<cgrid, kExtractThreads, 0, w->stream>>>(store_ref(c), fv_x, vx.depth, bitmaps, d_vu, (int)chunk.size(), mag, sign);
-                CUDA_TRY(cudaGetLastError());
-                q.launches += 2;
-                vl.cols = vcols; vl.mag = mag; vl.sign = sign; vl.n = vn;
-            }
-            if (x_int) {                                     // x's keys: the chunk's columns holding a listed value, sorted
-                SortPairs& k = dk[(size_t)nr];
-                k.n = 0;
-                rc = k.reserve(vn); if (rc) return rc;
-                CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
-                const unsigned xgrid = (unsigned)std::min<uint64_t>((vn + 255) / 256, (uint64_t)c->sm_count * 8);
-                sparse_xkeys_kernel<<<xgrid, 256, 0, w->stream>>>(vl.cols, vl.mag, vl.sign, vn, d_xs, dx->n, xbits, cursor, k.keys(k.cur));
-                CUDA_TRY(cudaGetLastError()); q.launches++;
-                CUDA_TRY(cudaMemcpyAsync(w->h_out.p, cursor, 8, cudaMemcpyDeviceToHost, w->stream));
-                CUDA_TRY(cudaStreamSynchronize(w->stream));
-                k.n = *(const uint64_t*)w->h_out.p;
-                rc = sort_pairs(q, k, ebits + 16 + xbits, ~0ull); if (rc) return rc;
-                jn.keys[nr] = k.keys(k.cur); jn.n[nr] = k.n;
-            }
-            // the join, over ranges of dimension 0's entries that give at most kSortChunk cells (at least one entry)
-            const uint64_t n0 = jn.n[0];
-            const unsigned jgrid = (unsigned)std::min<uint64_t>((n0 + 255) / 256, (uint64_t)c->sm_count * 8);
-            for (uint64_t e0 = 0; e0 < n0;) {
-                uint64_t e1 = n0, got = 0;
-                for (;;) {
-                    CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
-                    sparse_join_kernel<SrOut::kCount><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, nullptr, SpVals{});
-                    CUDA_TRY(cudaGetLastError()); q.launches++;
-                    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, cursor, 8, cudaMemcpyDeviceToHost, w->stream));
-                    CUDA_TRY(cudaStreamSynchronize(w->stream));
-                    got = *(const uint64_t*)w->h_out.p;
-                    if (got <= kSortChunk || e1 - e0 == 1) break;
-                    e1 = e0 + (e1 - e0) / 2;
-                }
-                if (got) {
-                    cs.n = 0;
-                    rc = cs.reserve(got); if (rc) return rc;
-                    CUDA_TRY(cudaMemsetAsync(cursor, 0, 8, w->stream));
-                    if (agg) {
-                        vl.out = cs.cols(cs.cur);
-                        sparse_join_kernel<SrOut::kSum><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, cs.keys(cs.cur), vl);
-                    } else {
-                        sparse_join_kernel<SrOut::kEmit><<<jgrid, 256, 0, w->stream>>>(jn, e0, e1, cursor, cs.keys(cs.cur), SpVals{});
-                    }
-                    CUDA_TRY(cudaGetLastError()); q.launches++;
-                    cs.n = got;
-                    if (dx) {
-                        rc = distinct_keys(q, cs, cell_bits); if (rc) return rc;
-                        rc = sparse_union(q, cs, acc, cell_bits); if (rc) return rc;
-                    } else {
-                        rc = sort_pairs(q, cs, cell_bits, ~0ull); if (rc) return rc;
-                        rc = sparse_merge(q, cs, acc, agg ? &acc_sums : nullptr, cell_bits, limit, &jn.hi); if (rc) return rc;
-                    }
-                }
-                e0 = e1;
-            }
-            a = b;
-        }
-        CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
-        CUDA_TRY(cudaStreamSynchronize(w->stream));
-        q.add_elapsed();
     }
-    // with dx, the distinct (cell, x) keys as their cells, run-length coded into (cell, distinct count) pairs
-    SortPairs& res = dx ? acc_sums : acc;
-    if (dx && acc.n) {
+    DevBuf& vb = s.sb.b[kSpMaxDims + 2]; DevBuf& ub = s.sb.b[kSpMaxDims + 3];
+    const size_t sign_bytes = ((vn + 31) / 32) * 4;
+    if (vb.ensure(vn * 16 + sign_bytes) || ub.ensure(vunits.size() * sizeof(ColUnit))) return FBGPU_E_NOMEM;
+    unsigned long long* vcols = (unsigned long long*)vb.p; unsigned long long* mag = vcols + vn;
+    unsigned int* sign = (unsigned int*)(mag + vn);
+    const ColUnit* d_vu = (const ColUnit*)ub.p;
+    CUDA_TRY(cudaMemcpyAsync(ub.p, vunits.data(), vunits.size() * sizeof(ColUnit), cudaMemcpyHostToDevice, w->stream));
+    CUDA_TRY(cudaMemsetAsync(mag, 0, vn * 8 + sign_bytes, w->stream));
+    columns_emit_kernel<<<grid, kEmitThreads, 0, w->stream>>>(bt.bitmaps, d_vu + nc, nc, vcols);
+    CUDA_TRY(cudaGetLastError());
+    extract_values_kernel<<<grid, kExtractThreads, 0, w->stream>>>(store_ref(s.c), s.fv_x, s.r.x.depth, bt.bitmaps, d_vu, nc, mag, sign);
+    CUDA_TRY(cudaGetLastError());
+    s.q.launches += 2;
+    const SpVals& vl = ch.vl = SpVals{ vcols, mag, sign, vn, nullptr };
+    if (!s.x_int) return 0;
+    SortPairs& k = s.dk[s.dims.size()];
+    k.n = 0;
+    int rc = k.reserve(vn); if (rc) return rc;
+    CUDA_TRY(cudaMemsetAsync(s.cursor, 0, 8, w->stream));
+    const unsigned xgrid = (unsigned)std::min<uint64_t>((vn + 255) / 256, (uint64_t)s.c->sm_count * 8);
+    sparse_xkeys_kernel<<<xgrid, 256, 0, w->stream>>>(vl.cols, vl.mag, vl.sign, vn, s.d_xs, s.r.x.n_values, s.xbits, s.cursor, k.keys(k.cur));
+    CUDA_TRY(cudaGetLastError()); s.q.launches++;
+    CUDA_TRY(cudaMemcpyAsync(w->h_out.p, s.cursor, 8, cudaMemcpyDeviceToHost, w->stream));
+    CUDA_TRY(cudaStreamSynchronize(w->stream));
+    k.n = *(const uint64_t*)w->h_out.p;
+    rc = sort_pairs(s.q, k, bit_width((uint64_t)nc - 1) + 16 + s.xbits, ~0ull); if (rc) return rc;
+    s.jn.keys[s.dims.size()] = k.keys(k.cur); s.jn.n[s.dims.size()] = k.n;
+    return 0;
+}
+
+// the join-range search and emit: [e0, n0) of dimension 0's entries halved to [e0, *e1) until it gives at most kSortChunk cells
+// (at least one entry), and those cells emitted into cs, with kSum's values taken from the chunk's value list
+static int sparse_join_range(SpCall& s, SpChunk& ch, uint64_t e0, uint64_t* e1) {
+    Workspace* w = s.w;
+    const uint64_t n0 = s.jn.n[0];
+    const unsigned grid = (unsigned)std::min<uint64_t>((n0 + 255) / 256, (uint64_t)s.c->sm_count * 8);
+    uint64_t got = 0;
+    for (*e1 = n0;; *e1 = e0 + (*e1 - e0) / 2) {
+        CUDA_TRY(cudaMemsetAsync(s.cursor, 0, 8, w->stream));
+        sparse_join_kernel<SrOut::kCount><<<grid, 256, 0, w->stream>>>(s.jn, e0, *e1, s.cursor, nullptr, SpVals{});
+        CUDA_TRY(cudaGetLastError()); s.q.launches++;
+        CUDA_TRY(cudaMemcpyAsync(w->h_out.p, s.cursor, 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaStreamSynchronize(w->stream));
+        got = *(const uint64_t*)w->h_out.p;
+        if (got <= kSortChunk || *e1 - e0 == 1) break;
+    }
+    SortPairs& cs = s.cs;
+    cs.n = 0;
+    if (!got) return 0;
+    int rc = cs.reserve(got); if (rc) return rc;
+    CUDA_TRY(cudaMemsetAsync(s.cursor, 0, 8, w->stream));
+    if (s.r.agg == GvAgg::kSum) {
+        ch.vl.out = cs.cols(cs.cur);
+        sparse_join_kernel<SrOut::kSum><<<grid, 256, 0, w->stream>>>(s.jn, e0, *e1, s.cursor, cs.keys(cs.cur), ch.vl);
+    } else {
+        sparse_join_kernel<SrOut::kEmit><<<grid, 256, 0, w->stream>>>(s.jn, e0, *e1, s.cursor, cs.keys(cs.cur), SpVals{});
+    }
+    CUDA_TRY(cudaGetLastError()); s.q.launches++;
+    cs.n = got;
+    return 0;
+}
+
+// the distinct pair's final run-length coding of its keys' cells into acc_sums; then the read-back
+static int sparse_finish(SpCall& s, SpResult& out) {
+    Workspace* w = s.w;
+    SortPairs& acc = s.acc;
+    SortPairs& res = s.r.distinct() ? s.acc_sums : acc;
+    if (s.r.distinct() && acc.n) {
         CUDA_TRY(cudaEventRecord(w->ev0, w->stream));
-        const unsigned sgrid = (unsigned)std::min<uint64_t>((acc.n + 255) / 256, (uint64_t)c->sm_count * 8);
-        sparse_shift_kernel<<<sgrid, 256, 0, w->stream>>>(acc.keys(acc.cur), acc.n, xbits);
-        CUDA_TRY(cudaGetLastError()); q.launches++;
+        const unsigned grid = (unsigned)std::min<uint64_t>((acc.n + 255) / 256, (uint64_t)s.c->sm_count * 8);
+        sparse_shift_kernel<<<grid, 256, 0, w->stream>>>(acc.keys(acc.cur), acc.n, s.xbits);
+        CUDA_TRY(cudaGetLastError()); s.q.launches++;
         unsigned long long no_hi = ~0ull;
-        rc = sparse_merge(q, acc, acc_sums, nullptr, cell_bits, -1, &no_hi); if (rc) return rc;
+        int rc = sparse_merge(s.q, acc, s.acc_sums, nullptr, s.cell_bits, -1, &no_hi); if (rc) return rc;
         CUDA_TRY(cudaEventRecord(w->ev1, w->stream));
         CUDA_TRY(cudaStreamSynchronize(w->stream));
-        q.add_elapsed();
+        s.q.add_elapsed();
     }
-    cells.resize(res.n); counts.resize(res.n);
+    out.cells.resize(res.n); out.counts.resize(res.n);
     if (res.n) {
-        CUDA_TRY(cudaMemcpyAsync(cells.data(), res.keys(res.cur), res.n * 8, cudaMemcpyDeviceToHost, w->stream));
-        CUDA_TRY(cudaMemcpyAsync(counts.data(), res.cols(res.cur), res.n * 8, cudaMemcpyDeviceToHost, w->stream));
-        if (agg) {
-            sums->resize(acc.n);
-            CUDA_TRY(cudaMemcpyAsync(sums->data(), acc_sums.cols(acc_sums.cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaMemcpyAsync(out.cells.data(), res.keys(res.cur), res.n * 8, cudaMemcpyDeviceToHost, w->stream));
+        CUDA_TRY(cudaMemcpyAsync(out.counts.data(), res.cols(res.cur), res.n * 8, cudaMemcpyDeviceToHost, w->stream));
+        if (s.sums) {
+            out.sums.resize(acc.n);
+            CUDA_TRY(cudaMemcpyAsync(out.sums.data(), s.sums->cols(s.sums->cur), acc.n * 8, cudaMemcpyDeviceToHost, w->stream));
         }
         CUDA_TRY(cudaStreamSynchronize(w->stream));
     }
-    q.finish();
+    return 0;
+}
+
+// r's non-empty cells >= start, ascending, at most `limit` of them, and their counts (store lock held).  For kSum the filter is
+// <filter> ∩ exists(x), a cell is non-empty when its count there is, and each listed cell gets its wrapping sum of x's stored
+// values.  For the distinct pair, the cells in [start, end) where at least one listed x value (row) is held by a column of the
+// filter ∩ the cell's rows, and as counts the number of such x.
+static int groupby_sparse_run(fbgpu_ctx* c, uint32_t index, const SpRequest& r, SpResult& out) {
+    SpCall s{ c, index, r };
+    bool empty = false;
+    int rc = sparse_setup(s, &empty); if (rc) return rc;
+    if (empty) { s.q.finish(); return FBGPU_OK; }
+    const long long batch = std::min<long long>(c->unit_batch, 1ll << 16);     // a unit's place in a chunk takes 16 bits of a key
+    SpBatch bt;
+    SpChunk ch;
+    for (long long u0 = 0; u0 < s.q.n_units; u0 += batch) {
+        CUDA_TRY(cudaEventRecord(s.w->ev0, s.w->stream));
+        rc = sparse_batch(s, u0, std::min(batch, s.q.n_units - u0), bt); if (rc) return rc;
+        if (bt.units.empty()) continue;
+        for (size_t a = 0; a < bt.keep.size(); a = ch.b) {
+            rc = sparse_plan(s, bt, a, ch); if (rc) return rc;
+            rc = sparse_keys(s, bt, ch); if (rc) return rc;
+            rc = sparse_values(s, bt, ch); if (rc) return rc;
+            for (uint64_t e0 = 0, e1 = 0; e0 < s.jn.n[0]; e0 = e1) {
+                rc = sparse_join_range(s, ch, e0, &e1); if (rc) return rc;
+                if (s.cs.n) { rc = s.fold(s); if (rc) return rc; }
+            }
+        }
+        CUDA_TRY(cudaEventRecord(s.w->ev1, s.w->stream));
+        CUDA_TRY(cudaStreamSynchronize(s.w->stream));
+        s.q.add_elapsed();
+    }
+    rc = sparse_finish(s, out); if (rc) return rc;
+    s.q.finish();
     return FBGPU_OK;
 }
 
-// a (cell, count) list into the caller's arrays under the NOSPACE contract: *out_n = its size, nothing written when it exceeds cap
-static int write_cells(const std::vector<uint64_t>& cells, const std::vector<uint64_t>& counts, uint64_t* out_cells, uint64_t* out_counts, uint64_t cap, uint64_t* out_n) {
-    *out_n = cells.size();
-    if (cells.size() > cap) return fail(FBGPU_E_NOSPACE, "output needs room for %llu cells", (unsigned long long)cells.size());
-    if (!cells.empty()) { memcpy(out_cells, cells.data(), cells.size() * 8); memcpy(out_counts, counts.data(), counts.size() * 8); }
+// a (cell, count) list, with its sums when it has any, into the caller's arrays under the NOSPACE contract: *out_n = its size,
+// nothing written when it exceeds cap
+static int write_cells(const SpResult& r, uint64_t* out_cells, uint64_t* out_counts, int64_t* out_sums, uint64_t cap, uint64_t* out_n) {
+    *out_n = r.cells.size();
+    if (r.cells.size() > cap) return fail(FBGPU_E_NOSPACE, "output needs room for %llu cells", (unsigned long long)r.cells.size());
+    if (!r.cells.empty()) { memcpy(out_cells, r.cells.data(), r.cells.size() * 8); memcpy(out_counts, r.counts.data(), r.counts.size() * 8); }
+    if (!r.sums.empty()) memcpy(out_sums, r.sums.data(), r.sums.size() * 8);
     return FBGPU_OK;
+}
+
+// the sparse GroupBy entry point `name`: the argument checks, the refusal with ranks attached (group lists merge by cell and
+// distinct sets by union, neither by an all-reduce), then q over the dimensions of the flat arrays, the store locked, and the
+// list written out
+static int groupby_sparse_call(fbgpu_ctx* c, const char* name, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views,
+                               int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows, SpRequest q,
+                               uint64_t* out_cells, uint64_t* out_counts, int64_t* out_sums, uint64_t cap, uint64_t* out_n) {
+    int rc = groupby_sparse_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, q, out_cells, out_counts, out_sums, cap, out_n);
+    if (rc) return rc;
+    if (c->comm || c->n_ranks > 1)
+        return q.distinct() ? fail(FBGPU_E_COMM, "%s is local to one context: distinct sets of the ranks merge by union, not by sum", name)
+                            : fail(FBGPU_E_COMM, "%s is local to one context: group lists merge by cell, not by an all-reduce", name);
+    q.dims = gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows);
+    std::shared_lock<std::shared_mutex> lk;
+    rc = begin_query(c, lk); if (rc) return rc;
+    SpResult r;
+    rc = groupby_sparse_run(c, index, q, r); if (rc) return rc;
+    return write_cells(r, out_cells, out_counts, out_sums, cap, out_n);
 }
 
 // GroupBy over set-like dimensions of any number of rows: fbgpu_groupby_views' cells, as the sorted list of the non-empty ones
@@ -3055,39 +3199,10 @@ extern "C" int fbgpu_groupby_sparse(fbgpu_ctx* c, uint32_t index, const uint32_t
                                     const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
                                     const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
                                     uint64_t* out_cells, uint64_t* out_counts, uint64_t cap, uint64_t* out_n) try {
-    int rc = groupby_sparse_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards,
-                                 out_cells, out_counts, cap, out_n);
-    if (rc) return rc;
-    if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_groupby_sparse is local to one context: group lists merge by cell, not by an all-reduce");
-    std::shared_lock<std::shared_mutex> lk;
-    rc = begin_query(c, lk); if (rc) return rc;
-    std::vector<uint64_t> cells, counts;
-    rc = groupby_sparse_run(c, index, gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows), filter, n_filter_ops, shards, n_shards,
-                            start, limit, cells, counts);
-    if (rc) return rc;
-    return write_cells(cells, counts, out_cells, out_counts, cap, out_n);
+    return groupby_sparse_call(c, "fbgpu_groupby_sparse", index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
+                               SpRequest{ {}, GvAgg::kCount, {}, filter, n_filter_ops, shards, n_shards, start, ~0ull, limit },
+                               out_cells, out_counts, nullptr, cap, out_n);
 } FBGPU_CATCH
-
-// the argument checks of fbgpu_groupby_sparse_sum and its node form: fbgpu_groupby_sparse's, then the aggregate's
-static int groupby_sparse_sum_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
-                                   const uint64_t* row_ids_flat, const int32_t* n_rows, int32_t a_depth, const fbgpu_op* filter, int32_t n_filter_ops,
-                                   const uint64_t* shards, int64_t n_shards, const uint64_t* out_cells, const uint64_t* out_counts, const int64_t* out_sums,
-                                   uint64_t cap, const uint64_t* out_n) {
-    int rc = groupby_sparse_args(handle, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards,
-                                 out_cells, out_counts, cap, out_n);
-    if (rc) return rc;
-    if (a_depth < 0 || a_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", a_depth);
-    if (cap && !out_sums) return fail(FBGPU_E_INVALID, "bad argument");
-    return 0;
-}
-
-// write_cells with each cell's sum beside its count
-static int write_cells(const std::vector<uint64_t>& cells, const std::vector<uint64_t>& counts, const std::vector<int64_t>& sums,
-                       uint64_t* out_cells, uint64_t* out_counts, int64_t* out_sums, uint64_t cap, uint64_t* out_n) {
-    int rc = write_cells(cells, counts, out_cells, out_counts, cap, out_n);
-    if (rc == FBGPU_OK && !sums.empty()) memcpy(out_sums, sums.data(), sums.size() * 8);
-    return rc;
-}
 
 // GroupBy(..., aggregate=Sum(field=x)) over set-like dimensions of any number of rows: fbgpu_groupby_sparse's list, where a cell is
 // listed when filter ∩ its rows ∩ exists(x) is non-empty, with that count and the wrapping sum of the columns' stored values
@@ -3096,63 +3211,10 @@ extern "C" int fbgpu_groupby_sparse_sum(fbgpu_ctx* c, uint32_t index, const uint
                                         const uint64_t* row_ids_flat, const int32_t* n_rows, uint32_t afield, uint32_t aview, int32_t a_depth,
                                         const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
                                         uint64_t* out_cells, uint64_t* out_counts, int64_t* out_sums, uint64_t cap, uint64_t* out_n) try {
-    int rc = groupby_sparse_sum_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, a_depth, filter, n_filter_ops, shards, n_shards,
-                                     out_cells, out_counts, out_sums, cap, out_n);
-    if (rc) return rc;
-    if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "fbgpu_groupby_sparse_sum is local to one context: group lists merge by cell, not by an all-reduce");
-    std::shared_lock<std::shared_mutex> lk;
-    rc = begin_query(c, lk); if (rc) return rc;
-    std::vector<uint64_t> cells, counts; std::vector<int64_t> sums;
-    const SpAgg agg{ afield, aview, a_depth };
-    rc = groupby_sparse_run(c, index, gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows), filter, n_filter_ops, shards, n_shards,
-                            start, limit, cells, counts, &agg, &sums);
-    if (rc) return rc;
-    return write_cells(cells, counts, sums, out_cells, out_counts, out_sums, cap, out_n);
+    return groupby_sparse_call(c, "fbgpu_groupby_sparse_sum", index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
+                               SpRequest{ {}, GvAgg::kSum, GvInt{ afield, aview, a_depth, nullptr, 0 }, filter, n_filter_ops, shards, n_shards, start, ~0ull, limit },
+                               out_cells, out_counts, out_sums, cap, out_n);
 } FBGPU_CATCH
-
-// the argument checks of fbgpu_groupby_sparse_distinct(_rows): fbgpu_groupby_sparse's, then at most kSpMaxDims - 1 dimensions
-// (x takes the join's last slot), x's list (values for an int x, rows for a set-like one) and depth, the range, and room in a
-// u64 for cell << bit_width(n_x - 1)
-static int groupby_sparse_distinct_args(const void* handle, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
-                                        const uint64_t* row_ids_flat, const int32_t* n_rows, const int64_t* x_values, const uint64_t* x_rows, int32_t n_x,
-                                        int32_t x_depth, const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards,
-                                        uint64_t start, uint64_t end, const uint64_t* out_cells, const uint64_t* out_distinct, uint64_t cap, const uint64_t* out_n) {
-    int rc = groupby_sparse_args(handle, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards,
-                                 out_cells, out_distinct, cap, out_n);
-    if (rc) return rc;
-    if (n_fields > kSpMaxDims - 1) return fail(FBGPU_E_INVALID, "n_fields=%d outside 1..%d", n_fields, kSpMaxDims - 1);
-    if (!x_values && !x_rows) return fail(FBGPU_E_INVALID, "bad argument");
-    if (n_x < 1) return fail(FBGPU_E_INVALID, "n_x=%d < 1", n_x);
-    for (int32_t i = 1; i < n_x; i++) {
-        if (x_values && x_values[i] <= x_values[i - 1]) return fail(FBGPU_E_INVALID, "x_values are not strictly ascending at position %d", i);
-        if (x_rows && x_rows[i] <= x_rows[i - 1]) return fail(FBGPU_E_INVALID, "x_rows are not strictly ascending at position %d", i);
-    }
-    if (x_depth < 0 || x_depth > 64) return fail(FBGPU_E_INVALID, "bit depth %d outside 0..64", x_depth);
-    if (start > end) return fail(FBGPU_E_INVALID, "start=%llu > end=%llu", (unsigned long long)start, (unsigned long long)end);
-    uint64_t cells = 1;
-    for (int32_t i = 0; i < n_fields; i++) cells *= (uint64_t)n_rows[i];                 // fits: checked above
-    const int xbits = bit_width((uint64_t)n_x - 1);
-    if (cells > (~0ull >> xbits)) return fail(FBGPU_E_INVALID, "product of n_rows times 2^%d exceeds 2^64 - 1", xbits);
-    return 0;
-}
-
-// fbgpu_groupby_sparse_distinct and fbgpu_groupby_sparse_distinct_rows, x described by dx
-static int groupby_sparse_distinct_call(fbgpu_ctx* c, const char* name, uint32_t index, const uint32_t* fields, const uint32_t* views_flat,
-                                        const int32_t* n_views, int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows, const SpDistinct& dx,
-                                        const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t start, uint64_t end,
-                                        uint64_t* out_cells, uint64_t* out_distinct, uint64_t cap, uint64_t* out_n) {
-    int rc = groupby_sparse_distinct_args(c, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, dx.values, dx.rows, dx.n, dx.depth,
-                                          filter, n_filter_ops, shards, n_shards, start, end, out_cells, out_distinct, cap, out_n);
-    if (rc) return rc;
-    if (c->comm || c->n_ranks > 1) return fail(FBGPU_E_COMM, "%s is local to one context: distinct sets of the ranks merge by union, not by sum", name);
-    std::shared_lock<std::shared_mutex> lk;
-    rc = begin_query(c, lk); if (rc) return rc;
-    std::vector<uint64_t> cells, distinct;
-    rc = groupby_sparse_run(c, index, gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows), filter, n_filter_ops, shards, n_shards,
-                            start, -1, cells, distinct, nullptr, nullptr, &dx, end);
-    if (rc) return rc;
-    return write_cells(cells, distinct, out_cells, out_distinct, cap, out_n);
-}
 
 // GroupBy(..., aggregate=Count(Distinct(field=x))) over set-like dimensions of any number of rows, x an int field: per cell of
 // fbgpu_groupby_sparse's in [start, end), the number of listed stored values of x that a column of filter ∩ the cell's rows
@@ -3162,9 +3224,9 @@ extern "C" int fbgpu_groupby_sparse_distinct(fbgpu_ctx* c, uint32_t index, const
                                              int32_t x_depth, const int64_t* x_values, int32_t n_x, const fbgpu_op* filter, int32_t n_filter_ops,
                                              const uint64_t* shards, int64_t n_shards, uint64_t start, uint64_t end,
                                              uint64_t* out_cells, uint64_t* out_distinct, uint64_t cap, uint64_t* out_n) try {
-    return groupby_sparse_distinct_call(c, "fbgpu_groupby_sparse_distinct", index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
-                                        SpDistinct{ xfield, xview, x_depth, x_values, nullptr, n_x }, filter, n_filter_ops, shards, n_shards,
-                                        start, end, out_cells, out_distinct, cap, out_n);
+    return groupby_sparse_call(c, "fbgpu_groupby_sparse_distinct", index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
+                               SpRequest{ {}, GvAgg::kDistinct, GvInt{ xfield, xview, x_depth, x_values, n_x }, filter, n_filter_ops, shards, n_shards, start, end, -1 },
+                               out_cells, out_distinct, nullptr, cap, out_n);
 } FBGPU_CATCH
 
 // the same with a set, mutex, bool or time field x: per cell, the number of listed rows of x holding a column of filter ∩ the
@@ -3174,9 +3236,10 @@ extern "C" int fbgpu_groupby_sparse_distinct_rows(fbgpu_ctx* c, uint32_t index, 
                                                   const uint64_t* x_rows, int32_t n_x, const fbgpu_op* filter, int32_t n_filter_ops,
                                                   const uint64_t* shards, int64_t n_shards, uint64_t start, uint64_t end,
                                                   uint64_t* out_cells, uint64_t* out_distinct, uint64_t cap, uint64_t* out_n) try {
-    return groupby_sparse_distinct_call(c, "fbgpu_groupby_sparse_distinct_rows", index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
-                                        SpDistinct{ xfield, xview, 0, nullptr, x_rows, n_x }, filter, n_filter_ops, shards, n_shards,
-                                        start, end, out_cells, out_distinct, cap, out_n);
+    return groupby_sparse_call(c, "fbgpu_groupby_sparse_distinct_rows", index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
+                               SpRequest{ {}, GvAgg::kDistinctRows, GvInt{ xfield, xview, 0, nullptr, n_x, x_rows }, filter, n_filter_ops, shards, n_shards,
+                                          start, end, -1 },
+                               out_cells, out_distinct, nullptr, cap, out_n);
 } FBGPU_CATCH
 
 // ------------------------------------------------------------------ comm

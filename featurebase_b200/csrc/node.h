@@ -334,78 +334,62 @@ extern "C" int fbgpu_node_groupby_sum(fbgpu_node* n, uint32_t index, const uint3
                                              filter, n_filter_ops, shards, n_shards }, out_counts, out_sums);
 } FBGPU_CATCH
 
-// GroupBy as a list of non-empty cells: every device lists its own shards' cells from `start` on, at most `limit`; the lists merge
-// by cell with the counts summed, and the window is cut after the merge.  Exact: a cell among the first K non-empty cells of the
-// node is among the first K of every device where it is non-empty, as for the all-rows branch of fbgpu_node_topn_cutoffs.
+// a sparse GroupBy node form (kCount or kSum): every device lists its own shards' cells with the same window; the lists merge by
+// cell with the counts and the (wrapping) sums added, and the window is cut after the merge.  Exact: a cell is listed on a device
+// exactly when its count there is non-zero, so a cell among the first K non-empty cells of the node is among the first K of every
+// device where it is non-empty, as for the all-rows branch of fbgpu_node_topn_cutoffs.
+static int node_groupby_sparse(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
+                               const uint64_t* row_ids_flat, const int32_t* n_rows, SpRequest q,
+                               uint64_t* out_cells, uint64_t* out_counts, int64_t* out_sums, uint64_t cap, uint64_t* out_n) {
+    int rc = groupby_sparse_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, q, out_cells, out_counts, out_sums, cap, out_n);
+    if (rc) return rc;
+    q.dims = gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows);
+    const NodeSplit sp = node_split(n, q.shards, q.n_shards);
+    std::vector<int> devs = node_owners(sp);
+    if (devs.empty()) devs.push_back(0);                 // no shard listed: still validate the filter
+    std::vector<SpResult> part(n->ctx.size());
+    rc = node_fan_out(n, devs, [&](int d) {
+        fbgpu_ctx* c = n->ctx[(size_t)d];
+        SpRequest qd = q; qd.shards = sp.shards[(size_t)d].data(); qd.n_shards = (int64_t)sp.shards[(size_t)d].size();
+        std::shared_lock<std::shared_mutex> lk;
+        int r = begin_query(c, lk); if (r) return r;
+        return groupby_sparse_run(c, index, qd, part[(size_t)d]);
+    });
+    if (rc) return rc;
+    std::vector<std::pair<uint64_t, std::pair<uint64_t, uint64_t>>> all;          // (cell, (count, sum))
+    for (int d : devs) {
+        const SpResult& p = part[(size_t)d];
+        for (size_t i = 0; i < p.cells.size(); i++) all.push_back({ p.cells[i], { p.counts[i], p.sums.empty() ? 0 : (uint64_t)p.sums[i] } });
+    }
+    std::sort(all.begin(), all.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
+    SpResult m;
+    for (const auto& e : all) {
+        if (!m.cells.empty() && m.cells.back() == e.first) { m.counts.back() += e.second.first; m.sums.back() = (int64_t)((uint64_t)m.sums.back() + e.second.second); }
+        else { m.cells.push_back(e.first); m.counts.push_back(e.second.first); m.sums.push_back((int64_t)e.second.second); }
+    }
+    const size_t keep = q.limit >= 0 ? std::min(m.cells.size(), (size_t)q.limit) : m.cells.size();
+    m.cells.resize(keep); m.counts.resize(keep); m.sums.resize(q.agg == GvAgg::kSum ? keep : 0);
+    return write_cells(m, out_cells, out_counts, out_sums, cap, out_n);
+}
+
+// fbgpu_groupby_sparse over a node: the non-empty cells from `start` on, at most `limit` of them, merged over the devices
 extern "C" int fbgpu_node_groupby_sparse(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views, int32_t n_fields,
                                          const uint64_t* row_ids_flat, const int32_t* n_rows, const fbgpu_op* filter, int32_t n_filter_ops,
                                          const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
                                          uint64_t* out_cells, uint64_t* out_counts, uint64_t cap, uint64_t* out_n) try {
-    int rc = groupby_sparse_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, filter, n_filter_ops, shards, n_shards,
-                                 out_cells, out_counts, cap, out_n);
-    if (rc) return rc;
-    const std::vector<GbDim> dims = gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows);
-    const NodeSplit sp = node_split(n, shards, n_shards);
-    std::vector<int> devs = node_owners(sp);
-    if (devs.empty()) devs.push_back(0);                 // no shard listed: still validate the filter
-    std::vector<std::vector<uint64_t>> cells(n->ctx.size()), counts(n->ctx.size());
-    rc = node_fan_out(n, devs, [&](int d) {
-        fbgpu_ctx* c = n->ctx[(size_t)d];
-        const auto& s = sp.shards[(size_t)d];
-        std::shared_lock<std::shared_mutex> lk;
-        int r = begin_query(c, lk); if (r) return r;
-        return groupby_sparse_run(c, index, dims, filter, n_filter_ops, s.data(), (int64_t)s.size(), start, limit, cells[(size_t)d], counts[(size_t)d]);
-    });
-    if (rc) return rc;
-    std::vector<std::pair<uint64_t, uint64_t>> all;
-    for (int d : devs) for (size_t i = 0; i < cells[(size_t)d].size(); i++) all.emplace_back(cells[(size_t)d][i], counts[(size_t)d][i]);
-    std::sort(all.begin(), all.end());
-    std::vector<uint64_t> mc, mn;
-    for (const auto& p : all) {
-        if (!mc.empty() && mc.back() == p.first) mn.back() += p.second;
-        else { mc.push_back(p.first); mn.push_back(p.second); }
-    }
-    if (limit >= 0 && mc.size() > (uint64_t)limit) { mc.resize((size_t)limit); mn.resize((size_t)limit); }
-    return write_cells(mc, mn, out_cells, out_counts, cap, out_n);
+    return node_groupby_sparse(n, index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
+                               SpRequest{ {}, GvAgg::kCount, {}, filter, n_filter_ops, shards, n_shards, start, ~0ull, limit },
+                               out_cells, out_counts, nullptr, cap, out_n);
 } FBGPU_CATCH
 
-// fbgpu_node_groupby_sparse with a Sum: every device lists its own shards' cells with the same window; the lists merge by cell
-// with counts and sums added (the sums wrap), and the window is cut after the merge.  Exact for the reason given above: a cell is
-// listed on a device exactly when its count there is non-zero, and its node count is the sum of those.
+// fbgpu_groupby_sparse_sum over a node: the same window, with each listed cell's wrapping sum merged beside its count
 extern "C" int fbgpu_node_groupby_sparse_sum(fbgpu_node* n, uint32_t index, const uint32_t* fields, const uint32_t* views_flat, const int32_t* n_views,
                                              int32_t n_fields, const uint64_t* row_ids_flat, const int32_t* n_rows, uint32_t afield, uint32_t aview, int32_t a_depth,
                                              const fbgpu_op* filter, int32_t n_filter_ops, const uint64_t* shards, int64_t n_shards, uint64_t start, int64_t limit,
                                              uint64_t* out_cells, uint64_t* out_counts, int64_t* out_sums, uint64_t cap, uint64_t* out_n) try {
-    int rc = groupby_sparse_sum_args(n, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows, a_depth, filter, n_filter_ops, shards, n_shards,
-                                     out_cells, out_counts, out_sums, cap, out_n);
-    if (rc) return rc;
-    const std::vector<GbDim> dims = gb_set_dims(fields, views_flat, n_views, n_fields, row_ids_flat, n_rows);
-    const SpAgg agg{ afield, aview, a_depth };
-    const NodeSplit sp = node_split(n, shards, n_shards);
-    std::vector<int> devs = node_owners(sp);
-    if (devs.empty()) devs.push_back(0);                 // no shard listed: still validate the filter
-    std::vector<std::vector<uint64_t>> cells(n->ctx.size()), counts(n->ctx.size());
-    std::vector<std::vector<int64_t>> sums(n->ctx.size());
-    rc = node_fan_out(n, devs, [&](int d) {
-        fbgpu_ctx* c = n->ctx[(size_t)d];
-        const auto& s = sp.shards[(size_t)d];
-        std::shared_lock<std::shared_mutex> lk;
-        int r = begin_query(c, lk); if (r) return r;
-        return groupby_sparse_run(c, index, dims, filter, n_filter_ops, s.data(), (int64_t)s.size(), start, limit, cells[(size_t)d], counts[(size_t)d],
-                                  &agg, &sums[(size_t)d]);
-    });
-    if (rc) return rc;
-    std::vector<std::pair<uint64_t, std::pair<uint64_t, uint64_t>>> all;
-    for (int d : devs)
-        for (size_t i = 0; i < cells[(size_t)d].size(); i++) all.push_back({ cells[(size_t)d][i], { counts[(size_t)d][i], (uint64_t)sums[(size_t)d][i] } });
-    std::sort(all.begin(), all.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
-    std::vector<uint64_t> mc, mn; std::vector<int64_t> ms;
-    for (const auto& p : all) {
-        if (!mc.empty() && mc.back() == p.first) { mn.back() += p.second.first; ms.back() = (int64_t)((uint64_t)ms.back() + p.second.second); }
-        else { mc.push_back(p.first); mn.push_back(p.second.first); ms.push_back((int64_t)p.second.second); }
-    }
-    if (limit >= 0 && mc.size() > (uint64_t)limit) { mc.resize((size_t)limit); mn.resize((size_t)limit); ms.resize((size_t)limit); }
-    return write_cells(mc, mn, ms, out_cells, out_counts, out_sums, cap, out_n);
+    return node_groupby_sparse(n, index, fields, views_flat, n_views, n_fields, row_ids_flat, n_rows,
+                               SpRequest{ {}, GvAgg::kSum, GvInt{ afield, aview, a_depth, nullptr, 0 }, filter, n_filter_ops, shards, n_shards, start, ~0ull, limit },
+                               out_cells, out_counts, out_sums, cap, out_n);
 } FBGPU_CATCH
 
 // Sum / Min / Max of an int field: per-device partials merged as ValCount.Add / Smaller / Larger do (executor.go:8446-8560)

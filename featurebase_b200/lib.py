@@ -4,6 +4,7 @@ import ctypes as C
 import os
 import threading
 import types
+from functools import partial
 
 import numpy as np
 
@@ -647,28 +648,13 @@ class Context:
         sums): a count is the number of the cell's columns holding a value of x, a cell is listed when it is non-zero, and sums
         (int64) are the wrapping sums of those columns' stored values (value - Base)."""
         g = _groupby_args(set_dims, [], shards, filter_ops)
-        n = C.c_uint64(0)
         cap = max(getattr(self, "_sparse_cap", 0), 1 << 12) if limit is None else max(min(int(limit), 1 << 16), 1)
-        lim = -1 if limit is None else int(limit)
-        while True:
-            cells, counts = np.empty(cap, dtype=np.uint64), np.empty(cap, dtype=np.uint64)
-            if agg is None:
-                rc = self.L.fbgpu_groupby_sparse(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, g.filter, g.n_filter,
-                                                 g.shards, g.n_shards, int(start), lim, cells.ctypes.data, counts.ctypes.data, cap, C.byref(n))
-            else:
-                sums = np.empty(cap, dtype=np.int64)
-                rc = self.L.fbgpu_groupby_sparse_sum(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows,
-                                                     int(agg[0]), int(agg[1]), int(agg[2]), g.filter, g.n_filter, g.shards, g.n_shards,
-                                                     int(start), lim, cells.ctypes.data, counts.ctypes.data, sums.ctypes.data, cap, C.byref(n))
-            if rc == E_NOSPACE:
-                cap = int(n.value)
-                continue
-            self._check(rc)
-            if limit is None:
-                self._sparse_cap = cap
-            if agg is None:
-                return cells[: n.value].copy(), counts[: n.value].copy()
-            return cells[: n.value].copy(), counts[: n.value].copy(), sums[: n.value].copy()
+        head = (self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows)
+        tail = (g.filter, g.n_filter, g.shards, g.n_shards, int(start), -1 if limit is None else int(limit))
+        if agg is None:
+            return self._sparse_list(partial(self.L.fbgpu_groupby_sparse, *head, *tail), (np.uint64, np.uint64), cap, limit is None)
+        return self._sparse_list(partial(self.L.fbgpu_groupby_sparse_sum, *head, int(agg[0]), int(agg[1]), int(agg[2]), *tail),
+                                 (np.uint64, np.uint64, np.int64), cap, limit is None)
 
     def groupby_sparse_distinct(self, index, set_dims, x, shards, filter_ops=None, start=0, end=None):
         """GroupBy(..., aggregate=Count(Distinct(field=x))) over groupby_sparse's dimensions (1..7 of them), x an int field, in one
@@ -684,26 +670,31 @@ class Context:
 
     def _groupby_sparse_distinct(self, index, set_dims, x, shards, filter_ops, start, end, rows):
         g = _groupby_args(set_dims, [], shards, filter_ops)
-        xs = _u64arr(x[2]) if rows else np.ascontiguousarray(np.asarray(x[3], dtype=np.int64))
-        end = (1 << 64) - 1 if end is None else int(end)
+        head = (self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, int(x[0]), int(x[1]))
+        tail = (g.filter, g.n_filter, g.shards, g.n_shards, int(start), (1 << 64) - 1 if end is None else int(end))
+        if rows:
+            xs = _u64arr(x[2])
+            call = partial(self.L.fbgpu_groupby_sparse_distinct_rows, *head, xs.ctypes.data, len(xs), *tail)
+        else:
+            xs = np.ascontiguousarray(np.asarray(x[3], dtype=np.int64))
+            call = partial(self.L.fbgpu_groupby_sparse_distinct, *head, int(x[2]), xs.ctypes.data, len(xs), *tail)
+        return self._sparse_list(call, (np.uint64, np.uint64), max(getattr(self, "_sparse_cap", 0), 1 << 12), True)
+
+    def _sparse_list(self, call, dtypes, cap, remember):
+        """call(*outputs, cap, &n) under the NOSPACE contract: on E_NOSPACE the outputs (one array per dtype) grow to the n it
+        reports and the call runs again.  Returns the outputs cut to n; with `remember` the cap that fitted is the next call's
+        starting cap."""
         n = C.c_uint64(0)
-        cap = max(getattr(self, "_sparse_cap", 0), 1 << 12)
         while True:
-            cells, distinct = np.empty(cap, dtype=np.uint64), np.empty(cap, dtype=np.uint64)
-            if rows:
-                rc = self.L.fbgpu_groupby_sparse_distinct_rows(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, int(x[0]), int(x[1]),
-                                                               xs.ctypes.data, len(xs), g.filter, g.n_filter, g.shards, g.n_shards, int(start), end,
-                                                               cells.ctypes.data, distinct.ctypes.data, cap, C.byref(n))
-            else:
-                rc = self.L.fbgpu_groupby_sparse_distinct(self.h, index, g.fields, g.views, g.n_views, g.n_fields, g.rows, g.n_rows, int(x[0]), int(x[1]),
-                                                          int(x[2]), xs.ctypes.data, len(xs), g.filter, g.n_filter, g.shards, g.n_shards, int(start), end,
-                                                          cells.ctypes.data, distinct.ctypes.data, cap, C.byref(n))
-            if rc == E_NOSPACE:
-                cap = int(n.value)
-                continue
-            self._check(rc)
+            out = [np.empty(cap, dtype=t) for t in dtypes]
+            rc = call(*[a.ctypes.data for a in out], cap, C.byref(n))
+            if rc != E_NOSPACE:
+                break
+            cap = int(n.value)
+        self._check(rc)
+        if remember:
             self._sparse_cap = cap
-            return cells[: n.value].copy(), distinct[: n.value].copy()
+        return tuple(a[: n.value].copy() for a in out)
 
     def rows_payload_bytes(self, index, field, view, shards, row_ids=None):
         sh = _u64arr(shards)
